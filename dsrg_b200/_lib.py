@@ -86,6 +86,14 @@ SIGNATURES = {
     "dsrg_seedloss_backward_host": (_i, [_vp, _i, _i, _vp, _vp, _f, _vp]),
     "dsrg_seedloss_forward_dev": (_i, [_vp, _i, _vp, _vp, _vp, _vp]),
     "dsrg_seedloss_backward_dev": (_i, [_vp, _i, _i, _vp, _vp, _f, _vp, _vp]),
+    "dsrg_seedloss_plain_forward_dev": (_i, [_vp, _i, _vp, _vp, _vp, _vp]),
+    "dsrg_seedloss_plain_backward_dev": (_i, [_vp, _i, _i, _vp, _vp, _vp, _vp]),
+    "dsrg_seedloss_plain_forward_host": (_i, [_vp, _i, _vp, _vp, _vp]),
+    "dsrg_seedloss_plain_backward_host": (_i, [_vp, _i, _i, _vp, _vp, _vp]),
+    "dsrg_expandloss_forward_dev": (_i, [_vp, _i, _vp, _vp, _d, _d, _vp, _vp]),
+    "dsrg_expandloss_backward_dev": (_i, [_vp, _i, _i, _vp, _vp, _d, _d, _vp, _vp]),
+    "dsrg_expandloss_forward_host": (_i, [_vp, _i, _vp, _vp, _d, _d, _vp]),
+    "dsrg_expandloss_backward_host": (_i, [_vp, _i, _i, _vp, _vp, _d, _d, _vp]),
     "dsrg_profile_tag_count": (_i, []),
     "dsrg_profile_tag_name": (C.c_char_p, [_i]),
     "dsrg_engine_profile": (_i, [_vp, _i]),

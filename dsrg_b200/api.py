@@ -179,6 +179,63 @@ class Engine(object):
                                                  float(top_diff), _dptr(grad_out), _stream(stream)))
         return grad_out
 
+    # ---- SEC losses: SeedLossLayer / ExpandLossLayer (pylayers.py:95-118, :183-233) ----
+    def seedloss_plain_forward_dev(self, probs, seeds, terms_out, stream=None):
+        """terms_out[0] = sum_n S(n) / cnt(n); loss = -terms[0] / N_global."""
+        B = probs.shape[0]
+        check(self._L.dsrg_seedloss_plain_forward_dev(self.h, B, _dptr(probs), _dptr(seeds), _dptr(terms_out),
+                                                      _stream(stream)))
+        return terms_out
+
+    def seedloss_plain_backward_dev(self, probs, seeds, grad_out, n_global=None, stream=None):
+        B = probs.shape[0]
+        check(self._L.dsrg_seedloss_plain_backward_dev(self.h, B, int(n_global or B), _dptr(probs), _dptr(seeds),
+                                                       _dptr(grad_out), _stream(stream)))
+        return grad_out
+
+    def expandloss_forward_dev(self, probs, labels, terms_out, q_fg=0.996, q_bg=0.999, stream=None):
+        """terms_out (3 floats): the local sums of the three terms; loss = -sum(terms) / N_global."""
+        B = probs.shape[0]
+        check(self._L.dsrg_expandloss_forward_dev(self.h, B, _dptr(probs), _dptr(labels), float(q_fg), float(q_bg),
+                                                  _dptr(terms_out), _stream(stream)))
+        return terms_out
+
+    def expandloss_backward_dev(self, probs, labels, grad_out, n_global=None, q_fg=0.996, q_bg=0.999, stream=None):
+        B = probs.shape[0]
+        check(self._L.dsrg_expandloss_backward_dev(self.h, B, int(n_global or B), _dptr(probs), _dptr(labels),
+                                                   float(q_fg), float(q_bg), _dptr(grad_out), _stream(stream)))
+        return grad_out
+
+    def seedloss_plain_forward_host(self, probs, seeds):
+        terms = np.zeros(1, np.float32)
+        check(self._L.dsrg_seedloss_plain_forward_host(self.h, probs.shape[0], _hptr(probs, np.float32),
+                                                       _hptr(seeds, np.float32), _hptr(terms, np.float32)))
+        return terms
+
+    def seedloss_plain_backward_host(self, probs, seeds, n_global=None, grad=None):
+        if grad is None:
+            grad = np.empty(probs.shape, np.float32)
+        check(self._L.dsrg_seedloss_plain_backward_host(self.h, probs.shape[0], int(n_global or probs.shape[0]),
+                                                        _hptr(probs, np.float32), _hptr(seeds, np.float32),
+                                                        _hptr(grad, np.float32)))
+        return grad
+
+    def expandloss_forward_host(self, probs, labels, q_fg=0.996, q_bg=0.999):
+        """labels: (B,1,1,M) or (B,M) float32 -> the three local sums (see expandloss_forward_dev)."""
+        terms = np.zeros(3, np.float32)
+        check(self._L.dsrg_expandloss_forward_host(self.h, probs.shape[0], _hptr(probs, np.float32),
+                                                   _hptr(labels, np.float32), float(q_fg), float(q_bg),
+                                                   _hptr(terms, np.float32)))
+        return terms
+
+    def expandloss_backward_host(self, probs, labels, n_global=None, q_fg=0.996, q_bg=0.999, grad=None):
+        if grad is None:
+            grad = np.empty(probs.shape, np.float32)
+        check(self._L.dsrg_expandloss_backward_host(self.h, probs.shape[0], int(n_global or probs.shape[0]),
+                                                    _hptr(probs, np.float32), _hptr(labels, np.float32),
+                                                    float(q_fg), float(q_bg), _hptr(grad, np.float32)))
+        return grad
+
     # ---- host entry points (numpy; H2D / D2H inside the call) ----
     def crf_host(self, unary, image, params, out=None, unary_layout=LAYOUT_NHWC, out_layout=LAYOUT_NHWC):
         B = image.shape[0]

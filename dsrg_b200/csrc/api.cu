@@ -406,6 +406,11 @@ dsrg_engine *dsrg_engine_create(int device, int max_batch, int H, int W, int M) 
     rc |= dalloc(e, &e->parent, bn);
     rc |= dalloc(e, &e->hc, bn);
     rc |= dalloc(e, &e->loss_acc, (size_t)max_batch * 4);
+    e->sec_wcap = e->Ncap < DSRG_GWRP_MAX_PLANE ? e->Ncap : DSRG_GWRP_MAX_PLANE;
+    rc |= dalloc(e, &e->sec_rec, (size_t)max_batch * M);
+    rc |= dalloc(e, &e->sec_img, (size_t)max_batch * 3);
+    rc |= dalloc(e, &e->sec_part, (size_t)max_batch * kSecPlainChunks);
+    rc |= dalloc(e, &e->sec_w, (size_t)2 * e->sec_wcap);
     rc |= dalloc(e, &e->dev_err, 1);
     rc |= dalloc(e, &e->hy_list, (size_t)max_batch * e->ntiles);
     rc |= dalloc(e, &e->hy_count, 1);
@@ -439,8 +444,8 @@ void dsrg_engine_destroy(dsrg_engine *h) {
     lattice_free(e->sp);
     lattice_free(e->bi);
     void *ptrs[] = {e->U, e->Q0, e->spA, e->spB, e->spC, e->biA, e->biB, e->biC, e->nvA, e->nvB, e->lmap,
-                    e->lflag, e->parent, e->hc, e->loss_acc, e->dev_err, e->hy_list, e->hy_count, e->st_unary, e->st_out,
-                    e->st_cues, e->st_labels, e->st_image, e->st_lmap, e->st_raw, e->st_idx};
+                    e->lflag, e->parent, e->hc, e->loss_acc, e->sec_rec, e->sec_img, e->sec_part, e->sec_w, e->dev_err,
+                    e->hy_list, e->hy_count, e->st_unary, e->st_out, e->st_cues, e->st_labels, e->st_image, e->st_lmap, e->st_raw, e->st_idx};
     for (void *p : ptrs) cudaFree(p);
     if (e->own_stream) cudaStreamDestroy(e->own_stream);
     if (e->in_stream) cudaStreamDestroy(e->in_stream);

@@ -157,6 +157,8 @@ int seedloss_forward(Engine *e, int B, const float *probs, const float *seeds, f
                      cudaStream_t s);
 int seedloss_backward(Engine *e, int B, int n_global, const float *probs, const float *seeds,
                       float top_diff, float *grad, cudaStream_t s);
+// ---- sec_loss.cu ----
+constexpr int kSecPlainChunks = 16;  // CTAs per image of SeedLossLayer's sums (fixed, so is their order)
 
 struct Engine {
     int device = 0;
@@ -189,6 +191,15 @@ struct Engine {
     uint8_t *hc = nullptr;     // [B][N] high-confidence flag per root
     // loss scratch
     double *loss_acc = nullptr;  // [B][4]
+    // SEC losses (sec_loss.cu): per-plane GWRP records, per-image sums, SeedLoss partials, the q^i tables
+    double2 *sec_rec = nullptr;   // [B][M] (G, max)
+    double *sec_img = nullptr;    // [B][3]
+    double2 *sec_part = nullptr;  // [B][kSecPlainChunks]
+    double *sec_w = nullptr;      // [2][sec_wcap]: q_fg table, then q_bg table
+    int sec_wcap = 0;             // min(Ncap, DSRG_GWRP_MAX_PLANE)
+    double sec_q[2] = {0, 0}, sec_z[2] = {0, 0};
+    int sec_n[2] = {0, 0};        // (q, n) the device tables hold; 0 = none yet
+    std::vector<double> sec_w_host[2];
     // staging for the *_host entry points
     float *st_unary = nullptr, *st_out = nullptr, *st_cues = nullptr, *st_labels = nullptr;
     uint8_t *st_image = nullptr;

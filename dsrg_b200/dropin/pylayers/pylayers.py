@@ -11,6 +11,9 @@ in train-s.prototxt:746-812 keeps working:
 * ``SoftmaxLayer`` / ``ConstrainLossLayer`` (pylayers.py:23-51, :154-180), the producer and the
   other consumer of the hot path's blobs (SURVEY 8f rank 1) -> dsrg_softmax_* / dsrg_constrainloss_*,
   so that the module covers every Python layer train-s.prototxt names except the data layer.
+* ``SeedLossLayer`` / ``ExpandLossLayer`` (pylayers.py:95-118, :183-233), SEC's seeding and expansion losses
+  (the seed-loss blocks train-s.prototxt:821-910 keeps commented out, and SEC-style baselines)
+  -> dsrg_seedloss_plain_* / dsrg_expandloss_*.
 
 The blobs Caffe hands to a Python layer are host numpy views, so the ``*_host`` entry points of
 the C ABI are used: one H2D of the bottoms and one D2H of the tops per call, everything else --
@@ -186,6 +189,67 @@ class BalancedSeedLossLayer(caffe.Layer):
         # like the reference (pylayers.py:150-152) the incoming top diff is NOT applied
         bottom[0].diff[...] = _engine(n, c, h, w).seedloss_backward_host(_f32(bottom[0].data), _f32(bottom[1].data),
                                                                            n_global=n_global, top_diff=1.0)
+
+
+class SeedLossLayer(caffe.Layer):
+    """pylayers.py:95-118, SEC's seeding loss -> dsrg_seedloss_plain_{forward,backward}_host.  The mean over this
+    solver's batch of sum(lab log p) / sum(lab); no floor on the count, so an image without seeds gives NaN like the
+    reference."""
+
+    def setup(self, bottom, top):
+        if len(bottom) != 2:
+            raise Exception("The layer needs two inputs!")
+
+    def reshape(self, bottom, top):
+        top[0].reshape(1)
+
+    def forward(self, bottom, top):
+        n = bottom[0].data.shape[0]
+        terms = _engine(*bottom[0].data.shape).seedloss_plain_forward_host(_f32(bottom[0].data), _f32(bottom[1].data))
+        top[0].data[...] = -float(terms[0]) / n
+
+    def backward(self, top, prop_down, bottom):
+        # like the reference (pylayers.py:116-118) the incoming top diff is NOT applied
+        bottom[0].diff[...] = _engine(*bottom[0].data.shape).seedloss_plain_backward_host(_f32(bottom[0].data),
+                                                                                          _f32(bottom[1].data))
+
+
+class ExpandLossLayer(caffe.Layer):
+    """pylayers.py:183-233, SEC's expansion loss (global weighted rank pooling, q_fg = 0.996, q_bg = 0.999)
+    -> dsrg_expandloss_{forward,backward}_host.  Bottoms: probs (N, 21, 41, 41) and the labels blob (N, 1, 1, 21).
+    The reference's graph reshapes to (-1, 20, 41*41) (:201, :208): any other shape fails inside Theano or mixes
+    planes of different images, so it is refused here."""
+
+    Q_FG, Q_BG = 0.996, 0.999   # pylayers.py:200, :207
+
+    def setup(self, bottom, top):
+        if len(bottom) != 2:
+            raise Exception("The layer needs two inputs!")
+
+    def reshape(self, bottom, top):
+        top[0].reshape(1)
+
+    @staticmethod
+    def _check(bottom):
+        shape = bottom[0].data.shape
+        if len(shape) != 4 or shape[1] != 21 or shape[2] * shape[3] != 41 * 41:
+            raise Exception("ExpandLossLayer needs probs of shape (N, 21, H, W) with H*W = 41*41 (pylayers.py:201), "
+                            "got %s" % (shape,))
+        if bottom[1].data.size != shape[0] * 21:
+            raise Exception("ExpandLossLayer needs labels of shape (N, 1, 1, 21), got %s" % (bottom[1].data.shape,))
+        return shape
+
+    def forward(self, bottom, top):
+        shape = self._check(bottom)
+        terms = _engine(*shape).expandloss_forward_host(_f32(bottom[0].data), _f32(bottom[1].data),
+                                                        self.Q_FG, self.Q_BG)
+        top[0].data[...] = -(float(terms[0]) + float(terms[1]) + float(terms[2])) / shape[0]
+
+    def backward(self, top, prop_down, bottom):
+        shape = self._check(bottom)
+        # like the reference (pylayers.py:231-233) the incoming top diff is NOT applied
+        bottom[0].diff[...] = _engine(*shape).expandloss_backward_host(_f32(bottom[0].data), _f32(bottom[1].data),
+                                                                       q_fg=self.Q_FG, q_bg=self.Q_BG)
 
 
 def _allreduce_terms(terms, n_local):

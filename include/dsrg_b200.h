@@ -39,6 +39,9 @@ extern "C" {
  * DenseCRF(W, H, 81), training/tools/test-coco.py.  The Softmax / ConstrainLoss layers and the predict_mask
  * post-processing are built for at most DSRG_MAX_LABELS. */
 #define DSRG_MAX_LABELS_WIDE 255
+/* pixels per class plane the GWRP kernels of dsrg_expandloss_* sort in shared memory (41x41 and the 65x65 maps
+ * of a 513 crop fit; larger planes return DSRG_E_INVALID) */
+#define DSRG_GWRP_MAX_PLANE 8192
 
 int dsrg_version(void);               /* 10000*major + 100*minor + patch */
 const char *dsrg_last_error(void);    /* message of the last failing call on this thread */
@@ -311,6 +314,44 @@ int dsrg_seedloss_forward_host(dsrg_engine *e, int B, const float *probs_host,
                                const float *seeds_host, float *terms_out_host /* 2 floats */);
 int dsrg_seedloss_backward_host(dsrg_engine *e, int B, int n_global, const float *probs_host,
                                 const float *seeds_host, float top_diff, float *grad_out_host);
+
+/*
+ * SeedLossLayer (pylayers.py:95-118), SEC's plain seeding loss: loss = -mean_n S(n) / cnt(n) with
+ * S(n) = sum_{c,h,w} lab log p and cnt(n) = sum lab -- no max(cnt, 1e-4) floor, so an image without seeds gives
+ * NaN like the reference.  Forward writes the LOCAL sum terms_out[0] = sum_n S(n) / cnt(n), so that
+ * loss = -terms[0] / N_global.  Backward writes d loss / d probs = -lab / (p * cnt * N_global); the layer's top
+ * diff is not applied (the reference ignores it).
+ */
+int dsrg_seedloss_plain_forward_dev(dsrg_engine *e, int B, const float *probs_dev, const float *seeds_dev,
+                                    float *terms_out_dev /* 1 float */, void *stream);
+int dsrg_seedloss_plain_backward_dev(dsrg_engine *e, int B, int n_global, const float *probs_dev,
+                                     const float *seeds_dev, float *grad_out_dev, void *stream);
+int dsrg_seedloss_plain_forward_host(dsrg_engine *e, int B, const float *probs_host, const float *seeds_host,
+                                     float *terms_out_host /* 1 float */);
+int dsrg_seedloss_plain_backward_host(dsrg_engine *e, int B, int n_global, const float *probs_host,
+                                      const float *seeds_host, float *grad_out_host);
+
+/*
+ * ExpandLossLayer (pylayers.py:183-233), SEC's expansion loss by global weighted rank pooling (GWRP).  probs
+ * [B][M][H][W] (channel 0 = background), labels [B][M] (the N x 1 x 1 M labels blob; class k >= 1 is present when
+ * labels > 0.5).  G_q(x) = sum_i sort(x)_i q^(n-1-i) / Z, Z = sum_i q^i, n = H*W <= DSRG_GWRP_MAX_PLANE; the
+ * reference's q_fg = 0.996, q_bg = 0.999 (:200, :207).  Forward writes the LOCAL sums
+ *   terms_out[0] = sum_n sum_k s_k log G_fg(p_k) / P,  terms_out[1] = sum_n sum_k (1-s_k) log(1 - max p_k) / A,
+ *   terms_out[2] = sum_n log G_bg(p_0)
+ * (P, A: present / absent foreground classes of image n), so that loss = -(terms[0]+terms[1]+terms[2]) / N_global.
+ * Backward writes d loss / d probs as Theano's T.grad forms it: through the sort permutation and, IN FULL, to every
+ * element equal to a plane's max; P = 0 or A = 0 makes the loss NaN and the image's foreground gradient NaN.
+ * Both are deterministic: two identical calls give bit-identical results.
+ */
+int dsrg_expandloss_forward_dev(dsrg_engine *e, int B, const float *probs_dev, const float *labels_dev, double q_fg,
+                                double q_bg, float *terms_out_dev /* 3 floats */, void *stream);
+int dsrg_expandloss_backward_dev(dsrg_engine *e, int B, int n_global, const float *probs_dev,
+                                 const float *labels_dev, double q_fg, double q_bg, float *grad_out_dev,
+                                 void *stream);
+int dsrg_expandloss_forward_host(dsrg_engine *e, int B, const float *probs_host, const float *labels_host,
+                                 double q_fg, double q_bg, float *terms_out_host /* 3 floats */);
+int dsrg_expandloss_backward_host(dsrg_engine *e, int B, int n_global, const float *probs_host,
+                                  const float *labels_host, double q_fg, double q_bg, float *grad_out_host);
 
 /* Optional per-kernel timing for the roofline report: while enabled every kernel launch of the
  * engine is bracketed by CUDA events on its launching stream.  dsrg_engine_profile_read()
