@@ -104,7 +104,8 @@ static int lattice_alloc(Engine *e, Lattice &L, int d, int shared) {
     const size_t nt = n * e->ntiles;
     rc |= dalloc(e, &L.tl_nloc, nt);
     rc |= dalloc(e, &L.tl_hy, nt);
-    L.entcap = kTileThreads * (d + 1) + L.maxloc;  // every segment is padded to an even entry count
+    // every segment is padded to an even entry count; a tile's block starts on 16 bytes (8 entries)
+    L.entcap = (kTileThreads * (d + 1) + L.maxloc + 7) & ~7;
     rc |= dalloc(e, &L.tl_hdr, nt * L.maxloc);
     rc |= dalloc(e, &L.tl_pack, nt * L.entcap);
     rc |= dalloc(e, &L.tl_loc, n * (d + 1) * L.N);

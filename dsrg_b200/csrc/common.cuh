@@ -60,9 +60,9 @@ struct Lattice {
     int32_t *tl_nloc = nullptr;    // [nimg][ntiles] local vertices of the tile; | kTileHybrid: hybrid tile; -1: overflow tile without a list
     uint8_t *tl_hy = nullptr;      // [nimg][ntiles] 1: hybrid tile, k_mf_tile skips it (bilateral only)
     int2 *tl_hdr = nullptr;        // [nimg][ntiles][maxloc] per local vertex: (first entry | count<<16, local row id)
-    int2 *tl_pack = nullptr;       // [nimg][ntiles][entcap] CSR entries grouped by local vertex:
-                                   // (byte offset of the pixel's Q row in the tile, weight bits)
-    int entcap = 0;                // 256*(d+1) + 2
+    uint16_t *tl_pack = nullptr;   // [nimg][ntiles][entcap] CSR entries grouped by local vertex:
+                                   // r << 8 | pixel's thread index in the tile (see kEntZero)
+    int entcap = 0;                // 256*(d+1) + maxloc, a multiple of 8 (16-byte blocks for the bulk copy)
     uint16_t *tl_loc = nullptr;    // [nimg][d+1][N] local vertex index of (pixel, r), kLocRemote if not in the tile's list
     float *wn = nullptr;           // [nimg][d+1][N] barycentric weight * norm
     float scale[5] = {0, 0, 0, 0, 0};  // elevation scale factors (permutohedral.cpp:179-182)
@@ -118,6 +118,14 @@ constexpr int kSplatUnroll = DSRG_SPLAT_UNROLL;
 // tl_loc value of a (pixel, vertex) incidence that is NOT in the tile-local list, and the flag in tl_nloc of a tile
 // that has such incidences (a hybrid tile, tiles.cu)
 constexpr int kLocRemote = 0xFFFF, kTileHybrid = 1 << 16;
+// A CSR entry (tl_pack) is 16 bits, r << 8 | t: t is the pixel's thread index in the tile (its Q row), r its
+// incidence index in one index space for both lattices (spatial 0..2, bilateral 3..8).  The mean-field kernels
+// keep the weights of the current tile in a shared table wtab[r][kTileThreads], so the entry indexes it directly;
+// the padding entry that evens a segment out points at the table's zero slot.
+static_assert(kTileThreads == 256, "the entry's low byte is the thread index");
+constexpr int kEntRows = 9;
+constexpr int kEntZero = kEntRows << 8;  // wtab[kEntZero] = 0; its Q row (t = 0) is a valid one
+__host__ __device__ constexpr int ent_r0(int dp1) { return dp1 == 3 ? 0 : 3; }  // first r of a lattice
 // an overflow tile becomes a hybrid one when its local list would cover at least this share (percent) of its
 // incidences; below that (uniform-noise images, the sigma/12 training lattices) the plain direct path is faster
 // ... and only when the batch has at least DSRG_HY_MIN_TILES hybrid tiles per SM (tiles.cu: k_tile_demote)

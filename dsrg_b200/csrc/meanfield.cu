@@ -85,7 +85,7 @@ struct TileLat {
     const int32_t *tl_nloc;
     const uint8_t *tl_hy;    // [nimg][ntiles] 1: hybrid tile (bilateral view only)
     const int2 *tl_hdr;
-    const int2 *tl_pack;
+    const uint16_t *tl_pack;
     const uint16_t *tl_loc;
     const float *wn;         // [nimg][dp1][N]
     const float *val_in;     // blurred values of the previous splat (slice source)
@@ -148,17 +148,39 @@ struct TileRow {
     static constexpr int CHP = CH + DSRG_ROW_PAD;  // float4 per staged row (padded)
 };
 
+// A tile's staging area: its local vertices' value rows (later its Q rows), its CSR entry blocks and the mbarrier
+// the bulk copies complete on; TileSmem adds the weight table the entries index.
 template <int MP, int MAXBI = kMaxLocBi>
-struct TileSmem {
+struct TileStage {
     static constexpr int CH = MP / 4;
     static constexpr int CHP = TileRow<MP>::CHP;
     static constexpr int kRows = kMaxLocSp + MAXBI;
     static constexpr int kBufF4 = (kRows * CHP > kTileThreads * CHP) ? kRows * CHP : kTileThreads * CHP;  // staged rows / Q alias
-    static constexpr int kEntSp = kTileThreads * 3 + kMaxLocSp, kEntBi = kTileThreads * 6 + MAXBI;  // segments padded to even
+    // segments padded to even, each block a whole number of 16-byte units
+    static constexpr int kEntSp = (kTileThreads * 3 + kMaxLocSp + 7) & ~7, kEntBi = (kTileThreads * 6 + MAXBI + 7) & ~7;
     float4 buf[kBufF4];
-    int2 ent[kEntSp + kEntBi];  // CSR entries (byte offset of the pixel's Q row, weight bits)
+    uint16_t ent[kEntSp + kEntBi];  // CSR entries (r << 8 | thread, common.cuh:kEntZero)
     uint64_t bar;
 };
+
+template <int MP, int MAXBI = kMaxLocBi>
+struct TileSmem {
+    TileStage<MP, MAXBI> st;
+    float wtab[kEntZero + 4];  // [r][thread] weights of the tile being splatted, then the zero slot
+};
+
+// the size of a lattice's CSR entry block as bulk-copied, from the header of its last segment
+__device__ __forceinline__ uint32_t ent_block_bytes(int2 last) {
+    return ((uint32_t)((last.x & 0xffff) + (((last.x >> 16) + 1) & ~1)) * 2u + 15u) & ~15u;
+}
+
+// the current tile's weights into the table its CSR entries index; the CTA's thread t is the tile's pixel t
+__device__ __forceinline__ void tile_put_weights(float *wtab, const float *w_sp, const float *w_bi) {
+#pragma unroll
+    for (int r = 0; r < 3; r++) wtab[(ent_r0(3) + r) * kTileThreads + threadIdx.x] = w_sp[r];
+#pragma unroll
+    for (int r = 0; r < 6; r++) wtab[(ent_r0(6) + r) * kTileThreads + threadIdx.x] = w_bi[r];
+}
 
 // slice one lattice from the staged rows (shared memory): t += coef * sum_r wn_r * row_r
 // tail1: M = MP - 3 (e.g. 21 labels in 24 lanes): the last chunk holds ONE real channel, so a 32-bit load
@@ -264,12 +286,13 @@ __device__ __forceinline__ unsigned tile_remote_mask(const uint16_t *loc, size_t
 // CSR splat of both lattices: one thread per (local vertex, label quad) walks the vertex's segment
 // serially and issues ONE vector reduction; vertices are ordered by segment length (tiles.cu), so the
 // lanes of a warp run similar trip counts, and no cross-lane reduction is needed.
+// An entry e names the pixel's Q row (e & 255) and its weight wtab[e].
 template <int MP>
 __device__ __forceinline__ void tile_splat_csr(float4 *vout_sp, float4 *vout_bi, int n_sp, int n_bi,
                                                const int2 *hdr_sp, const int2 *hdr_bi, int base_sp, int base_bi,
-                                               const int2 *ent_sp, const int2 *ent_bi,
-                                               const unsigned char *qs_bytes) {
-    constexpr int CH = MP / 4;
+                                               const uint16_t *ent_sp, const uint16_t *ent_bi, const float4 *qs,
+                                               const float *wtab) {
+    constexpr int CH = MP / 4, CHP = TileRow<MP>::CHP;
     // 8 lanes per vertex (CH of them active): every quarter-warp of an LDS.128 then reads ONE pixel
     // row (contiguous 96 B), which is bank-conflict free (packing CH lanes is not)
     constexpr int LPV = 8;
@@ -290,16 +313,17 @@ __device__ __forceinline__ void tile_splat_csr(float4 *vout_sp, float4 *vout_bi,
         const int2 h = hn;  // (first entry | count << 16, local row id)
         if (p + kTileThreads < pairs) hn = hdr_of(p + kTileThreads);
         // segments start on even entries and are padded to an even count (weight-0 entry): two per load
-        const int4 *ep = reinterpret_cast<const int4 *>((is_sp ? ent_sp : ent_bi) + (h.x & 0xffff));
+        const uint32_t *ep = reinterpret_cast<const uint32_t *>((is_sp ? ent_sp : ent_bi) + (h.x & 0xffff));
         const int n2 = ((h.x >> 16) + 1) >> 1;
-        const unsigned char *qbase = qs_bytes + cq * 16;
+        const float4 *qb = qs + cq;
         float4 a = make_float4(0.f, 0.f, 0.f, 0.f);
 #pragma unroll kPairUnroll
         for (int it = 0; it < n2; ++it) {
-            const int4 en = ep[it];
-            const float w0 = __int_as_float(en.y), w1 = __int_as_float(en.w);
-            const float4 q0 = *reinterpret_cast<const float4 *>(qbase + en.x);
-            const float4 q1 = *reinterpret_cast<const float4 *>(qbase + en.z);
+            const uint32_t en = ep[it];
+            const uint32_t e0 = en & 0xffffu, e1 = en >> 16;
+            const float w0 = wtab[e0], w1 = wtab[e1];
+            const float4 q0 = qb[(e0 & 255u) * CHP];
+            const float4 q1 = qb[(e1 & 255u) * CHP];
             a.x = fmaf(w0, q0.x, a.x);
             a.y = fmaf(w0, q0.y, a.y);
             a.z = fmaf(w0, q0.z, a.z);
@@ -351,8 +375,10 @@ k_mf_tile(const float *U, float *U_rw, int clamp, float *__restrict__ Qout, Tile
     constexpr int CH = MP / 4;
     constexpr int kRowBytes = MP * 4;
     using SM = TileSmem<MP>;
+    using ST = TileStage<MP>;
     extern __shared__ __align__(128) unsigned char smem_raw[];
-    SM &sm = *reinterpret_cast<SM *>(smem_raw);
+    SM &smt = *reinterpret_cast<SM *>(smem_raw);
+    ST &sm = smt.st;
     // A hybrid tile is k_mf_tile_hy's.  The test reads a byte map of its own and stands before anything else: the
     // same test on the tile's vertex count, wherever it was placed, made ptxas allocate this kernel's 64 registers
     // differently (more spill traffic in the splat loop, also on images that have no such tile at all).
@@ -368,10 +394,10 @@ k_mf_tile(const float *U, float *U_rw, int clamp, float *__restrict__ Qout, Tile
     const bool fb_sp = nl_sp < 0, fb_bi = nl_bi < 0;
     const int n_sp = fb_sp ? 0 : nl_sp, n_bi = fb_bi ? 0 : nl_bi;
     const int base_sp = sp.rowbase[b], base_bi = bi.rowbase[b];
-    constexpr int CHP = SM::CHP;
+    constexpr int CHP = ST::CHP;
     float4 *vs_sp = sm.buf, *vs_bi = sm.buf + kMaxLocSp * CHP;
     const int2 *hdr_sp = sp.tl_hdr + ti_sp * kMaxLocSp, *hdr_bi = bi.tl_hdr + ti_bi * kMaxLocHy;  // global, L1/L2-resident
-    int2 *ent_sp = sm.ent, *ent_bi = sm.ent + SM::kEntSp;
+    uint16_t *ent_sp = sm.ent, *ent_bi = sm.ent + ST::kEntSp;
     const size_t strideN = (size_t)N;
     const size_t px_sp = (size_t)sb_sp * 3 * N + pix, px_bi = (size_t)sb_bi * 6 * N + pix;
 
@@ -380,6 +406,7 @@ k_mf_tile(const float *U, float *U_rw, int clamp, float *__restrict__ Qout, Tile
     const int n_copies = (MODE != MODE_FIRST ? n_sp + n_bi : 0) + (MODE != MODE_LAST ? (n_sp > 0) + (n_bi > 0) : 0);
     if (tid == 0) {
         mbar_init(&sm.bar, n_copies > 0 ? n_copies : 1);
+        smt.wtab[kEntZero] = 0.0f;
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
     __syncthreads();
@@ -394,7 +421,7 @@ k_mf_tile(const float *U, float *U_rw, int clamp, float *__restrict__ Qout, Tile
                      kRowBytes, &sm.bar);
         }
         if (MODE != MODE_LAST && lv == (is_sp ? n_sp : n_bi) - 1) {  // the last segment tells the block's length
-            const uint32_t bytes = (uint32_t)((h.x & 0xffff) + (((h.x >> 16) + 1) & ~1)) * 8u;
+            const uint32_t bytes = ent_block_bytes(h);
             mbar_arrive_expect_tx(&sm.bar, bytes);
             bulk_g2s(is_sp ? ent_sp : ent_bi,
                      is_sp ? sp.tl_pack + ti_sp * sp.entcap : bi.tl_pack + ti_bi * bi.entcap, bytes, &sm.bar);
@@ -482,13 +509,13 @@ k_mf_tile(const float *U, float *U_rw, int clamp, float *__restrict__ Qout, Tile
     float4 *qs = sm.buf;
 #pragma unroll
     for (int c = 0; c < CH; c++) qs[tid * CHP + c] = make_float4(t[4 * c], t[4 * c + 1], t[4 * c + 2], t[4 * c + 3]);
+    tile_put_weights(smt.wtab, w_sp, w_bi);
     __syncthreads();
     // ---- splat ----
     float4 *vout_sp = reinterpret_cast<float4 *>(sp.val_out), *vout_bi = reinterpret_cast<float4 *>(bi.val_out);
     if (fb_sp && in) tile_splat_direct<MP, 3>(vout_sp, sp.off + px_sp, strideN, base_sp, w_sp, t);
     if (fb_bi && in) tile_splat_direct<MP, 6>(vout_bi, bi.off + px_bi, strideN, base_bi, w_bi, t);
-    tile_splat_csr<MP>(vout_sp, vout_bi, n_sp, n_bi, hdr_sp, hdr_bi, base_sp, base_bi, ent_sp, ent_bi,
-                       reinterpret_cast<const unsigned char *>(qs));
+    tile_splat_csr<MP>(vout_sp, vout_bi, n_sp, n_bi, hdr_sp, hdr_bi, base_sp, base_bi, ent_sp, ent_bi, qs, smt.wtab);
 }
 
 // Hybrid tiles (tiles.cu: more distinct vertices than the shared-memory path of k_mf_tile holds -- textured images,
@@ -504,15 +531,17 @@ k_mf_tile_hy(const float *U, float *U_rw, int clamp, float *__restrict__ Qout, T
              const int2 *hy_list, const int *hy_count) {
     constexpr int CH = MP / 4;
     constexpr int kRowBytes = MP * 4;
-    using SM = TileSmem<MP, kMaxLocHy>;
-    constexpr int CHP = SM::CHP;
+    using ST = TileStage<MP, kMaxLocHy>;
+    constexpr int CHP = ST::CHP;
     extern __shared__ __align__(128) unsigned char smem_raw[];
-    SM &sm = *reinterpret_cast<SM *>(smem_raw);
+    TileSmem<MP, kMaxLocHy> &smt = *reinterpret_cast<TileSmem<MP, kMaxLocHy> *>(smem_raw);
+    ST &sm = smt.st;
     const int tid = threadIdx.x;
     const int nhy = *hy_count;
     const size_t strideN = (size_t)N;
     float4 *vs_sp = sm.buf, *vs_bi = sm.buf + kMaxLocSp * CHP;
-    int2 *ent_sp = sm.ent, *ent_bi = sm.ent + SM::kEntSp;
+    uint16_t *ent_sp = sm.ent, *ent_bi = sm.ent + ST::kEntSp;
+    if (tid == 0) smt.wtab[kEntZero] = 0.0f;  // visible after the first tile's barriers
     float4 *vout_sp = reinterpret_cast<float4 *>(sp.val_out), *vout_bi = reinterpret_cast<float4 *>(bi.val_out);
     for (int item = blockIdx.x; item < nhy; item += gridDim.x) {
         const int2 bt = hy_list[item];
@@ -553,7 +582,7 @@ k_mf_tile_hy(const float *U, float *U_rw, int clamp, float *__restrict__ Qout, T
                          kRowBytes, &sm.bar);
             }
             if (MODE != MODE_LAST && lv == (is_sp ? n_sp : n_bi) - 1) {  // the last segment tells the block's length
-                const uint32_t bytes = (uint32_t)((h.x & 0xffff) + (((h.x >> 16) + 1) & ~1)) * 8u;
+                const uint32_t bytes = ent_block_bytes(h);
                 mbar_arrive_expect_tx(&sm.bar, bytes);
                 bulk_g2s(is_sp ? ent_sp : ent_bi,
                          is_sp ? sp.tl_pack + ti_sp * sp.entcap : bi.tl_pack + ti_bi * bi.entcap, bytes, &sm.bar);
@@ -634,9 +663,10 @@ k_mf_tile_hy(const float *U, float *U_rw, int clamp, float *__restrict__ Qout, T
             float4 *qs = sm.buf;
 #pragma unroll
             for (int c = 0; c < CH; c++) qs[tid * CHP + c] = make_float4(t[4 * c], t[4 * c + 1], t[4 * c + 2], t[4 * c + 3]);
+            tile_put_weights(smt.wtab, w_sp, w_bi);
             __syncthreads();
-            tile_splat_csr<MP>(vout_sp, vout_bi, n_sp, n_bi, hdr_sp, hdr_bi, base_sp, base_bi, ent_sp, ent_bi,
-                               reinterpret_cast<const unsigned char *>(qs));
+            tile_splat_csr<MP>(vout_sp, vout_bi, n_sp, n_bi, hdr_sp, hdr_bi, base_sp, base_bi, ent_sp, ent_bi, qs,
+                               smt.wtab);
         }
         __syncthreads();  // the tile is done with the shared buffers and the barrier
         if (tid == 0) asm volatile("mbarrier.inval.shared::cta.b64 [%0];" ::"r"(smem_u32(&sm.bar)) : "memory");

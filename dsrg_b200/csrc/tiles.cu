@@ -6,18 +6,19 @@
 // finds them once per lattice build: per tile the distinct rows with, for each, its segment of the
 // transposed incidence (tl_hdr), per pixel the index into that list (tl_loc), and the incidence
 // itself as a CSR grouped by local vertex whose entries are already in the form the mean-field
-// kernel consumes (tl_pack: byte offset of the pixel's Q row inside the tile, weight); the whole
-// entry list of a tile is one 16-byte-aligned block for a bulk copy.  Local vertices are numbered
+// kernel consumes (tl_pack: 16 bits, r << 8 | pixel's thread index, which locate both the pixel's Q row
+// and its weight in the kernel's shared tables, common.cuh:kEntZero); the whole entry list of a tile is
+// one 16-byte-aligned block for a bulk copy.  Local vertices are numbered
 // by decreasing segment length.  Tiles with too many distinct rows keep their most-shared ones (hybrid tiles).
 // The symmetric normalisation is folded into the weights: wn = bary * norm (pairwise.cpp:66,79).
 #include "common.cuh"
 
 namespace dsrg {
 
-template <int DP1, int MAXA, int MAXLOC, int MP>
+template <int DP1, int MAXA, int MAXLOC>
 __global__ void __launch_bounds__(kTileThreads)
 k_tile_build(const int32_t *off, const float *bary, const float *norm, int32_t *tl_nloc, uint8_t *tl_hy, int2 *tl_hdr,
-             int2 *tl_pack, uint16_t *tl_loc, float *wn, int N, int W, int H, int tiles_x, int ntiles,
+             uint16_t *tl_pack, uint16_t *tl_loc, float *wn, int N, int W, int H, int tiles_x, int ntiles,
              int entcap, int tile_w, int2 *hy_list, int *hy_count) {
     constexpr int HS = kTileThreads * 8;  // >= kTileThreads*DP1 distinct rows in the worst case, power of two
     constexpr int HBITS = (HS == 1024) ? 10 : (HS == 2048) ? 11 : (HS == 4096) ? 12 : -1;
@@ -197,7 +198,7 @@ k_tile_build(const int32_t *off, const float *bary, const float *norm, int32_t *
     }
     __syncthreads();
     // exclusive scan of the reordered counts, each rounded up to an even number -> ptr: every segment then
-    // starts on a 16-byte boundary and the consumer reads its entries two at a time (one LDS.128)
+    // starts on a 4-byte boundary and the consumer reads its entries two at a time (one LDS.32)
     {
         const int v = tid < nloc ? ((scnt[tid] + 1) & ~1) : 0;
         int incl = v;
@@ -216,7 +217,7 @@ k_tile_build(const int32_t *off, const float *bary, const float *norm, int32_t *
         }
     }
     __syncthreads();
-    int2 *pack = tl_pack + ((size_t)b * ntiles + tile) * entcap;
+    uint16_t *pack = tl_pack + ((size_t)b * ntiles + tile) * entcap;
     if (in) {
 #pragma unroll
         for (int r = 0; r < DP1; r++) {
@@ -228,13 +229,13 @@ k_tile_build(const int32_t *off, const float *bary, const float *norm, int32_t *
             const int nv = perm[lv[r]];
             *loc = (uint16_t)nv;
             const int pos = ptr[nv] + atomicAdd(&cnt[nv], 1);
-            pack[pos] = make_int2(tid * ((MP + 4 * DSRG_ROW_PAD) * 4), __float_as_int(w[r]));  // byte offset of the pixel's (padded) Q row
+            pack[pos] = (uint16_t)((ent_r0(DP1) + r) << 8 | tid);  // the weight is w[r] = wn, which the consumer holds
         }
     }
     if (tid < nloc) {
         const int nv = perm[tid];
         tl_hdr[((size_t)b * ntiles + tile) * MAXLOC + nv] = make_int2(ptr[nv] | (mycnt << 16), rows_s[tid]);
-        if (mycnt & 1) pack[ptr[nv] + mycnt] = make_int2(0, 0);  // padding entry: pixel 0 with weight 0
+        if (mycnt & 1) pack[ptr[nv] + mycnt] = (uint16_t)kEntZero;  // padding entry: pixel 0 with weight 0
     }
     if (tid == 0) {
         tl_nloc[tile] = nloc | (hybrid ? kTileHybrid : 0);
@@ -263,26 +264,14 @@ int tiles_build(Engine *e, Lattice &L, int nb, cudaStream_t s) {
     dim3 g(e->ntiles, nb);
     const bool hy_on = L.d == 5 && hybrid_tiles_on(e, nb);
     if (L.d == 5) DSRG_CUDA_TRY(cudaMemsetAsync(e->hy_count, 0, sizeof(int), s));  // the list of hybrid tiles is rebuilt (or stays empty)
-#define DSRG_TILE_BUILD(DP1, MAXA, MAXLOC, MPV)                                                             \
+#define DSRG_TILE_BUILD(DP1, MAXA, MAXLOC)                                                                   \
     DSRG_LAUNCH(e, T_LAT_MISC, s,                                                                            \
-                (k_tile_build<DP1, MAXA, MAXLOC, MPV><<<g, kTileThreads, 0, s>>>(L.off, L.bary, L.norm, L.tl_nloc, L.tl_hy, L.tl_hdr, \
+                (k_tile_build<DP1, MAXA, MAXLOC><<<g, kTileThreads, 0, s>>>(L.off, L.bary, L.norm, L.tl_nloc, L.tl_hy, L.tl_hdr, \
                                                                   L.tl_pack, L.tl_loc, L.wn, L.N, e->W, e->H,  \
                                                                   e->tiles_x, e->ntiles, L.entcap, e->tile_w,  \
                                                                   hy_on ? e->hy_list : nullptr, e->hy_count)))
-#define DSRG_TILE_BUILD_MP(MPV)                                      \
-    if (L.d == 2) { DSRG_TILE_BUILD(3, kMaxLocSp, kMaxLocSp, MPV); } \
-    else { DSRG_TILE_BUILD(6, kMaxLocBi, kMaxLocHy, MPV); }
-    switch (e->MP) {
-        case 4: DSRG_TILE_BUILD_MP(4); break;
-        case 8: DSRG_TILE_BUILD_MP(8); break;
-        case 12: DSRG_TILE_BUILD_MP(12); break;
-        case 16: DSRG_TILE_BUILD_MP(16); break;
-        case 20: DSRG_TILE_BUILD_MP(20); break;
-        case 24: DSRG_TILE_BUILD_MP(24); break;
-        case 28: DSRG_TILE_BUILD_MP(28); break;
-        case 32: DSRG_TILE_BUILD_MP(32); break;
-        default: set_error("unsupported label count"); return DSRG_E_INVALID;
-    }
+    if (L.d == 2) DSRG_TILE_BUILD(3, kMaxLocSp, kMaxLocSp);
+    else DSRG_TILE_BUILD(6, kMaxLocBi, kMaxLocHy);
     if (hy_on)
         DSRG_LAUNCH(e, T_LAT_MISC, s,
                     k_tile_demote<<<1, kThreads, 0, s>>>(e->hy_list, e->hy_count, L.tl_nloc, L.tl_hy, e->ntiles, DSRG_HY_MIN_TILES * e->sm_count));
