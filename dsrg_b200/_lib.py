@@ -76,6 +76,12 @@ SIGNATURES = {
     "dsrg_predict_mask_host": (_i, [_vp, _i, _i, _vp, _vp, _vp, _vp, _f, _i, _pp, _vp, _i, _vp, _vp]),
     "dsrg_annotation_forward_dev": (_i, [_vp, _i, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _vp, _vp, _vp, _vp]),
     "dsrg_annotation_forward_host": (_i, [_vp, _i, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _vp, _vp, _vp]),
+    "dsrg_confusion_create": (_vp, [_i, _i]),
+    "dsrg_confusion_destroy": (None, [_vp]),
+    "dsrg_confusion_reset": (_i, [_vp, _vp]),
+    "dsrg_confusion_add_dev": (_i, [_vp, _sz, _vp, _vp, _i, _vp]),
+    "dsrg_confusion_add_host": (_i, [_vp, _sz, _vp, _vp, _i]),
+    "dsrg_confusion_read": (_i, [_vp, _vp, _vp]),
     "dsrg_wire_pack_mask": (_i, [_vp, _vp, _sz]),
     "dsrg_wire_unpack_mask": (None, [_vp, _vp, _sz]),
     "dsrg_wire_apply_clamp_mask": (None, [_vp, _vp, _sz]),

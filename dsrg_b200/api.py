@@ -462,6 +462,74 @@ class Engine(object):
         return ns, nb
 
 
+def _pred_host(pred, K):
+    """pred as a flat C-contiguous uint8 or int32 array.  Other integer predictions (np.argmax gives int64) are
+    narrowed on the host: values outside [0, K) become -1, so they are counted as invalid and never wrapped."""
+    pred = np.ascontiguousarray(pred).reshape(-1)
+    if pred.dtype in (np.uint8, np.int32):
+        return pred
+    if pred.dtype.kind not in "iu":
+        raise TypeError("pred must be an integer array, not %s" % pred.dtype)
+    ok = (pred >= 0) & (pred < K)
+    out = np.full(pred.size, -1, np.int32)
+    out[ok] = pred[ok]
+    return out
+
+
+class Confusion(object):
+    """dsrg_confusion: a K x K uint64 confusion matrix (row = gt, column = pred) on the device, plus the counters
+    of pixels that were not binned -- invalid[0]: gt >= K other than 255, invalid[1]: gt < K with pred outside
+    [0, K).  The rules are generateM's (training/tools/evaluate.py:61-68): pixels with gt >= K are skipped."""
+
+    def __init__(self, K, device=None):
+        self._L = _lib.lib()
+        if device is None:
+            device = self._L.dsrg_current_device()
+        self.K, self.device = int(K), int(device)
+        self.h = self._L.dsrg_confusion_create(self.device, self.K)
+        if not self.h:
+            raise DsrgError(_lib.E_CUDA, self._L.dsrg_last_error().decode())
+
+    def close(self):
+        if getattr(self, "h", None):
+            self._L.dsrg_confusion_destroy(self.h)
+            self.h = None
+
+    __del__ = close
+
+    def reset(self, stream=None):
+        """Zero the matrix and the counters (stream None: the legacy default stream; ordered after every add)."""
+        check(self._L.dsrg_confusion_reset(self.h, None if stream is None else C.c_void_p(int(stream))))
+
+    def add_host(self, gt, pred):
+        """gt: uint8 array; pred: uint8 / int32 (taken as they are) or any other integer array of the same size."""
+        gt = np.ascontiguousarray(gt).reshape(-1)
+        if gt.dtype != np.uint8:
+            raise TypeError("gt must be uint8 (a label PNG), not %s" % gt.dtype)
+        pred = _pred_host(pred, self.K)
+        if pred.size != gt.size:
+            raise ValueError("gt and pred differ in size (%d vs %d)" % (gt.size, pred.size))
+        check(self._L.dsrg_confusion_add_host(self.h, gt.size, C.c_void_p(gt.ctypes.data),
+                                              C.c_void_p(pred.ctypes.data), pred.itemsize))
+
+    def add_dev(self, gt, pred, stream=None):
+        """gt: contiguous uint8 CUDA tensor; pred: contiguous uint8 or int32 CUDA tensor of the same size."""
+        import torch
+        if gt.dtype != torch.uint8 or pred.dtype not in (torch.uint8, torch.int32):
+            raise TypeError("gt must be uint8 and pred uint8 or int32 (got %s, %s)" % (gt.dtype, pred.dtype))
+        if gt.numel() != pred.numel():
+            raise ValueError("gt and pred differ in size (%d vs %d)" % (gt.numel(), pred.numel()))
+        check(self._L.dsrg_confusion_add_dev(self.h, gt.numel(), _dptr(gt), _dptr(pred), pred.element_size(),
+                                             _stream(stream)))
+
+    def read(self):
+        """(matrix (K, K) uint64, invalid (2,) uint64) after every add so far (synchronises)."""
+        m = np.empty((self.K, self.K), np.uint64)
+        inv = np.empty(2, np.uint64)
+        check(self._L.dsrg_confusion_read(self.h, C.c_void_p(m.ctypes.data), C.c_void_p(inv.ctypes.data)))
+        return m, inv
+
+
 class DenseCRF(object):
     """Same surface as the reference's Cython extension type krahenbuhl2013.wrapper.DenseCRF
     (CRF/krahenbuhl2013/wrapper.pyx:20-60), backed by dsrg_densecrf_* (host pointers)."""

@@ -358,13 +358,14 @@ __device__ __forceinline__ double numpy_sum(F get, int n_rt) {
 struct DeviceScope {
     int prev = -1;
     bool switched = false;
-    explicit DeviceScope(const Engine *e) {
-        if (!e) return;
+    explicit DeviceScope(const Engine *e) : DeviceScope(e ? e->device : -1) {}
+    explicit DeviceScope(int device) {  // device < 0: nothing to select
+        if (device < 0) return;
         if (cudaGetDevice(&prev) != cudaSuccess) {
             cudaGetLastError();
             prev = -1;
         }
-        if (prev != e->device) switched = cudaSetDevice(e->device) == cudaSuccess && prev >= 0;
+        if (prev != device) switched = cudaSetDevice(device) == cudaSuccess && prev >= 0;
     }
     ~DeviceScope() {
         if (switched) cudaSetDevice(prev);

@@ -71,6 +71,46 @@ k_post_softmax(const float *in, float *out, float *probs, int npix, int M, long 
         }
 }
 
+// The same for M > DSRG_MAX_LABELS (the COCO tools' 81 labels): the label vector does not fit in registers, so
+// exp(s - max) is parked in `out` (in may alias out: each thread owns its pixel) and read back for the division.
+// Same float32 operations in the same order as k_post_softmax.
+template <bool CLAMPLOG>
+__global__ void __launch_bounds__(kThreads)
+k_post_softmax_wide(const float *in, float *out, float *probs, int npix, int M, long long ls, long long ps,
+                    float eps) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= npix) return;
+    const float *s = in + (size_t)i * ps;
+    float *o = out + (size_t)i * ps;
+    float m = -INFINITY;
+    for (int l = 0; l < M; l++) m = fmaxf(m, s[(size_t)l * ls]);
+    float sum = 0.f;
+    for (int l = 0; l < M; l++) {
+        const float v = expf(__fsub_rn(s[(size_t)l * ls], m));
+        o[(size_t)l * ls] = v;
+        sum = __fadd_rn(sum, v);
+    }
+    for (int l = 0; l < M; l++) {
+        float p = __fdiv_rn(o[(size_t)l * ls], sum);
+        if (CLAMPLOG) {
+            if (p < eps) p = eps;
+            if (probs) probs[(size_t)i * ps + (size_t)l * ls] = p;
+            p = logf(p);
+        }
+        o[(size_t)l * ls] = p;
+    }
+}
+
+template <bool CLAMPLOG>
+static void post_softmax(Engine *e, const float *in, float *out, float *probs, int npix, long long ls, long long ps,
+                         float eps, cudaStream_t s) {
+    const int g = cdiv(npix, kThreads), M = e->M;
+    if (M > DSRG_MAX_LABELS)
+        DSRG_LAUNCH(e, T_POST, s, k_post_softmax_wide<CLAMPLOG><<<g, kThreads, 0, s>>>(in, out, probs, npix, M, ls, ps, eps));
+    else
+        DSRG_LAUNCH(e, T_POST, s, k_post_softmax<CLAMPLOG><<<g, kThreads, 0, s>>>(in, out, probs, npix, M, ls, ps, eps));
+}
+
 // probs[probs < eps] = eps; unary = np.log(probs)   (generate_train_gt.py:90-94), element-wise
 __global__ void __launch_bounds__(kThreads)
 k_post_clamp_log(const float *in, float *out, float *probs, long long n, float eps) {
@@ -82,9 +122,9 @@ k_post_clamp_log(const float *in, float *out, float *probs, long long n, float e
     out[i] = logf(p);
 }
 
-struct LabelSel {
+struct LabelSel {   // 1 KB of kernel parameters
     int n;
-    int id[DSRG_MAX_LABELS];
+    int id[DSRG_MAX_LABELS_WIDE];
 };
 
 // np.argmax (first maximum) over the selected labels, result = the selected label's id
@@ -129,14 +169,11 @@ static int predict_mask_body(Engine *e, int mode, int n_scales, const float *con
     if (mode == DSRG_POST_SUM_SCORES) {
         for (int k = 0; k < n_scales; k++)
             if ((rc = zoom_scores(e, scores[k], hs[k], ws[k], unary, k > 0, s))) return rc;
-        DSRG_LAUNCH(e, T_POST, s,
-                    k_post_softmax<true><<<cdiv(N, kThreads), kThreads, 0, s>>>(unary, unary, clamped, N, M, 1, M, eps));
+        post_softmax<true>(e, unary, unary, clamped, N, 1, M, eps, s);
     } else {
         const int np = hs[0] * ws[0];
         float *small = e->st_cues;                    // [M][h][w] probabilities at network resolution
-        DSRG_LAUNCH(e, T_POST, s,
-                    k_post_softmax<false><<<cdiv(np, kThreads), kThreads, 0, s>>>(scores[0], small, nullptr, np, M,
-                                                                                   np, 1, eps));
+        post_softmax<false>(e, scores[0], small, nullptr, np, np, 1, eps, s);
         if ((rc = zoom_scores(e, small, hs[0], ws[0], unary, 0, s))) return rc;
         const long long n = (long long)N * M;
         DSRG_LAUNCH(e, T_POST, s, k_post_clamp_log<<<cdiv(n, kThreads), kThreads, 0, s>>>(unary, unary, clamped, n, eps));
@@ -161,12 +198,8 @@ static int predict_mask(Engine *e, int mode, int n_scales, const float *const *s
         set_error("bad mode %d", mode);
         return DSRG_E_INVALID;
     }
-    if (e->M > DSRG_MAX_LABELS) {
-        set_error("predict_mask post-processing supports at most %d labels (engine has %d)", DSRG_MAX_LABELS, e->M);
-        return DSRG_E_INVALID;
-    }
     if (n_scales < 1 || (mode == DSRG_POST_ZOOM_PROBS && n_scales != 1) || !scores || !hs || !ws || !result ||
-        (smooth && (!image || !p)) || n_sel < 0 || n_sel > DSRG_MAX_LABELS || (n_sel > 0 && !labels_sel)) {
+        (smooth && (!image || !p)) || n_sel < 0 || n_sel > DSRG_MAX_LABELS_WIDE || (n_sel > 0 && !labels_sel)) {
         set_error("bad argument");
         return DSRG_E_INVALID;
     }

@@ -34,10 +34,10 @@ extern "C" {
 #define DSRG_LAYOUT_NCHW 1
 
 #define DSRG_MAX_LABELS 32 /* labels per pixel of the fused, register-tiled kernels (the 21-class hot path) */
-/* CRF (batch, layer and DenseCRF-object entry points) and SRG accept up to this many labels: above DSRG_MAX_LABELS
- * the mean field runs on a generic label-chunked path (csrc/meanfield_wide.cu) -- the reference's COCO tool uses
- * DenseCRF(W, H, 81), training/tools/test-coco.py.  The Softmax / ConstrainLoss layers and the predict_mask
- * post-processing are built for at most DSRG_MAX_LABELS. */
+/* CRF (batch, layer and DenseCRF-object entry points), SRG, the predict_mask post-processing and the confusion
+ * matrix accept up to this many labels: above DSRG_MAX_LABELS the mean field runs on a generic label-chunked path
+ * (csrc/meanfield_wide.cu) -- the reference's COCO tool uses DenseCRF(W, H, 81), training/tools/test-coco.py.
+ * The Softmax / ConstrainLoss layers are built for at most DSRG_MAX_LABELS. */
 #define DSRG_MAX_LABELS_WIDE 255
 /* pixels per class plane the GWRP kernels of dsrg_expandloss_* sort in shared memory (41x41 and the 65x65 maps
  * of a 513 crop fit; larger planes return DSRG_E_INVALID) */
@@ -263,6 +263,37 @@ int dsrg_annotation_forward_host(dsrg_engine *e, int B, const int32_t *tag_offse
                                  const int32_t *cue_offsets, const int32_t *cue_idx, const int32_t *flip,
                                  const float *images_in_host, int Hi, int Wi, float *labels_out_host,
                                  float *cues_out_host, float *images_out_host);
+
+/* ------------------------------------------------------------------------------------------
+ * Confusion matrix of a segmentation run, the scoring step of the evaluation tools:
+ *   ConfusionMatrix (training/tools/evaluate.py:17-68, ap.py:19-72); its generateM (:61-68 / :65-72) counts
+ *     m[gt[i], pred[i]] += 1 for every pixel with gt[i] < nclass, one Python iteration per pixel
+ *   get_confusion_matrix (training/tools/test-coco.py:62-81): the same matrix via np.bincount(gt * K + pred)
+ * An object owns a K x K uint64 matrix on `device` (-1: dsrg_current_device()), K <= DSRG_MAX_LABELS_WIDE, and
+ * two uint64 counters of pixels that are not binned:
+ *   invalid[0] : gt >= K other than 255 (the ignore label); such pixels are skipped, as generateM skips them
+ *   invalid[1] : gt < K but pred outside [0, K) (numpy raises IndexError there; the Python layer raises)
+ * The counts are exact and independent of the order of the calls.  Unlike test-coco.py, gt * K is never computed in
+ * uint8: that product wraps mod 256 there for K = 81 (gt = 4, pred = 4 lands in bin 72).
+ * Every call restores the caller's current device.
+ * ------------------------------------------------------------------------------------------ */
+typedef struct dsrg_confusion dsrg_confusion;
+
+dsrg_confusion *dsrg_confusion_create(int device, int K);      /* ConfusionMatrix(nclass), evaluate.py:19-22 */
+void dsrg_confusion_destroy(dsrg_confusion *c);
+/* zero the matrix and the counters, queued on `stream` */
+int dsrg_confusion_reset(dsrg_confusion *c, void *stream);
+/* generateM over n pixels and accumulate (ConfM.addM(m) of evaluate.py:155-156): gt uint8, pred uint8 (pred_bytes
+ * 1, a prediction PNG read back, evaluate.py:144) or int32 (4, the result of dsrg_predict_mask_dev).  Device
+ * pointers may have any offset (int32 pred: 4-byte aligned); queued on `stream`. */
+int dsrg_confusion_add_dev(dsrg_confusion *c, size_t n, const uint8_t *gt_dev, const void *pred_dev,
+                           int pred_bytes /* 1 or 4 */, void *stream);
+/* the same from host memory, streamed in chunks through the object's pinned staging (the copy of chunk k+1
+ * overlaps the counting of chunk k); returns when the pixels are counted */
+int dsrg_confusion_add_host(dsrg_confusion *c, size_t n, const uint8_t *gt, const void *pred, int pred_bytes);
+/* wait for every add / reset so far and copy the K*K matrix (row = gt, column = pred) and the 2 invalid counters
+ * out; either pointer may be NULL */
+int dsrg_confusion_read(dsrg_confusion *c, uint64_t *matrix_out /* K*K */, uint64_t *invalid_out /* 2 */);
 
 /* Host-only helpers of the *_host wire format (0/1 planes cross PCIe as 1 bit per value, see
  * csrc/wire.cu); exported for unit tests.  pack returns 1 if every value was exactly 0 or 1. */

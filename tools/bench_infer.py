@@ -3,7 +3,10 @@ training/tools/test-ms.py on VOC-sized images, one image per call, sizes changin
 through postprocess.predict_mask_ms (host numpy in, host label map out).  Not the headline metric
 (that is bench.py); prints one JSON line.
 
-usage: python tools/bench_infer.py [--images 40] [--cpu 2]
+With --labels 81 it times the COCO tool's post-processing instead (training/tools/test-coco.py:108-133: one
+481-pixel scale, 81 labels, the mean field on the label-chunked path) on COCO-sized images.
+
+usage: python tools/bench_infer.py [--images 40] [--cpu 2] [--labels 21|81]
 """
 import argparse
 import json
@@ -16,16 +19,24 @@ import numpy as np
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 
 SIZES = [(375, 500), (500, 375), (333, 500), (500, 334), (366, 500), (281, 500), (500, 500), (375, 500)]
+COCO_SIZES = [(480, 640), (640, 480), (427, 640), (640, 427), (480, 640), (612, 612), (426, 640), (480, 640)]
 
 
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--images", type=int, default=40)
-    ap.add_argument("--cpu", type=int, default=2, help="images timed through the CPU oracle (0 = skip)")
+    ap.add_argument("--cpu", type=int, default=None, help="images timed through the CPU oracle (0 = skip; "
+                                                          "default 2 at 21 labels, 0 at 81)")
+    ap.add_argument("--labels", type=int, default=21, choices=(21, 81))
     args = ap.parse_args()
+    if args.cpu is None:
+        args.cpu = 2 if args.labels == 21 else 0
     import torch
     from dsrg_b200 import pool, postprocess, synth
-    cases = [synth.make_score_blobs(100 + i, H, W, (31, 41, 51)) for i, (H, W) in enumerate(SIZES)]
+    coco = args.labels == 81
+    sizes = COCO_SIZES if coco else SIZES
+    scales = (61,) if coco else (31, 41, 51)        # fc8 of the 481 input (test-coco.py:116) / of 241, 321, 401
+    cases = [synth.make_score_blobs(100 + i, H, W, scales, C=args.labels) for i, (H, W) in enumerate(sizes)]
     for c in cases:                                   # warm-up: engine growth, lazy allocations
         postprocess.predict_mask_ms(c["image"], c["blobs"])
     eng = list(pool._ENGINES.values())[0]
@@ -43,10 +54,12 @@ def main():
     eng.profile(False)
     launches = eng.take_launch_count()
     gpu_ms = sum(v[0] for v in prof.values()) / len(cases)
-    out = {"metric": "images/s, predict_mask post-processing (3 score scales -> zoom/sum -> softmax -> CRF 10 it -> argmax), "
-                     "one VOC-sized image per call, host in / host out",
+    what = ("81 labels, 1 score scale -> zoom -> softmax -> CRF 10 it -> argmax), one COCO-sized image per call"
+            if coco else "3 score scales -> zoom/sum -> softmax -> CRF 10 it -> argmax), one VOC-sized image per call")
+    out = {"metric": "images/s, predict_mask post-processing (" + what + ", host in / host out",
+           "labels": args.labels, "gpu": torch.cuda.get_device_name(0),
            "value": args.images / dt, "ms_per_image": 1e3 * dt / args.images, "images": args.images,
-           "sizes": SIZES, "engine_capacity": list(eng.capacity), "engine_device_MB": eng.device_bytes / 1e6,
+           "sizes": sizes, "engine_capacity": list(eng.capacity), "engine_device_MB": eng.device_bytes / 1e6,
            "kernel_ms_per_image": gpu_ms, "launches_per_image": launches / len(cases),
            "kernel_classes_ms_per_image": {k: v[0] / len(cases) for k, v in sorted(prof.items())}}
     if args.cpu:
