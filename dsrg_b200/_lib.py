@@ -47,7 +47,6 @@ SIGNATURES = {
     "dsrg_engine_set_size": (_i, [_vp, _i, _i]),
     "dsrg_engine_get_size": (_i, [_vp, _vp, _vp, _vp, _vp]),
     "dsrg_engine_set_host_chunk": (_i, [_vp, _i]),
-    "dsrg_engine_set_lanes": (_i, [_vp, _i]),
     "dsrg_engine_set_graphs": (_i, [_vp, _i]),
     "dsrg_engine_graph_replays": (_ll, [_vp]),
     "dsrg_engine_take_launch_count": (_ll, [_vp]),

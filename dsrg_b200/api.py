@@ -122,9 +122,6 @@ class Engine(object):
     def graph_replays(self):
         return int(self._L.dsrg_engine_graph_replays(self.h))
 
-    def set_lanes(self, lanes):
-        check(self._L.dsrg_engine_set_lanes(self.h, int(lanes)))
-
     @property
     def hybrid_tiles(self):
         """Tiles of the last mean-field pass that took the hybrid path (textured images); synchronises."""

@@ -270,7 +270,7 @@ using namespace dsrg;
 
 extern "C" {
 
-int dsrg_version(void) { return 100; }
+int dsrg_version(void) { return 101; }
 
 const char *dsrg_last_error(void) { return g_err; }
 
@@ -419,11 +419,7 @@ dsrg_engine *dsrg_engine_create(int device, int max_batch, int H, int W, int M) 
     if (!rc && cudaMemset(e->dev_err, 0, sizeof(int)) != cudaSuccess) rc = DSRG_E_CUDA;
     if (!rc && cudaStreamCreateWithFlags(&e->own_stream, cudaStreamNonBlocking) != cudaSuccess) rc = DSRG_E_CUDA;
     if (!rc && cudaStreamCreateWithFlags(&e->in_stream, cudaStreamNonBlocking) != cudaSuccess) rc = DSRG_E_CUDA;
-    if (!rc && cudaStreamCreateWithFlags(&e->aux_stream, cudaStreamNonBlocking) != cudaSuccess) rc = DSRG_E_CUDA;
-    if (!rc && cudaEventCreateWithFlags(&e->fork_event, cudaEventDisableTiming) != cudaSuccess) rc = DSRG_E_CUDA;
-    if (!rc && cudaEventCreateWithFlags(&e->join_event, cudaEventDisableTiming) != cudaSuccess) rc = DSRG_E_CUDA;
     if (!rc && cudaEventCreateWithFlags(&e->order_event, cudaEventDisableTiming) != cudaSuccess) rc = DSRG_E_CUDA;
-    if (const char *ev = getenv("DSRG_B200_LANES")) e->lanes = atoi(ev) == 2 ? 2 : 1;
     if (const char *ev = getenv("DSRG_B200_WIRE")) e->wire_compress = atoi(ev) != 0;
     if (const char *ev = getenv("DSRG_B200_GRAPHS")) e->use_graphs = atoi(ev) != 0;
     if (const char *ev = getenv("DSRG_B200_HOST_CHUNK")) e->host_chunk = atoi(ev) > 0 ? atoi(ev) : e->host_chunk;
@@ -450,9 +446,6 @@ void dsrg_engine_destroy(dsrg_engine *h) {
     for (void *p : ptrs) cudaFree(p);
     if (e->own_stream) cudaStreamDestroy(e->own_stream);
     if (e->in_stream) cudaStreamDestroy(e->in_stream);
-    if (e->aux_stream) cudaStreamDestroy(e->aux_stream);
-    if (e->fork_event) cudaEventDestroy(e->fork_event);
-    if (e->join_event) cudaEventDestroy(e->join_event);
     if (e->order_event) cudaEventDestroy(e->order_event);
     if (e->out_stream) cudaStreamDestroy(e->out_stream);
     for (auto ev : e->pipe_events) cudaEventDestroy(ev);
@@ -513,7 +506,7 @@ long long dsrg_engine_take_launch_count(dsrg_engine *h) {
 static const char *kTagNames[T_COUNT] = {
     "lattice_insert", "lattice_misc", "lattice_norm", "mf_init", "mf_zero", "mf_blur_spatial",
     "mf_blur_bilateral", "mf_tile", "mf_export", "srg_label", "srg_merge", "srg_flag", "srg_emit",
-    "seedloss", "wire_bits", "prepare_image", "postprocess", "annotation", "mf_blur_fused", "mf_tile_hybrid"};
+    "seedloss", "wire_bits", "prepare_image", "postprocess", "annotation", "mf_tile_hybrid"};
 
 int dsrg_profile_tag_count(void) { return T_COUNT; }
 
@@ -550,13 +543,6 @@ long long dsrg_engine_hybrid_tiles(dsrg_engine *h) {
         return -1;
     }
     return n;
-}
-
-int dsrg_engine_set_lanes(dsrg_engine *h, int lanes) {
-    Engine *e = (Engine *)h;
-    if (!e || lanes < 1 || lanes > 2) return DSRG_E_INVALID;
-    e->lanes = lanes;
-    return DSRG_OK;
 }
 
 int dsrg_engine_profile(dsrg_engine *h, int enable) {

@@ -75,16 +75,13 @@ struct Engine;
 enum KTag {
     T_LAT_INSERT = 0, T_LAT_MISC, T_LAT_NORM, T_MF_INIT, T_MF_ZERO, T_MF_BLUR_SP,
     T_MF_BLUR_BI, T_MF_TILE, T_MF_EXPORT, T_SRG_LABEL, T_SRG_MERGE, T_SRG_FLAG, T_SRG_EMIT,
-    T_LOSS, T_WIRE, T_PREP, T_POST, T_ANNOT, T_MF_BLUR_FUSED, T_MF_TILE_HY, T_COUNT
+    T_LOSS, T_WIRE, T_PREP, T_POST, T_ANNOT, T_MF_TILE_HY, T_COUNT
 };
 
 // ---- lattice.cu ----
 int lattice_build(Engine *e, Lattice &L, int B, const uint8_t *image_dev, cudaStream_t s);
 // ---- tiles.cu ----
-#ifndef DSRG_TILE_H
-#define DSRG_TILE_H 8
-#endif
-constexpr int kTileW = 32, kTileH = DSRG_TILE_H;   // one thread per pixel, one warp per tile row
+constexpr int kTileW = 32, kTileH = 8;   // one thread per pixel, one warp per tile row
 constexpr int kTileThreads = kTileW * kTileH;
 #ifndef DSRG_MAXLOC_BI
 #define DSRG_MAXLOC_BI 192
@@ -216,13 +213,11 @@ struct Engine {
     int32_t *st_idx = nullptr;  // index lists of the annotation entry points
     size_t st_idx_cap = 0;
     int32_t *st_lmap = nullptr;
-    cudaStream_t own_stream = nullptr, in_stream = nullptr, out_stream = nullptr, aux_stream = nullptr;
-    cudaEvent_t fork_event = nullptr, join_event = nullptr;
+    cudaStream_t own_stream = nullptr, in_stream = nullptr, out_stream = nullptr;
     // order of the passes of this engine across streams (StreamScope)
     cudaEvent_t order_event = nullptr;
     cudaStream_t last_stream = nullptr;
     bool last_stream_valid = false;
-    int lanes = 1;  // 2 = run the mean-field loop as two half-batches on two streams (off by default)
     std::vector<cudaEvent_t> pipe_events;
     int host_chunk = 0;   // > 0 caps the images per pipeline stage of the *_host entry points
     // 0/1 planes travel over PCIe as bit masks (wire.cu): device + pinned host staging, [maxB][words/image]

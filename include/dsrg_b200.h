@@ -99,10 +99,6 @@ int dsrg_engine_get_size(const dsrg_engine *e, int *H, int *W, int *H_capacity, 
 /* The *_host full-pass entry points pipeline the batch in chunks (default B/8, 3B/8, B/2 images) through
  * H2D | kernels | D2H streams; `images` > 0 caps the chunk size, 0 restores the default. */
 int dsrg_engine_set_host_chunk(dsrg_engine *e, int images);
-/* Experimental: run the mean-field loop as `lanes` (1 or 2, default 1) half-batches on separate
- * streams so that the DRAM-latency-bound blur passes of one half overlap the shared-memory-bound tile
- * kernel of the other (off by default). */
-int dsrg_engine_set_lanes(dsrg_engine *e, int lanes);
 /* Device passes (*_dev entry points, and through them the chunks of the *_host ones) are captured into CUDA
  * graphs the second time a pass is issued with the same arguments and replayed afterwards -- one launch instead
  * of 40-130 dependent ones.  Needs a real stream (not the legacy default stream); enable = 0 turns it off and
