@@ -54,17 +54,6 @@ k_annot_images(const float *in, float *out, const int32_t *flip, long long per_i
     out[i] = in[src];
 }
 
-static int grow_idx(Engine *e, size_t ints) {
-    if (ints <= e->st_idx_cap) return DSRG_OK;
-    cudaFree(e->st_idx);
-    e->st_idx = nullptr;
-    e->st_idx_cap = 0;
-    int rc = dalloc(e, &e->st_idx, ints);
-    if (rc) return rc;
-    e->st_idx_cap = ints;
-    return DSRG_OK;
-}
-
 // host-side validation with numpy's rules: -dim <= index < dim, else IndexError
 static int check_indices(const int32_t *v, long long n, int dim, const char *what) {
     for (long long k = 0; k < n; k++)
@@ -79,11 +68,6 @@ static int annotation_forward(Engine *e, int B, const int32_t *tag_off, const in
                               const int32_t *cue_off, const int32_t *cue_idx, const int32_t *flip,
                               const float *images_in, int Hi, int Wi, float *labels_out, float *cues_out,
                               float *images_out, cudaStream_t s) {
-    if (!tag_off || !cue_off || !labels_out || !cues_out || (images_out && (!images_in || Hi < 1 || Wi < 1)) ||
-        (images_out && images_in == images_out)) {
-        set_error("bad argument");
-        return DSRG_E_INVALID;
-    }
     const long long nt = tag_off[B], nk = cue_off[B];
     if (tag_off[0] != 0 || cue_off[0] != 0 || nt < 0 || nk < 0 || (nt && !tags) || (nk && !cue_idx)) {
         set_error("bad offsets");
@@ -101,7 +85,7 @@ static int annotation_forward(Engine *e, int B, const int32_t *tag_off, const in
     if ((rc = check_indices(cue_idx + 2 * nk, nk, e->W, "axis 3 (column)"))) return rc;
     // device copy of the index lists: [tag_off B+1][cue_off B+1][flip B][tags nt][cue_idx 3*nk]
     const size_t n_ints = (size_t)(2 * (B + 1) + B) + nt + 3 * nk;
-    if ((rc = grow_idx(e, n_ints))) return rc;
+    if ((rc = grow_staging(e, (void **)&e->st_idx, &e->st_idx_cap, n_ints * sizeof(int32_t)))) return rc;
     std::vector<int32_t> pack(n_ints);
     int32_t *p = pack.data();
     memcpy(p, tag_off, sizeof(int32_t) * (B + 1));
@@ -133,55 +117,47 @@ static int annotation_forward(Engine *e, int B, const int32_t *tag_off, const in
 
 using namespace dsrg;
 
+// the pointers every call needs, and the image pair when the images are copied
+static bool annot_args_ok(const int32_t *tag_off, const int32_t *cue_off, const float *images_in, int Hi, int Wi,
+                          const float *labels_out, const float *cues_out, const float *images_out) {
+    return tag_off && cue_off && labels_out && cues_out && (!images_out || (images_in && Hi >= 1 && Wi >= 1));
+}
+
 extern "C" int dsrg_annotation_forward_dev(dsrg_engine *h, int B, const int32_t *tag_offsets, const int32_t *tags,
                                            const int32_t *cue_offsets, const int32_t *cue_idx, const int32_t *flip,
                                            const float *images_in_dev, int Hi, int Wi, float *labels_out_dev,
                                            float *cues_out_dev, float *images_out_dev, void *stream) {
-    Engine *e = (Engine *)h;
-    DeviceScope dev_scope(e);
-    int rc = check_batch(e, B);
-    if (rc) return rc;
-    StreamScope stream_scope(e, (cudaStream_t)stream);
-    return annotation_forward(e, B, tag_offsets, tags, cue_offsets, cue_idx, flip, images_in_dev, Hi, Wi,
-                              labels_out_dev, cues_out_dev, images_out_dev, (cudaStream_t)stream);
+    const cudaStream_t s = (cudaStream_t)stream;
+    // the mirror reads and writes whole rows: the two image buffers must be distinct
+    const bool ok = annot_args_ok(tag_offsets, cue_offsets, images_in_dev, Hi, Wi, labels_out_dev, cues_out_dev,
+                                  images_out_dev) && (!images_out_dev || images_in_dev != images_out_dev);
+    return dev_call(h, B, s, ok, [&](Engine *e) {
+        return annotation_forward(e, B, tag_offsets, tags, cue_offsets, cue_idx, flip, images_in_dev, Hi, Wi,
+                                  labels_out_dev, cues_out_dev, images_out_dev, s);
+    });
 }
 
 extern "C" int dsrg_annotation_forward_host(dsrg_engine *h, int B, const int32_t *tag_offsets, const int32_t *tags,
                                             const int32_t *cue_offsets, const int32_t *cue_idx, const int32_t *flip,
                                             const float *images_in, int Hi, int Wi, float *labels_out,
                                             float *cues_out, float *images_out) {
-    Engine *e = (Engine *)h;
-    DeviceScope dev_scope(e);
-    int rc = check_batch(e, B);
-    if (rc) return rc;
-    if ((rc = ensure_staging(e))) return rc;
-    cudaStream_t s = e->own_stream;
-    StreamScope stream_scope(e, s);
-    float *d_in = nullptr, *d_out = nullptr;
-    const size_t nimg = images_out ? (size_t)B * 3 * Hi * Wi : 0;
-    if (images_out) {
-        if (!images_in || Hi < 1 || Wi < 1) {
-            set_error("bad argument");
-            return DSRG_E_INVALID;
+    const bool ok = annot_args_ok(tag_offsets, cue_offsets, images_in, Hi, Wi, labels_out, cues_out, images_out);
+    return host_call(h, B, ok, false, [&](Engine *e, cudaStream_t s) {
+        float *d_in = nullptr, *d_out = nullptr;
+        const size_t nimg = images_out ? (size_t)B * 3 * Hi * Wi : 0;
+        if (images_out) {
+            if (int rc = grow_staging(e, (void **)&e->st_raw, &e->st_raw_cap, 2 * nimg * sizeof(float))) return rc;
+            d_in = e->st_raw;
+            d_out = e->st_raw + nimg;
+            DSRG_CUDA_TRY(cudaMemcpyAsync(d_in, images_in, nimg * sizeof(float), cudaMemcpyHostToDevice, s));
         }
-        if (2 * nimg > e->st_raw_cap) {
-            cudaFree(e->st_raw);
-            e->st_raw = nullptr;
-            e->st_raw_cap = 0;
-            if ((rc = dalloc(e, &e->st_raw, 2 * nimg))) return rc;
-            e->st_raw_cap = 2 * nimg;
-        }
-        d_in = e->st_raw;
-        d_out = e->st_raw + nimg;
-        DSRG_CUDA_TRY(cudaMemcpyAsync(d_in, images_in, nimg * sizeof(float), cudaMemcpyHostToDevice, s));
-    }
-    if ((rc = annotation_forward(e, B, tag_offsets, tags, cue_offsets, cue_idx, flip, d_in, Hi, Wi, e->st_labels,
-                                 e->st_cues, d_out, s)))
-        return rc;
-    DSRG_CUDA_TRY(cudaMemcpyAsync(labels_out, e->st_labels, sizeof(float) * (size_t)B * e->M, cudaMemcpyDeviceToHost, s));
-    DSRG_CUDA_TRY(cudaMemcpyAsync(cues_out, e->st_cues, sizeof(float) * (size_t)B * e->M * e->N, cudaMemcpyDeviceToHost, s));
-    if (images_out)
-        DSRG_CUDA_TRY(cudaMemcpyAsync(images_out, d_out, nimg * sizeof(float), cudaMemcpyDeviceToHost, s));
-    DSRG_CUDA_TRY(cudaStreamSynchronize(s));
-    return DSRG_OK;
+        if (int rc = annotation_forward(e, B, tag_offsets, tags, cue_offsets, cue_idx, flip, d_in, Hi, Wi,
+                                        e->st_labels, e->st_cues, d_out, s))
+            return rc;
+        DSRG_CUDA_TRY(cudaMemcpyAsync(labels_out, e->st_labels, sizeof(float) * (size_t)B * e->M, cudaMemcpyDeviceToHost, s));
+        DSRG_CUDA_TRY(cudaMemcpyAsync(cues_out, e->st_cues, sizeof(float) * (size_t)B * e->M * e->N, cudaMemcpyDeviceToHost, s));
+        if (images_out)
+            DSRG_CUDA_TRY(cudaMemcpyAsync(images_out, d_out, nimg * sizeof(float), cudaMemcpyDeviceToHost, s));
+        return DSRG_OK;
+    });
 }

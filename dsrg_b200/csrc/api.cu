@@ -219,10 +219,6 @@ static GraphKey pass_key(const Engine *e, int entry, int B, const dsrg_crf_param
 
 static int crf_core(Engine *e, int B, const float *unary, int layout, bool clamp, float *unary_rw,
                     const uint8_t *image, const dsrg_crf_params *p, cudaStream_t s) {
-    if (!unary || !image || !p) {
-        set_error("NULL pointer argument");
-        return DSRG_E_INVALID;
-    }
     if (layout != DSRG_LAYOUT_NHWC && layout != DSRG_LAYOUT_NCHW) {
         set_error("bad layout %d", layout);
         return DSRG_E_INVALID;
@@ -264,13 +260,37 @@ int ensure_staging(Engine *e) {
     return rc ? DSRG_E_NOMEM : DSRG_OK;
 }
 
+int grow_staging(Engine *e, void **buf, size_t *cap_bytes, size_t bytes) {
+    if (bytes <= *cap_bytes) return DSRG_OK;
+    cudaFree(*buf);  // synchronises with anything still reading it
+    *buf = nullptr;
+    *cap_bytes = 0;
+    if (int rc = device_alloc(e, buf, bytes)) return rc;
+    *cap_bytes = bytes;
+    return DSRG_OK;
+}
+
+static int no_engine() {
+    set_error("engine is NULL");
+    return DSRG_E_INVALID;
+}
+
+// the *_last_* entry points read what the engine's last mean-field pass left behind
+static int last_crf_held(const Engine *e, int B) {
+    if (e->last_crf_B == B) return DSRG_OK;
+    set_error("no mean-field result for a batch of %d is held by this engine (last: %d)", B, e->last_crf_B);
+    return DSRG_E_STATE;
+}
+
+static bool layout_ok(int layout) { return layout == DSRG_LAYOUT_NHWC || layout == DSRG_LAYOUT_NCHW; }
+
 }  // namespace dsrg
 
 using namespace dsrg;
 
 extern "C" {
 
-int dsrg_version(void) { return 101; }
+int dsrg_version(void) { return 102; }
 
 const char *dsrg_last_error(void) { return g_err; }
 
@@ -462,10 +482,7 @@ size_t dsrg_engine_device_bytes(const dsrg_engine *h) { return h ? ((const Engin
 
 int dsrg_engine_set_size(dsrg_engine *h, int H, int W) {
     Engine *e = (Engine *)h;
-    if (!e) {
-        set_error("engine is NULL");
-        return DSRG_E_INVALID;
-    }
+    if (!e) return no_engine();
     if (H < 1 || W < 1 || H > e->Hcap || W > e->Wcap) {
         set_error("size %dx%d outside the engine's capacity %dx%d", H, W, e->Hcap, e->Wcap);
         return DSRG_E_INVALID;
@@ -484,10 +501,7 @@ int dsrg_engine_set_size(dsrg_engine *h, int H, int W) {
 
 int dsrg_engine_get_size(const dsrg_engine *h, int *H, int *W, int *Hcap, int *Wcap) {
     const Engine *e = (const Engine *)h;
-    if (!e) {
-        set_error("engine is NULL");
-        return DSRG_E_INVALID;
-    }
+    if (!e) return no_engine();
     if (H) *H = e->H;
     if (W) *W = e->W;
     if (Hcap) *Hcap = e->Hcap;
@@ -514,14 +528,15 @@ const char *dsrg_profile_tag_name(int tag) { return (tag >= 0 && tag < T_COUNT) 
 
 int dsrg_engine_set_host_chunk(dsrg_engine *h, int images) {
     Engine *e = (Engine *)h;
-    if (!e || images < 0) return DSRG_E_INVALID;
+    if (!e) return no_engine();
+    if (images < 0) return DSRG_E_INVALID;
     e->host_chunk = images;
     return DSRG_OK;
 }
 
 int dsrg_engine_set_graphs(dsrg_engine *h, int enable) {
     Engine *e = (Engine *)h;
-    if (!e) return DSRG_E_INVALID;
+    if (!e) return no_engine();
     e->use_graphs = enable != 0;
     if (!enable) {
         DeviceScope dev_scope(e);
@@ -547,14 +562,15 @@ long long dsrg_engine_hybrid_tiles(dsrg_engine *h) {
 
 int dsrg_engine_profile(dsrg_engine *h, int enable) {
     Engine *e = (Engine *)h;
-    if (!e) return DSRG_E_INVALID;
+    if (!e) return no_engine();
     e->prof = enable != 0;
     return DSRG_OK;
 }
 
 int dsrg_engine_profile_read(dsrg_engine *h, float *ms_out, long long *count_out) {
     Engine *e = (Engine *)h;
-    if (!e || !ms_out || !count_out) return DSRG_E_INVALID;
+    if (!e) return no_engine();
+    if (!ms_out || !count_out) return DSRG_E_INVALID;
     DeviceScope dev_scope(e);
     DSRG_CUDA_TRY(cudaDeviceSynchronize());
     for (int t = 0; t < T_COUNT; t++) {
@@ -577,95 +593,65 @@ int dsrg_engine_profile_read(dsrg_engine *h, float *ms_out, long long *count_out
 int dsrg_crf_batch_dev(dsrg_engine *h, int B, const float *unary, int unary_layout,
                        const uint8_t *image, const dsrg_crf_params *params, float *out,
                        int out_layout, void *stream) {
-    Engine *e = (Engine *)h;
-    DeviceScope dev_scope(e);
-    int rc = check_batch(e, B);
-    if (rc) return rc;
-    StreamScope stream_scope(e, (cudaStream_t)stream);
-    if (!out || (out_layout != DSRG_LAYOUT_NHWC && out_layout != DSRG_LAYOUT_NCHW)) {
-        set_error("bad output argument");
-        return DSRG_E_INVALID;
-    }
-    cudaStream_t s = (cudaStream_t)stream;
-    GraphKey key = pass_key(e, 1, B, params);
-    key.add(unary).add(unary_layout).add(image).add(out).add(out_layout);
-    // krahenbuhl2013.CRF runs on this entry point with a size that changes from call to call: like the other
-    // per-image callers its graph carries the rebuild of the shared spatial lattice when one is due
-    const bool rebuild = params && post_pass_needs_spatial(e, params);
-    key.add(rebuild);
-    if (rebuild) e->sp_valid = false;
-    rc = run_pass(e, s, key, params != nullptr, [&]() {
-        int r = crf_core(e, B, unary, unary_layout, false, nullptr, image, params, s);
-        if (r) return r;
-        return meanfield_export(e, B, out, out_layout, s);
+    const cudaStream_t s = (cudaStream_t)stream;
+    return dev_call(h, B, s, unary && image && params && out && layout_ok(out_layout), [&](Engine *e) {
+        GraphKey key = pass_key(e, 1, B, params);
+        key.add(unary).add(unary_layout).add(image).add(out).add(out_layout);
+        // krahenbuhl2013.CRF runs on this entry point with a size that changes from call to call: like the other
+        // per-image callers its graph carries the rebuild of the shared spatial lattice when one is due
+        const bool rebuild = post_pass_needs_spatial(e, params);
+        key.add(rebuild);
+        if (rebuild) e->sp_valid = false;
+        const int rc = run_pass(e, s, key, true, [&]() {
+            int r = crf_core(e, B, unary, unary_layout, false, nullptr, image, params, s);
+            if (r) return r;
+            return meanfield_export(e, B, out, out_layout, s);
+        });
+        post_pass_done(e, params, B, rc);
+        return rc;
     });
-    post_pass_done(e, params, B, rc);
-    return rc;
 }
 
 int dsrg_crf_map_batch_dev(dsrg_engine *h, int B, const float *unary, int unary_layout,
                            const uint8_t *image, const dsrg_crf_params *params, int32_t *labels_out,
                            void *stream) {
-    Engine *e = (Engine *)h;
-    DeviceScope dev_scope(e);
-    int rc = check_batch(e, B);
-    if (rc) return rc;
-    StreamScope stream_scope(e, (cudaStream_t)stream);
-    if (!labels_out) {
-        set_error("labels_out is NULL");
-        return DSRG_E_INVALID;
-    }
-    cudaStream_t s = (cudaStream_t)stream;
-    GraphKey key = pass_key(e, 2, B, params);
-    key.add(unary).add(unary_layout).add(image).add(labels_out);
-    return crf_pass_done(e, B, run_pass(e, s, key, spatial_ready(e, params), [&]() {
-        int r = crf_core(e, B, unary, unary_layout, false, nullptr, image, params, s);
-        if (r) return r;
-        return meanfield_export_map(e, B, labels_out, s);
-    }));
+    const cudaStream_t s = (cudaStream_t)stream;
+    return dev_call(h, B, s, unary && image && params && labels_out, [&](Engine *e) {
+        GraphKey key = pass_key(e, 2, B, params);
+        key.add(unary).add(unary_layout).add(image).add(labels_out);
+        return crf_pass_done(e, B, run_pass(e, s, key, spatial_ready(e, params), [&]() {
+            int r = crf_core(e, B, unary, unary_layout, false, nullptr, image, params, s);
+            if (r) return r;
+            return meanfield_export_map(e, B, labels_out, s);
+        }));
+    });
 }
 
 int dsrg_crf_batch_host(dsrg_engine *h, int B, const float *unary, int unary_layout,
                         const uint8_t *image, const dsrg_crf_params *params, float *out,
                         int out_layout) {
-    Engine *e = (Engine *)h;
-    DeviceScope dev_scope(e);
-    int rc = check_batch(e, B);
-    if (rc) return rc;
-    if (!unary || !image || !out) {
-        set_error("NULL pointer argument");
-        return DSRG_E_INVALID;
-    }
-    if ((rc = ensure_staging(e))) return rc;
-    cudaStream_t s = e->own_stream;
-    StreamScope stream_scope(e, s);
-    const size_t n = (size_t)B * e->M * e->N;
-    DSRG_CUDA_TRY(cudaMemcpyAsync(e->st_unary, unary, n * sizeof(float), cudaMemcpyHostToDevice, s));
-    DSRG_CUDA_TRY(cudaMemcpyAsync(e->st_image, image, (size_t)B * e->N * 3, cudaMemcpyHostToDevice, s));
-    rc = dsrg_crf_batch_dev(h, B, e->st_unary, unary_layout, e->st_image, params, e->st_out, out_layout, s);
-    if (rc) return rc;
-    DSRG_CUDA_TRY(cudaMemcpyAsync(out, e->st_out, n * sizeof(float), cudaMemcpyDeviceToHost, s));
-    return check_device_flag(e, s);
+    return host_call(h, B, unary && image && params && out, true, [&](Engine *e, cudaStream_t s) {
+        const size_t n = (size_t)B * e->M * e->N;
+        DSRG_CUDA_TRY(cudaMemcpyAsync(e->st_unary, unary, n * sizeof(float), cudaMemcpyHostToDevice, s));
+        DSRG_CUDA_TRY(cudaMemcpyAsync(e->st_image, image, (size_t)B * e->N * 3, cudaMemcpyHostToDevice, s));
+        if (int rc = dsrg_crf_batch_dev(h, B, e->st_unary, unary_layout, e->st_image, params, e->st_out, out_layout, s))
+            return rc;
+        DSRG_CUDA_TRY(cudaMemcpyAsync(out, e->st_out, n * sizeof(float), cudaMemcpyDeviceToHost, s));
+        return DSRG_OK;
+    });
 }
 
 int dsrg_srg_batch_dev(dsrg_engine *h, int B, const float *labels, const float *probs,
                        const float *cues, double th1, double th2, int renorm, float *seeds_out,
                        int32_t *label_map_out, void *stream) {
-    Engine *e = (Engine *)h;
-    DeviceScope dev_scope(e);
-    int rc = check_batch(e, B);
-    if (rc) return rc;
-    StreamScope stream_scope(e, (cudaStream_t)stream);
-    if (!labels || !probs || !cues || !seeds_out) {
-        set_error("NULL pointer argument");
-        return DSRG_E_INVALID;
-    }
-    if (e->M > 255) {
-        set_error("SRG supports at most 255 classes");
-        return DSRG_E_INVALID;
-    }
-    return srg_run(e, B, labels, probs, cues, th1, th2, renorm, seeds_out, label_map_out,
-                   (cudaStream_t)stream);
+    const cudaStream_t s = (cudaStream_t)stream;
+    return dev_call(h, B, s, labels && probs && cues && seeds_out, [&](Engine *e) {
+        if (e->M > 255) {
+            set_error("SRG supports at most 255 classes");
+            return DSRG_E_INVALID;
+        }
+        return srg_run(e, B, labels, probs, cues, th1, th2, renorm, seeds_out, label_map_out, s);
+    });
 }
 
 }  // extern "C"
@@ -693,184 +679,64 @@ extern "C" {
 int dsrg_dsrg_forward_dev(dsrg_engine *h, int B, const float *labels, float *probs,
                           const float *cues, const uint8_t *image, const dsrg_crf_params *params,
                           double th1, double th2, float *seeds_out, float *crf_out, void *stream) {
-    Engine *e = (Engine *)h;
-    DeviceScope dev_scope(e);
-    int rc = check_batch(e, B);
-    if (rc) return rc;
-    StreamScope stream_scope(e, (cudaStream_t)stream);
-    if (!labels || !probs || !cues || !seeds_out) {
-        set_error("NULL pointer argument");
-        return DSRG_E_INVALID;
-    }
-    return dsrg_forward_core(e, B, labels, probs, cues, nullptr, image, params, th1, th2, seeds_out, nullptr, crf_out,
-                             (cudaStream_t)stream);
+    const cudaStream_t s = (cudaStream_t)stream;
+    return dev_call(h, B, s, labels && probs && cues && image && params && seeds_out, [&](Engine *e) {
+        return dsrg_forward_core(e, B, labels, probs, cues, nullptr, image, params, th1, th2, seeds_out, nullptr,
+                                 crf_out, s);
+    });
 }
 
 int dsrg_crflayer_forward_dev(dsrg_engine *h, int B, float *probs, const uint8_t *image,
                               const dsrg_crf_params *params, float *log_out, float *result,
                               void *stream) {
-    Engine *e = (Engine *)h;
-    DeviceScope dev_scope(e);
-    int rc = check_batch(e, B);
-    if (rc) return rc;
-    StreamScope stream_scope(e, (cudaStream_t)stream);
-    if (!probs || !log_out) {
-        set_error("NULL pointer argument");
-        return DSRG_E_INVALID;
-    }
-    cudaStream_t s = (cudaStream_t)stream;
-    GraphKey key = pass_key(e, 4, B, params);
-    key.add(probs).add(image).add(log_out).add(result);
-    return crf_pass_done(e, B, run_pass(e, s, key, spatial_ready(e, params), [&]() {
-        int r = crf_core(e, B, probs, DSRG_LAYOUT_NCHW, true, probs, image, params, s);
-        if (r) return r;
-        return meanfield_export_renorm(e, B, result, log_out, s);
-    }));
+    const cudaStream_t s = (cudaStream_t)stream;
+    return dev_call(h, B, s, probs && image && params && log_out, [&](Engine *e) {
+        GraphKey key = pass_key(e, 4, B, params);
+        key.add(probs).add(image).add(log_out).add(result);
+        return crf_pass_done(e, B, run_pass(e, s, key, spatial_ready(e, params), [&]() {
+            int r = crf_core(e, B, probs, DSRG_LAYOUT_NCHW, true, probs, image, params, s);
+            if (r) return r;
+            return meanfield_export_renorm(e, B, result, log_out, s);
+        }));
+    });
 }
 
 // ---- one refinement, two consumers (train-s.prototxt:758-786: CRFLayer and DSRGLayer read the same blobs) ----
 int dsrg_srg_last_crf_host(dsrg_engine *h, int B, const float *labels, const float *cues, double th1, double th2,
                            float *seeds_out) {
-    Engine *e = (Engine *)h;
-    DeviceScope dev_scope(e);
-    int rc = check_batch(e, B);
-    if (rc) return rc;
-    if (!labels || !cues || !seeds_out) {
-        set_error("NULL pointer argument");
-        return DSRG_E_INVALID;
-    }
-    if (e->last_crf_B != B) {
-        set_error("no mean-field result for a batch of %d is held by this engine (last: %d)", B, e->last_crf_B);
-        return DSRG_E_STATE;
-    }
-    if ((rc = ensure_staging(e))) return rc;
-    cudaStream_t s = e->own_stream;
-    StreamScope stream_scope(e, s);
-    const size_t n = (size_t)B * e->M * e->N;
-    DSRG_CUDA_TRY(cudaMemcpyAsync(e->st_labels, labels, (size_t)B * e->M * sizeof(float), cudaMemcpyHostToDevice, s));
-    DSRG_CUDA_TRY(cudaMemcpyAsync(e->st_cues, cues, n * sizeof(float), cudaMemcpyHostToDevice, s));
-    // SRG on the raw marginals of the last pass, float64 clamp + renormalisation fused in (pylayers.py:328-344)
-    if ((rc = srg_run(e, B, e->st_labels, e->Qcur, e->st_cues, th1, th2, 1, e->st_out, nullptr, s))) return rc;
-    DSRG_CUDA_TRY(cudaMemcpyAsync(seeds_out, e->st_out, n * sizeof(float), cudaMemcpyDeviceToHost, s));
-    return check_device_flag(e, s);
+    return host_call(h, B, labels && cues && seeds_out, true, [&](Engine *e, cudaStream_t s) {
+        const size_t n = (size_t)B * e->M * e->N;
+        DSRG_CUDA_TRY(cudaMemcpyAsync(e->st_labels, labels, (size_t)B * e->M * sizeof(float), cudaMemcpyHostToDevice, s));
+        DSRG_CUDA_TRY(cudaMemcpyAsync(e->st_cues, cues, n * sizeof(float), cudaMemcpyHostToDevice, s));
+        // SRG on the raw marginals of the last pass, float64 clamp + renormalisation fused in (pylayers.py:328-344)
+        if (int rc = srg_run(e, B, e->st_labels, e->Qcur, e->st_cues, th1, th2, 1, e->st_out, nullptr, s)) return rc;
+        DSRG_CUDA_TRY(cudaMemcpyAsync(seeds_out, e->st_out, n * sizeof(float), cudaMemcpyDeviceToHost, s));
+        return DSRG_OK;
+    }, last_crf_held);
 }
 
 int dsrg_crf_last_marginals_host(dsrg_engine *h, int B, float *out, int out_layout) {
-    Engine *e = (Engine *)h;
-    DeviceScope dev_scope(e);
-    int rc = check_batch(e, B);
-    if (rc) return rc;
-    if (!out || (out_layout != DSRG_LAYOUT_NHWC && out_layout != DSRG_LAYOUT_NCHW)) {
-        set_error("bad output argument");
-        return DSRG_E_INVALID;
-    }
-    if (e->last_crf_B != B) {
-        set_error("no mean-field result for a batch of %d is held by this engine (last: %d)", B, e->last_crf_B);
-        return DSRG_E_STATE;
-    }
-    if ((rc = ensure_staging(e))) return rc;
-    cudaStream_t s = e->own_stream;
-    StreamScope stream_scope(e, s);
-    if ((rc = meanfield_export(e, B, e->st_out, out_layout, s))) return rc;
-    DSRG_CUDA_TRY(cudaMemcpyAsync(out, e->st_out, (size_t)B * e->M * e->N * sizeof(float), cudaMemcpyDeviceToHost, s));
-    DSRG_CUDA_TRY(cudaStreamSynchronize(s));
-    return DSRG_OK;
+    return host_call(h, B, out && layout_ok(out_layout), false, [&](Engine *e, cudaStream_t s) {
+        if (int rc = meanfield_export(e, B, e->st_out, out_layout, s)) return rc;
+        DSRG_CUDA_TRY(cudaMemcpyAsync(out, e->st_out, (size_t)B * e->M * e->N * sizeof(float), cudaMemcpyDeviceToHost, s));
+        return DSRG_OK;
+    }, last_crf_held);
 }
 
 int dsrg_crflayer_forward_host(dsrg_engine *h, int B, float *probs, const uint8_t *image,
                                const dsrg_crf_params *params, float *log_out, float *result) {
-    Engine *e = (Engine *)h;
-    DeviceScope dev_scope(e);
-    int rc = check_batch(e, B);
-    if (rc) return rc;
-    if (!probs || !image || !log_out) {
-        set_error("NULL pointer argument");
-        return DSRG_E_INVALID;
-    }
-    if ((rc = ensure_staging(e))) return rc;
-    cudaStream_t s = e->own_stream;
-    StreamScope stream_scope(e, s);
-    const size_t n = (size_t)B * e->M * e->N;
-    DSRG_CUDA_TRY(cudaMemcpyAsync(e->st_unary, probs, n * sizeof(float), cudaMemcpyHostToDevice, s));
-    DSRG_CUDA_TRY(cudaMemcpyAsync(e->st_image, image, (size_t)B * e->N * 3, cudaMemcpyHostToDevice, s));
-    rc = dsrg_crflayer_forward_dev(h, B, e->st_unary, e->st_image, params, e->st_out, result ? e->st_cues : nullptr, s);
-    if (rc) return rc;
-    DSRG_CUDA_TRY(cudaMemcpyAsync(log_out, e->st_out, n * sizeof(float), cudaMemcpyDeviceToHost, s));
-    DSRG_CUDA_TRY(cudaMemcpyAsync(probs, e->st_unary, n * sizeof(float), cudaMemcpyDeviceToHost, s));
-    if (result) DSRG_CUDA_TRY(cudaMemcpyAsync(result, e->st_cues, n * sizeof(float), cudaMemcpyDeviceToHost, s));
-    return check_device_flag(e, s);
-}
-
-int dsrg_seedloss_forward_host(dsrg_engine *h, int B, const float *probs, const float *seeds,
-                               float *terms_out) {
-    Engine *e = (Engine *)h;
-    DeviceScope dev_scope(e);
-    int rc = check_batch(e, B);
-    if (rc) return rc;
-    if (!probs || !seeds || !terms_out) {
-        set_error("NULL pointer argument");
-        return DSRG_E_INVALID;
-    }
-    if ((rc = ensure_staging(e))) return rc;
-    cudaStream_t s = e->own_stream;
-    StreamScope stream_scope(e, s);
-    const size_t n = (size_t)B * e->M * e->N;
-    DSRG_CUDA_TRY(cudaMemcpyAsync(e->st_unary, probs, n * sizeof(float), cudaMemcpyHostToDevice, s));
-    DSRG_CUDA_TRY(cudaMemcpyAsync(e->st_cues, seeds, n * sizeof(float), cudaMemcpyHostToDevice, s));
-    if ((rc = seedloss_forward(e, B, e->st_unary, e->st_cues, e->st_labels, s))) return rc;
-    DSRG_CUDA_TRY(cudaMemcpyAsync(terms_out, e->st_labels, 2 * sizeof(float), cudaMemcpyDeviceToHost, s));
-    DSRG_CUDA_TRY(cudaStreamSynchronize(s));
-    return DSRG_OK;
-}
-
-int dsrg_seedloss_backward_host(dsrg_engine *h, int B, int n_global, const float *probs,
-                                const float *seeds, float top_diff, float *grad) {
-    Engine *e = (Engine *)h;
-    DeviceScope dev_scope(e);
-    int rc = check_batch(e, B);
-    if (rc) return rc;
-    if (!probs || !seeds || !grad || n_global < 1) {
-        set_error("bad argument");
-        return DSRG_E_INVALID;
-    }
-    if ((rc = ensure_staging(e))) return rc;
-    cudaStream_t s = e->own_stream;
-    StreamScope stream_scope(e, s);
-    const size_t n = (size_t)B * e->M * e->N;
-    DSRG_CUDA_TRY(cudaMemcpyAsync(e->st_unary, probs, n * sizeof(float), cudaMemcpyHostToDevice, s));
-    DSRG_CUDA_TRY(cudaMemcpyAsync(e->st_cues, seeds, n * sizeof(float), cudaMemcpyHostToDevice, s));
-    if ((rc = seedloss_backward(e, B, n_global, e->st_unary, e->st_cues, top_diff, e->st_out, s))) return rc;
-    DSRG_CUDA_TRY(cudaMemcpyAsync(grad, e->st_out, n * sizeof(float), cudaMemcpyDeviceToHost, s));
-    DSRG_CUDA_TRY(cudaStreamSynchronize(s));
-    return DSRG_OK;
-}
-
-int dsrg_seedloss_forward_dev(dsrg_engine *h, int B, const float *probs, const float *seeds,
-                              float *terms_out, void *stream) {
-    Engine *e = (Engine *)h;
-    DeviceScope dev_scope(e);
-    int rc = check_batch(e, B);
-    if (rc) return rc;
-    StreamScope stream_scope(e, (cudaStream_t)stream);
-    if (!probs || !seeds || !terms_out) {
-        set_error("NULL pointer argument");
-        return DSRG_E_INVALID;
-    }
-    return seedloss_forward(e, B, probs, seeds, terms_out, (cudaStream_t)stream);
-}
-
-int dsrg_seedloss_backward_dev(dsrg_engine *h, int B, int n_global, const float *probs,
-                               const float *seeds, float top_diff, float *grad, void *stream) {
-    Engine *e = (Engine *)h;
-    DeviceScope dev_scope(e);
-    int rc = check_batch(e, B);
-    if (rc) return rc;
-    StreamScope stream_scope(e, (cudaStream_t)stream);
-    if (!probs || !seeds || !grad || n_global < 1) {
-        set_error("bad argument");
-        return DSRG_E_INVALID;
-    }
-    return seedloss_backward(e, B, n_global, probs, seeds, top_diff, grad, (cudaStream_t)stream);
+    return host_call(h, B, probs && image && params && log_out, true, [&](Engine *e, cudaStream_t s) {
+        const size_t n = (size_t)B * e->M * e->N;
+        DSRG_CUDA_TRY(cudaMemcpyAsync(e->st_unary, probs, n * sizeof(float), cudaMemcpyHostToDevice, s));
+        DSRG_CUDA_TRY(cudaMemcpyAsync(e->st_image, image, (size_t)B * e->N * 3, cudaMemcpyHostToDevice, s));
+        if (int rc = dsrg_crflayer_forward_dev(h, B, e->st_unary, e->st_image, params, e->st_out,
+                                               result ? e->st_cues : nullptr, s))
+            return rc;
+        DSRG_CUDA_TRY(cudaMemcpyAsync(log_out, e->st_out, n * sizeof(float), cudaMemcpyDeviceToHost, s));
+        DSRG_CUDA_TRY(cudaMemcpyAsync(probs, e->st_unary, n * sizeof(float), cudaMemcpyDeviceToHost, s));
+        if (result) DSRG_CUDA_TRY(cudaMemcpyAsync(result, e->st_cues, n * sizeof(float), cudaMemcpyDeviceToHost, s));
+        return DSRG_OK;
+    });
 }
 
 int dsrg_engine_lattice_sizes(dsrg_engine *h, int B, int *v_spatial, int *v_bilateral) {
@@ -888,7 +754,7 @@ int dsrg_engine_lattice_sizes(dsrg_engine *h, int B, int *v_spatial, int *v_bila
 int dsrg_engine_copy_norm(dsrg_engine *h, int which, int B, float *norm_out) {
     Engine *e = (Engine *)h;
     DeviceScope dev_scope(e);
-    int rc = check_batch(e, B);
+    int rc = check_entry(e, B, norm_out != nullptr);
     if (rc) return rc;
     DSRG_CUDA_TRY(cudaDeviceSynchronize());
     if (which == 0)
@@ -1003,23 +869,22 @@ int dsrg_densecrf_add_pairwise_energy(dsrg_densecrf *c, float w1, float theta_al
     return DSRG_OK;
 }
 
-// runs the mean field on the borrowed engine; the caller holds g_pool_mu until its export + copy are done
-static int densecrf_run(dsrg_densecrf *c, int n_iters, Engine **eng) {
-    if (!c) {
-        set_error("NULL object");
+// the engine an object borrows; the caller holds g_pool_mu until its export + copy are done
+static int densecrf_engine(dsrg_densecrf *c, const void *out, Engine **e) {
+    if (!c || !out) {
+        set_error("bad argument (NULL pointer or value out of range)");
         return DSRG_E_INVALID;
     }
-    Engine *e = pool_engine(c->H, c->W, c->M);
-    if (!e) return DSRG_E_CUDA;
-    *eng = e;
-    DeviceScope dev_scope(e);
+    *e = pool_engine(c->H, c->W, c->M);
+    return *e ? DSRG_OK : DSRG_E_CUDA;
+}
+
+// runs the mean field on the borrowed engine, inside its host_call
+static int densecrf_run(dsrg_densecrf *c, int n_iters, Engine *e, cudaStream_t s) {
     int rc = dsrg_engine_set_size((dsrg_engine *)e, c->H, c->W);
     if (rc) return rc;
-    if ((rc = ensure_staging(e))) return rc;
     if (!c->has_unary) c->unary.assign((size_t)c->W * c->H * c->M, 0.0f);  // unary.fill(0), densecrf.cpp:117
     c->params.n_iters = n_iters;
-    cudaStream_t s = e->own_stream;
-    StreamScope stream_scope(e, s);
     DSRG_CUDA_TRY(cudaMemcpyAsync(e->st_unary, c->unary.data(), c->unary.size() * sizeof(float), cudaMemcpyHostToDevice, s));
     if (!c->has_pairwise) {
         // no pairwise term: every mean-field step reproduces Q = softmax(-unary) (densecrf.cpp:120-128 with an
@@ -1041,37 +906,27 @@ static int densecrf_run(dsrg_densecrf *c, int n_iters, Engine **eng) {
 }
 
 int dsrg_densecrf_inference(dsrg_densecrf *c, int n_iters, float *probs_out) {
-    if (!probs_out) {
-        set_error("NULL pointer argument");
-        return DSRG_E_INVALID;
-    }
     std::lock_guard<std::mutex> lk(g_pool_mu);
-    Engine *e = nullptr;
-    int rc = densecrf_run(c, n_iters, &e);
-    if (rc) return rc;
-    DeviceScope dev_scope(e);
-    cudaStream_t s = e->own_stream;
-    StreamScope stream_scope(e, s);
-    if ((rc = meanfield_export(e, 1, e->st_out, DSRG_LAYOUT_NHWC, s))) return rc;
-    DSRG_CUDA_TRY(cudaMemcpyAsync(probs_out, e->st_out, c->unary.size() * sizeof(float), cudaMemcpyDeviceToHost, s));
-    return check_device_flag(e, s);
+    Engine *eng = nullptr;
+    if (int rc = densecrf_engine(c, probs_out, &eng)) return rc;
+    return host_call((dsrg_engine *)eng, 1, true, true, [&](Engine *e, cudaStream_t s) {
+        int rc = densecrf_run(c, n_iters, e, s);
+        if (rc || (rc = meanfield_export(e, 1, e->st_out, DSRG_LAYOUT_NHWC, s))) return rc;
+        DSRG_CUDA_TRY(cudaMemcpyAsync(probs_out, e->st_out, c->unary.size() * sizeof(float), cudaMemcpyDeviceToHost, s));
+        return DSRG_OK;
+    });
 }
 
 int dsrg_densecrf_map(dsrg_densecrf *c, int n_iters, int *labels) {
-    if (!labels) {
-        set_error("NULL pointer argument");
-        return DSRG_E_INVALID;
-    }
     std::lock_guard<std::mutex> lk(g_pool_mu);
-    Engine *e = nullptr;
-    int rc = densecrf_run(c, n_iters, &e);
-    if (rc) return rc;
-    DeviceScope dev_scope(e);
-    cudaStream_t s = e->own_stream;
-    StreamScope stream_scope(e, s);
-    if ((rc = meanfield_export_map(e, 1, e->st_lmap, s))) return rc;
-    DSRG_CUDA_TRY(cudaMemcpyAsync(labels, e->st_lmap, (size_t)c->W * c->H * sizeof(int), cudaMemcpyDeviceToHost, s));
-    return check_device_flag(e, s);
+    Engine *eng = nullptr;
+    if (int rc = densecrf_engine(c, labels, &eng)) return rc;
+    return host_call((dsrg_engine *)eng, 1, true, true, [&](Engine *e, cudaStream_t s) {
+        int rc = densecrf_run(c, n_iters, e, s);
+        if (rc || (rc = meanfield_export_map(e, 1, e->st_lmap, s))) return rc;
+        DSRG_CUDA_TRY(cudaMemcpyAsync(labels, e->st_lmap, (size_t)c->W * c->H * sizeof(int), cudaMemcpyDeviceToHost, s));
+        return DSRG_OK;
+    });
 }
 
 }  // extern "C"

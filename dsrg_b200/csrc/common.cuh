@@ -157,11 +157,6 @@ int dsrg_forward_core(Engine *e, int B, const float *labels, float *probs, const
                       uint32_t *seed_bits, float *crf_out, cudaStream_t s);
 bool post_pass_needs_spatial(const Engine *e, const dsrg_crf_params *p);
 void post_pass_done(Engine *e, const dsrg_crf_params *p, int B, int rc);
-// ---- loss.cu ----
-int seedloss_forward(Engine *e, int B, const float *probs, const float *seeds, float *terms_out,
-                     cudaStream_t s);
-int seedloss_backward(Engine *e, int B, int n_global, const float *probs, const float *seeds,
-                      float top_diff, float *grad, cudaStream_t s);
 // ---- sec_loss.cu ----
 constexpr int kSecPlainChunks = 16;  // CTAs per image of SeedLossLayer's sums (fixed, so is their order)
 
@@ -208,7 +203,8 @@ struct Engine {
     // staging for the *_host entry points
     float *st_unary = nullptr, *st_out = nullptr, *st_cues = nullptr, *st_labels = nullptr;
     uint8_t *st_image = nullptr;
-    float *st_raw = nullptr;   // raw (un-zoomed) images of the *_host preprocessing entry point
+    // staging whose size depends on the call, grown on demand (grow_staging); capacities in bytes
+    float *st_raw = nullptr;   // raw (un-zoomed) images and score maps of the *_host entry points
     size_t st_raw_cap = 0;
     int32_t *st_idx = nullptr;  // index lists of the annotation entry points
     size_t st_idx_cap = 0;
@@ -414,11 +410,54 @@ inline int run_pass(Engine *e, cudaStream_t s, const GraphKey &key, bool allow_g
 int device_alloc(Engine *e, void **p, size_t bytes);
 int check_batch(Engine *e, int B);
 int ensure_staging(Engine *e);
+int grow_staging(Engine *e, void **buf, size_t *cap_bytes, size_t bytes);  // frees the old buffer first
 int check_device_flag(Engine *e, cudaStream_t s);
 void wire_free(Engine *e);
 template <typename T>
 inline int dalloc(Engine *e, T **p, size_t count) {
     return device_alloc(e, (void **)p, count * sizeof(T));
+}
+
+// ---- the prologue of every engine entry point of the C ABI ----
+// In this order: the engine's device for the whole call (DeviceScope, restored on every path), the NULL engine and
+// the batch range (check_batch), the arguments, and only then the stream (StreamScope).  `args_ok` is false when a
+// required pointer is NULL or a plain argument is out of range; a call rejected here allocates and queues nothing.
+// Checks that need the engine's shape or labels stay in the body.
+inline int check_entry(Engine *e, int B, bool args_ok) {
+    if (int rc = check_batch(e, B)) return rc;
+    if (args_ok) return DSRG_OK;
+    set_error("bad argument (NULL pointer or value out of range)");
+    return DSRG_E_INVALID;
+}
+
+// *_dev entry points: body(e) runs on the caller's stream `s`
+template <typename F>
+inline int dev_call(dsrg_engine *h, int B, cudaStream_t s, bool args_ok, F body) {
+    Engine *e = (Engine *)h;
+    DeviceScope dev_scope(e);
+    if (int rc = check_entry(e, B, args_ok)) return rc;
+    StreamScope stream_scope(e, s);
+    return body(e);
+}
+
+// *_host entry points: the same prologue, then `state` (a check of what the engine holds, if given), the staging
+// buffers (ensure_staging), and body(e, s) on the engine's own stream, which copies in, runs what the *_dev twin runs
+// and copies out.  Returns once those copies have landed: through check_device_flag for the passes that end in it
+// (`flag`), else a stream synchronisation.
+template <typename F>
+inline int host_call(dsrg_engine *h, int B, bool args_ok, bool flag, F body,
+                     int (*state)(const Engine *, int) = nullptr) {
+    Engine *e = (Engine *)h;
+    DeviceScope dev_scope(e);
+    int rc = check_entry(e, B, args_ok);
+    if (!rc && state) rc = state(e, B);
+    if (rc || (rc = ensure_staging(e))) return rc;
+    cudaStream_t s = e->own_stream;
+    StreamScope stream_scope(e, s);
+    if ((rc = body(e, s))) return rc;
+    if (flag) return check_device_flag(e, s);
+    DSRG_CUDA_TRY(cudaStreamSynchronize(s));
+    return DSRG_OK;
 }
 
 }  // namespace dsrg

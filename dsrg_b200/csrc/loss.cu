@@ -283,85 +283,105 @@ int constrain_backward(Engine *e, int B, const float *probs, const float *logs, 
 
 using namespace dsrg;
 
-// generic host wrapper: up to two planar inputs in, up to two planar outputs (or one scalar) out
-static int host_elementwise(dsrg_engine *h, int B, const float *in0, const float *in1, float *out0, float *out1,
-                            float *scalar_out, int op) {
-    Engine *e = (Engine *)h;
-    DeviceScope dev_scope(e);
-    int rc = check_batch(e, B);
-    if (rc) return rc;
-    if (!in0 || (op != 0 && !in1)) {
-        set_error("NULL pointer argument");
-        return DSRG_E_INVALID;
-    }
-    if ((rc = ensure_staging(e))) return rc;
-    cudaStream_t s = e->own_stream;
-    StreamScope stream_scope(e, s);
-    const size_t n = (size_t)B * e->M * e->N;
-    DSRG_CUDA_TRY(cudaMemcpyAsync(e->st_unary, in0, n * sizeof(float), cudaMemcpyHostToDevice, s));
-    if (in1) DSRG_CUDA_TRY(cudaMemcpyAsync(e->st_cues, in1, n * sizeof(float), cudaMemcpyHostToDevice, s));
-    switch (op) {
-        case 0: rc = softmax_forward(e, B, e->st_unary, e->st_out, s); break;
-        case 1: rc = softmax_backward(e, B, e->st_unary, e->st_cues, e->st_out, s); break;
-        case 2: rc = constrain_forward(e, B, e->st_unary, e->st_cues, e->st_labels, s); break;
-        case 3: rc = constrain_backward(e, B, e->st_unary, e->st_cues, e->st_out, e->U, s); break;
-    }
-    if (rc) return rc;
-    if (out0) DSRG_CUDA_TRY(cudaMemcpyAsync(out0, e->st_out, n * sizeof(float), cudaMemcpyDeviceToHost, s));
-    if (out1) DSRG_CUDA_TRY(cudaMemcpyAsync(out1, e->U, n * sizeof(float), cudaMemcpyDeviceToHost, s));
-    if (scalar_out) DSRG_CUDA_TRY(cudaMemcpyAsync(scalar_out, e->st_labels, sizeof(float), cudaMemcpyDeviceToHost, s));
-    DSRG_CUDA_TRY(cudaStreamSynchronize(s));
-    return DSRG_OK;
+extern "C" {
+int dsrg_seedloss_forward_dev(dsrg_engine *h, int B, const float *probs, const float *seeds, float *terms_out,
+                              void *stream) {
+    const cudaStream_t s = (cudaStream_t)stream;
+    return dev_call(h, B, s, probs && seeds && terms_out,
+                    [&](Engine *e) { return seedloss_forward(e, B, probs, seeds, terms_out, s); });
+}
+int dsrg_seedloss_backward_dev(dsrg_engine *h, int B, int n_global, const float *probs, const float *seeds,
+                               float top_diff, float *grad, void *stream) {
+    const cudaStream_t s = (cudaStream_t)stream;
+    return dev_call(h, B, s, probs && seeds && grad && n_global >= 1, [&](Engine *e) {
+        return seedloss_backward(e, B, n_global, probs, seeds, top_diff, grad, s);
+    });
+}
+int dsrg_seedloss_forward_host(dsrg_engine *h, int B, const float *probs, const float *seeds, float *terms_out) {
+    return host_call(h, B, probs && seeds && terms_out, false, [&](Engine *e, cudaStream_t s) {
+        const size_t n = (size_t)B * e->M * e->N;
+        DSRG_CUDA_TRY(cudaMemcpyAsync(e->st_unary, probs, n * sizeof(float), cudaMemcpyHostToDevice, s));
+        DSRG_CUDA_TRY(cudaMemcpyAsync(e->st_cues, seeds, n * sizeof(float), cudaMemcpyHostToDevice, s));
+        if (int rc = seedloss_forward(e, B, e->st_unary, e->st_cues, e->st_labels, s)) return rc;
+        DSRG_CUDA_TRY(cudaMemcpyAsync(terms_out, e->st_labels, 2 * sizeof(float), cudaMemcpyDeviceToHost, s));
+        return DSRG_OK;
+    });
+}
+int dsrg_seedloss_backward_host(dsrg_engine *h, int B, int n_global, const float *probs, const float *seeds,
+                                float top_diff, float *grad) {
+    return host_call(h, B, probs && seeds && grad && n_global >= 1, false, [&](Engine *e, cudaStream_t s) {
+        const size_t n = (size_t)B * e->M * e->N;
+        DSRG_CUDA_TRY(cudaMemcpyAsync(e->st_unary, probs, n * sizeof(float), cudaMemcpyHostToDevice, s));
+        DSRG_CUDA_TRY(cudaMemcpyAsync(e->st_cues, seeds, n * sizeof(float), cudaMemcpyHostToDevice, s));
+        if (int rc = seedloss_backward(e, B, n_global, e->st_unary, e->st_cues, top_diff, e->st_out, s)) return rc;
+        DSRG_CUDA_TRY(cudaMemcpyAsync(grad, e->st_out, n * sizeof(float), cudaMemcpyDeviceToHost, s));
+        return DSRG_OK;
+    });
 }
 
-extern "C" {
 int dsrg_softmax_forward_dev(dsrg_engine *h, int B, const float *preds, float *probs_out, void *stream) {
-    Engine *e = (Engine *)h;
-    DeviceScope dev_scope(e);
-    int rc = check_batch(e, B);
-    if (rc) return rc;
-    StreamScope stream_scope(e, (cudaStream_t)stream);
-    return softmax_forward(e, B, preds, probs_out, (cudaStream_t)stream);
+    const cudaStream_t s = (cudaStream_t)stream;
+    return dev_call(h, B, s, preds && probs_out, [&](Engine *e) { return softmax_forward(e, B, preds, probs_out, s); });
 }
 int dsrg_softmax_backward_dev(dsrg_engine *h, int B, const float *preds, const float *top_diff, float *grad_out,
                               void *stream) {
-    Engine *e = (Engine *)h;
-    DeviceScope dev_scope(e);
-    int rc = check_batch(e, B);
-    if (rc) return rc;
-    StreamScope stream_scope(e, (cudaStream_t)stream);
-    return softmax_backward(e, B, preds, top_diff, grad_out, (cudaStream_t)stream);
+    const cudaStream_t s = (cudaStream_t)stream;
+    return dev_call(h, B, s, preds && top_diff && grad_out,
+                    [&](Engine *e) { return softmax_backward(e, B, preds, top_diff, grad_out, s); });
 }
 int dsrg_constrainloss_forward_dev(dsrg_engine *h, int B, const float *probs, const float *log_smooth,
                                    float *loss_out, void *stream) {
-    Engine *e = (Engine *)h;
-    DeviceScope dev_scope(e);
-    int rc = check_batch(e, B);
-    if (rc) return rc;
-    StreamScope stream_scope(e, (cudaStream_t)stream);
-    return constrain_forward(e, B, probs, log_smooth, loss_out, (cudaStream_t)stream);
+    const cudaStream_t s = (cudaStream_t)stream;
+    return dev_call(h, B, s, probs && log_smooth && loss_out,
+                    [&](Engine *e) { return constrain_forward(e, B, probs, log_smooth, loss_out, s); });
 }
 int dsrg_constrainloss_backward_dev(dsrg_engine *h, int B, const float *probs, const float *log_smooth,
                                     float *grad_probs, float *grad_log, void *stream) {
-    Engine *e = (Engine *)h;
-    DeviceScope dev_scope(e);
-    int rc = check_batch(e, B);
-    if (rc) return rc;
-    StreamScope stream_scope(e, (cudaStream_t)stream);
-    return constrain_backward(e, B, probs, log_smooth, grad_probs, grad_log, (cudaStream_t)stream);
+    const cudaStream_t s = (cudaStream_t)stream;
+    return dev_call(h, B, s, probs && log_smooth && grad_probs && grad_log,
+                    [&](Engine *e) { return constrain_backward(e, B, probs, log_smooth, grad_probs, grad_log, s); });
 }
 int dsrg_softmax_forward_host(dsrg_engine *h, int B, const float *preds, float *probs_out) {
-    return host_elementwise(h, B, preds, nullptr, probs_out, nullptr, nullptr, 0);
+    return host_call(h, B, preds && probs_out, false, [&](Engine *e, cudaStream_t s) {
+        const size_t n = (size_t)B * e->M * e->N;
+        DSRG_CUDA_TRY(cudaMemcpyAsync(e->st_unary, preds, n * sizeof(float), cudaMemcpyHostToDevice, s));
+        if (int rc = softmax_forward(e, B, e->st_unary, e->st_out, s)) return rc;
+        DSRG_CUDA_TRY(cudaMemcpyAsync(probs_out, e->st_out, n * sizeof(float), cudaMemcpyDeviceToHost, s));
+        return DSRG_OK;
+    });
 }
 int dsrg_softmax_backward_host(dsrg_engine *h, int B, const float *preds, const float *top_diff, float *grad_out) {
-    return host_elementwise(h, B, preds, top_diff, grad_out, nullptr, nullptr, 1);
+    return host_call(h, B, preds && top_diff && grad_out, false, [&](Engine *e, cudaStream_t s) {
+        const size_t n = (size_t)B * e->M * e->N;
+        DSRG_CUDA_TRY(cudaMemcpyAsync(e->st_unary, preds, n * sizeof(float), cudaMemcpyHostToDevice, s));
+        DSRG_CUDA_TRY(cudaMemcpyAsync(e->st_cues, top_diff, n * sizeof(float), cudaMemcpyHostToDevice, s));
+        if (int rc = softmax_backward(e, B, e->st_unary, e->st_cues, e->st_out, s)) return rc;
+        DSRG_CUDA_TRY(cudaMemcpyAsync(grad_out, e->st_out, n * sizeof(float), cudaMemcpyDeviceToHost, s));
+        return DSRG_OK;
+    });
 }
 int dsrg_constrainloss_forward_host(dsrg_engine *h, int B, const float *probs, const float *log_smooth,
                                     float *loss_out) {
-    return host_elementwise(h, B, probs, log_smooth, nullptr, nullptr, loss_out, 2);
+    return host_call(h, B, probs && log_smooth && loss_out, false, [&](Engine *e, cudaStream_t s) {
+        const size_t n = (size_t)B * e->M * e->N;
+        DSRG_CUDA_TRY(cudaMemcpyAsync(e->st_unary, probs, n * sizeof(float), cudaMemcpyHostToDevice, s));
+        DSRG_CUDA_TRY(cudaMemcpyAsync(e->st_cues, log_smooth, n * sizeof(float), cudaMemcpyHostToDevice, s));
+        if (int rc = constrain_forward(e, B, e->st_unary, e->st_cues, e->st_labels, s)) return rc;
+        DSRG_CUDA_TRY(cudaMemcpyAsync(loss_out, e->st_labels, sizeof(float), cudaMemcpyDeviceToHost, s));
+        return DSRG_OK;
+    });
 }
 int dsrg_constrainloss_backward_host(dsrg_engine *h, int B, const float *probs, const float *log_smooth,
                                      float *grad_probs, float *grad_log) {
-    return host_elementwise(h, B, probs, log_smooth, grad_probs, grad_log, nullptr, 3);
+    return host_call(h, B, probs && log_smooth && grad_probs && grad_log, false, [&](Engine *e, cudaStream_t s) {
+        const size_t n = (size_t)B * e->M * e->N;
+        DSRG_CUDA_TRY(cudaMemcpyAsync(e->st_unary, probs, n * sizeof(float), cudaMemcpyHostToDevice, s));
+        DSRG_CUDA_TRY(cudaMemcpyAsync(e->st_cues, log_smooth, n * sizeof(float), cudaMemcpyHostToDevice, s));
+        // the second gradient is staged through U: every st_* buffer of this size already holds an input or output
+        if (int rc = constrain_backward(e, B, e->st_unary, e->st_cues, e->st_out, e->U, s)) return rc;
+        DSRG_CUDA_TRY(cudaMemcpyAsync(grad_probs, e->st_out, n * sizeof(float), cudaMemcpyDeviceToHost, s));
+        DSRG_CUDA_TRY(cudaMemcpyAsync(grad_log, e->U, n * sizeof(float), cudaMemcpyDeviceToHost, s));
+        return DSRG_OK;
+    });
 }
 }

@@ -198,9 +198,8 @@ static int predict_mask(Engine *e, int mode, int n_scales, const float *const *s
         set_error("bad mode %d", mode);
         return DSRG_E_INVALID;
     }
-    if (n_scales < 1 || (mode == DSRG_POST_ZOOM_PROBS && n_scales != 1) || !scores || !hs || !ws || !result ||
-        (smooth && (!image || !p)) || n_sel < 0 || n_sel > DSRG_MAX_LABELS_WIDE || (n_sel > 0 && !labels_sel)) {
-        set_error("bad argument");
+    if (n_scales < 1 || (mode == DSRG_POST_ZOOM_PROBS && n_scales != 1) || n_sel < 0 || n_sel > DSRG_MAX_LABELS_WIDE) {
+        set_error("bad argument (NULL pointer or value out of range)");
         return DSRG_E_INVALID;
     }
     LabelSel sel;
@@ -233,113 +232,83 @@ static int predict_mask(Engine *e, int mode, int n_scales, const float *const *s
     return rc;
 }
 
-static int grow_raw(Engine *e, size_t need) {
-    if (need <= e->st_raw_cap) return DSRG_OK;
-    cudaFree(e->st_raw);  // synchronises with anything still reading it
-    e->st_raw = nullptr;
-    e->st_raw_cap = 0;
-    int rc = dalloc(e, &e->st_raw, need);
-    if (rc) return rc;
-    e->st_raw_cap = need;
-    return DSRG_OK;
-}
-
 }  // namespace dsrg
 
 using namespace dsrg;
 
+// a predict_mask call's pointers: the score maps, hs / ws and the result always; the image and the CRF parameters
+// when it smooths; the label selection when it has one
+static bool post_args_ok(const float *const *scores, const int *hs, const int *ws, const uint8_t *image, int smooth,
+                         const dsrg_crf_params *params, const int32_t *labels_sel, int n_sel, const int32_t *result) {
+    return scores && hs && ws && result && (!smooth || (image && params)) && (n_sel <= 0 || labels_sel);
+}
+
 extern "C" int dsrg_zoom_scores_dev(dsrg_engine *h, const float *scores_dev, int hi, int wi, float *out_dev,
                                     int accumulate, void *stream) {
-    Engine *e = (Engine *)h;
-    DeviceScope dev_scope(e);
-    int rc = check_batch(e, 1);
-    if (rc) return rc;
-    StreamScope stream_scope(e, (cudaStream_t)stream);
-    if (!scores_dev || !out_dev || hi < 1 || wi < 1) {
-        set_error("bad argument");
-        return DSRG_E_INVALID;
-    }
-    return zoom_scores(e, scores_dev, hi, wi, out_dev, accumulate, (cudaStream_t)stream);
+    const cudaStream_t s = (cudaStream_t)stream;
+    return dev_call(h, 1, s, scores_dev && out_dev && hi >= 1 && wi >= 1,
+                    [&](Engine *e) { return zoom_scores(e, scores_dev, hi, wi, out_dev, accumulate, s); });
 }
 
 extern "C" int dsrg_zoom_scores_host(dsrg_engine *h, const float *scores, int hi, int wi, float *out,
                                      int accumulate) {
-    Engine *e = (Engine *)h;
-    DeviceScope dev_scope(e);
-    int rc = check_batch(e, 1);
-    if (rc) return rc;
-    if (!scores || !out || hi < 1 || wi < 1) {
-        set_error("bad argument");
-        return DSRG_E_INVALID;
-    }
-    if ((rc = ensure_staging(e))) return rc;
-    const size_t nin = (size_t)e->M * hi * wi, nout = (size_t)e->N * e->M;
-    if ((rc = grow_raw(e, nin))) return rc;
-    cudaStream_t s = e->own_stream;
-    StreamScope stream_scope(e, s);
-    DSRG_CUDA_TRY(cudaMemcpyAsync(e->st_raw, scores, nin * sizeof(float), cudaMemcpyHostToDevice, s));
-    if (accumulate)
-        DSRG_CUDA_TRY(cudaMemcpyAsync(e->st_unary, out, nout * sizeof(float), cudaMemcpyHostToDevice, s));
-    if ((rc = zoom_scores(e, e->st_raw, hi, wi, e->st_unary, accumulate, s))) return rc;
-    DSRG_CUDA_TRY(cudaMemcpyAsync(out, e->st_unary, nout * sizeof(float), cudaMemcpyDeviceToHost, s));
-    DSRG_CUDA_TRY(cudaStreamSynchronize(s));
-    return DSRG_OK;
+    return host_call(h, 1, scores && out && hi >= 1 && wi >= 1, false, [&](Engine *e, cudaStream_t s) {
+        const size_t nin = (size_t)e->M * hi * wi, nout = (size_t)e->N * e->M;
+        if (int rc = grow_staging(e, (void **)&e->st_raw, &e->st_raw_cap, nin * sizeof(float))) return rc;
+        DSRG_CUDA_TRY(cudaMemcpyAsync(e->st_raw, scores, nin * sizeof(float), cudaMemcpyHostToDevice, s));
+        if (accumulate)
+            DSRG_CUDA_TRY(cudaMemcpyAsync(e->st_unary, out, nout * sizeof(float), cudaMemcpyHostToDevice, s));
+        if (int rc = zoom_scores(e, e->st_raw, hi, wi, e->st_unary, accumulate, s)) return rc;
+        DSRG_CUDA_TRY(cudaMemcpyAsync(out, e->st_unary, nout * sizeof(float), cudaMemcpyDeviceToHost, s));
+        return DSRG_OK;
+    });
 }
 
 extern "C" int dsrg_predict_mask_dev(dsrg_engine *h, int mode, int n_scales, const float *const *scores_dev,
                                      const int *hs, const int *ws, const uint8_t *image_dev, float eps,
                                      int smooth, const dsrg_crf_params *params, const int32_t *labels_sel,
                                      int n_sel, int32_t *result_out_dev, float *probs_out_dev, void *stream) {
-    Engine *e = (Engine *)h;
-    DeviceScope dev_scope(e);
-    int rc = check_batch(e, 1);
-    if (rc) return rc;
-    StreamScope stream_scope(e, (cudaStream_t)stream);
-    return predict_mask(e, mode, n_scales, scores_dev, hs, ws, image_dev, eps, smooth, params, labels_sel, n_sel,
-                        result_out_dev, probs_out_dev, (cudaStream_t)stream);
+    const cudaStream_t s = (cudaStream_t)stream;
+    const bool ok = post_args_ok(scores_dev, hs, ws, image_dev, smooth, params, labels_sel, n_sel, result_out_dev);
+    return dev_call(h, 1, s, ok, [&](Engine *e) {
+        return predict_mask(e, mode, n_scales, scores_dev, hs, ws, image_dev, eps, smooth, params, labels_sel, n_sel,
+                            result_out_dev, probs_out_dev, s);
+    });
 }
 
 extern "C" int dsrg_predict_mask_host(dsrg_engine *h, int mode, int n_scales, const float *const *scores,
                                       const int *hs, const int *ws, const uint8_t *image, float eps, int smooth,
                                       const dsrg_crf_params *params, const int32_t *labels_sel, int n_sel,
                                       int32_t *result_out, float *probs_out) {
-    Engine *e = (Engine *)h;
-    DeviceScope dev_scope(e);
-    int rc = check_batch(e, 1);
-    if (rc) return rc;
-    if (n_scales < 1 || n_scales > 16 || !scores || !hs || !ws || !result_out || (smooth && !image)) {
-        set_error("bad argument");
-        return DSRG_E_INVALID;
-    }
-    if ((rc = ensure_staging(e))) return rc;
-    size_t total = 0;
-    for (int k = 0; k < n_scales; k++) {
-        if (!scores[k] || hs[k] < 1 || ws[k] < 1) {
-            set_error("score map %d: bad pointer or size", k);
-            return DSRG_E_INVALID;
+    const bool ok = n_scales >= 1 && n_scales <= 16 &&
+                    post_args_ok(scores, hs, ws, image, smooth, params, labels_sel, n_sel, result_out);
+    return host_call(h, 1, ok, false, [&](Engine *e, cudaStream_t s) {
+        size_t total = 0;
+        for (int k = 0; k < n_scales; k++) {
+            if (!scores[k] || hs[k] < 1 || ws[k] < 1) {
+                set_error("score map %d: bad pointer or size", k);
+                return DSRG_E_INVALID;
+            }
+            total += (size_t)e->M * hs[k] * ws[k];
         }
-        total += (size_t)e->M * hs[k] * ws[k];
-    }
-    if ((rc = grow_raw(e, total))) return rc;
-    cudaStream_t s = e->own_stream;
-    StreamScope stream_scope(e, s);
-    const float *dptr[16];
-    size_t at = 0;
-    for (int k = 0; k < n_scales; k++) {
-        const size_t n = (size_t)e->M * hs[k] * ws[k];
-        DSRG_CUDA_TRY(cudaMemcpyAsync(e->st_raw + at, scores[k], n * sizeof(float), cudaMemcpyHostToDevice, s));
-        dptr[k] = e->st_raw + at;
-        at += n;
-    }
-    if (smooth)
-        DSRG_CUDA_TRY(cudaMemcpyAsync(e->st_image, image, (size_t)e->N * 3, cudaMemcpyHostToDevice, s));
-    if ((rc = predict_mask(e, mode, n_scales, dptr, hs, ws, e->st_image, eps, smooth, params, labels_sel, n_sel,
-                           e->st_lmap, probs_out ? e->st_out : nullptr, s)))
-        return rc;
-    DSRG_CUDA_TRY(cudaMemcpyAsync(result_out, e->st_lmap, (size_t)e->N * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
-    if (probs_out)
-        DSRG_CUDA_TRY(cudaMemcpyAsync(probs_out, e->st_out, (size_t)e->N * e->M * sizeof(float),
-                                      cudaMemcpyDeviceToHost, s));
-    DSRG_CUDA_TRY(cudaStreamSynchronize(s));
-    return DSRG_OK;
+        if (int rc = grow_staging(e, (void **)&e->st_raw, &e->st_raw_cap, total * sizeof(float))) return rc;
+        const float *dptr[16];
+        size_t at = 0;
+        for (int k = 0; k < n_scales; k++) {
+            const size_t n = (size_t)e->M * hs[k] * ws[k];
+            DSRG_CUDA_TRY(cudaMemcpyAsync(e->st_raw + at, scores[k], n * sizeof(float), cudaMemcpyHostToDevice, s));
+            dptr[k] = e->st_raw + at;
+            at += n;
+        }
+        if (smooth)
+            DSRG_CUDA_TRY(cudaMemcpyAsync(e->st_image, image, (size_t)e->N * 3, cudaMemcpyHostToDevice, s));
+        if (int rc = predict_mask(e, mode, n_scales, dptr, hs, ws, e->st_image, eps, smooth, params, labels_sel, n_sel,
+                                  e->st_lmap, probs_out ? e->st_out : nullptr, s))
+            return rc;
+        DSRG_CUDA_TRY(cudaMemcpyAsync(result_out, e->st_lmap, (size_t)e->N * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
+        if (probs_out)
+            DSRG_CUDA_TRY(cudaMemcpyAsync(probs_out, e->st_out, (size_t)e->N * e->M * sizeof(float),
+                                          cudaMemcpyDeviceToHost, s));
+        return DSRG_OK;
+    });
 }

@@ -43,42 +43,21 @@ using namespace dsrg;
 
 extern "C" int dsrg_prepare_image_dev(dsrg_engine *h, int B, int Hi, int Wi, const float *images_dev,
                                       const double *mean_pixel, uint8_t *image_out_dev, void *stream) {
-    Engine *e = (Engine *)h;
-    DeviceScope dev_scope(e);
-    int rc = check_batch(e, B);
-    if (rc) return rc;
-    StreamScope stream_scope(e, (cudaStream_t)stream);
-    if (!images_dev || !mean_pixel || !image_out_dev || Hi < 1 || Wi < 1) {
-        set_error("bad argument");
-        return DSRG_E_INVALID;
-    }
-    return prepare_image(e, B, Hi, Wi, images_dev, mean_pixel, image_out_dev, (cudaStream_t)stream);
+    const cudaStream_t s = (cudaStream_t)stream;
+    return dev_call(h, B, s, images_dev && mean_pixel && image_out_dev && Hi >= 1 && Wi >= 1, [&](Engine *e) {
+        return prepare_image(e, B, Hi, Wi, images_dev, mean_pixel, image_out_dev, s);
+    });
 }
 
 extern "C" int dsrg_prepare_image_host(dsrg_engine *h, int B, int Hi, int Wi, const float *images,
                                        const double *mean_pixel, uint8_t *image_out) {
-    Engine *e = (Engine *)h;
-    DeviceScope dev_scope(e);
-    int rc = check_batch(e, B);
-    if (rc) return rc;
-    if (!images || !mean_pixel || !image_out || Hi < 1 || Wi < 1) {
-        set_error("bad argument");
-        return DSRG_E_INVALID;
-    }
-    if ((rc = ensure_staging(e))) return rc;
-    const size_t need = (size_t)B * 3 * Hi * Wi;
-    if (need > e->st_raw_cap) {  // raw images come in any size: grow on demand (not on the hot CRF path)
-        cudaFree(e->st_raw);
-        e->st_raw = nullptr;
-        e->st_raw_cap = 0;
-        if ((rc = dalloc(e, &e->st_raw, need))) return rc;
-        e->st_raw_cap = need;
-    }
-    cudaStream_t s = e->own_stream;
-    StreamScope stream_scope(e, s);
-    DSRG_CUDA_TRY(cudaMemcpyAsync(e->st_raw, images, need * sizeof(float), cudaMemcpyHostToDevice, s));
-    if ((rc = prepare_image(e, B, Hi, Wi, e->st_raw, mean_pixel, e->st_image, s))) return rc;
-    DSRG_CUDA_TRY(cudaMemcpyAsync(image_out, e->st_image, (size_t)B * e->N * 3, cudaMemcpyDeviceToHost, s));
-    DSRG_CUDA_TRY(cudaStreamSynchronize(s));
-    return DSRG_OK;
+    const bool ok = images && mean_pixel && image_out && Hi >= 1 && Wi >= 1;
+    return host_call(h, B, ok, false, [&](Engine *e, cudaStream_t s) {
+        const size_t need = (size_t)B * 3 * Hi * Wi;  // raw images come in any size
+        if (int rc = grow_staging(e, (void **)&e->st_raw, &e->st_raw_cap, need * sizeof(float))) return rc;
+        DSRG_CUDA_TRY(cudaMemcpyAsync(e->st_raw, images, need * sizeof(float), cudaMemcpyHostToDevice, s));
+        if (int rc = prepare_image(e, B, Hi, Wi, e->st_raw, mean_pixel, e->st_image, s)) return rc;
+        DSRG_CUDA_TRY(cudaMemcpyAsync(image_out, e->st_image, (size_t)B * e->N * 3, cudaMemcpyDeviceToHost, s));
+        return DSRG_OK;
+    });
 }

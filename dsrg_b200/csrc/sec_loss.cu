@@ -252,10 +252,6 @@ int gwrp_weights(Engine *e, int which, double q, cudaStream_t s) {
 
 int gwrp_setup(Engine *e, const float *probs, const float *labels, double q_fg, double q_bg, GwrpArgs *a,
                size_t *smem_fwd, size_t *smem_bwd, cudaStream_t s) {
-    if (!probs || !labels) {
-        set_error("NULL pointer argument");
-        return DSRG_E_INVALID;
-    }
     if (e->N > DSRG_GWRP_MAX_PLANE) {
         set_error("ExpandLoss: a %dx%d plane has %d pixels; the GWRP kernels sort at most %d", e->H, e->W, e->N,
                   DSRG_GWRP_MAX_PLANE);
@@ -340,97 +336,74 @@ int plainseed_backward(Engine *e, int B, int n_global, const float *probs, const
 
 using namespace dsrg;
 
-// host wrapper: probs and the per-image label rows in, the terms (forward) or the gradient (backward) out
-static int sec_host(dsrg_engine *h, int B, int n_global, const float *probs, const float *second, size_t second_n,
-                    float *terms_out, int n_terms, float *grad_out, int op, double q_fg, double q_bg) {
-    Engine *e = (Engine *)h;
-    DeviceScope dev_scope(e);
-    int rc = check_batch(e, B);
-    if (rc) return rc;
-    if (!probs || !second || (!terms_out && !grad_out) || n_global < 1) {
-        set_error("bad argument");
-        return DSRG_E_INVALID;
-    }
-    if ((rc = ensure_staging(e))) return rc;
-    cudaStream_t s = e->own_stream;
-    StreamScope stream_scope(e, s);
-    const size_t n = (size_t)B * e->M * e->N;
-    DSRG_CUDA_TRY(cudaMemcpyAsync(e->st_unary, probs, n * sizeof(float), cudaMemcpyHostToDevice, s));
-    DSRG_CUDA_TRY(cudaMemcpyAsync(e->st_cues, second, second_n * sizeof(float), cudaMemcpyHostToDevice, s));
-    switch (op) {
-        case 0: rc = expandloss_forward(e, B, e->st_unary, e->st_cues, q_fg, q_bg, e->st_labels, s); break;
-        case 1: rc = expandloss_backward(e, B, n_global, e->st_unary, e->st_cues, q_fg, q_bg, e->st_out, s); break;
-        case 2: rc = plainseed_forward(e, B, e->st_unary, e->st_cues, e->st_labels, s); break;
-        case 3: rc = plainseed_backward(e, B, n_global, e->st_unary, e->st_cues, e->st_out, s); break;
-    }
-    if (rc) return rc;
-    if (terms_out)
-        DSRG_CUDA_TRY(cudaMemcpyAsync(terms_out, e->st_labels, n_terms * sizeof(float), cudaMemcpyDeviceToHost, s));
-    if (grad_out) DSRG_CUDA_TRY(cudaMemcpyAsync(grad_out, e->st_out, n * sizeof(float), cudaMemcpyDeviceToHost, s));
-    DSRG_CUDA_TRY(cudaStreamSynchronize(s));
-    return DSRG_OK;
-}
-
-static int sec_dev_check(Engine *e, int B, int n_global, const void *probs, const void *second, const void *out) {
-    int rc = check_batch(e, B);
-    if (rc) return rc;
-    if (!probs || !second || !out || n_global < 1) {
-        set_error("bad argument");
-        return DSRG_E_INVALID;
-    }
-    return DSRG_OK;
-}
-
+// the *_host twins stage probs in st_unary and the labels or seeds in st_cues; the terms come back through
+// st_labels, the gradient through st_out
 extern "C" {
 int dsrg_expandloss_forward_dev(dsrg_engine *h, int B, const float *probs, const float *labels, double q_fg,
                                 double q_bg, float *terms_out, void *stream) {
-    Engine *e = (Engine *)h;
-    DeviceScope dev_scope(e);
-    if (int rc = sec_dev_check(e, B, 1, probs, labels, terms_out)) return rc;
-    StreamScope stream_scope(e, (cudaStream_t)stream);
-    return expandloss_forward(e, B, probs, labels, q_fg, q_bg, terms_out, (cudaStream_t)stream);
+    const cudaStream_t s = (cudaStream_t)stream;
+    return dev_call(h, B, s, probs && labels && terms_out,
+                    [&](Engine *e) { return expandloss_forward(e, B, probs, labels, q_fg, q_bg, terms_out, s); });
 }
 int dsrg_expandloss_backward_dev(dsrg_engine *h, int B, int n_global, const float *probs, const float *labels,
                                  double q_fg, double q_bg, float *grad_out, void *stream) {
-    Engine *e = (Engine *)h;
-    DeviceScope dev_scope(e);
-    if (int rc = sec_dev_check(e, B, n_global, probs, labels, grad_out)) return rc;
-    StreamScope stream_scope(e, (cudaStream_t)stream);
-    return expandloss_backward(e, B, n_global, probs, labels, q_fg, q_bg, grad_out, (cudaStream_t)stream);
+    const cudaStream_t s = (cudaStream_t)stream;
+    return dev_call(h, B, s, probs && labels && grad_out && n_global >= 1, [&](Engine *e) {
+        return expandloss_backward(e, B, n_global, probs, labels, q_fg, q_bg, grad_out, s);
+    });
 }
 int dsrg_expandloss_forward_host(dsrg_engine *h, int B, const float *probs, const float *labels, double q_fg,
                                  double q_bg, float *terms_out) {
-    Engine *e = (Engine *)h;
-    return sec_host(h, B, 1, probs, labels, (size_t)B * (e ? e->M : 0), terms_out, 3, nullptr, 0, q_fg, q_bg);
+    return host_call(h, B, probs && labels && terms_out, false, [&](Engine *e, cudaStream_t s) {
+        DSRG_CUDA_TRY(cudaMemcpyAsync(e->st_unary, probs, (size_t)B * e->M * e->N * sizeof(float), cudaMemcpyHostToDevice, s));
+        DSRG_CUDA_TRY(cudaMemcpyAsync(e->st_cues, labels, (size_t)B * e->M * sizeof(float), cudaMemcpyHostToDevice, s));
+        if (int rc = expandloss_forward(e, B, e->st_unary, e->st_cues, q_fg, q_bg, e->st_labels, s)) return rc;
+        DSRG_CUDA_TRY(cudaMemcpyAsync(terms_out, e->st_labels, 3 * sizeof(float), cudaMemcpyDeviceToHost, s));
+        return DSRG_OK;
+    });
 }
 int dsrg_expandloss_backward_host(dsrg_engine *h, int B, int n_global, const float *probs, const float *labels,
                                   double q_fg, double q_bg, float *grad_out) {
-    Engine *e = (Engine *)h;
-    return sec_host(h, B, n_global, probs, labels, (size_t)B * (e ? e->M : 0), nullptr, 0, grad_out, 1, q_fg, q_bg);
+    return host_call(h, B, probs && labels && grad_out && n_global >= 1, false, [&](Engine *e, cudaStream_t s) {
+        const size_t n = (size_t)B * e->M * e->N;
+        DSRG_CUDA_TRY(cudaMemcpyAsync(e->st_unary, probs, n * sizeof(float), cudaMemcpyHostToDevice, s));
+        DSRG_CUDA_TRY(cudaMemcpyAsync(e->st_cues, labels, (size_t)B * e->M * sizeof(float), cudaMemcpyHostToDevice, s));
+        if (int rc = expandloss_backward(e, B, n_global, e->st_unary, e->st_cues, q_fg, q_bg, e->st_out, s)) return rc;
+        DSRG_CUDA_TRY(cudaMemcpyAsync(grad_out, e->st_out, n * sizeof(float), cudaMemcpyDeviceToHost, s));
+        return DSRG_OK;
+    });
 }
 int dsrg_seedloss_plain_forward_dev(dsrg_engine *h, int B, const float *probs, const float *seeds, float *terms_out,
                                     void *stream) {
-    Engine *e = (Engine *)h;
-    DeviceScope dev_scope(e);
-    if (int rc = sec_dev_check(e, B, 1, probs, seeds, terms_out)) return rc;
-    StreamScope stream_scope(e, (cudaStream_t)stream);
-    return plainseed_forward(e, B, probs, seeds, terms_out, (cudaStream_t)stream);
+    const cudaStream_t s = (cudaStream_t)stream;
+    return dev_call(h, B, s, probs && seeds && terms_out,
+                    [&](Engine *e) { return plainseed_forward(e, B, probs, seeds, terms_out, s); });
 }
 int dsrg_seedloss_plain_backward_dev(dsrg_engine *h, int B, int n_global, const float *probs, const float *seeds,
                                      float *grad_out, void *stream) {
-    Engine *e = (Engine *)h;
-    DeviceScope dev_scope(e);
-    if (int rc = sec_dev_check(e, B, n_global, probs, seeds, grad_out)) return rc;
-    StreamScope stream_scope(e, (cudaStream_t)stream);
-    return plainseed_backward(e, B, n_global, probs, seeds, grad_out, (cudaStream_t)stream);
+    const cudaStream_t s = (cudaStream_t)stream;
+    return dev_call(h, B, s, probs && seeds && grad_out && n_global >= 1,
+                    [&](Engine *e) { return plainseed_backward(e, B, n_global, probs, seeds, grad_out, s); });
 }
 int dsrg_seedloss_plain_forward_host(dsrg_engine *h, int B, const float *probs, const float *seeds, float *terms_out) {
-    Engine *e = (Engine *)h;
-    return sec_host(h, B, 1, probs, seeds, (size_t)B * (e ? e->M * e->N : 0), terms_out, 1, nullptr, 2, 0, 0);
+    return host_call(h, B, probs && seeds && terms_out, false, [&](Engine *e, cudaStream_t s) {
+        const size_t n = (size_t)B * e->M * e->N;
+        DSRG_CUDA_TRY(cudaMemcpyAsync(e->st_unary, probs, n * sizeof(float), cudaMemcpyHostToDevice, s));
+        DSRG_CUDA_TRY(cudaMemcpyAsync(e->st_cues, seeds, n * sizeof(float), cudaMemcpyHostToDevice, s));
+        if (int rc = plainseed_forward(e, B, e->st_unary, e->st_cues, e->st_labels, s)) return rc;
+        DSRG_CUDA_TRY(cudaMemcpyAsync(terms_out, e->st_labels, sizeof(float), cudaMemcpyDeviceToHost, s));
+        return DSRG_OK;
+    });
 }
 int dsrg_seedloss_plain_backward_host(dsrg_engine *h, int B, int n_global, const float *probs, const float *seeds,
                                       float *grad_out) {
-    Engine *e = (Engine *)h;
-    return sec_host(h, B, n_global, probs, seeds, (size_t)B * (e ? e->M * e->N : 0), nullptr, 0, grad_out, 3, 0, 0);
+    return host_call(h, B, probs && seeds && grad_out && n_global >= 1, false, [&](Engine *e, cudaStream_t s) {
+        const size_t n = (size_t)B * e->M * e->N;
+        DSRG_CUDA_TRY(cudaMemcpyAsync(e->st_unary, probs, n * sizeof(float), cudaMemcpyHostToDevice, s));
+        DSRG_CUDA_TRY(cudaMemcpyAsync(e->st_cues, seeds, n * sizeof(float), cudaMemcpyHostToDevice, s));
+        if (int rc = plainseed_backward(e, B, n_global, e->st_unary, e->st_cues, e->st_out, s)) return rc;
+        DSRG_CUDA_TRY(cudaMemcpyAsync(grad_out, e->st_out, n * sizeof(float), cudaMemcpyDeviceToHost, s));
+        return DSRG_OK;
+    });
 }
 }

@@ -220,40 +220,34 @@ extern "C" void dsrg_wire_apply_clamp_mask(const uint32_t *src, float *probs, si
 }
 
 // srg_only: no CRF (probs are read-only, `renorm` as in dsrg_srg_batch_dev, optional label map out)
-static int host_pass_impl(dsrg_engine *h, int B, const float *labels, float *probs, const float *cues,
+static int host_pass_impl(Engine *e, int B, const float *labels, float *probs, const float *cues,
                           const uint8_t *image, const dsrg_crf_params *params, double th1, double th2,
                           float *seeds_out, float *crf_out, bool srg_only, int renorm, int32_t *label_map_out);
 
 static int host_pass(dsrg_engine *h, int B, const float *labels, float *probs, const float *cues,
                      const uint8_t *image, const dsrg_crf_params *params, double th1, double th2,
                      float *seeds_out, float *crf_out, bool srg_only, int renorm, int32_t *label_map_out) {
-    Engine *e = (Engine *)h;
-    DeviceScope dev_scope(e);
-    const int rc = host_pass_impl(h, B, labels, probs, cues, image, params, th1, th2, seeds_out, crf_out, srg_only,
-                                  renorm, label_map_out);
-    if (rc != DSRG_OK && e && e->in_stream) {
-        // a chunk failed mid-pipeline: copies of earlier chunks may still be reading or writing the caller's
-        // buffers -- wait for them before the error is reported (the outputs are then undefined, not in flight)
-        cudaStreamSynchronize(e->in_stream);
-        cudaStreamSynchronize(e->own_stream);
-        cudaStreamSynchronize(e->out_stream);
-        cudaGetLastError();
-    }
-    return rc;
+    const bool ok = labels && probs && cues && seeds_out && (srg_only || (image && params));
+    return host_call(h, B, ok, true, [&](Engine *e, cudaStream_t) {
+        const int rc = host_pass_impl(e, B, labels, probs, cues, image, params, th1, th2, seeds_out, crf_out, srg_only,
+                                      renorm, label_map_out);
+        if (rc != DSRG_OK) {
+            // a chunk failed mid-pipeline: copies of earlier chunks may still be reading or writing the caller's
+            // buffers -- wait for them before the error is reported (the outputs are then undefined, not in flight)
+            cudaStreamSynchronize(e->in_stream);
+            cudaStreamSynchronize(e->own_stream);
+            cudaStreamSynchronize(e->out_stream);
+            cudaGetLastError();
+        }
+        return rc;
+    });
 }
 
-static int host_pass_impl(dsrg_engine *h, int B, const float *labels, float *probs, const float *cues,
+static int host_pass_impl(Engine *e, int B, const float *labels, float *probs, const float *cues,
                           const uint8_t *image, const dsrg_crf_params *params, double th1, double th2,
                           float *seeds_out, float *crf_out, bool srg_only, int renorm, int32_t *label_map_out) {
-    Engine *e = (Engine *)h;
-    int rc = check_batch(e, B);
+    int rc = ensure_wire(e);
     if (rc) return rc;
-    if (!labels || !probs || !cues || (!image && !srg_only) || !seeds_out) {
-        set_error("NULL pointer argument");
-        return DSRG_E_INVALID;
-    }
-    if ((rc = ensure_staging(e))) return rc;
-    if ((rc = ensure_wire(e))) return rc;
     // chunk schedule: a small first chunk gets the GPU going early, then full-size chunks
     const int chunk = e->host_chunk > 0 ? e->host_chunk : B;
     std::vector<int> cb0, cnb;
@@ -305,7 +299,6 @@ static int host_pass_impl(dsrg_engine *h, int B, const float *labels, float *pro
         e->pipe_events.push_back(ev);
     }
     cudaStream_t s_in = e->in_stream, s = e->own_stream, s_out = e->out_stream;
-    StreamScope stream_scope(e, s);
     const size_t img_elems = (size_t)e->M * e->N;
     const int n_img = (int)img_elems;
     const size_t wpi = (img_elems + 31) / 32;
@@ -434,7 +427,7 @@ static int host_pass_impl(dsrg_engine *h, int B, const float *labels, float *pro
         fprintf(stderr, "[dsrg host pass] total %.2f ms: pack %.2f issue %.2f unpack %.2f wait %.2f (threads %d, chunks %d)\n",
                 1e3 * (omp_get_wtime() - t0), 1e3 * t_pack, 1e3 * t_issue, 1e3 * t_unpack, 1e3 * t_wait, host_threads(),
                 nchunks);
-    return check_device_flag(e, s);
+    return DSRG_OK;
 }
 
 extern "C" int dsrg_dsrg_forward_host(dsrg_engine *h, int B, const float *labels, float *probs,

@@ -390,7 +390,7 @@ int dsrg_engine_profile(dsrg_engine *e, int enable);
 int dsrg_engine_profile_read(dsrg_engine *e, float *ms_out, long long *count_out);
 
 /* Introspection used by the lattice-level parity tests: vertex counts of the lattices built by
- * the last CRF call (spatial, then bilateral per image). */
+ * the last CRF call (spatial, then bilateral per image); either pointer may be NULL. */
 int dsrg_engine_lattice_sizes(dsrg_engine *e, int B, int *v_spatial_out, int *v_bilateral_out);
 /* Per-pixel symmetric normalisation vectors (DenseKernel::norm_, pairwise.cpp:54-57) of the
  * last CRF call: which = 0 spatial [N] (shared by the batch), 1 bilateral [B][N]. */
