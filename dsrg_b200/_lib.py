@@ -69,6 +69,8 @@ SIGNATURES = {
     "dsrg_constrainloss_backward_host": (_i, [_vp, _i, _vp, _vp, _vp, _vp]),
     "dsrg_prepare_image_dev": (_i, [_vp, _i, _i, _i, _vp, _vp, _vp, _vp]),
     "dsrg_prepare_image_host": (_i, [_vp, _i, _i, _i, _vp, _vp, _vp]),
+    "dsrg_prepare_net_input_dev": (_i, [_vp, _vp, _i, _i, _i, _vp, _vp, _vp, _vp, _vp]),
+    "dsrg_prepare_net_input_host": (_i, [_vp, _vp, _i, _i, _i, _vp, _vp, _vp, _vp]),
     "dsrg_zoom_scores_dev": (_i, [_vp, _vp, _i, _i, _vp, _i, _vp]),
     "dsrg_zoom_scores_host": (_i, [_vp, _vp, _i, _i, _vp, _i]),
     "dsrg_predict_mask_dev": (_i, [_vp, _i, _i, _vp, _vp, _vp, _vp, _f, _i, _pp, _vp, _i, _vp, _vp, _vp]),

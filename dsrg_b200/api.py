@@ -304,6 +304,43 @@ class Engine(object):
                                              _stream(stream)))
         return out
 
+    # ---- network input of the evaluation tools (training/tools/test-ms.py:68-81 and its siblings) ----
+    @staticmethod
+    def _net_input_args(sizes, mean_pixel):
+        n = len(sizes)
+        hs = (C.c_int * n)(*[int(h) for h, _ in sizes])
+        ws = (C.c_int * n)(*[int(w) for _, w in sizes])
+        mean = np.ascontiguousarray(mean_pixel, np.float64)
+        if mean.shape != (3,):
+            raise ValueError("mean_pixel must have 3 elements")
+        return n, hs, ws, mean
+
+    def prepare_net_input_host(self, image, sizes, mean_pixel=(104.0, 117.0, 123.0)):
+        """(H,W,3) uint8 image -> one (1,3,h,w) float32 network input per (h, w) of `sizes`: preprocess(image, size)
+        of the evaluation tools, bit-exact.  Does not change the engine's size."""
+        H, W = image.shape[:2]
+        n, hs, ws, mean = self._net_input_args(sizes, mean_pixel)
+        outs = [np.empty((1, 3, h, w), np.float32) for h, w in zip(hs, ws)]
+        ptrs = (C.c_void_p * n)(*[o.ctypes.data for o in outs])
+        check(self._L.dsrg_prepare_net_input_host(self.h, _hptr(image, np.uint8), int(H), int(W), n, hs, ws,
+                                                  _hptr(mean, np.float64), ptrs))
+        return outs
+
+    def prepare_net_input_dev(self, image, outs, mean_pixel=(104.0, 117.0, 123.0), stream=None):
+        """image: (H,W,3) uint8 CUDA tensor; outs: float32 CUDA tensors of shape (3,h,w) or (1,3,h,w), one per
+        scale (their shapes give the sizes)."""
+        import torch
+        if image.dtype != torch.uint8 or image.dim() != 3 or image.shape[2] != 3:
+            raise ValueError("image must be an (H, W, 3) uint8 tensor")
+        for o in outs:
+            if o.dtype != torch.float32 or o.dim() < 3 or o.numel() != 3 * o.shape[-2] * o.shape[-1]:
+                raise ValueError("every output must be a float32 (3, h, w) or (1, 3, h, w) tensor")
+        n, hs, ws, mean = self._net_input_args([(o.shape[-2], o.shape[-1]) for o in outs], mean_pixel)
+        ptrs = (C.c_void_p * n)(*[_dptr(o).value for o in outs])
+        check(self._L.dsrg_prepare_net_input_dev(self.h, _dptr(image), int(image.shape[0]), int(image.shape[1]), n,
+                                                 hs, ws, _hptr(mean, np.float64), ptrs, _stream(stream)))
+        return outs
+
     def crflayer_forward_host(self, probs, image, params, log_out=None, result=None):
         B = probs.shape[0]
         if log_out is None:

@@ -290,7 +290,7 @@ using namespace dsrg;
 
 extern "C" {
 
-int dsrg_version(void) { return 102; }
+int dsrg_version(void) { return 103; }
 
 const char *dsrg_last_error(void) { return g_err; }
 
@@ -462,7 +462,8 @@ void dsrg_engine_destroy(dsrg_engine *h) {
     lattice_free(e->bi);
     void *ptrs[] = {e->U, e->Q0, e->spA, e->spB, e->spC, e->biA, e->biB, e->biC, e->nvA, e->nvB, e->lmap,
                     e->lflag, e->parent, e->hc, e->loss_acc, e->sec_rec, e->sec_img, e->sec_part, e->sec_w, e->dev_err,
-                    e->hy_list, e->hy_count, e->st_unary, e->st_out, e->st_cues, e->st_labels, e->st_image, e->st_lmap, e->st_raw, e->st_idx};
+                    e->hy_list, e->hy_count, e->st_unary, e->st_out, e->st_cues, e->st_labels, e->st_image, e->st_lmap, e->st_raw, e->st_idx,
+                    e->st_prep};
     for (void *p : ptrs) cudaFree(p);
     if (e->own_stream) cudaStreamDestroy(e->own_stream);
     if (e->in_stream) cudaStreamDestroy(e->in_stream);

@@ -208,6 +208,8 @@ struct Engine {
     size_t st_raw_cap = 0;
     int32_t *st_idx = nullptr;  // index lists of the annotation entry points
     size_t st_idx_cap = 0;
+    uint8_t *st_prep = nullptr;  // image and network inputs of dsrg_prepare_net_input_host
+    size_t st_prep_cap = 0;
     int32_t *st_lmap = nullptr;
     cudaStream_t own_stream = nullptr, in_stream = nullptr, out_stream = nullptr;
     // order of the passes of this engine across streams (StreamScope)

@@ -9,6 +9,7 @@
 //     float64 without contraction, then cast to float32 (the array dtype)
 #pragma once
 #include <cuda_runtime.h>
+#include <stdint.h>
 
 namespace dsrg {
 
@@ -35,14 +36,26 @@ __device__ __forceinline__ ZoomTap zoom_tap(int oy, int ox, int Hi, int Wi, int 
     return z;
 }
 
+// the four taps of z, `at(y, x)` giving the input value at (y, x) as float64
+template <typename At>
+__device__ __forceinline__ float zoom_taps(const ZoomTap &z, At at) {
+    if (z.oob) return 0.0f;
+    double t = __dmul_rn(__dmul_rn(at(z.y0, z.x0), z.wy0), z.wx0);
+    t = __dadd_rn(t, __dmul_rn(__dmul_rn(at(z.y0, z.x1), z.wy0), z.wx1));
+    t = __dadd_rn(t, __dmul_rn(__dmul_rn(at(z.y1, z.x0), z.wy1), z.wx0));
+    t = __dadd_rn(t, __dmul_rn(__dmul_rn(at(z.y1, z.x1), z.wy1), z.wx1));
+    return (float)t;
+}
+
 // p: one [Hi][Wi] float32 plane
 __device__ __forceinline__ float zoom_apply(const float *__restrict__ p, int Wi, const ZoomTap &z) {
-    if (z.oob) return 0.0f;
-    double t = __dmul_rn(__dmul_rn((double)p[(size_t)z.y0 * Wi + z.x0], z.wy0), z.wx0);
-    t = __dadd_rn(t, __dmul_rn(__dmul_rn((double)p[(size_t)z.y0 * Wi + z.x1], z.wy0), z.wx1));
-    t = __dadd_rn(t, __dmul_rn(__dmul_rn((double)p[(size_t)z.y1 * Wi + z.x0], z.wy1), z.wx0));
-    t = __dadd_rn(t, __dmul_rn(__dmul_rn((double)p[(size_t)z.y1 * Wi + z.x1], z.wy1), z.wx1));
-    return (float)t;
+    return zoom_taps(z, [&](int y, int x) { return (double)p[(size_t)y * Wi + x]; });
+}
+
+// p: an interleaved [Hi][Wi][3] uint8 image, channel c.  Its values are what image.astype('float32') hands to
+// scipy: the float32 cast of a uint8 is exact, and so is the float64 one.
+__device__ __forceinline__ float zoom_apply(const uint8_t *__restrict__ p, int Wi, int c, const ZoomTap &z) {
+    return zoom_taps(z, [&](int y, int x) { return (double)p[((size_t)y * Wi + x) * 3 + c]; });
 }
 
 }  // namespace dsrg

@@ -1,5 +1,6 @@
-"""Inference post-processing of the reference's evaluation tools on the GPU: everything predict_mask()
-does after net.forward() (training/tools/test-ms.py:84-111, training/tools/generate_train_gt.py:76-104).
+"""Inference pre- and post-processing of the reference's evaluation tools on the GPU: the network input of every
+scale (preprocess(), training/tools/test-ms.py:68-81) and everything predict_mask() does after net.forward()
+(training/tools/test-ms.py:84-111, training/tools/generate_train_gt.py:76-104).
 The network forward pass stays with the caller; pass the fc8 score blobs as they come out of
 ``net.blobs['fc8-SEC'].data[0]`` ((M, h, w) float32).  No CPU fallback: needs the CUDA library."""
 import numpy as np
@@ -8,6 +9,35 @@ from . import api as _api
 from .pool import engine_for as _engine_for
 
 EPS = 0.00001  # test-ms.py:103, generate_train_gt.py:90
+MEAN_PIXEL = (104.0, 117.0, 123.0)  # test-ms.py:48 and the other tools
+
+
+def net_input_size(H, W, size, relative=False):
+    """The (h, w) of preprocess(image, size) for an H x W image: scipy's int(round(in * factor)) with Python's
+    round, factor = size / float(in) (test-ms.py:73-74) or, with `relative`, the zoom factor itself
+    (test-ms-f.py:105).  So 334 * 1.25 = 417.5 gives 418 and 334 * 0.75 = 250.5 gives 250."""
+    fy, fx = (size, size) if relative else (size / float(H), size / float(W))
+    return int(round(H * fy)), int(round(W * fx))
+
+
+def preprocess(im, sizes, relative=False, M=21, mean_pixel=MEAN_PIXEL):
+    """preprocess(image, size) of the evaluation tools (test-ms.py:68-81, test.py, test-coco.py, generate_train_gt.py,
+    show-result.py; test-ms-f.py / test-coco-f.py with `relative` zoom factors) for every size of `sizes`, on the
+    device in one launch: zoom(order=1), RGB -> BGR, - mean_pixel, HWC -> CHW, bit-exact with scipy.  `im` is the
+    uint8 (H, W, 3) image as pylab.imread / cv2.imread return it.  Returns one (1, 3, h, w) float32 blob per size.
+    Runs on the pooled engine that predict_mask_* with the same M will use for this image, so the post-processing
+    that follows neither re-shapes the engine again nor drops its cached graphs."""
+    if not isinstance(im, np.ndarray) or im.dtype != np.uint8 or im.ndim != 3 or im.shape[2] != 3:
+        raise ValueError("image must be a uint8 (H, W, 3) array")
+    mean = np.asarray(mean_pixel, np.float64)
+    if mean.shape != (3,):
+        raise ValueError("mean_pixel must have 3 elements")
+    H, W = im.shape[:2]
+    shapes = [net_input_size(H, W, s, relative) for s in sizes]
+    if not shapes or min(min(s) for s in shapes) < 1:
+        raise ValueError("every scale must give at least one row and column (got %s)" % shapes)
+    eng = _engine_for(H, W, M)
+    return eng.prepare_net_input_host(np.ascontiguousarray(im), shapes, mean)
 
 
 def _blob(a):

@@ -209,6 +209,29 @@ int dsrg_prepare_image_host(dsrg_engine *e, int B, int Hi, int Wi, const float *
                             const double *mean_pixel /* host, 3 */, uint8_t *image_out_host);
 
 /*
+ * The network input of the evaluation tools: preprocess(image, size) of training/tools/test-ms.py:68-81,
+ * test.py:60-73, test-coco.py:92-105, generate_train_gt.py:62-75, show-result.py:64-77 (absolute sizes) and
+ * test-ms-f.py:100-112, test-coco-f.py:124-136 (zoom factors), for every scale of one image in one launch:
+ *   image = nd.zoom(image.astype('float32'), (h/H, w/W, 1.0), order=1)   scipy.ndimage.zoom order=1 semantics,
+ *                                                                         float64 arithmetic, float32 result
+ *   image = image[:, :, [2, 1, 0]]; image = image - mean_pixel            float64, like numpy with the tools'
+ *   image = image.transpose([2, 0, 1])                                    np.array([104.0, 117.0, 123.0])
+ * stored into the float32 `images` blob; bit-exact.
+ *   image   : [H][W][3] uint8, interleaved, as pylab.imread / cv2.imread return it
+ *   hs, ws  : n_scales output sizes, host memory in both variants (1 <= n_scales <= DSRG_PREP_MAX_SCALES); the
+ *             tools' sizes are int(round(H * f)), int(round(W * f)) -- scipy's output shape
+ *   out     : host array of n_scales pointers to [3][hs[k]][ws[k]] float32
+ * H and W are the image's: the call neither reads nor changes the engine's size (dsrg_engine_set_size).
+ */
+#define DSRG_PREP_MAX_SCALES 16
+int dsrg_prepare_net_input_dev(dsrg_engine *e, const uint8_t *image_dev, int H, int W, int n_scales,
+                               const int *hs, const int *ws, const double *mean_pixel /* host, 3 */,
+                               float *const *out_dev, void *stream);
+int dsrg_prepare_net_input_host(dsrg_engine *e, const uint8_t *image_host, int H, int W, int n_scales,
+                                const int *hs, const int *ws, const double *mean_pixel /* host, 3 */,
+                                float *const *out_host);
+
+/*
  * Full-resolution inference post-processing: what predict_mask() of the evaluation / ground-truth tools
  * does between the network's score blob and the label map (engine batch 1, size = the image's):
  *   DSRG_POST_SUM_SCORES  training/tools/test-ms.py:84-111: scores_all = sum_k zoom(scores_k, order=1);

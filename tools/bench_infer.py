@@ -6,7 +6,10 @@ through postprocess.predict_mask_ms (host numpy in, host label map out).  Not th
 With --labels 81 it times the COCO tool's post-processing instead (training/tools/test-coco.py:108-133: one
 481-pixel scale, 81 labels, the mean field on the label-chunked path) on COCO-sized images.
 
-usage: python tools/bench_infer.py [--images 40] [--cpu 2] [--labels 21|81]
+With --preprocess it also times the step before the network, preprocess(image, size) of every scale of an image
+(postprocess.preprocess, one launch), next to the same statements with scipy on one core.
+
+usage: python tools/bench_infer.py [--images 40] [--cpu 2] [--labels 21|81] [--preprocess [--cpu-preprocess 8]]
 """
 import argparse
 import json
@@ -28,6 +31,9 @@ def main():
     ap.add_argument("--cpu", type=int, default=None, help="images timed through the CPU oracle (0 = skip; "
                                                           "default 2 at 21 labels, 0 at 81)")
     ap.add_argument("--labels", type=int, default=21, choices=(21, 81))
+    ap.add_argument("--preprocess", action="store_true", help="also time the network input of every scale "
+                                                              "(postprocess.preprocess) and its scipy statements")
+    ap.add_argument("--cpu-preprocess", type=int, default=8, help="images whose preprocess is timed with scipy")
     args = ap.parse_args()
     if args.cpu is None:
         args.cpu = 2 if args.labels == 21 else 0
@@ -70,7 +76,52 @@ def main():
         cdt = (time.perf_counter() - t0) / args.cpu
         out["cpu_oracle"] = {"ms_per_image": 1e3 * cdt, "images": args.cpu, "cores": 1,
                              "kind": "port (scipy zoom + numpy + oracle/crf_oracle.c)"}
+    if args.preprocess:
+        out["preprocess"] = time_preprocess(args, cases, eng, coco)
     print(json.dumps(out), flush=True)
+
+
+def time_preprocess(args, cases, eng, coco):
+    """preprocess(image, size) of every scale of an image (test-ms.py:68-81 at 241/321/401, test-coco.py:92-105 at
+    481) through postprocess.preprocess: host uint8 image in, host float32 blobs out; the kernel time from the
+    profile; and the same statements with scipy (oracle/prep_oracle.py) on one core of this host."""
+    import torch
+    from dsrg_b200 import postprocess
+    from oracle import prep_oracle
+    sizes = (481,) if coco else (241, 321, 401)
+    for c in cases:                                   # warm-up: staging growth
+        postprocess.preprocess(c["image"], sizes, M=args.labels)
+    torch.cuda.synchronize()
+    t0 = time.perf_counter()
+    for i in range(args.images):
+        c = cases[i % len(cases)]
+        postprocess.preprocess(c["image"], sizes, M=args.labels)
+    dt = (time.perf_counter() - t0) / args.images
+    eng.take_launch_count()
+    eng.profile(True)
+    for c in cases:
+        postprocess.preprocess(c["image"], sizes, M=args.labels)
+    prof = eng.profile_read()
+    eng.profile(False)
+    launches = eng.take_launch_count()
+    kms = prof["prepare_image"][0] / len(cases)
+    nbytes = 0
+    for c in cases:
+        H, W = c["image"].shape[:2]
+        nbytes += 3 * H * W + sum(12 * h * w for h, w in (postprocess.net_input_size(H, W, s) for s in sizes))
+    nbytes /= len(cases)
+    res = {"sizes": list(sizes), "ms_per_image": 1e3 * dt, "images": args.images, "kernel_ms_per_image": kms,
+           "launches_per_image": launches / len(cases), "algorithmic_MB_per_image": nbytes / 1e6,
+           "kernel_GB_per_s": nbytes / (kms * 1e6)}
+    n = max(1, args.cpu_preprocess)
+    t0 = time.perf_counter()
+    for i in range(n):
+        c = cases[i % len(cases)]
+        for s in sizes:
+            prep_oracle.preprocess(c["image"], s)
+    res["cpu_scipy"] = {"ms_per_image": 1e3 * (time.perf_counter() - t0) / n, "images": n, "cores": 1,
+                        "kind": "the reference's statements (scipy.ndimage.zoom + numpy)"}
+    return res
 
 
 if __name__ == "__main__":
