@@ -341,9 +341,17 @@ template <int NT, typename F>
 __device__ __forceinline__ double numpy_sum(F get, int n_rt) {
     const int n = NT ? NT : n_rt;
     if (n <= 128) return numpy_sum_block<NT>(get, 0, n);
-    int n2 = n / 2;  // n <= 255 here (DSRG_MAX_LABELS, SRG's 255): one level of the recursion
+    // n <= 255 here (DSRG_MAX_LABELS_WIDE, SRG's 255).  NumPy splits at n/2 rounded down to a multiple of 8 and
+    // recurses into both halves: the first (<= 127) is one block, the second (<= 135) is split once more when it
+    // exceeds 128, which happens from n = 249 on
+    int n2 = n / 2;
     n2 -= n2 % 8;
-    return numpy_sum_block<0>(get, 0, n2) + numpy_sum_block<0>(get, n2, n - n2);
+    const double lo = numpy_sum_block<0>(get, 0, n2);
+    const int m = n - n2;
+    if (m <= 128) return lo + numpy_sum_block<0>(get, n2, m);
+    int m2 = m / 2;
+    m2 -= m2 % 8;
+    return lo + (numpy_sum_block<0>(get, n2, m2) + numpy_sum_block<0>(get, n2 + m2, m - m2));
 }
 
 // Entry points run on the engine's device and hand the calling thread back on the device it came with: a Caffe

@@ -39,3 +39,143 @@ def crf_case_inputs(name):
             im, unary = make_golden.crf_inputs(H, W, var, kind, i)
             return im, unary, sf
     raise KeyError(name)
+
+
+# ---- label counts: the cases of test_gpu_label_counts.py (checked on the CPU by test_label_counts_cpu.py) ----
+MAX_FUSED = 32                       # DSRG_MAX_LABELS: above it the label-chunked path (meanfield_wide.cu)
+FUSED_SHAPES = {"smooth": (37, 45), "noise": (41, 41)}
+FUSED_CONFIGS = [("smooth", 1.0), ("noise", 1.0), ("smooth", 12.0)]   # (image, scale factor), B = 2
+FUSED_ITER_M = [1, 6, 12, 15, 17, 24, 27, 32]                          # one M per MP for n_iters 1 and 2
+HYBRID_M = [1, 6, 9, 16, 18, 24, 25, 32]                               # one M per MP on textured 321x321 images
+HYBRID_SHAPE, HYBRID_B, HYBRID_START = (321, 321), 5, 70
+WIDE_M = [33, 34, 35, 36, 64, 127, 128, 129, 200, 253, 255]
+WIDE_SHAPES = {"smooth": (29, 37), "noise": (19, 23)}
+RENORM_M = [1, 7, 8, 9, 16, 17, 21, 32, 33, 127, 128, 129, 136, 255]
+
+
+def padded(M):
+    """MP: the label count rounded up to the lane width of the value rows (api.cu)."""
+    return (M + 3) // 4 * 4
+
+
+def tail1(M):
+    """The fused kernels' last label quad holds one real label (meanfield.cu: tile_slice_smem)."""
+    return M == padded(M) - 3
+
+
+def small_image(rng, H, W, img):
+    """synth's images at a small shape.  "smooth" is the corner of an image eight times larger: synth blurs in
+    proportion to the size, and at 40 pixels its smooth image already overflows every bilateral tile."""
+    if img == "smooth":
+        return np.ascontiguousarray(synth.make_image(rng, 8 * H, 8 * W, img)[:H, :W])
+    return synth.make_image(rng, H, W, img)
+
+
+def fused_images(img, B=2):
+    H, W = FUSED_SHAPES[img]
+    return np.stack([small_image(np.random.RandomState(17 + b), H, W, img) for b in range(B)])
+
+
+def wide_images(img, B=2):
+    H, W = WIDE_SHAPES[img]
+    return np.stack([small_image(np.random.RandomState(29 + b), H, W, img) for b in range(B)])
+
+
+def hybrid_images():
+    return synth.make_batch(HYBRID_B, *HYBRID_SHAPE, image="photo", start=HYBRID_START)["image"]
+
+
+def log_unary(B, H, W, M, seed, scale=2.0):
+    """(B,H,W,M) float32 log-probabilities with a few confident regions (label 0 and label M-1 win a block each)."""
+    rng = np.random.RandomState(seed)
+    logits = rng.randn(B, H, W, M) * scale
+    logits[:, : H // 3, : W // 2, 0] += 4
+    logits[:, H // 2:, W // 3:, M - 1] += 4
+    pr = np.exp(logits - logits.max(-1, keepdims=True))
+    pr /= pr.sum(-1, keepdims=True)
+    return np.log(np.maximum(pr, 1e-5)).astype(np.float32)
+
+
+_CONSTS = None
+
+
+def csrc_constants():
+    """The compile-time defaults of the tile geometry and the tile-path thresholds, read from csrc/common.cuh."""
+    global _CONSTS
+    if _CONSTS is None:
+        import re
+        src = open(os.path.join(os.path.dirname(os.path.abspath(__file__)), "..", "dsrg_b200", "csrc",
+                                "common.cuh")).read()
+        c = {k: int(v) for k, v in re.findall(r"#define\s+(DSRG_\w+)\s+(\d+)\s*$", src, re.M)}
+        m = re.search(r"constexpr int kTileW = (\d+), kTileH = (\d+);", src)
+        c["kTileW"], c["kTileH"] = int(m.group(1)), int(m.group(2))
+        _CONSTS = c
+    return _CONSTS
+
+
+def tile_geometry(H, W):
+    """api.cu:engine_shape: tiles of tile_w x kTileH pixels, the width split evenly."""
+    k = csrc_constants()
+    tiles_x = -(-W // k["kTileW"])
+    tile_w = -(-W // tiles_x)
+    tiles_y = -(-H // k["kTileH"])
+    return tiles_x, tile_w, tiles_y
+
+
+def _hybrid_cover_ok(counts, npix, k):
+    """k_tile_build's rule for an overflow tile (tiles.cu): the smallest incidence count c >= 2 whose vertices (those
+    touched c times or more) fit into DSRG_MAXLOC_HY, plus the first `extra` vertices of the next bucket, must cover
+    DSRG_HY_MIN_COVER percent of the tile's incidences."""
+    maxloc = k["DSRG_MAXLOC_HY"]
+    threads = k["kTileW"] * k["kTileH"]
+    hist = np.bincount(counts, minlength=threads + 2)
+    nv_ge = np.cumsum(hist[::-1])[::-1]                          # vertices with >= c incidences
+    ni_ge = np.cumsum((hist * np.arange(hist.size))[::-1])[::-1]  # their incidences
+    c = next(c for c in range(2, threads + 1) if nv_ge[c] <= maxloc)
+    extra = maxloc - nv_ge[c] if c - 1 >= 2 else 0
+    covered = ni_ge[c] + extra * (c - 1)
+    return covered * 100 >= npix * 6 * k["DSRG_HY_MIN_COVER"]
+
+
+def predict_tile_paths(images, sf, sm_count, cf=13):
+    """What tiles.cu does to each tile of a mean-field pass over `images` (B,H,W,3) with crf_params(sf, cf), from the
+    oracle's own lattices.  Returns {"sp": kinds (ntiles,), "bi": kinds (B, ntiles), "hybrid_tiles": n}; a kind is
+    "smem" (the tile's distinct vertices fit the shared-memory list), "direct" (overflow tile on k_mf_tile's direct
+    path) or "hybrid" (k_mf_tile_hy).  Only the bilateral lattice has hybrid tiles; `hybrid_tiles` is the count the
+    engine reports after k_tile_demote."""
+    from oracle import crf_oracle
+    k = csrc_constants()
+    B, H, W = images.shape[:3]
+    tiles_x, tile_w, tiles_y = tile_geometry(H, W)
+    ntiles = tiles_x * tiles_y
+    ys, xs = np.mgrid[0:H, 0:W]
+    tile_of = ((ys // k["kTileH"]) * tiles_x + xs // tile_w).ravel()
+    npix = np.bincount(tile_of, minlength=ntiles)
+    gate = ntiles * B >= 16 * sm_count                             # common.cuh: hybrid_tiles_on
+    sp_kinds, bi_kinds = None, np.empty((B, ntiles), object)
+    for b in range(B):
+        c = crf_oracle.DenseCRF(W, H, 1)
+        c.set_unary_energy(np.zeros(H * W, np.float32))
+        c.add_pairwise_energy(10, 80 / sf, 80 / sf, cf, cf, cf, 3, 3 / sf, 3 / sf, images[b].ravel())
+        for lat, maxa in ((0, k["DSRG_MAXLOC_SP"]), (1, k["DSRG_MAXLOC_BI"])):
+            if lat == 0 and b > 0:
+                continue                                           # one spatial lattice serves the batch
+            off = c.lattice(lat).offset.astype(np.int64)          # (N, d+1): the vertex of every (pixel, r)
+            keys = tile_of[:, None] * (int(off.max()) + 1) + off
+            uniq, cnt = np.unique(keys.ravel(), return_counts=True)
+            utile = uniq // (int(off.max()) + 1)
+            nvert = np.bincount(utile, minlength=ntiles)
+            kinds = np.where(nvert > maxa, "direct", "smem").astype(object)
+            if lat == 1 and gate:
+                for t in np.nonzero(nvert > maxa)[0]:
+                    if _hybrid_cover_ok(cnt[utile == t], npix[t], k):
+                        kinds[t] = "hybrid"
+            if lat == 0:
+                sp_kinds = kinds
+            else:
+                bi_kinds[b] = kinds
+    nhy = int((bi_kinds == "hybrid").sum())
+    if nhy < k["DSRG_HY_MIN_TILES"] * sm_count:                    # k_tile_demote
+        bi_kinds[bi_kinds == "hybrid"] = "direct"
+        nhy = 0
+    return {"sp": sp_kinds, "bi": bi_kinds, "hybrid_tiles": nhy}
