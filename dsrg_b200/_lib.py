@@ -77,6 +77,9 @@ SIGNATURES = {
     "dsrg_predict_mask_host": (_i, [_vp, _i, _i, _vp, _vp, _vp, _vp, _f, _i, _pp, _vp, _i, _vp, _vp]),
     "dsrg_annotation_forward_dev": (_i, [_vp, _i, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _vp, _vp, _vp, _vp]),
     "dsrg_annotation_forward_host": (_i, [_vp, _i, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _vp, _vp, _vp]),
+    "dsrg_annotation_coco_forward_dev": (_i, [_vp, _vp, _vp, _vp, _i, _vp, _vp, _i, _i, _vp, _i, _vp, _vp, _vp, _vp,
+                                              _vp]),
+    "dsrg_annotation_coco_forward_host": (_i, [_vp, _vp, _vp, _vp, _i, _vp, _vp, _i, _i, _vp, _i, _vp, _vp, _vp]),
     "dsrg_confusion_create": (_vp, [_i, _i]),
     "dsrg_confusion_destroy": (None, [_vp]),
     "dsrg_confusion_reset": (_i, [_vp, _vp]),

@@ -469,6 +469,64 @@ class Engine(object):
                                                   _dptr(images_out), _stream(stream)))
         return labels_out, cues_out
 
+    # ---- AnnotationLayerCOCO.forward (pylayers.py:432-512) ----
+    @staticmethod
+    def _coco_args(shapes, flip, new_size, mean_pixel):
+        B = len(shapes)
+        Hs = (C.c_int * B)(*[int(s[0]) for s in shapes])
+        Ws = (C.c_int * B)(*[int(s[1]) for s in shapes])
+        fl = None if flip is None else np.ascontiguousarray(flip, np.int32)
+        if fl is not None and fl.shape != (B,):
+            raise ValueError("flip must have one entry per image")
+        mean = np.ascontiguousarray(mean_pixel, np.float64)
+        if mean.shape != (3,):
+            raise ValueError("mean_pixel must have 3 elements")
+        new_h, new_w = (int(v) for v in new_size)
+        return B, Hs, Ws, fl, mean, new_h, new_w
+
+    def annotation_coco_forward_host(self, images, label_maps, new_size, mean_pixel, flip=None, ignore_label=255,
+                                     out=None):
+        """images: B (H_b, W_b, 3) uint8 BGR arrays; label_maps: (B, H, W) uint8 at the engine's size ->
+        labels (B,1,1,M), cues (B,M,H,W), images (B,3,new_h,new_w) float32, written into `out` when it is given
+        (three C-contiguous float32 arrays of those shapes).  A label value >= M other than ignore_label raises
+        DsrgError with numpy's IndexError message."""
+        for im in images:
+            _hptr(im, np.uint8)
+            if im.ndim != 3 or im.shape[2] != 3:
+                raise ValueError("every image must be an (H, W, 3) uint8 array")
+        B, Hs, Ws, fl, mean, new_h, new_w = self._coco_args([im.shape for im in images], flip, new_size, mean_pixel)
+        if label_maps.shape != (B, self.H, self.W):
+            raise ValueError("label_maps must have shape (%d, %d, %d)" % (B, self.H, self.W))
+        if out is None:
+            out = (np.empty((B, 1, 1, self.M), np.float32), np.empty((B, self.M, self.H, self.W), np.float32),
+                   np.empty((B, 3, new_h, new_w), np.float32))
+        ptrs = (C.c_void_p * B)(*[im.ctypes.data for im in images])
+        check(self._L.dsrg_annotation_coco_forward_host(
+            self.h, ptrs, Hs, Ws, B, _hptr(label_maps, np.uint8), _hptr(fl, np.int32), new_h, new_w,
+            _hptr(mean, np.float64), int(ignore_label), _hptr(out[0], np.float32), _hptr(out[1], np.float32),
+            _hptr(out[2], np.float32)))
+        return out
+
+    def annotation_coco_forward_dev(self, images, label_maps, labels_out, cues_out, images_out, mean_pixel,
+                                    flip=None, ignore_label=255, bad_out=None, stream=None):
+        """images: B (H_b, W_b, 3) uint8 CUDA tensors; label_maps: (B, H, W) uint8 CUDA tensor; the outputs are
+        float32 CUDA tensors, images_out (B, 3, new_h, new_w) giving the size.  bad_out: optional (B,) int32 CUDA
+        tensor, per image the raster index of the first label value >= M other than ignore_label, or -1."""
+        import torch
+        for im in images:
+            if im.dtype != torch.uint8 or im.dim() != 3 or im.shape[2] != 3:
+                raise ValueError("every image must be an (H, W, 3) uint8 tensor")
+        if images_out.dim() != 4:
+            raise ValueError("images_out must be a (B, 3, new_h, new_w) tensor")
+        B, Hs, Ws, fl, mean, new_h, new_w = self._coco_args([im.shape for im in images], flip,
+                                                            images_out.shape[2:], mean_pixel)
+        ptrs = (C.c_void_p * B)(*[_dptr(im).value for im in images])
+        check(self._L.dsrg_annotation_coco_forward_dev(
+            self.h, ptrs, Hs, Ws, B, _dptr(label_maps), _hptr(fl, np.int32), new_h, new_w, _hptr(mean, np.float64),
+            int(ignore_label), _dptr(labels_out), _dptr(cues_out), _dptr(images_out), _dptr(bad_out),
+            _stream(stream)))
+        return labels_out, cues_out, images_out
+
     # ---- per-kernel timing ----
     def profile(self, enable):
         check(self._L.dsrg_engine_profile(self.h, int(bool(enable))))

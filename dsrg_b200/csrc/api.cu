@@ -290,7 +290,7 @@ using namespace dsrg;
 
 extern "C" {
 
-int dsrg_version(void) { return 103; }
+int dsrg_version(void) { return 104; }
 
 const char *dsrg_last_error(void) { return g_err; }
 

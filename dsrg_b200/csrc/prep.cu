@@ -66,11 +66,7 @@ k_prepare_net_input(const uint8_t *__restrict__ im, int H, int W, NetInputScales
     const int oy = pix / w, ox = pix - oy * w;
     const ZoomTap tap = zoom_tap(oy, ox, H, W, h, w);
     float *o = sc.out[k];
-#pragma unroll
-    for (int c = 0; c < 3; c++) {
-        const float z = zoom_apply(im, W, 2 - c, tap);                     // float32, like nd.zoom's result
-        o[(size_t)c * h * w + pix] = (float)__dsub_rn((double)z, sc.mean[c]);  // - mean_pixel (float64)
-    }
+    net_input_pixel(im, W, tap, sc.mean, o, h, w, pix);
 }
 
 static int prepare_net_input(Engine *e, int H, int W, const uint8_t *image, int n, const int *hs, const int *ws,

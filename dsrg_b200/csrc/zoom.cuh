@@ -58,4 +58,17 @@ __device__ __forceinline__ float zoom_apply(const uint8_t *__restrict__ p, int W
     return zoom_taps(z, [&](int y, int x) { return (double)p[((size_t)y * Wi + x) * 3 + c]; });
 }
 
+// One pixel of a network input built the way the evaluation tools' preprocess() and AnnotationLayerCOCO build it:
+//   nd.zoom(image.astype('float32'), (h/H, w/W, 1.0), order=1)[:, :, [2, 1, 0]] - mean, transposed to CHW
+// The zoom of channel 2 - c of the interleaved [H][W][3] image at `tap` (zoom_tap of the pixel in an h x w output),
+// minus mean[c] in float64 (numpy promotes against the float64 mean), stored as float32 at o[c * h * w + pix].
+__device__ __forceinline__ void net_input_pixel(const uint8_t *__restrict__ im, int W, const ZoomTap &tap,
+                                                const double *mean, float *o, int h, int w, int pix) {
+#pragma unroll
+    for (int c = 0; c < 3; c++) {
+        const float z = zoom_apply(im, W, 2 - c, tap);                     // float32, like nd.zoom's result
+        o[(size_t)c * h * w + pix] = (float)__dsub_rn((double)z, mean[c]);  // - mean_pixel (float64)
+    }
+}
+
 }  // namespace dsrg

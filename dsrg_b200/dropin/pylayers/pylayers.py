@@ -14,11 +14,16 @@ in train-s.prototxt:746-812 keeps working:
 * ``SeedLossLayer`` / ``ExpandLossLayer`` (pylayers.py:95-118, :183-233), SEC's seeding and expansion losses
   (the seed-loss blocks train-s.prototxt:821-910 keeps commented out, and SEC-style baselines)
   -> dsrg_seedloss_plain_* / dsrg_expandloss_*.
+* ``AnnotationLayer`` / ``AnnotationLayerCOCO`` (pylayers.py:346-387, :389-512), the VOC and COCO training inputs
+  -> dsrg_annotation_forward_* / dsrg_annotation_coco_forward_*.
 
 The blobs Caffe hands to a Python layer are host numpy views, so the ``*_host`` entry points of
 the C ABI are used: one H2D of the bottoms and one D2H of the tops per call, everything else --
 including the image zoom / mean / round preprocessing -- on the GPU.  There is no multiprocessing.Pool (pylayers.py:292) and no CPU fallback.
 """
+import ast
+import re
+
 import numpy as np
 import yaml
 
@@ -46,19 +51,22 @@ def _f32(a):
     return np.ascontiguousarray(a, dtype=np.float32)
 
 
-_PINNED_REGIONS = {}   # data pointer -> nbytes of blob buffers page-locked with dsrg_host_register
+_PINNED_REGIONS = {}   # data pointer -> (nbytes, the array) of blob buffers page-locked with dsrg_host_register
 
 
 def _pin(a):
     """Page-lock a blob's buffer once (Caffe keeps its blobs for the life of the net; in GPU mode their CPU side
     already is pinned memory): the host entry points then stream it at the PCIe rate instead of going through the
-    driver's staged pageable copies.  DSRG_B200_PIN_BLOBS=0 turns it off; failures are ignored."""
+    driver's staged pageable copies.  DSRG_B200_PIN_BLOBS=0 turns it off; failures are ignored.
+    The table holds a reference to every array it registered, so a registered buffer is never freed: memory that is
+    freed while still registered and then handed to another array makes the driver refuse later copies from it
+    (cudaErrorInvalidValue).  At most 16 arrays are held; the oldest is unregistered and released first."""
     import os
     if os.environ.get("DSRG_B200_PIN_BLOBS", "1") == "0" or not isinstance(a, np.ndarray) or a.nbytes < (1 << 20):
         return a
     from dsrg_b200 import _lib
     ptr = a.ctypes.data
-    if _PINNED_REGIONS.get(ptr) != a.nbytes:
+    if _PINNED_REGIONS.get(ptr, (None,))[0] != a.nbytes:
         L = _lib.lib()
         if ptr in _PINNED_REGIONS:
             L.dsrg_host_unregister(ptr)
@@ -68,7 +76,7 @@ def _pin(a):
             L.dsrg_host_unregister(old)
             del _PINNED_REGIONS[old]
         if L.dsrg_host_register(ptr, a.nbytes) == 0:
-            _PINNED_REGIONS[ptr] = a.nbytes
+            _PINNED_REGIONS[ptr] = (a.nbytes, a)
     return a
 
 
@@ -404,3 +412,94 @@ class AnnotationLayer(caffe.Layer):
 
     def backward(self, top, propagate_down, bottom):
         pass
+
+
+_IMREAD_GRAYSCALE, _IMREAD_COLOR = 0, 1   # cv2's values of the two flags
+
+
+def _imread(path, flag):
+    """cv2.imread(path, flag).  OpenCV is imported on first use, so that the module loads without it; tests and
+    tools that feed decoded arrays replace this function."""
+    import cv2
+    return cv2.imread(path, flag)
+
+
+def _read(path, flag):
+    im = _imread(path, flag)
+    if im is None:
+        raise IOError("cannot read %r" % path)
+    im = np.asarray(im)
+    if im.dtype != np.uint8 or im.ndim != (3 if flag == _IMREAD_COLOR else 2) or (im.ndim == 3 and im.shape[2] != 3):
+        raise ValueError("%r: expected %s uint8, got %s %s" % (
+            path, "(H, W, 3)" if flag == _IMREAD_COLOR else "(H, W)", im.shape, im.dtype))
+    return im
+
+
+class AnnotationLayerCOCO(caffe.Layer):
+    """pylayers.py:389-512 -> dsrg_annotation_coco_forward_host.  The files are decoded on the host (``_imread``)
+    and the random numbers drawn there in the reference's order: ``numpy.random.shuffle`` of the list when an epoch
+    is over, then per image ``np.random.choice`` when mirroring.  The zoom, the mean, the mirror, the cue planes and
+    the tags of the whole batch are one device call.  ``param_str`` keys as in the reference: `source`, `root`,
+    `batch_size`, `mean` (3 values) and `new_size` are required; `mirror` defaults to False, `ignore_label` to
+    255."""
+
+    K = 81
+
+    def setup(self, bottom, top):
+        layer_params = ast.literal_eval(self.param_str)
+        self.source = layer_params['source']
+        self.root_folder = layer_params['root']
+        self.batch_size = layer_params['batch_size']
+        self.is_mirror = layer_params.get('mirror', False)
+        self.mean = layer_params['mean']
+        self.new_h, self.new_w = layer_params['new_size']
+        self.ignore_label = layer_params.get('ignore_label', 255)
+        # image - self.mean subtracts per channel in float64 only when mean has three values; numpy would subtract
+        # a scalar in float32
+        if np.asarray(self.mean).shape != (3,):
+            raise ValueError("mean must have 3 values, got %r" % (self.mean,))
+        self._mean = np.asarray(self.mean, np.float64)
+        with open(self.source) as f:
+            self.indexlist = [line.strip().split() for line in f]
+        self._cur = 0
+        top[0].reshape(self.batch_size, 1, 1, self.K)
+        top[1].reshape(self.batch_size, self.K, self.new_h // 8 + 1, self.new_w // 8 + 1)
+        top[2].reshape(self.batch_size, 3, self.new_h, self.new_w)
+
+    def reshape(self, bottom, top):
+        pass
+
+    def backward(self, top, propagate_down, bottom):
+        pass
+
+    def forward(self, bottom, top):
+        B = self.batch_size
+        h, w = self.new_h // 8 + 1, self.new_w // 8 + 1
+        images, labels, flips = [], np.empty((B, h, w), np.uint8), []
+        for itt in range(B):
+            if self._cur == len(self.indexlist):                                      # pylayers.py:447-449
+                self._cur = 0
+                np.random.shuffle(self.indexlist)
+            image_file_path, label_file_path = self.indexlist[self._cur]
+            image = _read(self.root_folder + image_file_path, _IMREAD_COLOR)
+            label = _read(self.root_folder + label_file_path, _IMREAD_GRAYSCALE)
+            self._cur += 1
+            if self.is_mirror:
+                flips.append(int(np.random.choice(2) * 2 - 1 == -1))                 # pylayers.py:501
+            images.append(image)
+            labels[itt] = label   # broadcasts like top[1].data[itt, ...] = cues (:439); ValueError otherwise
+        tops = [t.data for t in top[:3]]
+        direct = all(isinstance(t, np.ndarray) and t.dtype == np.float32 and t.flags["C_CONTIGUOUS"] for t in tops)
+        eng = _engine(B, self.K, h, w)
+        try:
+            got = eng.annotation_coco_forward_host(images, labels, (self.new_h, self.new_w), self._mean,
+                                                   flips if self.is_mirror else None, self.ignore_label,
+                                                   out=tops if direct else None)
+        except _api.DsrgError as e:
+            m = re.search(r"index -?\d+ is out of bounds for axis 0 with size \d+", str(e))
+            if m:
+                raise IndexError(m.group(0)) from None
+            raise
+        if not direct:
+            for t, g in zip(top, got):
+                t.data[...] = g

@@ -37,7 +37,8 @@ extern "C" {
 /* CRF (batch, layer and DenseCRF-object entry points), SRG, the predict_mask post-processing and the confusion
  * matrix accept up to this many labels: above DSRG_MAX_LABELS the mean field runs on a generic label-chunked path
  * (csrc/meanfield_wide.cu) -- the reference's COCO tool uses DenseCRF(W, H, 81), training/tools/test-coco.py.
- * The Softmax / ConstrainLoss layers are built for at most DSRG_MAX_LABELS. */
+ * Of the layers, only Softmax is limited to DSRG_MAX_LABELS; ConstrainLoss, BalancedSeedLoss, the SEC losses and
+ * the COCO annotation layer have no label limit of their own. */
 #define DSRG_MAX_LABELS_WIDE 255
 /* pixels per class plane the GWRP kernels of dsrg_expandloss_* sort in shared memory (41x41 and the 65x65 maps
  * of a 513 crop fit; larger planes return DSRG_E_INVALID) */
@@ -282,6 +283,36 @@ int dsrg_annotation_forward_host(dsrg_engine *e, int B, const int32_t *tag_offse
                                  const int32_t *cue_offsets, const int32_t *cue_idx, const int32_t *flip,
                                  const float *images_in_host, int Hi, int Wi, float *labels_out_host,
                                  float *cues_out_host, float *images_out_host);
+
+/*
+ * AnnotationLayerCOCO.forward (pylayers/pylayers/pylayers.py:432-512), the COCO training input, after the caller
+ * has decoded the files and drawn the random numbers (the shuffle and `flip`) in the reference's order.  Per image b:
+ *   images[b]  : [Hs[b]][Ws[b]][3] uint8 BGR, as cv2.imread(..., IMREAD_COLOR) returns it; each image has its own size
+ *   label_maps : [B][H][W] uint8 (H x W = the engine's size), as cv2.imread(..., IMREAD_GRAYSCALE) returns them
+ *   flip [B] or NULL : 1 = mirror this image's pixels and cues along the width (flip == -1, :500-503)
+ * ->
+ *   images_out : [B][3][new_h][new_w] float32: zoom(image.astype('float32'), (new_h/H, new_w/W, 1.0), order=1),
+ *                channels reversed, - mean_pixel in float64 (scipy.ndimage.zoom order=1 semantics, bit-exact; the
+ *                arithmetic of dsrg_prepare_net_input_*)
+ *   cues_out   : [B][K][H][W] float32 0/1, cues[v, y, x] = 1 for every pixel with value v != ignore_label
+ *   labels_out : [B][1][1][K] float32 0/1, 1 for every value present other than ignore_label (label 0 is not forced)
+ * K is the engine's M (81 for COCO).  The arrays of image pointers, Hs, Ws, flip and mean_pixel live on the host in
+ * both variants.  The images are staged through a table in device memory, so B is bounded by the engine only.
+ * A label value v >= K other than ignore_label is what numpy refuses with IndexError:
+ *   _host: DSRG_E_INVALID before any copy or launch, with numpy's message ("index 90 is out of bounds for axis 0
+ *          with size 81") for the first such pixel, image by image in raster order.
+ *   _dev : such pixels are skipped (no cue plane, no tag; nothing is written out of bounds).  bad_out_dev [B] int32
+ *          (may be NULL) receives per image the raster index, in the label map as given (before the mirror), of the
+ *          first such pixel, or -1 if there is none; the caller checks it once the stream has run.
+ */
+int dsrg_annotation_coco_forward_dev(dsrg_engine *e, const uint8_t *const *images_dev, const int *Hs, const int *Ws,
+                                     int B, const uint8_t *label_maps_dev, const int32_t *flip, int new_h, int new_w,
+                                     const double *mean_pixel /* host, 3 */, int ignore_label, float *labels_out_dev,
+                                     float *cues_out_dev, float *images_out_dev, int32_t *bad_out_dev, void *stream);
+int dsrg_annotation_coco_forward_host(dsrg_engine *e, const uint8_t *const *images_host, const int *Hs,
+                                      const int *Ws, int B, const uint8_t *label_maps_host, const int32_t *flip,
+                                      int new_h, int new_w, const double *mean_pixel /* host, 3 */, int ignore_label,
+                                      float *labels_out_host, float *cues_out_host, float *images_out_host);
 
 /* ------------------------------------------------------------------------------------------
  * Confusion matrix of a segmentation run, the scoring step of the evaluation tools:
