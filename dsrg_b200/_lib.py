@@ -109,6 +109,7 @@ SIGNATURES = {
     "dsrg_engine_profile": (_i, [_vp, _i]),
     "dsrg_engine_profile_read": (_i, [_vp, _vp, _vp]),
     "dsrg_engine_lattice_sizes": (_i, [_vp, _i, _vp, _vp]),
+    "dsrg_engine_lattice_tables": (_i, [_vp, _i, _i, _vp, _vp]),
     "dsrg_engine_copy_norm": (_i, [_vp, _i, _i, _vp]),
     "dsrg_densecrf_create": (_vp, [_i, _i, _i]),
     "dsrg_densecrf_destroy": (None, [_vp]),

@@ -546,6 +546,17 @@ class Engine(object):
         check(self._L.dsrg_engine_lattice_sizes(self.h, B, _hptr(vs, np.int32), _hptr(vb, np.int32)))
         return int(vs[0]), vb
 
+    def lattice_tables(self, which, b):
+        """Image b's lattice of the last CRF call (which = 0 spatial, 1 bilateral) in the engine's numbering:
+        off (d+1, N) 1-based rows of every (r, pixel), nbr (d+1, V+1, 2) the blur neighbours of rows 0..V."""
+        d = 2 if which == 0 else 5
+        vs, vb = self.lattice_sizes(b + 1)
+        V = vs if which == 0 else int(vb[b])
+        off = np.zeros((d + 1, self.H * self.W), np.int32)
+        nbr = np.zeros((d + 1, V + 1, 2), np.int32)
+        check(self._L.dsrg_engine_lattice_tables(self.h, which, b, _hptr(off, np.int32), _hptr(nbr, np.int32)))
+        return off, nbr
+
     def norms(self, B):
         ns = np.zeros(self.H * self.W, np.float32)
         nb = np.zeros((B, self.H * self.W), np.float32)

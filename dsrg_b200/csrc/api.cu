@@ -98,6 +98,11 @@ static int lattice_alloc(Engine *e, Lattice &L, int d, int shared) {
     rc |= dalloc(e, &L.hval, n * L.cap);
     rc |= dalloc(e, &L.vslot, n * L.capv);
     rc |= dalloc(e, &L.vcount, n);
+    rc |= dalloc(e, &L.aslot, n * L.capv);
+    rc |= dalloc(e, &L.vkey, n * L.capv);
+    const long long rn_words = renum_words(e->ntiles, d + 1);  // the capacity shape has the most tiles
+    rc |= dalloc(e, &L.rn_words, n * rn_words);
+    rc |= dalloc(e, &L.rn_chunk, n * (rn_words / kRenumChunk));
     rc |= dalloc(e, &L.rowbase, (size_t)e->maxB + 1);
     rc |= dalloc(e, &L.nbr, (size_t)(d + 1) * L.nbr_stride);
     L.maxloc = (d == 2) ? kMaxLocSp : kMaxLocHy;
@@ -114,6 +119,7 @@ static int lattice_alloc(Engine *e, Lattice &L, int d, int shared) {
     if (cudaMemset(L.hkeys, 0xFF, sizeof(uint64_t) * n * L.cap) != cudaSuccess) return DSRG_E_CUDA;
     if (cudaMemset(L.tl_hy, 0, nt) != cudaSuccess) return DSRG_E_CUDA;
     if (cudaMemset(L.hval, 0xFF, sizeof(int32_t) * n * L.cap) != cudaSuccess) return DSRG_E_CUDA;
+    if (cudaMemset(L.vkey, 0x7F, sizeof(int32_t) * n * L.capv) != cudaSuccess) return DSRG_E_CUDA;  // kNoKey
     return DSRG_OK;
 }
 
@@ -125,6 +131,10 @@ static void lattice_free(Lattice &L) {
     cudaFree(L.hval);
     cudaFree(L.vslot);
     cudaFree(L.vcount);
+    cudaFree(L.aslot);
+    cudaFree(L.vkey);
+    cudaFree(L.rn_words);
+    cudaFree(L.rn_chunk);
     cudaFree(L.rowbase);
     cudaFree(L.nbr);
     cudaFree(L.tl_nloc);
@@ -290,7 +300,7 @@ using namespace dsrg;
 
 extern "C" {
 
-int dsrg_version(void) { return 104; }
+int dsrg_version(void) { return 105; }
 
 const char *dsrg_last_error(void) { return g_err; }
 
@@ -749,6 +759,32 @@ int dsrg_engine_lattice_sizes(dsrg_engine *h, int B, int *v_spatial, int *v_bila
     if (v_spatial) DSRG_CUDA_TRY(cudaMemcpy(v_spatial, e->sp.vcount, sizeof(int), cudaMemcpyDeviceToHost));
     if (v_bilateral)
         DSRG_CUDA_TRY(cudaMemcpy(v_bilateral, e->bi.vcount, sizeof(int) * B, cudaMemcpyDeviceToHost));
+    return DSRG_OK;
+}
+
+int dsrg_engine_lattice_tables(dsrg_engine *h, int which, int b, int *off_out, int *nbr_out) {
+    Engine *e = (Engine *)h;
+    DeviceScope dev_scope(e);
+    int rc = check_entry(e, 1, e && (which == 0 || which == 1) && b >= 0 && b < e->maxB);
+    if (rc) return rc;
+    const Lattice &L = which == 0 ? e->sp : e->bi;
+    const int sb = L.shared ? 0 : b;
+    DSRG_CUDA_TRY(cudaDeviceSynchronize());
+    int V = 0, base = 0;
+    DSRG_CUDA_TRY(cudaMemcpy(&V, L.vcount + sb, sizeof(int), cudaMemcpyDeviceToHost));
+    if (!L.shared) DSRG_CUDA_TRY(cudaMemcpy(&base, L.rowbase + b, sizeof(int), cudaMemcpyDeviceToHost));
+    const int dp1 = L.d + 1;
+    if (off_out)
+        DSRG_CUDA_TRY(cudaMemcpy(off_out, L.off + (size_t)sb * dp1 * L.N, sizeof(int32_t) * dp1 * L.N,
+                                 cudaMemcpyDeviceToHost));
+    if (nbr_out) {
+        for (int j = 0; j < dp1; j++) {
+            int *dst = nbr_out + (size_t)j * (V + 1) * 2;
+            DSRG_CUDA_TRY(cudaMemcpy(dst, L.nbr + (size_t)j * L.nbr_stride + base, sizeof(int2) * (V + 1),
+                                     cudaMemcpyDeviceToHost));
+            for (int k = 0; k < 2 * (V + 1); k++) dst[k] -= base;
+        }
+    }
     return DSRG_OK;
 }
 

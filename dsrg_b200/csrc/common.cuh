@@ -51,6 +51,13 @@ struct Lattice {
     int32_t *hval = nullptr;    // [nimg][cap] local vertex id of the slot
     int32_t *vslot = nullptr;   // [nimg][capv] slot of local vertex id
     int32_t *vcount = nullptr;  // [nimg]
+    // build scratch of the renumbering (lattice.cu): the slot and the key (first incidence) of each vertex in
+    // arrival order (vkey is kNoKey between builds), the key-space bitmap with its per-word prefix, and the
+    // per-chunk prefix
+    int32_t *aslot = nullptr;   // [nimg][capv]
+    int32_t *vkey = nullptr;    // [nimg][capv]
+    uint2 *rn_words = nullptr;  // [nimg][renum_words()]
+    int32_t *rn_chunk = nullptr;  // [nimg][renum_words() / chunk]
     int32_t *rowbase = nullptr; // [max_batch+1]
     int2 *nbr = nullptr;        // [d+1][rows] (n1,n2): global rows (per-image) or local rows (shared)
     long long nbr_stride = 0;   // rows per axis in nbr
@@ -80,6 +87,9 @@ enum KTag {
 
 // ---- lattice.cu ----
 int lattice_build(Engine *e, Lattice &L, int B, const uint8_t *image_dev, cudaStream_t s);
+constexpr int kNoKey = 0x7F7F7F7F;  // renumbering key of no incidence yet (a byte pattern, for cudaMemset)
+constexpr int kRenumChunk = 4 * kThreads;  // bitmap words per renumbering chunk: 4 per thread of k_renum_scan
+long long renum_words(int ntiles, int dp1);  // bitmap words per image, a whole number of chunks
 // ---- tiles.cu ----
 constexpr int kTileW = 32, kTileH = 8;   // one thread per pixel, one warp per tile row
 constexpr int kTileThreads = kTileW * kTileH;

@@ -5,8 +5,15 @@
 // once.  The arithmetic that decides WHICH simplex a pixel falls into follows the reference's
 // SSE code path operation by operation (round-to-nearest-even, no FMA contraction: every float
 // op is an explicit __f*_rn intrinsic); the hash table itself is a GPU design (64-bit packed
-// keys, CAS insertion, ids in arrival order) because vertex numbering does not influence the
-// filter result.
+// keys, CAS insertion).
+//
+// Vertex numbering does not change the filter's values, but it decides the blur's memory traffic: a blur pass
+// reads 3 to 27 rows per output row through the neighbour table.  Insertion hands out ids in arrival order, which
+// with all of an image's insert blocks in flight at once scatters neighbouring vertices over a buffer larger than
+// the L2.  So the build renumbers every lattice (k_renum_*): a vertex's key is its first incidence in tile-major
+// pixel order (tile, pixel's thread index in the tile, r; tiles.cu's geometry), and the ids are the ranks of the
+// keys.  Lattice neighbours then sit a few ids apart for the spatial lattice and mostly so for the bilateral one,
+// each tile's rows are a few contiguous runs, and the numbering is deterministic.
 #include "common.cuh"
 
 namespace dsrg {
@@ -55,7 +62,8 @@ __device__ __forceinline__ uint64_t ld_relaxed_u64(const uint64_t *p) {
     return v;
 }
 
-// insert-or-find; the winner of an empty slot allocates the next vertex id of its image
+// insert-or-find; the winner of an empty slot allocates the next vertex id of its image (in arrival order: the
+// renumbering replaces it before anything else reads it)
 __device__ __forceinline__ int hash_insert(uint64_t *keys, int32_t *hval, int32_t *vslot,
                                            int32_t *vcount, uint32_t cap, uint64_t k) {
     uint32_t s = hash_slot(k, cap);
@@ -90,6 +98,7 @@ __device__ __forceinline__ int hash_lookup(const uint64_t *keys, uint32_t cap, u
 
 struct BuildArgs {
     int N, P, W;
+    int tile_w, tiles_x, ntiles;
     uint32_t cap;
     int capv;
     float sigma[5];
@@ -98,9 +107,17 @@ struct BuildArgs {
     int32_t *off;
     float *bary;
     uint64_t *hkeys;
-    int32_t *hval, *vslot, *vcount;
+    int32_t *hval, *aslot, *vcount, *vkey;
     int *err;
 };
+
+// A pixel's position in tile-major order (tiles.cu: tile index, then the pixel's thread index in the tile); the
+// phantom lanes all sit at position ntiles * kTileThreads, after every pixel.  Renumbering key of incidence
+// (pixel, r): pos * (d+1) + r.
+__device__ __forceinline__ int tile_major_pos(int x, int y, int tile_w, int tiles_x) {
+    const int tx = x / tile_w, ty = y / kTileH;
+    return (ty * tiles_x + tx) * kTileThreads + (y - ty * kTileH) * kTileW + (x - tx * tile_w);
+}
 
 // ---------------------------------------------------------------------------------------------
 // Kernel 1: one thread per pixel (plus the phantom tail lanes): features -> elevate -> simplex ->
@@ -116,8 +133,10 @@ __global__ void __launch_bounds__(kThreads) k_lattice_insert(BuildArgs a) {
     float f[D];
 #pragma unroll
     for (int j = 0; j < D; j++) f[j] = 0.0f;  // phantom lanes carry feature 0 (:196)
+    int pos = a.ntiles * kTileThreads;
     if (real) {
         const int x = i % a.W, y = i / a.W;
+        pos = tile_major_pos(x, y, a.tile_w, a.tiles_x);
         f[0] = __fdiv_rn((float)x, a.sigma[0]);  // densecrf.cpp:65-66 / :74-75
         f[1] = __fdiv_rn((float)y, a.sigma[1]);
         if (D == 5) {
@@ -192,7 +211,8 @@ __global__ void __launch_bounds__(kThreads) k_lattice_insert(BuildArgs a) {
     // vertices (:268-275)
     uint64_t *keys = a.hkeys + (size_t)b * a.cap;
     int32_t *hval = a.hval + (size_t)b * a.cap;
-    int32_t *vslot = a.vslot + (size_t)b * a.capv;
+    int32_t *aslot = a.aslot + (size_t)b * a.capv;
+    int32_t *vkey = a.vkey + (size_t)b * a.capv;
     int32_t *vcount = a.vcount + b;
     const unsigned lane = threadIdx.x & 31;
     bool range_bad = false;
@@ -210,14 +230,17 @@ __global__ void __launch_bounds__(kThreads) k_lattice_insert(BuildArgs a) {
         unsigned peers = __match_any_sync(0xffffffffu, valid ? pk : (kEmptyKey - 1 - lane));
         int leader = __ffs(peers) - 1;
         int id = 0;
+        // the first incidence of the vertex among the lanes, for the renumbering key (vkey is kNoKey between builds)
+        const int kmin = __reduce_min_sync(peers, valid ? pos * (D + 1) + r : kNoKey);
         if (valid && (int)lane == leader) {
-            const int slot = hash_insert(keys, hval, vslot, vcount, a.cap, pk);
+            const int slot = hash_insert(keys, hval, aslot, vcount, a.cap, pk);
             // the slot's owner publishes the vertex id right after winning the CAS; owners of the
             // same key always sit in other warps (one leader per key per warp), so this cannot
             // wait on a lane of the same warp
             do {
                 asm volatile("ld.relaxed.gpu.global.s32 %0, [%1];" : "=r"(id) : "l"(hval + slot) : "memory");
             } while (id < 0);
+            atomicMin(vkey + id, kmin);
         }
         id = __shfl_sync(0xffffffffu, id, leader);
         if (real) {
@@ -237,6 +260,102 @@ __global__ void k_rowbase(const int32_t *vcount, int32_t *rowbase, int B, int sh
             rowbase[b] = acc;
             if (b < B) acc += vcount[shared ? 0 : b] + 1;
         }
+    }
+}
+
+// ---------------------------------------------------------------------------------------------
+// Renumbering: new id = rank of the vertex's key (vkey, its first incidence, from k_lattice_insert) among its
+// image's keys.  The keys are marked in a bitmap over the key space (one bit per (pixel, r)); the rank of a key is
+// the number of marked bits before it: a per-chunk prefix (k_renum_scan, words of 32 bits, kRenumChunk words per
+// chunk), a per-image prefix over the chunks (k_renum_chunks) and the popcount inside the word.
+// ---------------------------------------------------------------------------------------------
+// words of the key-space bitmap per image (a whole number of chunks)
+long long renum_words(int ntiles, int dp1) {
+    const long long keys = ((long long)ntiles * kTileThreads + 1) * dp1;
+    return (keys + 32LL * kRenumChunk - 1) / (32LL * kRenumChunk) * kRenumChunk;
+}
+
+__global__ void __launch_bounds__(kThreads)
+k_renum_mark(const int32_t *vcount, const int32_t *vkey, uint2 *words, int capv, long long nwords) {
+    const int b = blockIdx.y;
+    const int V = vcount[b];
+    for (int v = blockIdx.x * blockDim.x + threadIdx.x; v < V; v += gridDim.x * blockDim.x) {
+        const int k = vkey[(size_t)b * capv + v];
+        atomicOr(&words[b * nwords + (k >> 5)].x, 1u << (k & 31));
+    }
+}
+
+// exclusive block-wide scan of one value per thread (kThreads threads); *total gets the block's sum
+__device__ __forceinline__ int block_exclusive_scan(int v, int *total) {
+    __shared__ int wsum[kThreads / 32];
+    const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+    int incl = v;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+        const int n = __shfl_up_sync(0xffffffffu, incl, o);
+        if (lane >= o) incl += n;
+    }
+    if (lane == 31) wsum[wid] = incl;
+    __syncthreads();
+    int base = 0, all = 0;
+#pragma unroll
+    for (int k = 0; k < kThreads / 32; k++) {
+        base += k < wid ? wsum[k] : 0;
+        all += wsum[k];
+    }
+    __syncthreads();  // wsum may be reused by the next call
+    *total = all;
+    return base + incl - v;
+}
+
+// per word: the marked bits before it inside its chunk (.y); per chunk: its marked bits
+__global__ void __launch_bounds__(kThreads) k_renum_scan(uint2 *words, int32_t *chunk_sum, long long nwords, int nchunks) {
+    const int b = blockIdx.y, c = blockIdx.x;
+    uint2 *w = words + b * nwords + (long long)c * kRenumChunk + 4 * threadIdx.x;
+    int n[4], s = 0;
+#pragma unroll
+    for (int q = 0; q < 4; q++) s += n[q] = __popc(w[q].x);
+    int total;
+    int pre = block_exclusive_scan(s, &total);
+#pragma unroll
+    for (int q = 0; q < 4; q++) {
+        w[q].y = (uint32_t)pre;
+        pre += n[q];
+    }
+    if (threadIdx.x == 0) chunk_sum[(size_t)b * nchunks + c] = total;
+}
+
+// per image: chunk sums -> exclusive prefix
+__global__ void __launch_bounds__(kThreads) k_renum_chunks(int32_t *chunk_sum, int nchunks) {
+    int32_t *cs = chunk_sum + (size_t)blockIdx.x * nchunks;
+    int carry = 0;
+    for (int c0 = 0; c0 < nchunks; c0 += kThreads) {
+        const int c = c0 + threadIdx.x;
+        const int v = c < nchunks ? cs[c] : 0;
+        int total;
+        const int pre = block_exclusive_scan(v, &total);
+        if (c < nchunks) cs[c] = carry + pre;
+        carry += total;
+    }
+}
+
+// old id v -> new id: vkey[v] becomes the new id (k_norm_splat rewrites off with it), hval and vslot follow the new
+// numbering
+__global__ void __launch_bounds__(kThreads)
+k_renum_rank(const int32_t *vcount, int32_t *vkey, const uint2 *words, const int32_t *chunk_sum, const int32_t *aslot,
+             int32_t *hval, int32_t *vslot, uint32_t cap, int capv, long long nwords, int nchunks) {
+    const int b = blockIdx.y;
+    const int V = vcount[b];
+    for (int v = blockIdx.x * blockDim.x + threadIdx.x; v < V; v += gridDim.x * blockDim.x) {
+        const size_t at = (size_t)b * capv + v;
+        const int k = vkey[at];
+        const uint2 w = words[b * nwords + (k >> 5)];
+        const int id = chunk_sum[(size_t)b * nchunks + (k >> 5) / kRenumChunk] + (int)w.y +
+                       __popc(w.x & ((1u << (k & 31)) - 1u));
+        vkey[at] = id;
+        const int slot = aslot[at];
+        hval[(size_t)b * cap + slot] = id;
+        vslot[(size_t)b * capv + id] = slot;
     }
 }
 
@@ -301,16 +420,20 @@ k_lattice_cleanup(uint64_t *hkeys, int32_t *hval, const int32_t *vslot, const in
 // Normalisation: norm = 1/sqrt(K 1 + 1e-20), pairwise.cpp:44,54-57, with K 1 evaluated like
 // Permutohedral::seqCompute(value_size=1) (permutohedral.cpp:476-527).
 // ---------------------------------------------------------------------------------------------
+// also finishes the renumbering: off still holds arrival-order ids, vkey maps them to the new ones (k_renum_rank)
 __global__ void __launch_bounds__(kThreads)
-k_norm_splat(const int32_t *off, const float *bary, const int32_t *rowbase, float *nv, int N,
-             int dp1) {
+k_norm_splat(int32_t *off, const float *bary, const int32_t *rowbase, const int32_t *vkey, float *nv, int N,
+             int dp1, int capv) {
     const int b = blockIdx.y;
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= N) return;
     const int base = rowbase[b];
+    const int32_t *perm = vkey + (size_t)b * capv;
     for (int r = 0; r < dp1; r++) {
         size_t at = ((size_t)b * dp1 + r) * N + i;
-        atomicAdd(nv + base + off[at], bary[at]);  // values[o] += w * 1 (:491)
+        const int row = perm[off[at] - 1] + 1;
+        off[at] = row;
+        atomicAdd(nv + base + row, bary[at]);  // values[o] += w * 1 (:491)
     }
 }
 
@@ -324,12 +447,14 @@ k_norm_blur(const float *in, float *out, const int2 *nbr, const int32_t *rowbase
     }
 }
 
+// also resets the renumbering keys for the next build (vkey is kNoKey between builds; k_norm_splat was its last reader)
 __global__ void __launch_bounds__(kThreads)
 k_norm_slice(const int32_t *off, const float *bary, const int32_t *rowbase, const float *nv,
-             float *norm, int N, int dp1, float alpha) {
+             float *norm, int N, int dp1, float alpha, int32_t *vkey, const int32_t *vcount, int capv) {
     const int b = blockIdx.y;
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= N) return;
+    for (int v = i, V = vcount[b]; v < V; v += N) vkey[(size_t)b * capv + v] = kNoKey;
     const int base = rowbase[b];
     float acc = 0.0f;
     for (int r = 0; r < dp1; r++) {
@@ -347,6 +472,9 @@ static int build_impl(Engine *e, Lattice &L, int nb, const uint8_t *image, cudaS
     a.N = L.N;
     a.P = L.P;
     a.W = e->W;
+    a.tile_w = e->tile_w;
+    a.tiles_x = e->tiles_x;
+    a.ntiles = e->ntiles;
     a.cap = (uint32_t)L.cap;
     a.capv = L.capv;
     for (int i = 0; i < 5; i++) {
@@ -358,18 +486,29 @@ static int build_impl(Engine *e, Lattice &L, int nb, const uint8_t *image, cudaS
     a.bary = L.bary;
     a.hkeys = L.hkeys;
     a.hval = L.hval;
-    a.vslot = L.vslot;
+    a.aslot = L.aslot;
     a.vcount = L.vcount;
+    a.vkey = L.vkey;
     a.err = e->dev_err;
     DSRG_CUDA_TRY(cudaMemsetAsync(L.vcount, 0, sizeof(int32_t) * nb, s));
+    const long long nwords = renum_words(e->ntiles, D + 1);
+    const int nchunks = (int)(nwords / kRenumChunk);
+    DSRG_CUDA_TRY(cudaMemsetAsync(L.rn_words, 0, sizeof(uint2) * nb * nwords, s));
     dim3 gp(cdiv(L.N + L.P, kThreads), nb);
     DSRG_LAUNCH(e, T_LAT_INSERT, s, k_lattice_insert<D><<<gp, kThreads, 0, s>>>(a));
     DSRG_LAUNCH(e, T_LAT_MISC, s, k_rowbase<<<1, 32, 0, s>>>(L.vcount, L.rowbase, L.shared ? e->maxB : nb, L.shared));
     dim3 gv(2 * e->sm_count, nb);
+    DSRG_LAUNCH(e, T_LAT_MISC, s, k_renum_mark<<<gv, kThreads, 0, s>>>(L.vcount, L.vkey, L.rn_words, L.capv, nwords));
+    DSRG_LAUNCH(e, T_LAT_MISC, s, k_renum_scan<<<dim3(nchunks, nb), kThreads, 0, s>>>(L.rn_words, L.rn_chunk, nwords, nchunks));
+    DSRG_LAUNCH(e, T_LAT_MISC, s, k_renum_chunks<<<nb, kThreads, 0, s>>>(L.rn_chunk, nchunks));
+    DSRG_LAUNCH(e, T_LAT_MISC, s,
+                k_renum_rank<<<gv, kThreads, 0, s>>>(L.vcount, L.vkey, L.rn_words, L.rn_chunk, L.aslot, L.hval, L.vslot,
+                                                     a.cap, L.capv, nwords, nchunks));
     DSRG_LAUNCH(e, T_LAT_MISC, s,
                 k_lattice_neighbors<D><<<gv, kThreads, 0, s>>>(L.hkeys, L.hval, L.vslot, L.vcount, L.rowbase,
                                                                L.nbr, L.nbr_stride, a.cap, L.capv, L.shared));
-    DSRG_LAUNCH(e, T_LAT_MISC, s, k_lattice_cleanup<<<gv, kThreads, 0, s>>>(L.hkeys, L.hval, L.vslot, L.vcount, a.cap, L.capv));
+    DSRG_LAUNCH(e, T_LAT_MISC, s,
+                k_lattice_cleanup<<<gv, kThreads, 0, s>>>(L.hkeys, L.hval, L.vslot, L.vcount, a.cap, L.capv));
     return DSRG_OK;
 }
 
@@ -384,7 +523,7 @@ int lattice_build(Engine *e, Lattice &L, int B, const uint8_t *image_dev, cudaSt
     const long long rows_nb = L.shared ? (long long)L.capv + 1 : L.rows_cap;
     DSRG_CUDA_TRY(cudaMemsetAsync(e->nvA, 0, sizeof(float) * rows_nb, s));
     dim3 gp(cdiv(L.N, kThreads), nb);
-    DSRG_LAUNCH(e, T_LAT_NORM, s, k_norm_splat<<<gp, kThreads, 0, s>>>(L.off, L.bary, L.rowbase, e->nvA, L.N, dp1));
+    DSRG_LAUNCH(e, T_LAT_NORM, s, k_norm_splat<<<gp, kThreads, 0, s>>>(L.off, L.bary, L.rowbase, L.vkey, e->nvA, L.N, dp1, L.capv));
     float *src = e->nvA, *dst = e->nvB;
     for (int j = 0; j < dp1; j++) {
         DSRG_LAUNCH(e, T_LAT_NORM, s,
@@ -395,7 +534,8 @@ int lattice_build(Engine *e, Lattice &L, int B, const uint8_t *image_dev, cudaSt
         dst = t;
     }
     const float alpha = 1.0f / (1 + powf(2, -L.d));  // permutohedral.cpp:510
-    DSRG_LAUNCH(e, T_LAT_NORM, s, k_norm_slice<<<gp, kThreads, 0, s>>>(L.off, L.bary, L.rowbase, src, L.norm, L.N, dp1, alpha));
+    DSRG_LAUNCH(e, T_LAT_NORM, s, k_norm_slice<<<gp, kThreads, 0, s>>>(L.off, L.bary, L.rowbase, src, L.norm, L.N, dp1, alpha,
+                                                                       L.vkey, L.vcount, L.capv));
     DSRG_CUDA_TRY(cudaGetLastError());
     // the tile-local views serve the fused kernel (up to DSRG_MAX_LABELS labels); the wide path only needs bary * norm
     return e->MP > DSRG_MAX_LABELS ? wide_weights(e, L, nb, s) : tiles_build(e, L, nb, s);

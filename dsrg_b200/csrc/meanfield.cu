@@ -691,20 +691,31 @@ __device__ __forceinline__ void blur_reduce(float4 *v) {
     for (int i = 0; i < N; i++) v[i] = blur_step(v[3 * i], v[3 * i + 1], v[3 * i + 2]);
 }
 
-// A pair pass gets 64 registers (4 CTAs per SM) so that all its row loads are in flight at once.  At 32
-// registers (full occupancy) the 9 loads of a pair go out in batches: faster on lattices that stay in the L2,
-// but on large scattered ones (uniform-noise images, ~176 k bilateral vertices per image) each batch waits on
-// HBM and the pair pass cost 2.1x a single-axis pass instead of 1.65x (H100 SXM, 400 W).
-template <int MP, int AX>
-__global__ void __launch_bounds__(kThreads, AX == 1 ? 8 : 4)
+// A pair pass over a large scattered lattice (uniform-noise images, ~176 k bilateral vertices per image) gets 64
+// registers (4 CTAs per SM) so that all its row loads are in flight at once: at 32 registers (full occupancy) the 9
+// loads go out in batches, each batch waits on HBM, and the pair pass cost 2.1x a single-axis pass instead of 1.65x
+// (H100 SXM, 400 W).  Where the rows a pass reads mostly hit in the caches (smooth and photo-like images on the
+// tile-major numbering, lattice.cu) full occupancy is faster.  The vertex counts live on the device, so a bilateral
+// pair pass launches both (blur_all) and `gate` lets the one that fits run: 1 = at most kBlurCachedRows rows per
+// image on average, 2 = more, 0 = always.
+#ifndef DSRG_BLUR_CACHED_ROWS
+#define DSRG_BLUR_CACHED_ROWS 65536
+#endif
+constexpr int kBlurCachedRows = DSRG_BLUR_CACHED_ROWS;
+// CTAs per SM of the full-occupancy pair pass: at 32 registers ptxas spills a few bytes for MP = 4, 12 and 28, at 40
+// (6 CTAs) none
+__host__ __device__ constexpr int blur_cached_ctas(int mp) { return (mp == 4 || mp == 12 || mp == 28) ? 6 : 8; }
+template <int MP, int AX, int CTAS>
+__global__ void __launch_bounds__(kThreads, CTAS)
 k_mf_blur(const float4 *in, float4 *out, const int2 *nbr, long long nbr_stride, const int32_t *rowbase, int B,
-          int shared, float4 *zero) {
+          int shared, float4 *zero, int gate) {
     constexpr int CH = MP / 4;
     constexpr int K = AX == 1 ? 3 : 9;  // rows of `in` per output row
     static_assert(AX == 1 || AX == 2, "one or two axes per pass");
     // r0 = rowbase[0] is 0.  Without it the compiler unswitches the loop on `shared` and reorders the row loads,
     // which made the bilateral blur 9 % slower on uniform-noise images (H100 SXM, 400 W)
     const long long r0 = rowbase[0], rows = rowbase[B] - r0;
+    if (gate && (rows > (long long)kBlurCachedRows * B) != (gate == 2)) return;
     const int rows_img = shared ? rowbase[1] : 0;
     const long long total = rows * CH;
     for (long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x; t < total;
@@ -813,7 +824,9 @@ static TileLat make_tile_view(const Lattice &L, const float *val_in, float *val_
 // lives.  A pass streams its source and destination buffers through HBM (at batch 64 @ 321² each lattice's
 // buffers are ~80 MB, beyond the L2), so a pair halves that traffic for 3x the row reads, most of which the
 // caches serve.  On an H100 SXM at a 400 W limit the blur of a dsrg321 step went from 6.6 to 5.2 ms; one
-// three-axis spatial pass (27 rows) was slower than pair + single.
+// three-axis spatial pass (27 rows) was slower than pair + single.  Re-measured on the tile-major vertex numbering
+// (lattice.cu), same card and limit: three-axis passes (spatial one pass, bilateral two, 2 CTAs per SM) took 6.1 ms
+// against 4.6 for this grouping.  Bilateral pair passes pick their occupancy by the lattice's size (k_mf_blur).
 template <int MP>
 static float *blur_all(Engine *e, const Lattice &L, float *buf, float *tmp, float *dead, int B, int tag, int grid,
                        cudaStream_t s) {
@@ -822,12 +835,21 @@ static float *blur_all(Engine *e, const Lattice &L, float *buf, float *tmp, floa
         const float4 *in = (const float4 *)src;
         const int2 *nbr = L.nbr + (size_t)j * L.nbr_stride;
         float4 *zero = j == 0 ? (float4 *)dead : nullptr;
-        if (j < L.d)
-            DSRG_LAUNCH(e, tag, s, (k_mf_blur<MP, 2><<<grid, kThreads, 0, s>>>(in, (float4 *)dst, nbr, L.nbr_stride,
-                                                                             L.rowbase, B, L.shared, zero)));
-        else
-            DSRG_LAUNCH(e, tag, s, (k_mf_blur<MP, 1><<<grid, kThreads, 0, s>>>(in, (float4 *)dst, nbr, L.nbr_stride,
-                                                                             L.rowbase, B, L.shared, zero)));
+        if (j == L.d) {
+            DSRG_LAUNCH(e, tag, s, (k_mf_blur<MP, 1, 8><<<grid, kThreads, 0, s>>>(in, (float4 *)dst, nbr, L.nbr_stride,
+                                                                                L.rowbase, B, L.shared, zero, 0)));
+        } else if (L.shared) {  // the spatial lattice: ~13.5 k rows per image at 321², always cached
+            DSRG_LAUNCH(e, tag, s, (k_mf_blur<MP, 2, 4><<<grid, kThreads, 0, s>>>(in, (float4 *)dst, nbr, L.nbr_stride,
+                                                                                L.rowbase, B, L.shared, zero, 0)));
+        } else if (L.capv <= kBlurCachedRows) {  // no image of this size can have more rows
+            DSRG_LAUNCH(e, tag, s, (k_mf_blur<MP, 2, blur_cached_ctas(MP)><<<grid, kThreads, 0, s>>>(
+                                       in, (float4 *)dst, nbr, L.nbr_stride, L.rowbase, B, L.shared, zero, 0)));
+        } else {
+            DSRG_LAUNCH(e, tag, s, (k_mf_blur<MP, 2, blur_cached_ctas(MP)><<<grid, kThreads, 0, s>>>(in, (float4 *)dst, nbr, L.nbr_stride,
+                                                                                L.rowbase, B, L.shared, zero, 1)));
+            DSRG_LAUNCH(e, tag, s, (k_mf_blur<MP, 2, 4><<<grid, kThreads, 0, s>>>(in, (float4 *)dst, nbr, L.nbr_stride,
+                                                                                L.rowbase, B, L.shared, zero, 2)));
+        }
         float *t = src;
         src = dst;
         dst = t;

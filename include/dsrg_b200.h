@@ -446,6 +446,11 @@ int dsrg_engine_profile_read(dsrg_engine *e, float *ms_out, long long *count_out
 /* Introspection used by the lattice-level parity tests: vertex counts of the lattices built by
  * the last CRF call (spatial, then bilateral per image); either pointer may be NULL. */
 int dsrg_engine_lattice_sizes(dsrg_engine *e, int B, int *v_spatial_out, int *v_bilateral_out);
+/* Image b's lattice tables of the last CRF call (which = 0 spatial, shared by the batch; 1 bilateral), in the
+ * engine's vertex numbering: off_out [d+1][N] the 1-based row of every (r, pixel) (0 is the zero row), nbr_out
+ * [d+1][V+1][2] the two blur neighbours of rows 0..V (V from dsrg_engine_lattice_sizes) as rows of the same image,
+ * 0 for a missing one.  Either pointer may be NULL.  For tests. */
+int dsrg_engine_lattice_tables(dsrg_engine *e, int which, int b, int *off_out, int *nbr_out);
 /* Per-pixel symmetric normalisation vectors (DenseKernel::norm_, pairwise.cpp:54-57) of the
  * last CRF call: which = 0 spatial [N] (shared by the batch), 1 bilateral [B][N]. */
 int dsrg_engine_copy_norm(dsrg_engine *e, int which, int B, float *norm_out_host);
