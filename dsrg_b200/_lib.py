@@ -80,6 +80,10 @@ SIGNATURES = {
     "dsrg_annotation_coco_forward_dev": (_i, [_vp, _vp, _vp, _vp, _i, _vp, _vp, _i, _i, _vp, _i, _vp, _vp, _vp, _vp,
                                               _vp]),
     "dsrg_annotation_coco_forward_host": (_i, [_vp, _vp, _vp, _vp, _i, _vp, _vp, _i, _i, _vp, _i, _vp, _vp, _vp]),
+    "dsrg_seg_data_forward_dev": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _vp, _vp, _vp, _i, _i, _vp, _f, _i, _i,
+                                       _vp, _vp, _vp]),
+    "dsrg_seg_data_forward_host": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _vp, _vp, _vp, _i, _i, _vp, _f, _i, _i,
+                                        _vp, _vp]),
     "dsrg_confusion_create": (_vp, [_i, _i]),
     "dsrg_confusion_destroy": (None, [_vp]),
     "dsrg_confusion_reset": (_i, [_vp, _vp]),

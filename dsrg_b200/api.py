@@ -527,6 +527,83 @@ class Engine(object):
             _stream(stream)))
         return labels_out, cues_out, images_out
 
+    # ---- ImageSegDataLayer.forward (layer.py:51-61, SimpleTransformer :147-236) ----
+    @staticmethod
+    def _seg_args(image_shapes, label_shapes, h_off, w_off, flip, mean):
+        B = len(image_shapes)
+        ints = lambda v: (C.c_int * B)(*[int(x) for x in v])  # noqa: E731
+        if len(h_off) != B or len(w_off) != B or (label_shapes is not None and len(label_shapes) != B):
+            raise ValueError("labels, h_off and w_off must have one entry per image")
+        Hs, Ws = ints(s[0] for s in image_shapes), ints(s[1] for s in image_shapes)
+        Hl = Wl = None
+        if label_shapes is not None:
+            Hl, Wl = ints(s[0] for s in label_shapes), ints(s[1] for s in label_shapes)
+        fl = None if flip is None else np.ascontiguousarray(flip, np.int32)
+        if fl is not None and fl.shape != (B,):
+            raise ValueError("flip must have one entry per image")
+        mean = np.ascontiguousarray(mean, np.float64)
+        if mean.shape != (3,):
+            raise ValueError("mean must have 3 elements")
+        return B, Hs, Ws, Hl, Wl, ints(h_off), ints(w_off), fl, mean
+
+    def seg_data_forward_host(self, images, labels, h_off, w_off, crop_size, mean, scale=1.0, flip=None,
+                              swap_rb=False, pad_label=255, out=None):
+        """images: B (H_b, W_b, 3) uint8 BGR arrays; labels: B (Hl_b, Wl_b) uint8 arrays, or None for the image-only
+        paths; h_off, w_off: per image the window's corner in the padded arrays; flip: B 0/1 flags or None ->
+        (images (B, 3, crop_h, crop_w), labels (B, 1, crop_h, crop_w) or None) float32, written into `out` when it is
+        given (a pair of C-contiguous float32 arrays of those shapes, the second None without labels).  pad_label is
+        the byte the label is padded with, saturate_cast<uchar>(ignore_label)."""
+        for im in images:
+            _hptr(im, np.uint8)
+            if im.ndim != 3 or im.shape[2] != 3:
+                raise ValueError("every image must be an (H, W, 3) uint8 array")
+        if labels is not None:
+            for lab in labels:
+                _hptr(lab, np.uint8)
+                if lab.ndim != 2:
+                    raise ValueError("every label must be an (H, W) uint8 array")
+        B, Hs, Ws, Hl, Wl, ho, wo, fl, mean = self._seg_args(
+            [im.shape for im in images], None if labels is None else [lab.shape for lab in labels], h_off, w_off,
+            flip, mean)
+        crop_h, crop_w = (int(v) for v in crop_size)
+        if out is None:
+            out = (np.empty((B, 3, crop_h, crop_w), np.float32),
+                   None if labels is None else np.empty((B, 1, crop_h, crop_w), np.float32))
+        ptrs = (C.c_void_p * B)(*[im.ctypes.data for im in images])
+        lptrs = None if labels is None else (C.c_void_p * B)(*[lab.ctypes.data for lab in labels])
+        check(self._L.dsrg_seg_data_forward_host(
+            self.h, ptrs, Hs, Ws, lptrs, Hl, Wl, B, ho, wo, _hptr(fl, np.int32), crop_h, crop_w,
+            _hptr(mean, np.float64), float(scale), int(bool(swap_rb)), int(pad_label), _hptr(out[0], np.float32),
+            _hptr(out[1], np.float32)))
+        return out
+
+    def seg_data_forward_dev(self, images, labels, h_off, w_off, images_out, labels_out, mean, scale=1.0, flip=None,
+                             swap_rb=False, pad_label=255, stream=None):
+        """images: B (H_b, W_b, 3) uint8 CUDA tensors; labels: B (Hl_b, Wl_b) uint8 CUDA tensors or None;
+        images_out (B, 3, crop_h, crop_w), giving the crop size, and labels_out (B, 1, crop_h, crop_w) or None: float32
+        CUDA tensors."""
+        import torch
+        for im in images:
+            if im.dtype != torch.uint8 or im.dim() != 3 or im.shape[2] != 3:
+                raise ValueError("every image must be an (H, W, 3) uint8 tensor")
+        if labels is not None:
+            for lab in labels:
+                if lab.dtype != torch.uint8 or lab.dim() != 2:
+                    raise ValueError("every label must be an (H, W) uint8 tensor")
+        if images_out.dim() != 4:
+            raise ValueError("images_out must be a (B, 3, crop_h, crop_w) tensor")
+        B, Hs, Ws, Hl, Wl, ho, wo, fl, mean = self._seg_args(
+            [im.shape for im in images], None if labels is None else [lab.shape for lab in labels], h_off, w_off,
+            flip, mean)
+        ptrs = (C.c_void_p * B)(*[_dptr(im).value for im in images])
+        lptrs = None if labels is None else (C.c_void_p * B)(*[_dptr(lab).value for lab in labels])
+        crop_h, crop_w = (int(v) for v in images_out.shape[2:])
+        check(self._L.dsrg_seg_data_forward_dev(
+            self.h, ptrs, Hs, Ws, lptrs, Hl, Wl, B, ho, wo, _hptr(fl, np.int32), crop_h, crop_w,
+            _hptr(mean, np.float64), float(scale), int(bool(swap_rb)), int(pad_label), _dptr(images_out),
+            _dptr(labels_out), _stream(stream)))
+        return images_out, labels_out
+
     # ---- per-kernel timing ----
     def profile(self, enable):
         check(self._L.dsrg_engine_profile(self.h, int(bool(enable))))

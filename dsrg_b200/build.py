@@ -12,7 +12,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIBDIR = os.path.join(HERE, "lib")
 LIB = os.path.join(LIBDIR, "libdsrg_b200.so")
-SOURCES = ["api.cu", "graph.cu", "lattice.cu", "tiles.cu", "meanfield.cu", "meanfield_wide.cu", "srg.cu", "loss.cu", "sec_loss.cu", "wire.cu", "numa.cu", "prep.cu", "post.cu", "annot.cu", "eval.cu"]
+SOURCES = ["api.cu", "graph.cu", "lattice.cu", "tiles.cu", "meanfield.cu", "meanfield_wide.cu", "srg.cu", "loss.cu", "sec_loss.cu", "wire.cu", "numa.cu", "prep.cu", "post.cu", "annot.cu", "segdata.cu", "eval.cu"]
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 NVCC_FLAGS = ARCH + ["-lineinfo", "-O3", "-std=c++17",
               "-Xcompiler", "-fPIC,-fopenmp", "--fmad=true"]

@@ -300,7 +300,7 @@ using namespace dsrg;
 
 extern "C" {
 
-int dsrg_version(void) { return 105; }
+int dsrg_version(void) { return 106; }
 
 const char *dsrg_last_error(void) { return g_err; }
 

@@ -16,6 +16,8 @@ in train-s.prototxt:746-812 keeps working:
   -> dsrg_seedloss_plain_* / dsrg_expandloss_*.
 * ``AnnotationLayer`` / ``AnnotationLayerCOCO`` (pylayers.py:346-387, :389-512), the VOC and COCO training inputs
   -> dsrg_annotation_forward_* / dsrg_annotation_coco_forward_*.
+* The package's ``layer`` submodule (pylayers/pylayers/layer.py) holds ``ImageSegDataLayer``, the stage-2 training
+  input of train-f.prototxt -> dsrg_seg_data_forward_*; it reads its files through ``_read`` / ``_imread`` below.
 
 The blobs Caffe hands to a Python layer are host numpy views, so the ``*_host`` entry points of
 the C ABI are used: one H2D of the bottoms and one D2H of the tops per call, everything else --

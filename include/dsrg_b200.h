@@ -314,6 +314,39 @@ int dsrg_annotation_coco_forward_host(dsrg_engine *e, const uint8_t *const *imag
                                       int new_h, int new_w, const double *mean_pixel /* host, 3 */, int ignore_label,
                                       float *labels_out_host, float *cues_out_host, float *images_out_host);
 
+/*
+ * ImageSegDataLayer.forward (pylayers/pylayers/layer.py:51-61, SimpleTransformer.preprocess :169-236), the stage-2
+ * training input of training/experiment/seed_mc/train-f.prototxt, after the caller has decoded the files and drawn
+ * the random numbers (the shuffle, the two randints and the mirror) in the reference's order.  Per image b:
+ *   images[b] : [Hs[b]][Ws[b]][3] uint8 BGR, as cv2.imread(..., IMREAD_COLOR) returns it; each image has its own size
+ *   labels[b] : [Hl[b]][Wl[b]] uint8, as cv2.imread(..., IMREAD_GRAYSCALE) returns it.  labels == NULL: image only
+ *               (preprocess(image), pre_test_image); Hl, Wl and labels_out are then not read
+ *   h_off[b], w_off[b] : top-left corner of the crop_h x crop_w window in the padded arrays
+ *   flip [B] or NULL : 1 = the window is read right to left (flip == -1, :231-234)
+ * The padding is max(crop - size, 0) rows and columns at the bottom and right, from the label's size (the image's
+ * without labels); the image gets the same.  ->
+ *   images_out : [B][3][crop_h][crop_w] float32: float32(double(v) - mean[c]) * float32 scale inside the image
+ *                (channel 2 - c of the pixel when swap_rb, else channel c), 0.0 in the padding
+ *   labels_out : [B][1][crop_h][crop_w] float32: the label inside it, pad_label in the padding.  pad_label is
+ *                saturate_cast<uchar>(ignore_label), what cv2.copyMakeBorder pads a uint8 label with
+ * The arrays of pointers, sizes, offsets, flip and mean live on the host in both variants.  The images are read
+ * through a table in device memory, so B is bounded by the engine only; the engine's shape, labels and retained
+ * marginals are neither read nor changed, so the smallest engine (1 x 1, one label, max_batch = B) serves.
+ * A negative offset, a window that leaves the padded image or the padded label (where the reference's slice comes
+ * back short and numpy refuses to store it) or a pad_label outside 0..255 returns DSRG_E_INVALID before any copy or
+ * launch.
+ */
+int dsrg_seg_data_forward_dev(dsrg_engine *e, const uint8_t *const *images_dev, const int *Hs, const int *Ws,
+                              const uint8_t *const *labels_dev, const int *Hl, const int *Wl, int B, const int *h_off,
+                              const int *w_off, const int32_t *flip, int crop_h, int crop_w,
+                              const double *mean /* host, 3 */, float scale, int swap_rb, int pad_label,
+                              float *images_out_dev, float *labels_out_dev, void *stream);
+int dsrg_seg_data_forward_host(dsrg_engine *e, const uint8_t *const *images_host, const int *Hs, const int *Ws,
+                               const uint8_t *const *labels_host, const int *Hl, const int *Wl, int B,
+                               const int *h_off, const int *w_off, const int32_t *flip, int crop_h, int crop_w,
+                               const double *mean /* host, 3 */, float scale, int swap_rb, int pad_label,
+                               float *images_out_host, float *labels_out_host);
+
 /* ------------------------------------------------------------------------------------------
  * Confusion matrix of a segmentation run, the scoring step of the evaluation tools:
  *   ConfusionMatrix (training/tools/evaluate.py:17-68, ap.py:19-72); its generateM (:61-68 / :65-72) counts
