@@ -94,7 +94,9 @@ SIGNATURES = {
     "dsrg_wire_unpack_mask": (None, [_vp, _vp, _sz]),
     "dsrg_wire_apply_clamp_mask": (None, [_vp, _vp, _sz]),
     "dsrg_crflayer_forward_host": (_i, [_vp, _i, _vp, _vp, _pp, _vp, _vp]),
+    "dsrg_crflayer_backward_dev": (_i, [_vp, _vp, _vp, _i, _vp, _vp]),
     "dsrg_srg_last_crf_host": (_i, [_vp, _i, _vp, _vp, _d, _d, _vp]),
+    "dsrg_srg_last_crf_dev": (_i, [_vp, _vp, _vp, _i, _d, _d, _vp, _vp]),
     "dsrg_crf_last_marginals_host": (_i, [_vp, _i, _vp, _i]),
     "dsrg_seedloss_forward_host": (_i, [_vp, _i, _vp, _vp, _vp]),
     "dsrg_seedloss_backward_host": (_i, [_vp, _i, _i, _vp, _vp, _f, _vp]),

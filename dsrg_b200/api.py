@@ -165,6 +165,42 @@ class Engine(object):
                                                 _dptr(log_out), _dptr(result), _stream(stream)))
         return log_out
 
+    def crflayer_backward_dev(self, result, top_diff, grad_out, stream=None):
+        """CRFLayer.backward: grad_out = (1 - result) * top_diff in float32, bit-identical to numpy."""
+        B = result.shape[0]
+        check(self._L.dsrg_crflayer_backward_dev(self.h, _dptr(result), _dptr(top_diff), B, _dptr(grad_out),
+                                                 _stream(stream)))
+        return grad_out
+
+    def srg_last_crf_dev(self, labels, cues, th1, th2, seeds_out, stream=None):
+        """SRG on the marginals of this engine's last CRF pass, on device arrays (one refinement, two consumers)."""
+        B = cues.shape[0]
+        check(self._L.dsrg_srg_last_crf_dev(self.h, _dptr(labels), _dptr(cues), B, float(th1), float(th2),
+                                            _dptr(seeds_out), _stream(stream)))
+        return seeds_out
+
+    # ---- SoftmaxLayer / ConstrainLossLayer (device arrays) ----
+    def softmax_forward_dev(self, preds, probs_out, stream=None):
+        check(self._L.dsrg_softmax_forward_dev(self.h, preds.shape[0], _dptr(preds), _dptr(probs_out),
+                                               _stream(stream)))
+        return probs_out
+
+    def softmax_backward_dev(self, preds, top_diff, grad_out, stream=None):
+        check(self._L.dsrg_softmax_backward_dev(self.h, preds.shape[0], _dptr(preds), _dptr(top_diff),
+                                                _dptr(grad_out), _stream(stream)))
+        return grad_out
+
+    def constrainloss_forward_dev(self, probs, log_smooth, loss_out, stream=None):
+        """loss_out: one float32 on the device."""
+        check(self._L.dsrg_constrainloss_forward_dev(self.h, probs.shape[0], _dptr(probs), _dptr(log_smooth),
+                                                     _dptr(loss_out), _stream(stream)))
+        return loss_out
+
+    def constrainloss_backward_dev(self, probs, log_smooth, grad_probs, grad_log, stream=None):
+        check(self._L.dsrg_constrainloss_backward_dev(self.h, probs.shape[0], _dptr(probs), _dptr(log_smooth),
+                                                      _dptr(grad_probs), _dptr(grad_log), _stream(stream)))
+        return grad_probs, grad_log
+
     def seedloss_forward_dev(self, probs, seeds, terms_out, stream=None):
         B = probs.shape[0]
         check(self._L.dsrg_seedloss_forward_dev(self.h, B, _dptr(probs), _dptr(seeds), _dptr(terms_out), _stream(stream)))

@@ -300,7 +300,7 @@ using namespace dsrg;
 
 extern "C" {
 
-int dsrg_version(void) { return 106; }
+int dsrg_version(void) { return 107; }
 
 const char *dsrg_last_error(void) { return g_err; }
 
@@ -724,6 +724,16 @@ int dsrg_srg_last_crf_host(dsrg_engine *h, int B, const float *labels, const flo
         DSRG_CUDA_TRY(cudaMemcpyAsync(seeds_out, e->st_out, n * sizeof(float), cudaMemcpyDeviceToHost, s));
         return DSRG_OK;
     }, last_crf_held);
+}
+
+int dsrg_srg_last_crf_dev(dsrg_engine *h, const float *labels, const float *cues, int B, double th1, double th2,
+                          float *seeds_out, void *stream) {
+    const cudaStream_t s = (cudaStream_t)stream;
+    return dev_call(h, B, s, labels && cues && seeds_out, [&](Engine *e) {
+        if (int rc = last_crf_held(e, B)) return rc;
+        // the device twin of the host entry point above: same kernels, queued behind the pass on the caller's stream
+        return srg_run(e, B, labels, e->Qcur, cues, th1, th2, 1, seeds_out, nullptr, s);
+    });
 }
 
 int dsrg_crf_last_marginals_host(dsrg_engine *h, int B, float *out, int out_layout) {

@@ -238,6 +238,23 @@ k_constrain_bwd(const float *probs, const float *logs, float *gp, float *gl, lon
     }
 }
 
+// CRFLayer.backward (pylayers.py:90-92): grad = (1 - result) * top_diff.  numpy evaluates it in float32, one rounding
+// per operation; the explicit _rn intrinsics keep nvcc from contracting the pair into an FMA.
+__global__ void __launch_bounds__(kThreads)
+k_crflayer_bwd(const float *result, const float *top, float *grad, long long total) {
+    for (long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x; t < total;
+         t += (long long)gridDim.x * blockDim.x)
+        grad[t] = __fmul_rn(__fsub_rn(1.0f, result[t]), top[t]);
+}
+
+int crflayer_backward(Engine *e, int B, const float *result, const float *top, float *grad, cudaStream_t s) {
+    const long long total = (long long)B * e->M * e->N;
+    const int grid = (int)(cdiv(total, kThreads) < 8 * e->sm_count ? cdiv(total, kThreads) : 8 * e->sm_count);
+    DSRG_LAUNCH(e, T_LOSS, s, k_crflayer_bwd<<<grid, kThreads, 0, s>>>(result, top, grad, total));
+    DSRG_CUDA_TRY(cudaGetLastError());
+    return DSRG_OK;
+}
+
 static int narrow_only(const Engine *e, const char *what) {
     if (e->M <= DSRG_MAX_LABELS) return DSRG_OK;
     set_error("%s supports at most %d labels (engine has %d)", what, DSRG_MAX_LABELS, e->M);
@@ -340,6 +357,12 @@ int dsrg_constrainloss_backward_dev(dsrg_engine *h, int B, const float *probs, c
     const cudaStream_t s = (cudaStream_t)stream;
     return dev_call(h, B, s, probs && log_smooth && grad_probs && grad_log,
                     [&](Engine *e) { return constrain_backward(e, B, probs, log_smooth, grad_probs, grad_log, s); });
+}
+int dsrg_crflayer_backward_dev(dsrg_engine *h, const float *result, const float *top_diff, int B, float *grad_out,
+                               void *stream) {
+    const cudaStream_t s = (cudaStream_t)stream;
+    return dev_call(h, B, s, result && top_diff && grad_out,
+                    [&](Engine *e) { return crflayer_backward(e, B, result, top_diff, grad_out, s); });
 }
 int dsrg_softmax_forward_host(dsrg_engine *h, int B, const float *preds, float *probs_out) {
     return host_call(h, B, preds && probs_out, false, [&](Engine *e, cudaStream_t s) {

@@ -396,6 +396,14 @@ int dsrg_crflayer_forward_dev(dsrg_engine *e, int B, float *probs_dev, const uin
 int dsrg_crflayer_forward_host(dsrg_engine *e, int B, float *probs_host, const uint8_t *image_host,
                                const dsrg_crf_params *params, float *log_out_host,
                                float *result_host);
+/*
+ * CRFLayer.backward (pylayers.py:90-92): grad = (1 - result) * top_diff over [B][M][H][W] float32, each element
+ * rounded like numpy's float32 arithmetic (no contraction to FMA), so it is bit-identical to the reference's
+ * statement on the same arrays.  result_dev is what dsrg_crflayer_forward_dev wrote to its `result` argument; the
+ * batch size follows the two arrays it describes.
+ */
+int dsrg_crflayer_backward_dev(dsrg_engine *e, const float *result_dev, const float *top_diff_dev, int B,
+                               float *grad_out_dev, void *stream);
 
 /*
  * One refinement, two consumers.  In the reference's net CRFLayer and DSRGLayer are fed the same two blobs
@@ -404,11 +412,16 @@ int dsrg_crflayer_forward_host(dsrg_engine *e, int B, float *probs_host, const u
  * use them instead of repeating the pass:
  *   dsrg_srg_last_crf_host       : generate_seed_step over the batch on those marginals (float64 clamp +
  *                                  renormalisation fused in, exactly what dsrg_dsrg_forward_* does after its CRF)
+ *   dsrg_srg_last_crf_dev        : the same on device arrays, queued on the caller's stream (no host
+ *                                  synchronisation; labels [B][M], cues / seeds_out [B][M][H][W]); the batch
+ *                                  size follows the arrays it describes
  *   dsrg_crf_last_marginals_host : the raw float32 marginals themselves
- * Both return DSRG_E_STATE unless the engine's last pass was a CRF over exactly B images.
+ * All return DSRG_E_STATE unless the engine's last pass was a CRF over exactly B images.
  */
 int dsrg_srg_last_crf_host(dsrg_engine *e, int B, const float *labels_host, const float *cues_host, double th1,
                            double th2, float *seeds_out_host);
+int dsrg_srg_last_crf_dev(dsrg_engine *e, const float *labels_dev, const float *cues_dev, int B, double th1,
+                          double th2, float *seeds_out_dev, void *stream);
 int dsrg_crf_last_marginals_host(dsrg_engine *e, int B, float *out_host, int out_layout);
 
 /*
