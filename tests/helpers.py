@@ -53,6 +53,105 @@ WIDE_SHAPES = {"smooth": (29, 37), "noise": (19, 23)}
 RENORM_M = [1, 7, 8, 9, 16, 17, 21, 32, 33, 127, 128, 129, 136, 255]
 
 
+def oracle_batch(image, unary, sf, n_iters=10):
+    from oracle import crf_oracle
+    return np.stack([crf_oracle.CRF(image[b], unary[b], n_iters, sf) for b in range(image.shape[0])])
+
+
+def crf_both_layouts(torch, eng, unary, image, params):
+    """crf_dev on NHWC unaries (init kernel) and on NCHW ones (read in place by the tile kernel); both NHWC out."""
+    from dsrg_b200 import api
+    d_im = torch.from_numpy(image).cuda()
+    d_un = torch.from_numpy(unary).cuda()
+    d_out = torch.empty_like(d_un)
+    eng.crf_dev(d_un, d_im, params, d_out)
+    nhwc = d_out.cpu().numpy()
+    d_nchw = d_un.permute(0, 3, 1, 2).contiguous()
+    d_out2 = torch.empty_like(d_nchw)
+    eng.crf_dev(d_nchw, d_im, params, d_out2, api.LAYOUT_NCHW, api.LAYOUT_NCHW)
+    return nhwc, d_out2.permute(0, 2, 3, 1).cpu().numpy()
+
+
+# ---- scale: the cases of test_gpu_scale.py (checked on the CPU by test_scale_cpu.py) ----
+# bench.py's workloads restated, not imported (test_scale_cpu.py pins them to bench.py's literals)
+BENCH_WORKLOADS = {
+    #            H    W    B   what
+    "train41": (41, 41, 20, "crf+srg"),
+    "dsrg321": (321, 321, 64, "crf+srg"),
+    "crf321": (321, 321, 64, "crf"),
+    "full513": (513, 513, 16, "crf+srg+loss"),
+}
+BENCH_M, BENCH_T_ITERS, BENCH_TH, BENCH_CF, BENCH_UNIQUE = 21, 10, (0.99, 0.85), 13, 8
+
+
+def bench_sf(workload):
+    return 12.0 if workload == "train41" else 1.0
+
+
+# (workload, image variant, the branch of the bilateral pair blur the batch takes: see blur_branch)
+SCALE_CASES = [("dsrg321", "smooth", "gate1"), ("dsrg321", "photo", "gate1"), ("dsrg321", "noise", "gate2"),
+               ("crf321", "smooth", "gate1"), ("full513", "smooth", "gate1"), ("train41", "smooth", "ungated")]
+
+
+def bench_unique(workload, variant):
+    """The distinct problems of bench.py's batch: synth_batch repeats the first BENCH_UNIQUE cyclically."""
+    H, W, B, _ = BENCH_WORKLOADS[workload]
+    return synth.make_batch(min(B, BENCH_UNIQUE), H, W, cues="cam", image=variant)
+
+
+def sample_indices(B, seed):
+    """The images of a batch that are compared with the oracle: both ends, the middle and one seeded draw."""
+    return sorted({0, 1, B // 2, B - 2, B - 1, int(np.random.RandomState(seed).randint(2, B - 2))})
+
+
+# gate 2 of the bilateral pair blur at every padded label count: two noise images of 224 x 224 (~96 k rows each)
+GATE2_M = HYBRID_M
+GATE2_SHAPE, GATE2_SEED = (224, 224), 60
+# (name, H, W, image of each batch entry, branch): both sides of the device-side row gate and of the host-side
+# capacity switch
+SWITCH_CASES = [("mixed224", 224, 224, ("noise", "smooth"), "gate1"),
+                ("noise200", 200, 200, ("noise", "noise"), "gate2"),
+                ("noise104x105", 104, 105, ("noise", "noise"), "ungated"),
+                ("noise105x105", 105, 105, ("noise", "noise"), "gate1")]
+COCO_SHAPE, COCO_M = (427, 640), 81                 # DenseCRF(W, H, 81) of the COCO tool at a COCO image's size
+WIDE_BIG_SHAPE, WIDE_BIG_M = (105, 105), 255        # the most labels, on a lattice above the capacity switch
+
+
+def seeded_images(H, W, kinds, seed):
+    return np.stack([synth.make_image(np.random.RandomState(seed + b), H, W, k) for b, k in enumerate(kinds)])
+
+
+def blur_cached_rows():
+    """meanfield.cu's default kBlurCachedRows (DSRG_BLUR_CACHED_ROWS)."""
+    import re
+    src = open(os.path.join(os.path.dirname(os.path.abspath(__file__)), "..", "dsrg_b200", "csrc",
+                            "meanfield.cu")).read()
+    return int(re.search(r"#define\s+DSRG_BLUR_CACHED_ROWS\s+(\d+)\s*$", src, re.M).group(1))
+
+
+def blur_branch(H, W, vb):
+    """Which kernel runs the bilateral pair passes (meanfield.cu: blur_all, k_mf_blur) for a batch of H x W images
+    whose bilateral lattices have vb[b] vertices: "ungated" when no image of this size can have more than
+    kBlurCachedRows rows (capv = (N + P) * 6, P the phantom lanes of api.cu:lattice_shape), else "gate1" (full
+    occupancy) when the batch has at most kBlurCachedRows rows per image on average (a row per vertex plus each
+    image's zero row), "gate2" (4 CTAs per SM) when it has more."""
+    rows = blur_cached_rows()
+    N = H * W
+    if (N + (4 - N % 4) % 4) * 6 <= rows:
+        return "ungated"
+    return "gate2" if sum(int(v) + 1 for v in vb) > rows * len(vb) else "gate1"
+
+
+def bilateral_vertices(image, sf=1.0, cf=13):
+    """The oracle's bilateral lattice size of one (H,W,3) image (phantom lanes included, as the engine counts)."""
+    from oracle import crf_oracle
+    H, W = image.shape[:2]
+    c = crf_oracle.DenseCRF(W, H, 1)
+    c.set_unary_energy(np.zeros(H * W, np.float32))
+    c.add_pairwise_energy(10, 80 / sf, 80 / sf, cf, cf, cf, 3, 3 / sf, 3 / sf, image.ravel())
+    return int(c.lattice(1).M)
+
+
 def padded(M):
     """MP: the label count rounded up to the lane width of the value rows (api.cu)."""
     return (M + 3) // 4 * 4

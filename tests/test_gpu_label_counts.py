@@ -14,30 +14,13 @@ layers refuse M > 32 (DSRG_E_INVALID), which test_gpu_crf.py::test_label_count_l
 import numpy as np
 import pytest
 
-from helpers import (FUSED_CONFIGS, FUSED_ITER_M, HYBRID_M, MAX_FUSED, RENORM_M, WIDE_M, fused_images, hybrid_images,
-                     log_unary, predict_tile_paths, small_image, wide_images)
+from helpers import (FUSED_CONFIGS, FUSED_ITER_M, HYBRID_M, MAX_FUSED, RENORM_M, WIDE_M, crf_both_layouts,
+                     fused_images, hybrid_images, log_unary, oracle_batch, predict_tile_paths, small_image, wide_images)
 from dsrg_b200 import api
 from oracle import crf_oracle, loss_oracle, srg_oracle
 
 pytestmark = pytest.mark.gpu
 TOL = 1e-4
-
-
-def oracle_batch(image, unary, sf, n_iters=10):
-    return np.stack([crf_oracle.CRF(image[b], unary[b], n_iters, sf) for b in range(image.shape[0])])
-
-
-def crf_both_layouts(torch, eng, unary, image, params):
-    """crf_dev on NHWC unaries (init kernel) and on NCHW ones (read in place by the tile kernel); both NHWC out."""
-    d_im = torch.from_numpy(image).cuda()
-    d_un = torch.from_numpy(unary).cuda()
-    d_out = torch.empty_like(d_un)
-    eng.crf_dev(d_un, d_im, params, d_out)
-    nhwc = d_out.cpu().numpy()
-    d_nchw = d_un.permute(0, 3, 1, 2).contiguous()
-    d_out2 = torch.empty_like(d_nchw)
-    eng.crf_dev(d_nchw, d_im, params, d_out2, api.LAYOUT_NCHW, api.LAYOUT_NCHW)
-    return nhwc, d_out2.permute(0, 2, 3, 1).cpu().numpy()
 
 
 def assert_close(got, want, what):
