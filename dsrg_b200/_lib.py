@@ -75,6 +75,8 @@ SIGNATURES = {
     "dsrg_zoom_scores_host": (_i, [_vp, _vp, _i, _i, _vp, _i]),
     "dsrg_predict_mask_dev": (_i, [_vp, _i, _i, _vp, _vp, _vp, _vp, _f, _i, _pp, _vp, _i, _vp, _vp, _vp]),
     "dsrg_predict_mask_host": (_i, [_vp, _i, _i, _vp, _vp, _vp, _vp, _f, _i, _pp, _vp, _i, _vp, _vp]),
+    "dsrg_predict_mask_batch_dev": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _vp, _f, _i, _pp, _vp, _vp, _vp, _vp]),
+    "dsrg_predict_mask_batch_host": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _vp, _f, _i, _pp, _vp, _vp, _vp]),
     "dsrg_annotation_forward_dev": (_i, [_vp, _i, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _vp, _vp, _vp, _vp]),
     "dsrg_annotation_forward_host": (_i, [_vp, _i, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _vp, _vp, _vp]),
     "dsrg_annotation_coco_forward_dev": (_i, [_vp, _vp, _vp, _vp, _i, _vp, _vp, _i, _i, _vp, _i, _vp, _vp, _vp, _vp,

@@ -466,6 +466,45 @@ class Engine(object):
                                             _dptr(result_out), _dptr(probs_out), _stream(stream)))
         return result_out
 
+    @staticmethod
+    def _post_batch_args(scores):
+        n = len(scores)
+        if not 1 <= n <= 16:
+            raise ValueError("between 1 and 16 score maps, not %d" % n)
+        if any(len(a.shape) != 4 or tuple(a.shape[:2]) != tuple(scores[0].shape[:2]) for a in scores):
+            raise ValueError("every score map must be (B, M, h, w) with the same B and M")
+        hs = (C.c_int * n)(*[int(a.shape[2]) for a in scores])
+        ws = (C.c_int * n)(*[int(a.shape[3]) for a in scores])
+        return n, int(scores[0].shape[0]), hs, ws
+
+    def predict_mask_batch_host(self, scores, images, params=None, mode=POST_SUM_SCORES, eps=0.00001, smooth=True,
+                                sel=None, want_probs=False):
+        """scores: list of (B,M,h,w) float32 arrays, one per scale; images (B,H,W,3) uint8 (None when not smooth);
+        sel: optional (B,M) int32 rows of label ids ending at the first -1 -> (B,H,W) int32 label maps
+        [, (B,H,W,M) float32 probabilities]."""
+        n, B, hs, ws = self._post_batch_args(scores)
+        ptrs = (C.c_void_p * n)(*[_hptr(a, np.float32).value for a in scores])
+        result = np.empty((B, self.H, self.W), np.int32)
+        probs = np.empty((B, self.H, self.W, self.M), np.float32) if want_probs else None
+        params = params if params is not None else crf_params()
+        check(self._L.dsrg_predict_mask_batch_host(self.h, ptrs, hs, ws, n, B, int(mode), _hptr(images, np.uint8),
+                                                   float(eps), int(bool(smooth)), C.byref(params),
+                                                   _hptr(sel, np.int32), _hptr(result, np.int32),
+                                                   _hptr(probs, np.float32)))
+        return (result, probs) if want_probs else result
+
+    def predict_mask_batch_dev(self, scores, images, result_out, params=None, mode=POST_SUM_SCORES, eps=0.00001,
+                               smooth=True, sel=None, probs_out=None, stream=None):
+        """The same on CUDA tensors, queued on `stream`: result_out (B,H,W) int32, probs_out optional (B,H,W,M)
+        float32, sel an optional (B,M) int32 tensor read when the pass runs."""
+        n, B, hs, ws = self._post_batch_args(scores)
+        ptrs = (C.c_void_p * n)(*[_dptr(a).value for a in scores])
+        params = params if params is not None else crf_params()
+        check(self._L.dsrg_predict_mask_batch_dev(self.h, ptrs, hs, ws, n, B, int(mode), _dptr(images), float(eps),
+                                                  int(bool(smooth)), C.byref(params), _dptr(sel), _dptr(result_out),
+                                                  _dptr(probs_out), _stream(stream)))
+        return result_out
+
     # ---- AnnotationLayer.forward (pylayers.py:369-387) ----
     @staticmethod
     def _annot_args(tags, cues, flip):

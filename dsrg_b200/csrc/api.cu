@@ -243,6 +243,11 @@ int crf_core_for_post(Engine *e, const float *unary_hwc, const uint8_t *image, c
     return crf_core(e, 1, unary_hwc, DSRG_LAYOUT_NHWC, false, nullptr, image, p, s);
 }
 
+int crf_core_batch_for_post(Engine *e, int B, const float *unary_hwc, const uint8_t *images,
+                            const dsrg_crf_params *p, cudaStream_t s) {
+    return crf_core(e, B, unary_hwc, DSRG_LAYOUT_NHWC, false, nullptr, images, p, s);
+}
+
 // Graph replay for the per-image callers (inference post-processing, DenseCRF objects), whose image size changes
 // from call to call: when the shared spatial lattice is not the one this call needs, the pass that rebuilds it is
 // captured as such (`rebuild` is part of the key), so its graph is self-contained and valid whatever the engine
@@ -300,7 +305,7 @@ using namespace dsrg;
 
 extern "C" {
 
-int dsrg_version(void) { return 107; }
+int dsrg_version(void) { return 108; }
 
 const char *dsrg_last_error(void) { return g_err; }
 

@@ -14,6 +14,10 @@
 // The zoom keeps scipy's arithmetic exactly (float64, scipy's tap order, float32 result; see zoom.cuh),
 // so with identical scores the unary handed to the CRF differs from the reference's only by the ulps of
 // expf/logf; the label map then follows the CRF's 1e-4 parity bound (ties within it may flip).
+//
+// dsrg_predict_mask_{dev,host} run one image per call on a batch-1 engine; dsrg_predict_mask_batch_{dev,host} run
+// B images of one size per pass (every scale's zoom and the sum in one launch, the batched CRF, a per-image label
+// selection read from device memory), with the per-image arithmetic, so without the CRF they are bit-identical.
 #include "common.cuh"
 #include "zoom.cuh"
 
@@ -232,6 +236,223 @@ static int predict_mask(Engine *e, int mode, int n_scales, const float *const *s
     return rc;
 }
 
+// ---- B images of the engine's size in one pass (dsrg_predict_mask_batch_*) ----
+// The per-image pass above is ~90 dependent launches whatever the image holds: at batch 1 it is bound by launch
+// latency.  The batched pass issues the same stages once for B images, and its CRF is the batched mean field.
+
+constexpr int kPostMaxScales = 16;
+
+// one batched network forward per scale: scale k is [B][M][h[k]][w[k]] float32 at p[k]
+struct ZoomScales {  // 264 bytes of kernel parameters
+    const float *p[kPostMaxScales];
+    int h[kPostMaxScales], w[kPostMaxScales];
+    int n;
+};
+
+// out [B][H][W][M] = sum_k zoom(scores_k[b]), one thread per output element.  The float32 sum is formed in the
+// per-image pass's order (scale 0 stored, then += each further scale, test-ms.py:97), so it is bit-identical.
+__global__ void __launch_bounds__(kThreads)
+k_zoom_sum_batch(ZoomScales sc, float *__restrict__ out, int B, int M, int Ho, int Wo) {
+    const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    const long long N = (long long)Ho * Wo;
+    if (idx >= (long long)B * N * M) return;
+    const int c = (int)(idx % M);
+    const long long bp = idx / M;
+    const int b = (int)(bp / N), pix = (int)(bp - b * N);
+    const int oy = pix / Wo, ox = pix - oy * Wo;
+    float acc = 0.f;
+#pragma unroll
+    for (int k = 0; k < kPostMaxScales; k++) {
+        if (k >= sc.n) break;
+        const int hi = sc.h[k], wi = sc.w[k];
+        const float z = zoom_apply(sc.p[k] + ((size_t)b * M + c) * hi * wi, wi, zoom_tap(oy, ox, hi, wi, Ho, Wo));
+        acc = k ? __fadd_rn(acc, z) : z;
+    }
+    out[idx] = acc;
+}
+
+// The soft-max at network resolution of generate_train_gt.py:88-89 over a [B][M][np] blob, pixel i of image b at
+// b * M * np + i: the float32 operations of k_post_softmax<false> (label stride np) in the same order
+__global__ void __launch_bounds__(kThreads)
+k_net_softmax_batch(const float *__restrict__ in, float *__restrict__ out, int B, int M, int np) {
+    const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= (long long)B * np) return;
+    const int b = (int)(t / np), i = (int)(t - (long long)b * np);
+    const size_t base = (size_t)b * M * np + i;
+    const float *s = in + base;
+    float *o = out + base;
+    float v[DSRG_MAX_LABELS];
+    float m = -INFINITY;
+#pragma unroll
+    for (int l = 0; l < DSRG_MAX_LABELS; l++)
+        if (l < M) {
+            v[l] = s[(size_t)l * np];
+            m = fmaxf(m, v[l]);
+        }
+    float sum = 0.f;
+#pragma unroll
+    for (int l = 0; l < DSRG_MAX_LABELS; l++)
+        if (l < M) {
+            v[l] = expf(__fsub_rn(v[l], m));
+            sum = __fadd_rn(sum, v[l]);
+        }
+#pragma unroll
+    for (int l = 0; l < DSRG_MAX_LABELS; l++)
+        if (l < M) o[(size_t)l * np] = __fdiv_rn(v[l], sum);
+}
+
+// the same above DSRG_MAX_LABELS: exp(s - max) is parked in `out`, as k_post_softmax_wide does
+__global__ void __launch_bounds__(kThreads)
+k_net_softmax_batch_wide(const float *__restrict__ in, float *__restrict__ out, int B, int M, int np) {
+    const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= (long long)B * np) return;
+    const int b = (int)(t / np), i = (int)(t - (long long)b * np);
+    const size_t base = (size_t)b * M * np + i;
+    const float *s = in + base;
+    float *o = out + base;
+    float m = -INFINITY;
+    for (int l = 0; l < M; l++) m = fmaxf(m, s[(size_t)l * np]);
+    float sum = 0.f;
+    for (int l = 0; l < M; l++) {
+        const float v = expf(__fsub_rn(s[(size_t)l * np], m));
+        o[(size_t)l * np] = v;
+        sum = __fadd_rn(sum, v);
+    }
+    for (int l = 0; l < M; l++) o[(size_t)l * np] = __fdiv_rn(o[(size_t)l * np], sum);
+}
+
+// Per (pixel, image b = blockIdx.y): np.argmax (first maximum) over image b's selected labels, result = the label's
+// id.  q holds image b at b * M * N: [M][N] (ls = N, ps = 1, the CRF marginals) or [N][M] (ls = 1, ps = M).
+// sel: [B][M] label ids, each row ending at its first -1; NULL or an empty row selects every label.  A row with
+// an entry outside [0, M) before its -1 is not read past: every pixel of that image gets -1.
+__global__ void __launch_bounds__(kThreads)
+k_post_argmax_batch(const float *q, int32_t *out, int N, int M, long long ls, long long ps, const int32_t *sel) {
+    __shared__ int s_id[DSRG_MAX_LABELS_WIDE];
+    __shared__ int s_n;
+    const int b = blockIdx.y;
+    for (int k = threadIdx.x; k < M; k += blockDim.x) s_id[k] = sel ? sel[(size_t)b * M + k] : k;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        int n = 0;
+        while (n < M && s_id[n] != -1) {
+            if (s_id[n] < 0 || s_id[n] >= M) {
+                n = -1;
+                break;
+            }
+            n++;
+        }
+        if (n == 0)
+            for (int k = 0; k < M; k++) s_id[k] = k;
+        s_n = n == 0 ? M : n;
+    }
+    __syncthreads();
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= N) return;
+    const int n = s_n;
+    if (n < 0) {
+        out[(size_t)b * N + i] = -1;
+        return;
+    }
+    const float *s = q + (size_t)b * M * N + (size_t)i * ps;
+    int arg = s_id[0];
+    float best = s[(size_t)arg * ls];
+    for (int k = 1; k < n; k++) {
+        const int id = s_id[k];
+        const float v = s[(size_t)id * ls];
+        if (v > best) {
+            best = v;
+            arg = id;
+        }
+    }
+    out[(size_t)b * N + i] = arg;
+}
+
+int crf_core_batch_for_post(Engine *e, int B, const float *unary_hwc, const uint8_t *images,
+                            const dsrg_crf_params *p, cudaStream_t s);  // api.cu
+
+static int predict_mask_batch_body(Engine *e, int B, int mode, const ZoomScales &sc, const uint8_t *images, float eps,
+                                   int smooth, const dsrg_crf_params *p, const int32_t *sel, int32_t *result,
+                                   float *probs_out, cudaStream_t s) {
+    const int N = e->N, M = e->M;
+    const long long n = (long long)B * N * M;
+    float *unary = e->st_unary;                       // [B][H][W][M]
+    float *clamped = smooth ? nullptr : (probs_out ? probs_out : e->st_out);
+    if (mode == DSRG_POST_SUM_SCORES) {
+        DSRG_LAUNCH(e, T_POST, s, k_zoom_sum_batch<<<cdiv(n, kThreads), kThreads, 0, s>>>(sc, unary, B, M, e->H, e->W));
+        post_softmax<true>(e, unary, unary, clamped, B * N, 1, M, eps, s);  // NHWC is contiguous across the batch
+    } else {
+        const int np = sc.h[0] * sc.w[0];
+        float *small = e->st_cues;                    // [B][M][h][w] probabilities at network resolution
+        const int g = cdiv((long long)B * np, kThreads);
+        if (M > DSRG_MAX_LABELS)
+            DSRG_LAUNCH(e, T_POST, s, k_net_softmax_batch_wide<<<g, kThreads, 0, s>>>(sc.p[0], small, B, M, np));
+        else
+            DSRG_LAUNCH(e, T_POST, s, k_net_softmax_batch<<<g, kThreads, 0, s>>>(sc.p[0], small, B, M, np));
+        ZoomScales zs = sc;
+        zs.p[0] = small;
+        DSRG_LAUNCH(e, T_POST, s, k_zoom_sum_batch<<<cdiv(n, kThreads), kThreads, 0, s>>>(zs, unary, B, M, e->H, e->W));
+        DSRG_LAUNCH(e, T_POST, s, k_post_clamp_log<<<cdiv(n, kThreads), kThreads, 0, s>>>(unary, unary, clamped, n, eps));
+    }
+    DSRG_CUDA_TRY(cudaGetLastError());
+    const dim3 ga(cdiv(N, kThreads), B);
+    if (smooth) {
+        if (int rc = crf_core_batch_for_post(e, B, unary, images, p, s)) return rc;
+        if (probs_out)
+            if (int rc = meanfield_export(e, B, probs_out, DSRG_LAYOUT_NHWC, s)) return rc;
+        DSRG_LAUNCH(e, T_POST, s, k_post_argmax_batch<<<ga, kThreads, 0, s>>>(e->Qcur, result, N, M, N, 1, sel));
+    } else {
+        DSRG_LAUNCH(e, T_POST, s, k_post_argmax_batch<<<ga, kThreads, 0, s>>>(clamped, result, N, M, 1, M, sel));
+    }
+    DSRG_CUDA_TRY(cudaGetLastError());
+    return DSRG_OK;
+}
+
+// what the batched pass checks before anything is staged or launched (B and the NULL pointers: the prologue)
+static int post_batch_check(const Engine *e, int mode, int n_scales, const float *const *scores, const int *hs,
+                            const int *ws) {
+    if (mode != DSRG_POST_SUM_SCORES && mode != DSRG_POST_ZOOM_PROBS) {
+        set_error("bad mode %d", mode);
+        return DSRG_E_INVALID;
+    }
+    if (mode == DSRG_POST_ZOOM_PROBS && n_scales != 1) {
+        set_error("DSRG_POST_ZOOM_PROBS takes one score map per image, not %d", n_scales);
+        return DSRG_E_INVALID;
+    }
+    for (int k = 0; k < n_scales; k++)
+        if (!scores[k] || hs[k] < 1 || ws[k] < 1 || (long long)hs[k] * ws[k] > e->Ncap) {
+            set_error("score map %d: bad pointer or size %dx%d (capacity %d pixels)", k, hs[k], ws[k], e->Ncap);
+            return DSRG_E_INVALID;
+        }
+    return DSRG_OK;
+}
+
+static int predict_mask_batch(Engine *e, int B, int mode, int n_scales, const float *const *scores, const int *hs,
+                              const int *ws, const uint8_t *images, float eps, int smooth, const dsrg_crf_params *p,
+                              const int32_t *sel, int32_t *result, float *probs_out, cudaStream_t s) {
+    int rc = post_batch_check(e, mode, n_scales, scores, hs, ws);
+    if (rc || (rc = ensure_staging(e))) return rc;
+    ZoomScales sc = {};
+    sc.n = n_scales;
+    for (int k = 0; k < n_scales; k++) {
+        sc.p[k] = scores[k];
+        sc.h[k] = hs[k];
+        sc.w[k] = ws[k];
+    }
+    // the selection is read by the pass, so its content is not part of the key: a replay follows what sel holds
+    const bool rebuild = smooth && post_pass_needs_spatial(e, p);
+    GraphKey key;
+    key.add(7).add(B).add(e->H).add(e->W).add(mode).add(n_scales).add(images).add(eps).add(smooth).add(sel)
+        .add(result).add(probs_out).add(rebuild);
+    for (int k = 0; k < n_scales; k++) key.add(scores[k]).add(hs[k]).add(ws[k]);
+    if (smooth) key.add(*p);
+    if (rebuild) e->sp_valid = false;
+    rc = run_pass(e, s, key, true, [&]() {
+        return predict_mask_batch_body(e, B, mode, sc, images, eps, smooth, p, sel, result, probs_out, s);
+    });
+    if (smooth) post_pass_done(e, p, B, rc);
+    return rc;
+}
+
 }  // namespace dsrg
 
 using namespace dsrg;
@@ -308,6 +529,67 @@ extern "C" int dsrg_predict_mask_host(dsrg_engine *h, int mode, int n_scales, co
         DSRG_CUDA_TRY(cudaMemcpyAsync(result_out, e->st_lmap, (size_t)e->N * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
         if (probs_out)
             DSRG_CUDA_TRY(cudaMemcpyAsync(probs_out, e->st_out, (size_t)e->N * e->M * sizeof(float),
+                                          cudaMemcpyDeviceToHost, s));
+        return DSRG_OK;
+    });
+}
+
+extern "C" int dsrg_predict_mask_batch_dev(dsrg_engine *h, const float *const *scores_dev, const int *hs,
+                                           const int *ws, int n_scales, int B, int mode, const uint8_t *images_dev,
+                                           float eps, int smooth, const dsrg_crf_params *params,
+                                           const int32_t *sel_dev, int32_t *result_out_dev, float *probs_out_dev,
+                                           void *stream) {
+    const cudaStream_t s = (cudaStream_t)stream;
+    const bool ok = n_scales >= 1 && n_scales <= kPostMaxScales &&
+                    post_args_ok(scores_dev, hs, ws, images_dev, smooth, params, nullptr, 0, result_out_dev);
+    return dev_call(h, B, s, ok, [&](Engine *e) {
+        return predict_mask_batch(e, B, mode, n_scales, scores_dev, hs, ws, images_dev, eps, smooth, params, sel_dev,
+                                  result_out_dev, probs_out_dev, s);
+    });
+}
+
+extern "C" int dsrg_predict_mask_batch_host(dsrg_engine *h, const float *const *scores, const int *hs, const int *ws,
+                                            int n_scales, int B, int mode, const uint8_t *images, float eps,
+                                            int smooth, const dsrg_crf_params *params, const int32_t *sel,
+                                            int32_t *result_out, float *probs_out) {
+    const bool ok = n_scales >= 1 && n_scales <= kPostMaxScales &&
+                    post_args_ok(scores, hs, ws, images, smooth, params, nullptr, 0, result_out);
+    return host_call(h, B, ok, false, [&](Engine *e, cudaStream_t s) {
+        const int M = e->M;
+        if (int rc = post_batch_check(e, mode, n_scales, scores, hs, ws)) return rc;
+        for (int b = 0; sel && b < B; b++)
+            for (int k = 0; k < M && sel[(size_t)b * M + k] != -1; k++) {
+                const int v = sel[(size_t)b * M + k];
+                if (v < 0 || v >= M) {
+                    set_error("image %d: selected label %d outside [0, %d)", b, v, M);
+                    return DSRG_E_INVALID;
+                }
+            }
+        size_t total = 0;
+        for (int k = 0; k < n_scales; k++) total += (size_t)B * M * hs[k] * ws[k];
+        if (int rc = grow_staging(e, (void **)&e->st_raw, &e->st_raw_cap, total * sizeof(float))) return rc;
+        if (sel)
+            if (int rc = grow_staging(e, (void **)&e->st_idx, &e->st_idx_cap, (size_t)B * M * sizeof(int32_t)))
+                return rc;
+        const float *dptr[kPostMaxScales];
+        size_t at = 0;
+        for (int k = 0; k < n_scales; k++) {
+            const size_t n = (size_t)B * M * hs[k] * ws[k];
+            DSRG_CUDA_TRY(cudaMemcpyAsync(e->st_raw + at, scores[k], n * sizeof(float), cudaMemcpyHostToDevice, s));
+            dptr[k] = e->st_raw + at;
+            at += n;
+        }
+        if (smooth)
+            DSRG_CUDA_TRY(cudaMemcpyAsync(e->st_image, images, (size_t)B * e->N * 3, cudaMemcpyHostToDevice, s));
+        if (sel)
+            DSRG_CUDA_TRY(cudaMemcpyAsync(e->st_idx, sel, (size_t)B * M * sizeof(int32_t), cudaMemcpyHostToDevice, s));
+        if (int rc = predict_mask_batch(e, B, mode, n_scales, dptr, hs, ws, e->st_image, eps, smooth, params,
+                                        sel ? e->st_idx : nullptr, e->st_lmap, probs_out ? e->st_out : nullptr, s))
+            return rc;
+        DSRG_CUDA_TRY(cudaMemcpyAsync(result_out, e->st_lmap, (size_t)B * e->N * sizeof(int32_t),
+                                      cudaMemcpyDeviceToHost, s));
+        if (probs_out)
+            DSRG_CUDA_TRY(cudaMemcpyAsync(probs_out, e->st_out, (size_t)B * e->N * M * sizeof(float),
                                           cudaMemcpyDeviceToHost, s));
         return DSRG_OK;
     });

@@ -6,6 +6,7 @@ The network forward pass stays with the caller; pass the fc8 score blobs as they
 import numpy as np
 
 from . import api as _api
+from .pool import batch_engine_for as _batch_engine_for
 from .pool import engine_for as _engine_for
 
 EPS = 0.00001  # test-ms.py:103, generate_train_gt.py:90
@@ -80,3 +81,147 @@ def predict_mask_gt(im, scores, labels, smooth=True, return_probs=False):
     if return_probs:
         return out[0].astype(np.int64), out[1]
     return out.astype(np.int64)
+
+
+# ---- many images per pass ----
+
+def _chunks(keys, batch):
+    """Indices of `keys` grouped by equal key (groups in order of first appearance, indices ascending), each group
+    cut into chunks of at most `batch`."""
+    groups = {}
+    for i, k in enumerate(keys):
+        groups.setdefault(k, []).append(i)
+    return [idx[a:a + batch] for idx in groups.values() for a in range(0, len(idx), batch)]
+
+
+def _run_batched(ims, blobs_per_image, sels, mode, smooth, batch, return_probs):
+    """Group the images by (H, W, score shapes), run each chunk as one batched pass, return per image in input
+    order.  `sels`: None or one selection list per image."""
+    n = len(ims)
+    if len(blobs_per_image) != n or (sels is not None and len(sels) != n):
+        raise ValueError("one set of score blobs%s per image" % ("" if sels is None else " and labels"))
+    batch = int(batch)
+    if batch < 1:
+        raise ValueError("batch must be at least 1")
+    shapes = []
+    for im, blobs in zip(ims, blobs_per_image):
+        shape = np.shape(im)
+        if len(shape) != 3 or shape[2] != 3:
+            raise ValueError("image must be (H, W, 3)")
+        if not blobs or any(b.shape[0] != blobs[0].shape[0] for b in blobs):
+            raise ValueError("every image needs at least one score blob, all with the same label count")
+        shapes.append((tuple(shape[:2]), tuple(b.shape for b in blobs)))
+    chunks = _chunks(shapes, batch)
+    # size each label count's engine for the largest chunk and image once, so no chunk re-creates it
+    need = {}
+    for idx in chunks:
+        (H, W), bs = shapes[idx[0]]
+        B0, H0, W0 = need.get(bs[0][0], (0, 0, 0))
+        need[bs[0][0]] = (max(B0, len(idx)), max(H0, H), max(W0, W))
+    for M, (B0, H0, W0) in need.items():
+        _batch_engine_for(B0, H0, W0, M)
+    labels, probs = [None] * n, [None] * n
+    params = _api.crf_params(1.0)
+    for idx in chunks:
+        (H, W), bs = shapes[idx[0]]
+        M = bs[0][0]
+        eng = _batch_engine_for(len(idx), H, W, M)
+        scores = [np.stack([blobs_per_image[i][k] for i in idx]) for k in range(len(bs))]
+        images = np.stack([_image(ims[i], True) for i in idx]) if smooth else None
+        sel = None
+        if sels is not None:
+            sel = np.full((len(idx), M), -1, np.int32)
+            for r, i in enumerate(idx):
+                sel[r, :len(sels[i])] = sels[i]
+        out = eng.predict_mask_batch_host(scores, images, params, mode, EPS, smooth, sel, return_probs)
+        res, pr = out if return_probs else (out, None)
+        for r, i in enumerate(idx):
+            labels[i] = res[r].astype(np.int64)
+            if return_probs:
+                probs[i] = pr[r]
+    return (labels, probs) if return_probs else labels
+
+
+def predict_masks_ms(ims, scores_per_image, smooth=True, batch=16, return_probs=False):
+    """predict_mask_ms over a list of images, up to `batch` of them per device pass: ims[i] is an (H,W,3) image and
+    scores_per_image[i] its list of (M,h,w) score blobs, of any sizes.  Images with the same (H, W) and score shapes
+    share passes.  Returns the list of (H,W) int64 label maps in input order [and the list of (H,W,M) float32
+    probabilities].  With smooth=False the results are bit-identical to predict_mask_ms image by image."""
+    blobs = [[_blob(s) for s in sc] for sc in scores_per_image]
+    return _run_batched(list(ims), blobs, None, _api.POST_SUM_SCORES, smooth, batch, return_probs)
+
+
+def predict_masks_gt(ims, scores, labels_per_image, smooth=True, batch=16):
+    """predict_mask_gt over a list of images, up to `batch` of them per device pass: scores[i] is image i's (M,h,w)
+    blob and labels_per_image[i] its tags.  Returns the list of (H,W) int64 label maps in input order."""
+    blobs = [[_blob(s)] for s in scores]
+    sels = []
+    for blob, tags in zip(blobs, labels_per_image):
+        M = blob[0].shape[0]
+        sel = [0] + [int(v) for v in np.asarray(tags).reshape(-1).tolist()]   # generate_train_gt.py:96-97
+        if min(sel) < 0 or max(sel) >= M:
+            raise ValueError("label ids must lie in [0, %d), got %s" % (M, sel))
+        # a repeated id can never be the first maximum again: keeping only its first occurrence changes nothing
+        sels.append(list(dict.fromkeys(sel)))
+    return _run_batched(list(ims), blobs, sels, _api.POST_ZOOM_PROBS, smooth, batch, False)
+
+
+_MODES = {"ms": _api.POST_SUM_SCORES, "gt": _api.POST_ZOOM_PROBS}
+
+
+def predict_mask_batch_dev(images, scores, labels=None, mode="ms", smooth=True, out=None):
+    """The post-processing of a batch that never leaves the device, queued on the current CUDA stream (so it can be
+    captured in a CUDA graph).
+      images : (B,H,W,3) uint8 CUDA tensor
+      scores : list of (B,M,h,w) float32 CUDA tensors, one batched forward per scale ("ms": 1 to 16 of them,
+               test-ms.py; "gt": exactly one, generate_train_gt.py)
+      labels : optional (B,M) or (B,1,1,M) 0/1 tag tensor (the labels blob): image b's arg-max runs over label 0 and
+               the labels tagged > 0.5, in ascending order.  The selection is built on the device, without a host
+               synchronisation, and read when the pass runs
+      out    : optional (B,H,W) int32 CUDA tensor to write into (a fixed output lets the engine replay its own graph)
+    Returns the (B,H,W) int32 label maps, which api.Confusion.add_dev counts directly.  Every argument is checked
+    (ValueError) before anything is queued."""
+    import torch
+    if mode not in _MODES:
+        raise ValueError("mode must be 'ms' or 'gt', not %r" % (mode,))
+    if not (isinstance(images, torch.Tensor) and images.is_cuda and images.dtype == torch.uint8 and images.dim() == 4
+            and images.shape[3] == 3 and images.is_contiguous()):
+        raise ValueError("images must be a contiguous (B, H, W, 3) uint8 CUDA tensor")
+    B, H, W = (int(v) for v in images.shape[:3])
+    dev = images.device
+    scores = list(scores)
+    if not 1 <= len(scores) <= 16 or (mode == "gt" and len(scores) != 1):
+        raise ValueError("mode %r takes %s score tensors, got %d" % (mode, "1" if mode == "gt" else "1 to 16",
+                                                                     len(scores)))
+    for s in scores:
+        if not (isinstance(s, torch.Tensor) and s.device == dev and s.dtype == torch.float32 and s.dim() == 4
+                and s.is_contiguous() and s.shape[0] == B and s.shape[1] == scores[0].shape[1] and min(s.shape) > 0):
+            raise ValueError("every score map must be a contiguous (B, M, h, w) float32 tensor on %s with B = %d and "
+                             "one M" % (dev, B))
+    M = int(scores[0].shape[1])
+    if B < 1 or H < 1 or W < 1 or M > 255:
+        raise ValueError("need B, H, W >= 1 and at most 255 labels (got B=%d, %dx%d, M=%d)" % (B, H, W, M))
+    if labels is not None and not (isinstance(labels, torch.Tensor) and labels.device == dev and
+                                   tuple(labels.shape) in ((B, M), (B, 1, 1, M))):
+        raise ValueError("labels must be a (B, M) or (B, 1, 1, M) tensor on %s" % dev)
+    if out is not None and not (isinstance(out, torch.Tensor) and out.device == dev and out.dtype == torch.int32
+                                and tuple(out.shape) == (B, H, W) and out.is_contiguous()):
+        raise ValueError("out must be a contiguous (B, H, W) int32 tensor on %s" % dev)
+    eng = _batch_engine_for(B, H, W, M, dev.index)
+    hc, wc = eng.capacity
+    for s in scores:
+        if s.shape[2] * s.shape[3] > hc * wc:
+            raise ValueError("score map %dx%d has more pixels than the engine holds (%d)" % (s.shape[2], s.shape[3],
+                                                                                           hc * wc))
+    sel = None
+    if labels is not None:
+        present = labels.reshape(B, M) > 0.5
+        present[:, 0] = True
+        ids = torch.arange(M, device=dev, dtype=torch.int32).expand(B, M)
+        order = torch.sort(torch.where(present, ids, ids + M), dim=1).values   # tagged ids first, ascending
+        sel = torch.where(order < M, order, torch.full_like(order, -1)).contiguous()
+    if out is None:
+        out = torch.empty((B, H, W), dtype=torch.int32, device=dev)
+    with torch.cuda.device(dev):
+        eng.predict_mask_batch_dev(scores, images, out, _api.crf_params(1.0), _MODES[mode], EPS, smooth, sel)
+    return out

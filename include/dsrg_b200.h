@@ -263,6 +263,34 @@ int dsrg_predict_mask_host(dsrg_engine *e, int mode, int n_scales, const float *
                            const int *hs, const int *ws, const uint8_t *image_host, float eps, int smooth,
                            const dsrg_crf_params *params, const int32_t *labels_sel, int n_sel,
                            int32_t *result_out_host, float *probs_out_host);
+/*
+ * The same post-processing for B images of the engine's current size in one pass (1 <= B <= max_batch): the
+ * pseudo-label run of test-ms.py / generate_train_gt.py over a dataset, or an evaluation loop that keeps fc8 on the
+ * device.  One batched pass replaces B per-image ones of ~90 dependent launches each.
+ *   scores    : n_scales pointers (1 <= n_scales <= 16) to [B][M][h_k][w_k] float32, one batched forward per
+ *               scale; the array of pointers and hs / ws live on the host in both variants
+ *   images    : [B][H][W][3] uint8 (may be NULL when smooth == 0)
+ *   mode, eps, smooth, params : as for dsrg_predict_mask_*; DSRG_POST_ZOOM_PROBS takes n_scales == 1
+ *   sel       : optional [B][M] int32; row b lists image b's label ids in the order the arg-max visits them (the
+ *               first maximum wins, generate_train_gt.py:96-100) and ends at its first -1.  NULL or an empty row
+ *               selects every label.  In _dev it is device memory read when the pass runs (its content is not
+ *               part of a cached graph's key)
+ *   result_out: [B][H][W] int32;  probs_out : optional [B][H][W][M] float32
+ * With smooth == 0 every image's result and probs_out are bit-identical to dsrg_predict_mask_* on that image alone;
+ * with smooth == 1 the CRF marginals follow the batched CRF's 1e-4 bound.
+ * A sel entry outside [0, M) before the row's -1:
+ *   _host: DSRG_E_INVALID before any copy or launch.
+ *   _dev : the row is not read past it, and every pixel of that image's result is -1 (a prediction that
+ *          dsrg_confusion_add_dev counts in invalid[1]); the caller checks it once the stream has run.
+ */
+int dsrg_predict_mask_batch_dev(dsrg_engine *e, const float *const *scores_dev, const int *hs, const int *ws,
+                                int n_scales, int B, int mode, const uint8_t *images_dev, float eps, int smooth,
+                                const dsrg_crf_params *params, const int32_t *sel_dev, int32_t *result_out_dev,
+                                float *probs_out_dev, void *stream);
+int dsrg_predict_mask_batch_host(dsrg_engine *e, const float *const *scores_host, const int *hs, const int *ws,
+                                 int n_scales, int B, int mode, const uint8_t *images_host, float eps, int smooth,
+                                 const dsrg_crf_params *params, const int32_t *sel_host, int32_t *result_out_host,
+                                 float *probs_out_host);
 
 /*
  * AnnotationLayer.forward (pylayers/pylayers/pylayers.py:369-387): image tags + sparse localisation cues
