@@ -12,6 +12,7 @@ LIB_PATH = os.environ.get("DSRG_B200_LIB") or os.path.join(_HERE, "lib", "libdsr
 OK, E_INVALID, E_CUDA, E_KEYRANGE, E_STATE, E_NOMEM = 0, -1, -2, -3, -4, -5
 LAYOUT_NHWC, LAYOUT_NCHW = 0, 1
 POST_SUM_SCORES, POST_ZOOM_PROBS = 0, 1
+PREP_IMAGES_PER_LAUNCH = 64      # DSRG_PREP_IMAGES_PER_LAUNCH
 
 
 class DsrgError(RuntimeError):
@@ -45,6 +46,7 @@ SIGNATURES = {
     "dsrg_engine_destroy": (None, [_vp]),
     "dsrg_engine_device_bytes": (_sz, [_vp]),
     "dsrg_engine_set_size": (_i, [_vp, _i, _i]),
+    "dsrg_engine_set_size_ordered": (_i, [_vp, _i, _i]),
     "dsrg_engine_get_size": (_i, [_vp, _vp, _vp, _vp, _vp]),
     "dsrg_engine_set_host_chunk": (_i, [_vp, _i]),
     "dsrg_engine_set_graphs": (_i, [_vp, _i]),
@@ -71,6 +73,8 @@ SIGNATURES = {
     "dsrg_prepare_image_host": (_i, [_vp, _i, _i, _i, _vp, _vp, _vp]),
     "dsrg_prepare_net_input_dev": (_i, [_vp, _vp, _i, _i, _i, _vp, _vp, _vp, _vp, _vp]),
     "dsrg_prepare_net_input_host": (_i, [_vp, _vp, _i, _i, _i, _vp, _vp, _vp, _vp]),
+    "dsrg_prepare_net_input_batch_dev": (_i, [_vp, _vp, _vp, _vp, _i, _i, _vp, _vp, _vp, _vp, _vp]),
+    "dsrg_prepare_net_input_batch_host": (_i, [_vp, _vp, _vp, _vp, _i, _i, _vp, _vp, _vp, _vp]),
     "dsrg_zoom_scores_dev": (_i, [_vp, _vp, _i, _i, _vp, _i, _vp]),
     "dsrg_zoom_scores_host": (_i, [_vp, _vp, _i, _i, _vp, _i]),
     "dsrg_predict_mask_dev": (_i, [_vp, _i, _i, _vp, _vp, _vp, _vp, _f, _i, _pp, _vp, _i, _vp, _vp, _vp]),

@@ -100,9 +100,12 @@ class Engine(object):
     def device_bytes(self):
         return self._L.dsrg_engine_device_bytes(self.h)
 
-    def set_size(self, H, W):
-        """Select an image size within the capacity the engine was created with (no reallocation)."""
-        check(self._L.dsrg_engine_set_size(self.h, int(H), int(W)))
+    def set_size(self, H, W, ordered=False):
+        """Select an image size within the capacity the engine was created with (no reallocation).  Waits for the
+        device when the size changes, unless `ordered`: then the caller drives this engine only through its entry
+        points (dsrg_engine_set_size_ordered), and no replay of a CUDA graph of its own holds the engine's launches."""
+        fn = self._L.dsrg_engine_set_size_ordered if ordered else self._L.dsrg_engine_set_size
+        check(fn(self.h, int(H), int(W)))
         self.H, self.W = int(H), int(W)
 
     @property
@@ -375,6 +378,43 @@ class Engine(object):
         ptrs = (C.c_void_p * n)(*[_dptr(o).value for o in outs])
         check(self._L.dsrg_prepare_net_input_dev(self.h, _dptr(image), int(image.shape[0]), int(image.shape[1]), n,
                                                  hs, ws, _hptr(mean, np.float64), ptrs, _stream(stream)))
+        return outs
+
+    @staticmethod
+    def _image_sizes(images):
+        B = len(images)
+        Hs = (C.c_int * B)(*[int(im.shape[0]) for im in images])
+        Ws = (C.c_int * B)(*[int(im.shape[1]) for im in images])
+        return B, Hs, Ws
+
+    def prepare_net_input_batch_host(self, images, sizes, mean_pixel=(104.0, 117.0, 123.0)):
+        """List of B (H_i,W_i,3) uint8 images -> one (B,3,h,w) float32 network input per (h, w) of `sizes`; image b
+        of each is bit-identical to prepare_net_input_host of that image alone.  Does not change the engine's size."""
+        B, Hs, Ws = self._image_sizes(images)
+        n, hs, ws, mean = self._net_input_args(sizes, mean_pixel)
+        ims = (C.c_void_p * B)(*[_hptr(im, np.uint8).value for im in images])
+        outs = [np.empty((B, 3, h, w), np.float32) for h, w in zip(hs, ws)]
+        ptrs = (C.c_void_p * n)(*[o.ctypes.data for o in outs])
+        check(self._L.dsrg_prepare_net_input_batch_host(self.h, ims, Hs, Ws, B, n, hs, ws, _hptr(mean, np.float64),
+                                                        ptrs))
+        return outs
+
+    def prepare_net_input_batch_dev(self, images, outs, mean_pixel=(104.0, 117.0, 123.0), stream=None):
+        """images: list of B contiguous (H_i,W_i,3) uint8 CUDA tensors; outs: one contiguous (B,3,h,w) float32 CUDA
+        tensor per scale (their shapes give the sizes).  Queued on `stream`; copies nothing from the host."""
+        import torch
+        for im in images:
+            if im.dtype != torch.uint8 or im.dim() != 3 or im.shape[2] != 3:
+                raise ValueError("every image must be an (H, W, 3) uint8 tensor")
+        for o in outs:
+            if o.dtype != torch.float32 or o.dim() != 4 or o.shape[:2] != (len(images), 3):
+                raise ValueError("every output must be a float32 (B, 3, h, w) tensor with B = %d" % len(images))
+        B, Hs, Ws = self._image_sizes(images)
+        n, hs, ws, mean = self._net_input_args([(o.shape[2], o.shape[3]) for o in outs], mean_pixel)
+        ims = (C.c_void_p * B)(*[_dptr(im).value for im in images])
+        ptrs = (C.c_void_p * n)(*[_dptr(o).value for o in outs])
+        check(self._L.dsrg_prepare_net_input_batch_dev(self.h, ims, Hs, Ws, B, n, hs, ws, _hptr(mean, np.float64),
+                                                       ptrs, _stream(stream)))
         return outs
 
     def crflayer_forward_host(self, probs, image, params, log_out=None, result=None):

@@ -305,7 +305,7 @@ using namespace dsrg;
 
 extern "C" {
 
-int dsrg_version(void) { return 108; }
+int dsrg_version(void) { return 109; }
 
 const char *dsrg_last_error(void) { return g_err; }
 
@@ -496,24 +496,31 @@ void dsrg_engine_destroy(dsrg_engine *h) {
 
 size_t dsrg_engine_device_bytes(const dsrg_engine *h) { return h ? ((const Engine *)h)->bytes : 0; }
 
-int dsrg_engine_set_size(dsrg_engine *h, int H, int W) {
-    Engine *e = (Engine *)h;
+// wait: for the work already queued on any stream.  Queued launches keep the old strides in their arguments, so the
+// wait is only needed for work the engine cannot order: dsrg_engine_set_size_ordered skips it.
+static int set_size(Engine *e, int H, int W, bool wait) {
     if (!e) return no_engine();
     if (H < 1 || W < 1 || H > e->Hcap || W > e->Wcap) {
         set_error("size %dx%d outside the engine's capacity %dx%d", H, W, e->Hcap, e->Wcap);
         return DSRG_E_INVALID;
     }
     if (H == e->H && W == e->W) return DSRG_OK;
-    // work already queued keeps the old strides in its launch arguments; wait for it before the
-    // buffers are re-interpreted with the new ones
-    DeviceScope dev_scope(e);
-    DSRG_CUDA_TRY(cudaDeviceSynchronize());
+    if (wait) {
+        DeviceScope dev_scope(e);
+        DSRG_CUDA_TRY(cudaDeviceSynchronize());
+    }
     engine_shape(e, H, W);
     e->last_crf_B = 0;
     // cached graphs stay: they are keyed by the shape (every stride is a function of it and of the capacity the
     // buffers were sized for), so a per-image caller that meets a size again replays that size's graph
     return DSRG_OK;
 }
+
+int dsrg_engine_set_size(dsrg_engine *h, int H, int W) { return set_size((Engine *)h, H, W, true); }
+
+// Every entry point orders its pass after the engine's previous one (StreamScope: the same stream, or a wait for the
+// order event on another), so between passes issued through the entry points the re-shape needs no wait
+int dsrg_engine_set_size_ordered(dsrg_engine *h, int H, int W) { return set_size((Engine *)h, H, W, false); }
 
 int dsrg_engine_get_size(const dsrg_engine *h, int *H, int *W, int *Hcap, int *Wcap) {
     const Engine *e = (const Engine *)h;

@@ -96,6 +96,11 @@ size_t dsrg_engine_device_bytes(const dsrg_engine *e); /* bytes of HBM held by t
  * without reallocating (the evaluation tools run one image at a time, each of its own size --
  * training/tools/test-ms.py:86-87).  Waits for queued work; the cached spatial lattice is rebuilt. */
 int dsrg_engine_set_size(dsrg_engine *e, int H, int W);
+/* The same re-shape without the wait, for a caller that drives the engine only through its entry points: each of
+ * them orders its pass after the engine's previous one (same stream, or a wait for its order event), and queued
+ * passes keep their own strides.  A replay of the caller's own CUDA graph of this engine's launches is not ordered
+ * that way: replays and later calls go on one stream, or the caller orders them. */
+int dsrg_engine_set_size_ordered(dsrg_engine *e, int H, int W);
 int dsrg_engine_get_size(const dsrg_engine *e, int *H, int *W, int *H_capacity, int *W_capacity);
 /* The *_host full-pass entry points pipeline the batch in chunks (default B/8, 3B/8, B/2 images) through
  * H2D | kernels | D2H streams; `images` > 0 caps the chunk size, 0 restores the default. */
@@ -231,6 +236,24 @@ int dsrg_prepare_net_input_dev(dsrg_engine *e, const uint8_t *image_dev, int H, 
 int dsrg_prepare_net_input_host(dsrg_engine *e, const uint8_t *image_host, int H, int W, int n_scales,
                                 const int *hs, const int *ws, const double *mean_pixel /* host, 3 */,
                                 float *const *out_host);
+/*
+ * The same network input for B images of any sizes (1 <= B <= the engine's max_batch): one network batch per scale.
+ * The evaluation tools pass absolute sizes, so every image of a list goes to the same (h_k, w_k) whatever its own size.
+ *   images  : host array of B pointers to [Hs[b]][Ws[b]][3] uint8 images (device memory in _dev)
+ *   Hs, Ws  : host arrays of the B image sizes
+ *   hs, ws  : as above; every image of the call is zoomed to (hs[k], ws[k])
+ *   out     : host array of n_scales pointers to [B][3][hs[k]][ws[k]] float32
+ * Image b of out[k] is bit-identical to dsrg_prepare_net_input_* of that image alone.  The image and scale tables are
+ * kernel parameters: _dev copies nothing from the host and can be captured in a CUDA graph.  One launch covers up to
+ * DSRG_PREP_IMAGES_PER_LAUNCH images.  Like the per-image call, it neither reads nor changes the engine's size.
+ */
+#define DSRG_PREP_IMAGES_PER_LAUNCH 64
+int dsrg_prepare_net_input_batch_dev(dsrg_engine *e, const uint8_t *const *images_dev, const int *Hs, const int *Ws,
+                                     int B, int n_scales, const int *hs, const int *ws,
+                                     const double *mean_pixel /* host, 3 */, float *const *out_dev, void *stream);
+int dsrg_prepare_net_input_batch_host(dsrg_engine *e, const uint8_t *const *images_host, const int *Hs,
+                                      const int *Ws, int B, int n_scales, const int *hs, const int *ws,
+                                      const double *mean_pixel /* host, 3 */, float *const *out_host);
 
 /*
  * Full-resolution inference post-processing: what predict_mask() of the evaluation / ground-truth tools
