@@ -273,6 +273,10 @@ int srg_run(Engine *e, int B, const float *labels, const float *probs, const flo
             double th1, double th2, int renorm, float *seeds_out, int32_t *label_map_out,
             cudaStream_t s, const uint32_t *cue_bits, uint32_t *seed_bits) {
     const int N = e->N, M = e->M;
+    if (seed_bits && !cue_bits) {  // seeds keep every cue value: they are a 0/1 mask only when the cues are
+        set_error("SRG seed bits need cue bits");
+        return DSRG_E_INVALID;
+    }
     const int wpi = (int)(((size_t)M * N + 31) / 32);
     dim3 g(cdiv(N, kThreads), B);
 #define DSRG_LABEL(MTV, CBV)                                                                                          \
@@ -292,7 +296,6 @@ int srg_run(Engine *e, int B, const float *labels, const float *probs, const flo
 #define DSRG_EMIT_MT(MTV)                                              \
     if (cue_bits && seed_bits) DSRG_EMIT(MTV, true, true);             \
     else if (cue_bits) DSRG_EMIT(MTV, true, false);                    \
-    else if (seed_bits) DSRG_EMIT(MTV, false, true);                   \
     else DSRG_EMIT(MTV, false, false)
     if (M == 21) { DSRG_EMIT_MT(21); } else { DSRG_EMIT_MT(0); }
 #undef DSRG_EMIT_MT

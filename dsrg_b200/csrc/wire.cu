@@ -8,7 +8,8 @@
 // only where a value was below 1e-4.  So the wire format is:
 //   in : probs (float32, as is), cues as 1 bit/value (packed by host threads, SSE2 movemask)
 //   out: seeds as 1 bit/value, clamp mask as 1 bit/value (the host applies probs[i] = 1e-4 itself)
-// Everything is exact; a chunk whose cues are not all exactly 0 or 1 falls back to float transfer.
+// Everything is exact.  The seeds are the cues with grown pixels set to 1, so they are a 0/1 mask only when the cues
+// are: a chunk whose cues are not all exactly 0 or 1 sends its cues and its seeds as floats (the clamp mask stays).
 // The batch is cut into chunks that flow through three streams (H2D | kernels | D2H) while the
 // calling thread packs the next chunk and unpacks finished ones.
 #include <emmintrin.h>
@@ -344,7 +345,8 @@ static int host_pass_impl(Engine *e, int B, const float *labels, float *probs, c
         const double tp = omp_get_wtime();
         const bool ok = e->wire_compress != 0 && many_threads &&
                         pack_mask(cues + (size_t)b0 * img_elems, e->h_cbits + (size_t)b0 * wpi, img_elems, wpi, nb);
-        const bool ok_s = e->wire_compress != 0 && many_threads;
+        // seeds keep every cue value as it is (pylayers.py:271-275): as bits only when the cues were 0/1
+        const bool ok_s = ok;
         const bool ok_m = e->wire_compress != 0 && !srg_only;
         t_pack += omp_get_wtime() - tp;
         ti = omp_get_wtime();

@@ -2,6 +2,7 @@
 import hashlib
 import importlib.util
 import os
+import re
 
 import numpy as np
 
@@ -115,6 +116,131 @@ SWITCH_CASES = [("mixed224", 224, 224, ("noise", "smooth"), "gate1"),
                 ("noise105x105", 105, 105, ("noise", "noise"), "gate1")]
 COCO_SHAPE, COCO_M = (427, 640), 81                 # DenseCRF(W, H, 81) of the COCO tool at a COCO image's size
 WIDE_BIG_SHAPE, WIDE_BIG_M = (105, 105), 255        # the most labels, on a lattice above the capacity switch
+
+
+# ---- host-buffer pipeline: the cases of test_gpu_wire.py (checked on the CPU by test_wire_cpu.py) ----
+# What crosses PCIe in each wire mode (wire.cu: host_pass_impl): name -> (environment, host threads it runs with)
+WIRE_MODES = {
+    "bits": ({"DSRG_B200_HOST_THREADS": "8"}, 8),                           # cue bits, seed bits, clamp mask
+    "floats": ({"DSRG_B200_HOST_THREADS": "1"}, 1),                         # floats plus the clamp mask
+    "raw": ({"DSRG_B200_HOST_THREADS": "8", "DSRG_B200_WIRE": "0"}, 8),     # floats and a full probs D2H
+}
+# case -> steps; a step is (engine (maxB, Hcap, Wcap, M), image size (H, W), batch B, host chunk cap,
+# DSRG_B200_HOST_SCHEDULE or None).  Consecutive steps with the same engine tuple share one engine.
+WIRE_CASES = {
+    "bench": [((64, 321, 321, 21), (321, 321), 64, 0, None)],
+    "mixed_cues": [((12, 45, 52, 21), (45, 52), 12, 0, "3,4,5")],
+    "wide": [((6, 37, 45, 81), (37, 45), 6, 2, None)],
+    "reshaped": [((8, 64, 80, 21), (41, 41), 5, 0, None), ((8, 64, 80, 21), (64, 80), 8, 0, None),
+                 ((4, 2, 3, 21), (1, 1), 4, 0, "1,1,2"), ((4, 2, 3, 21), (2, 3), 4, 0, "1,1,2")],
+}
+WIRE_SF = {"bench": 1.0, "mixed_cues": 12.0, "wide": 1.0, "reshaped": 12.0}
+# cue values that are neither 0 nor 1, as (image, value); each goes on a class the image does not have, so it is
+# never grown over and must come back unchanged
+WIRE_NONBINARY = {"mixed_cues": [(3, 0.5), (5, 2.0), (6, -1.0)], "wide": [(3, 0.5), (3, 2.0), (3, -1.0)]}
+# probs values at the clamp's edge (pylayers.py:312: p[p < 1e-4] = 1e-4), on the last image of the first chunk, the
+# first image of the second and the batch's last image
+WIRE_EDGE_IMAGES = (4, 5, 63)
+WIRE_EDGE_PROBS = np.array([1e-4, np.nextafter(np.float32(1e-4), np.float32(0)), 0.0, -0.0, -1e-3,
+                            np.finfo(np.float32).smallest_subnormal], np.float32)
+
+
+def host_schedule(B, maxB, host_chunk=0, schedule=None):
+    """wire.cu:host_pass_impl's chunk sizes for a batch of B: DSRG_B200_HOST_SCHEDULE's sizes (each at most maxB
+    and what is left; parsing stops at the first entry atoi reads as < 1) with the rest cut into chunks of
+    host_chunk (or one), else five chunks that end at 5/64, 14/64, 27/64, 44/64 and all of the batch, each
+    capped at host_chunk."""
+    def atoi(s):
+        m = re.match(r"\s*([+-]?\d+)", s)
+        return int(m.group(1)) if m else 0
+
+    sizes, b = [], 0
+    if schedule is not None:
+        chunk = host_chunk if host_chunk > 0 else B
+        for tok in schedule.split(",") if schedule else []:
+            if b >= B:
+                break
+            v = atoi(tok)
+            if v < 1:
+                break
+            v = min(v, maxB, B - b)
+            sizes.append(v)
+            b += v
+        while b < B:
+            sizes.append(min(B - b, chunk))
+            b += sizes[-1]
+    if sizes:
+        return sizes
+    cap = host_chunk if host_chunk > 0 else B
+    edges = (5.0 / 64, 14.0 / 64, 27.0 / 64, 44.0 / 64, 1.0)
+    k = 0
+    while b < B:
+        end = int(edges[k] * B + 0.5) if k < 5 else B
+        k += 1
+        if end <= b:
+            continue
+        if end > B or k >= 5:
+            end = B
+        while b < end:
+            sizes.append(min(end - b, cap))
+            b += sizes[-1]
+    return sizes
+
+
+def wire_inputs(case, step):
+    """labels (B, M), probs and cues (B, M, H, W), image (B, H, W, 3) of one step of a WIRE_CASES case.  "bench" is
+    bench.py's batch (bench_unique repeated to 64) with WIRE_EDGE_PROBS on WIRE_EDGE_IMAGES; the others are seeded
+    synth batches with the case's WIRE_NONBINARY cue values."""
+    _, (H, W), B, _, _ = WIRE_CASES[case][step]
+    M = WIRE_CASES[case][step][0][3]
+    if case == "bench":
+        uniq = bench_unique("dsrg321", "smooth")
+        pick = np.arange(B) % len(uniq["probs"])
+        d = {k: uniq[k][pick] for k in ("labels", "probs", "cues", "image")}
+        for b in WIRE_EDGE_IMAGES:
+            d["probs"][b, 2, 10, 10:10 + WIRE_EDGE_PROBS.size] = WIRE_EDGE_PROBS
+        return d
+    tiny = H * W < 64
+    d = synth.make_batch(B, H, W, C=M, cues="random" if tiny else "cam", image="noise" if tiny else "smooth",
+                         start=700 + 10 * step)
+    d = {k: np.ascontiguousarray(d[k]) for k in ("labels", "probs", "cues", "image")}
+    used = {}
+    for b, v in WIRE_NONBINARY.get(case, []):
+        k = used[b] = used.get(b, -1) + 1
+        c = np.nonzero(d["labels"][b] == 0)[0][k]
+        d["cues"][b, c, 1 + k, 2 + 2 * k] = v
+    return d
+
+
+def chunk_of(sizes, b):
+    """Index of the chunk that holds image b."""
+    return int(np.searchsorted(np.cumsum(sizes), b, side="right"))
+
+
+def wire_call_marker(B, maxB, host_chunk, schedule):
+    """The line the worker writes to stderr before each host-buffer call: what the call's schedule derives from."""
+    return "[wire call] B=%d maxB=%d chunk=%d schedule=%s" % (B, maxB, host_chunk, schedule or "")
+
+
+def parse_wire_log(text):
+    """Host-buffer calls in a worker's stderr: one dict per wire_call_marker line, with the B / maxB / chunk /
+    schedule it states and what the library's DSRG_B200_DEBUG_TIMING lines that follow it report -- the chunk
+    sizes of the timeline ("[n img: ...]") and the totals line's "(threads N, chunks K)"."""
+    calls = []
+    for line in text.splitlines():
+        m = re.match(r"\[wire call\] B=(\d+) maxB=(\d+) chunk=(\d+) schedule=(\S*)$", line.strip())
+        if m:
+            calls.append({"B": int(m.group(1)), "maxB": int(m.group(2)), "chunk": int(m.group(3)),
+                          "schedule": m.group(4) or None, "sizes": None, "threads": None, "chunks": None})
+            continue
+        if not calls:
+            continue
+        if line.startswith("[dsrg host pass] timeline"):
+            calls[-1]["sizes"] = [int(v) for v in re.findall(r"\[(\d+) img:", line)]
+        m = re.match(r"\[dsrg host pass\] total .*\(threads (\d+), chunks (\d+)\)\s*$", line)
+        if m:
+            calls[-1]["threads"], calls[-1]["chunks"] = int(m.group(1)), int(m.group(2))
+    return calls
 
 
 def seeded_images(H, W, kinds, seed):
