@@ -243,6 +243,63 @@ def parse_wire_log(text):
     return calls
 
 
+def mf64_problem_params(sf, zero=None, n_iters=10):
+    """api.crf_params(sf) for an n_iters run, with w1 ("w1") or w2 ("w2") set to 0 to isolate one lattice."""
+    from dsrg_b200 import api
+    p = api.crf_params(sf, maxiter=n_iters)
+    if zero:
+        setattr(p, zero, 0.0)
+    return p
+
+
+# ---- float64 mean field: the cases of test_gpu_meanfield64.py (checked on the CPU by test_meanfield64_cpu.py) ----
+MF64_ITERS = (1, 2, 3, 10)
+MF64_GATE2_M = [6, 24, 32]
+MF64_WIDE_M = [M for M in WIDE_M if M in (33, 81, 128, 255)]
+# (H, W, image): N % 4 = 0, 1, 2, 3, so the last 4-pixel block of the lattice build has 0..3 phantom lanes
+MF64_TINY = [(4, 4, "noise"), (3, 7, "noise"), (5, 6, "noise"), (3, 5, "noise")]
+MF64_TINY_M, MF64_TINY_SEED = 5, 90
+# (path, zeroed weight): each case runs on one lattice only, so a failure names the lattice
+MF64_ZERO_W = [(path, w) for path in ("smem", "bi_direct", "sp_direct", "hybrid", "wide") for w in ("w1", "w2")]
+MF64_ZERO_W_M = {"smem": 6, "bi_direct": 6, "sp_direct": 6, "hybrid": 24, "wide": 33}
+MF64_PATH_CONFIG = {"smem": ("smooth", 1.0), "bi_direct": ("noise", 1.0), "sp_direct": ("smooth", 12.0)}
+
+# The bar of a case after n iterations: BAR_K times the largest max|Q32 - Q64| over the float32 models, at least
+# BAR_FLOOR.  The models are the oracle's sequential splat, three shuffled splat orders (the device's float atomics
+# add in no fixed order) and two draws of the device's own operation order (meanfield64 arith="device": folded
+# weights, an fma slice, exp with a seeded 2^-22 relative error, a reciprocal); each is one draw of float32 rounding
+# noise, and the device is one more draw of the same size.  After ten iterations on noise images that noise is
+# heavy-tailed (over 40 draws of the device model the largest error was up to 3x the median), so BAR_K = 4 leaves
+# room for the device's draw to land beyond the largest of the six we sampled without letting through an error that
+# is itself several times the float32 noise.  A bar belongs to one image.  BAR_FLOOR covers the
+# exp of ex2.approx where the models agree exactly (M = 1, where Q is 1): a 2^-22 relative error in the numerator and
+# in the sum of the soft-max, on a Q of at most 1, is at most 2^-21; the floor is twice that.
+BAR_K = 4.0
+BAR_FLOOR = 2.0 ** -20
+BAR_MODELS = [dict(splat_order=None), dict(splat_order=1), dict(splat_order=2), dict(splat_order=3),
+              dict(splat_order=4, arith="device"), dict(splat_order=5, arith="device", exp_seed=1)]
+
+
+def mf64_truth_and_bar(problem, unary, iters=MF64_ITERS, extra=()):
+    """(Q64 after every n of `iters`, {n: bar}, {n: largest model error}) for one image's (H, W, M) unary; `extra`
+    are more float32 runs (meanfield64.Problem.run keywords) returned as a list of {n: Q}.  The float64 run and the
+    models run on threads (numpy's gathers and scipy's sparse products release the GIL)."""
+    import numpy as np
+    from concurrent.futures import ThreadPoolExecutor
+    T = max(iters)
+    problem.norms(np.float64)
+    jobs = [dict(dtype=np.float64)] + [dict(dtype=np.float32, **m) for m in BAR_MODELS] + \
+        [dict(dtype=np.float32, **e) for e in extra]
+    for j in jobs:
+        problem.norms(j["dtype"], j.get("splat_order"))
+    with ThreadPoolExecutor(min(len(jobs), os.cpu_count() or 1)) as ex:
+        runs = list(ex.map(lambda kw: problem.run(unary, T, **kw), jobs))
+    q64 = {n: runs[0][n] for n in iters}
+    spread = {n: max(float(np.abs(r[n] - q64[n]).max()) for r in runs[1:1 + len(BAR_MODELS)]) for n in iters}
+    bar = {n: max(BAR_K * spread[n], BAR_FLOOR) for n in iters}
+    return q64, bar, spread, [{n: r[n] for n in iters} for r in runs[1 + len(BAR_MODELS):]]
+
+
 def seeded_images(H, W, kinds, seed):
     return np.stack([synth.make_image(np.random.RandomState(seed + b), H, W, k) for b, k in enumerate(kinds)])
 
