@@ -238,11 +238,6 @@ static int crf_core(Engine *e, int B, const float *unary, int layout, bool clamp
     return meanfield_run(e, B, unary, layout, clamp, unary_rw, *p, s);
 }
 
-int crf_core_for_post(Engine *e, const float *unary_hwc, const uint8_t *image, const dsrg_crf_params *p,
-                      cudaStream_t s) {
-    return crf_core(e, 1, unary_hwc, DSRG_LAYOUT_NHWC, false, nullptr, image, p, s);
-}
-
 int crf_core_batch_for_post(Engine *e, int B, const float *unary_hwc, const uint8_t *images,
                             const dsrg_crf_params *p, cudaStream_t s) {
     return crf_core(e, B, unary_hwc, DSRG_LAYOUT_NHWC, false, nullptr, images, p, s);
@@ -272,6 +267,7 @@ int ensure_staging(Engine *e) {
     rc |= dalloc(e, &e->st_labels, (size_t)e->maxB * e->M);
     rc |= dalloc(e, &e->st_image, (size_t)e->maxB * e->Ncap * 3);
     rc |= dalloc(e, &e->st_lmap, (size_t)e->maxB * e->Ncap);
+    rc |= dalloc(e, &e->st_sel, (size_t)e->M);
     return rc ? DSRG_E_NOMEM : DSRG_OK;
 }
 
@@ -478,7 +474,7 @@ void dsrg_engine_destroy(dsrg_engine *h) {
     void *ptrs[] = {e->U, e->Q0, e->spA, e->spB, e->spC, e->biA, e->biB, e->biC, e->nvA, e->nvB, e->lmap,
                     e->lflag, e->parent, e->hc, e->loss_acc, e->sec_rec, e->sec_img, e->sec_part, e->sec_w, e->dev_err,
                     e->hy_list, e->hy_count, e->st_unary, e->st_out, e->st_cues, e->st_labels, e->st_image, e->st_lmap, e->st_raw, e->st_idx,
-                    e->st_prep};
+                    e->st_prep, e->st_sel};
     for (void *p : ptrs) cudaFree(p);
     if (e->own_stream) cudaStreamDestroy(e->own_stream);
     if (e->in_stream) cudaStreamDestroy(e->in_stream);

@@ -213,6 +213,7 @@ struct Engine {
     // staging for the *_host entry points
     float *st_unary = nullptr, *st_out = nullptr, *st_cues = nullptr, *st_labels = nullptr;
     uint8_t *st_image = nullptr;
+    int32_t *st_sel = nullptr;  // [M] label selection of dsrg_predict_mask_*, written by its pass (post.cu)
     // staging whose size depends on the call, grown on demand (grow_staging); capacities in bytes
     float *st_raw = nullptr;   // raw (un-zoomed) images and score maps of the *_host entry points
     size_t st_raw_cap = 0;

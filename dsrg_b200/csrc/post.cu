@@ -15,29 +15,55 @@
 // so with identical scores the unary handed to the CRF differs from the reference's only by the ulps of
 // expf/logf; the label map then follows the CRF's 1e-4 parity bound (ties within it may flip).
 //
-// dsrg_predict_mask_{dev,host} run one image per call on a batch-1 engine; dsrg_predict_mask_batch_{dev,host} run
-// B images of one size per pass (every scale's zoom and the sum in one launch, the batched CRF, a per-image label
-// selection read from device memory), with the per-image arithmetic, so without the CRF they are bit-identical.
+// One pass serves every entry point: B images of one size (every scale's zoom and the sum in one launch, the batched
+// CRF, a per-image label selection read from device memory).  dsrg_predict_mask_{dev,host} are that pass at B = 1,
+// their selection written into the engine by the pass; dsrg_zoom_scores_* is its zoom kernel on one scale.
 #include "common.cuh"
 #include "zoom.cuh"
 
 namespace dsrg {
 
-// in [M][h][w] float32 (the blob the reference transposes to (h,w,M) before zooming) -> out [H][W][M]
-template <bool ACC>
-__global__ void __launch_bounds__(kThreads)
-k_zoom_scores(const float *__restrict__ in, float *out, int M, int hi, int wi, int Ho, int Wo) {
+constexpr int kPostMaxScales = 16;
+
+// one batched network forward per scale: scale k is [B][M][h[k]][w[k]] float32 at p[k]
+struct ZoomScales {  // 264 bytes of kernel parameters
+    const float *p[kPostMaxScales];
+    int h[kPostMaxScales], w[kPostMaxScales];
+    int n;
+};
+
+// out [B][H][W][M] = sum_k zoom(scores_k[b]), one thread per output element, image b = blockIdx.y.  The float32 sum
+// is formed in the order of test-ms.py:97: scale 0 stored, then += each further scale; with `accumulate` every scale
+// is added to what out holds (`scores_all += scores`).  Capped at 40 registers, so that 6 CTAs fit on an SM: the
+// float64 tap arithmetic is latency-bound (one 81-label scale of a COCO-sized image: 248 us against 256 at 46
+// registers, H100 SXM at 700 W).
+__global__ void __launch_bounds__(kThreads, 6)
+k_zoom_sum_batch(ZoomScales sc, float *__restrict__ out, int M, int Ho, int Wo, int accumulate) {
     const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    if (idx >= (long long)Ho * Wo * M) return;
-    const int c = (int)(idx % M);
-    const int pix = (int)(idx / M);
+    const long long NM = (long long)Ho * Wo * M;
+    if (idx >= NM) return;
+    const int b = blockIdx.y, c = (int)(idx % M), pix = (int)(idx / M);
     const int oy = pix / Wo, ox = pix - oy * Wo;
-    const float z = zoom_apply(in + (size_t)c * hi * wi, wi, zoom_tap(oy, ox, hi, wi, Ho, Wo));
-    out[idx] = ACC ? __fadd_rn(out[idx], z) : z;  // scores_all += scores (float32)
+    out += b * NM;
+    float acc = accumulate ? out[idx] : 0.f;
+#pragma unroll
+    for (int k = 0; k < kPostMaxScales; k++) {
+        if (k >= sc.n) break;
+        const int hi = sc.h[k], wi = sc.w[k];
+        const float z = zoom_apply(sc.p[k] + ((size_t)b * M + c) * hi * wi, wi, zoom_tap(oy, ox, hi, wi, Ho, Wo));
+        acc = k || accumulate ? __fadd_rn(acc, z) : z;
+    }
+    out[idx] = acc;
 }
 
-// softmax over the labels of every pixel, strides in elements: label stride ls, pixel stride ps
-// (CHW blob: ls = npix, ps = 1; HWC map: ls = 1, ps = M).  Mirrors
+static void zoom_sum(Engine *e, int B, const ZoomScales &sc, float *out, int accumulate, cudaStream_t s) {
+    const dim3 g(cdiv((long long)e->N * e->M, kThreads), B);
+    DSRG_LAUNCH(e, T_POST, s, k_zoom_sum_batch<<<g, kThreads, 0, s>>>(sc, out, e->M, e->H, e->W, accumulate));
+}
+
+// softmax over the labels of every pixel of B images of npix pixels: pixel i of image b = blockIdx.y starts at
+// b * M * npix + i * ps and its labels are ls apart ([B][M][npix] blob: ls = npix, ps = 1; [B][npix][M] map: ls = 1,
+// ps = M).  Mirrors
 //   e = np.exp(s - np.max(s)); p = e / np.sum(e)            (float32)
 // and, when CLAMPLOG, the clamp at eps followed by np.log; `probs` (optional) receives the clamped p.
 template <bool CLAMPLOG>
@@ -46,7 +72,8 @@ k_post_softmax(const float *in, float *out, float *probs, int npix, int M, long 
                float eps) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= npix) return;
-    const float *s = in + (size_t)i * ps;
+    const size_t base = (size_t)blockIdx.y * M * npix + (size_t)i * ps;
+    const float *s = in + base;
     float v[DSRG_MAX_LABELS];
     float m = -INFINITY;
 #pragma unroll
@@ -68,10 +95,10 @@ k_post_softmax(const float *in, float *out, float *probs, int npix, int M, long 
             float p = __fdiv_rn(v[l], sum);
             if (CLAMPLOG) {
                 if (p < eps) p = eps;
-                if (probs) probs[(size_t)i * ps + (size_t)l * ls] = p;
+                if (probs) probs[base + (size_t)l * ls] = p;
                 p = logf(p);
             }
-            out[(size_t)i * ps + (size_t)l * ls] = p;
+            out[base + (size_t)l * ls] = p;
         }
 }
 
@@ -84,8 +111,9 @@ k_post_softmax_wide(const float *in, float *out, float *probs, int npix, int M, 
                     float eps) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= npix) return;
-    const float *s = in + (size_t)i * ps;
-    float *o = out + (size_t)i * ps;
+    const size_t base = (size_t)blockIdx.y * M * npix + (size_t)i * ps;
+    const float *s = in + base;
+    float *o = out + base;
     float m = -INFINITY;
     for (int l = 0; l < M; l++) m = fmaxf(m, s[(size_t)l * ls]);
     float sum = 0.f;
@@ -98,7 +126,7 @@ k_post_softmax_wide(const float *in, float *out, float *probs, int npix, int M, 
         float p = __fdiv_rn(o[(size_t)l * ls], sum);
         if (CLAMPLOG) {
             if (p < eps) p = eps;
-            if (probs) probs[(size_t)i * ps + (size_t)l * ls] = p;
+            if (probs) probs[base + (size_t)l * ls] = p;
             p = logf(p);
         }
         o[(size_t)l * ls] = p;
@@ -106,11 +134,13 @@ k_post_softmax_wide(const float *in, float *out, float *probs, int npix, int M, 
 }
 
 template <bool CLAMPLOG>
-static void post_softmax(Engine *e, const float *in, float *out, float *probs, int npix, long long ls, long long ps,
-                         float eps, cudaStream_t s) {
-    const int g = cdiv(npix, kThreads), M = e->M;
+static void post_softmax(Engine *e, const float *in, float *out, float *probs, int B, int npix, long long ls,
+                         long long ps, float eps, cudaStream_t s) {
+    const dim3 g(cdiv(npix, kThreads), B);
+    const int M = e->M;
     if (M > DSRG_MAX_LABELS)
-        DSRG_LAUNCH(e, T_POST, s, k_post_softmax_wide<CLAMPLOG><<<g, kThreads, 0, s>>>(in, out, probs, npix, M, ls, ps, eps));
+        DSRG_LAUNCH(e, T_POST, s,
+                    k_post_softmax_wide<CLAMPLOG><<<g, kThreads, 0, s>>>(in, out, probs, npix, M, ls, ps, eps));
     else
         DSRG_LAUNCH(e, T_POST, s, k_post_softmax<CLAMPLOG><<<g, kThreads, 0, s>>>(in, out, probs, npix, M, ls, ps, eps));
 }
@@ -126,199 +156,14 @@ k_post_clamp_log(const float *in, float *out, float *probs, long long n, float e
     out[i] = logf(p);
 }
 
-struct LabelSel {   // 1 KB of kernel parameters
-    int n;
-    int id[DSRG_MAX_LABELS_WIDE];
+// One selection row of k_post_argmax_batch, by value: the per-image entry points take their selection from host
+// memory the caller may reuse at once, and a replayed graph or a caller's capture has to write the same ids again.
+struct LabelRow {  // 1 KB of kernel parameters
+    int32_t id[DSRG_MAX_LABELS_WIDE];
 };
 
-// np.argmax (first maximum) over the selected labels, result = the selected label's id
-__global__ void __launch_bounds__(kThreads)
-k_post_argmax(const float *q, int32_t *out, int npix, long long ls, long long ps, LabelSel sel) {
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= npix) return;
-    const float *s = q + (size_t)i * ps;
-    float best = s[(size_t)sel.id[0] * ls];
-    int arg = sel.id[0];
-    for (int k = 1; k < sel.n; k++) {
-        const float v = s[(size_t)sel.id[k] * ls];
-        if (v > best) {
-            best = v;
-            arg = sel.id[k];
-        }
-    }
-    out[i] = arg;
-}
-
-int zoom_scores(Engine *e, const float *in, int hi, int wi, float *out, int accumulate, cudaStream_t s) {
-    const long long n = (long long)e->N * e->M;
-    const int g = cdiv(n, kThreads);
-    if (accumulate)
-        DSRG_LAUNCH(e, T_POST, s, k_zoom_scores<true><<<g, kThreads, 0, s>>>(in, out, e->M, hi, wi, e->H, e->W));
-    else
-        DSRG_LAUNCH(e, T_POST, s, k_zoom_scores<false><<<g, kThreads, 0, s>>>(in, out, e->M, hi, wi, e->H, e->W));
-    DSRG_CUDA_TRY(cudaGetLastError());
-    return DSRG_OK;
-}
-
-int crf_core_for_post(Engine *e, const float *unary_hwc, const uint8_t *image, const dsrg_crf_params *p,
-                      cudaStream_t s);  // api.cu
-
-static int predict_mask_body(Engine *e, int mode, int n_scales, const float *const *scores, const int *hs, const int *ws,
-                             const uint8_t *image, float eps, int smooth, const dsrg_crf_params *p, const LabelSel &sel,
-                             int32_t *result, float *probs_out, cudaStream_t s) {
-    int rc;
-    const int N = e->N, M = e->M;
-    float *unary = e->st_unary;                       // [H][W][M]
-    float *clamped = smooth ? nullptr : (probs_out ? probs_out : e->st_out);
-    if (mode == DSRG_POST_SUM_SCORES) {
-        for (int k = 0; k < n_scales; k++)
-            if ((rc = zoom_scores(e, scores[k], hs[k], ws[k], unary, k > 0, s))) return rc;
-        post_softmax<true>(e, unary, unary, clamped, N, 1, M, eps, s);
-    } else {
-        const int np = hs[0] * ws[0];
-        float *small = e->st_cues;                    // [M][h][w] probabilities at network resolution
-        post_softmax<false>(e, scores[0], small, nullptr, np, np, 1, eps, s);
-        if ((rc = zoom_scores(e, small, hs[0], ws[0], unary, 0, s))) return rc;
-        const long long n = (long long)N * M;
-        DSRG_LAUNCH(e, T_POST, s, k_post_clamp_log<<<cdiv(n, kThreads), kThreads, 0, s>>>(unary, unary, clamped, n, eps));
-    }
-    DSRG_CUDA_TRY(cudaGetLastError());
-    if (smooth) {
-        if ((rc = crf_core_for_post(e, unary, image, p, s))) return rc;
-        if (probs_out && (rc = meanfield_export(e, 1, probs_out, DSRG_LAYOUT_NHWC, s))) return rc;
-        DSRG_LAUNCH(e, T_POST, s, k_post_argmax<<<cdiv(N, kThreads), kThreads, 0, s>>>(e->Qcur, result, N, N, 1, sel));
-    } else {
-        DSRG_LAUNCH(e, T_POST, s, k_post_argmax<<<cdiv(N, kThreads), kThreads, 0, s>>>(clamped, result, N, 1, M, sel));
-    }
-    DSRG_CUDA_TRY(cudaGetLastError());
-    return DSRG_OK;
-}
-
-static int predict_mask(Engine *e, int mode, int n_scales, const float *const *scores, const int *hs,
-                        const int *ws, const uint8_t *image, float eps, int smooth, const dsrg_crf_params *p,
-                        const int32_t *labels_sel, int n_sel, int32_t *result, float *probs_out,
-                        cudaStream_t s) {
-    if (mode != DSRG_POST_SUM_SCORES && mode != DSRG_POST_ZOOM_PROBS) {
-        set_error("bad mode %d", mode);
-        return DSRG_E_INVALID;
-    }
-    if (n_scales < 1 || (mode == DSRG_POST_ZOOM_PROBS && n_scales != 1) || n_sel < 0 || n_sel > DSRG_MAX_LABELS_WIDE) {
-        set_error("bad argument (NULL pointer or value out of range)");
-        return DSRG_E_INVALID;
-    }
-    LabelSel sel;
-    sel.n = n_sel ? n_sel : e->M;
-    for (int k = 0; k < sel.n; k++) {
-        sel.id[k] = n_sel ? labels_sel[k] : k;
-        if (sel.id[k] < 0 || sel.id[k] >= e->M) {
-            set_error("selected label %d outside [0, %d)", sel.id[k], e->M);
-            return DSRG_E_INVALID;
-        }
-    }
-    for (int k = 0; k < n_scales; k++)
-        if (!scores[k] || hs[k] < 1 || ws[k] < 1 || (long long)hs[k] * ws[k] > e->Ncap) {
-            set_error("score map %d: bad pointer or size %dx%d (capacity %d pixels)", k, hs[k], ws[k], e->Ncap);
-            return DSRG_E_INVALID;
-        }
-    int rc = ensure_staging(e);
-    if (rc) return rc;
-    // the whole post-processing of one image as one graph per (shape, score sizes, options): the evaluation tools
-    // meet the same few dozen image sizes over and over (api.cu:post_pass_needs_spatial)
-    const bool rebuild = smooth && post_pass_needs_spatial(e, p);
-    GraphKey key;
-    key.add(6).add(e->H).add(e->W).add(mode).add(n_scales).add(image).add(eps).add(smooth).add(result).add(probs_out).add(rebuild);
-    for (int k = 0; k < n_scales; k++) key.add(scores[k]).add(hs[k]).add(ws[k]);
-    if (smooth) key.add(*p);
-    for (int k = 0; k < sel.n; k++) key.add(sel.id[k]);
-    if (rebuild) e->sp_valid = false;
-    rc = run_pass(e, s, key, true, [&]() { return predict_mask_body(e, mode, n_scales, scores, hs, ws, image, eps, smooth, p, sel, result, probs_out, s); });
-    if (smooth) post_pass_done(e, p, 1, rc);
-    return rc;
-}
-
-// ---- B images of the engine's size in one pass (dsrg_predict_mask_batch_*) ----
-// The per-image pass above is ~90 dependent launches whatever the image holds: at batch 1 it is bound by launch
-// latency.  The batched pass issues the same stages once for B images, and its CRF is the batched mean field.
-
-constexpr int kPostMaxScales = 16;
-
-// one batched network forward per scale: scale k is [B][M][h[k]][w[k]] float32 at p[k]
-struct ZoomScales {  // 264 bytes of kernel parameters
-    const float *p[kPostMaxScales];
-    int h[kPostMaxScales], w[kPostMaxScales];
-    int n;
-};
-
-// out [B][H][W][M] = sum_k zoom(scores_k[b]), one thread per output element.  The float32 sum is formed in the
-// per-image pass's order (scale 0 stored, then += each further scale, test-ms.py:97), so it is bit-identical.
-__global__ void __launch_bounds__(kThreads)
-k_zoom_sum_batch(ZoomScales sc, float *__restrict__ out, int B, int M, int Ho, int Wo) {
-    const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    const long long N = (long long)Ho * Wo;
-    if (idx >= (long long)B * N * M) return;
-    const int c = (int)(idx % M);
-    const long long bp = idx / M;
-    const int b = (int)(bp / N), pix = (int)(bp - b * N);
-    const int oy = pix / Wo, ox = pix - oy * Wo;
-    float acc = 0.f;
-#pragma unroll
-    for (int k = 0; k < kPostMaxScales; k++) {
-        if (k >= sc.n) break;
-        const int hi = sc.h[k], wi = sc.w[k];
-        const float z = zoom_apply(sc.p[k] + ((size_t)b * M + c) * hi * wi, wi, zoom_tap(oy, ox, hi, wi, Ho, Wo));
-        acc = k ? __fadd_rn(acc, z) : z;
-    }
-    out[idx] = acc;
-}
-
-// The soft-max at network resolution of generate_train_gt.py:88-89 over a [B][M][np] blob, pixel i of image b at
-// b * M * np + i: the float32 operations of k_post_softmax<false> (label stride np) in the same order
-__global__ void __launch_bounds__(kThreads)
-k_net_softmax_batch(const float *__restrict__ in, float *__restrict__ out, int B, int M, int np) {
-    const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    if (t >= (long long)B * np) return;
-    const int b = (int)(t / np), i = (int)(t - (long long)b * np);
-    const size_t base = (size_t)b * M * np + i;
-    const float *s = in + base;
-    float *o = out + base;
-    float v[DSRG_MAX_LABELS];
-    float m = -INFINITY;
-#pragma unroll
-    for (int l = 0; l < DSRG_MAX_LABELS; l++)
-        if (l < M) {
-            v[l] = s[(size_t)l * np];
-            m = fmaxf(m, v[l]);
-        }
-    float sum = 0.f;
-#pragma unroll
-    for (int l = 0; l < DSRG_MAX_LABELS; l++)
-        if (l < M) {
-            v[l] = expf(__fsub_rn(v[l], m));
-            sum = __fadd_rn(sum, v[l]);
-        }
-#pragma unroll
-    for (int l = 0; l < DSRG_MAX_LABELS; l++)
-        if (l < M) o[(size_t)l * np] = __fdiv_rn(v[l], sum);
-}
-
-// the same above DSRG_MAX_LABELS: exp(s - max) is parked in `out`, as k_post_softmax_wide does
-__global__ void __launch_bounds__(kThreads)
-k_net_softmax_batch_wide(const float *__restrict__ in, float *__restrict__ out, int B, int M, int np) {
-    const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    if (t >= (long long)B * np) return;
-    const int b = (int)(t / np), i = (int)(t - (long long)b * np);
-    const size_t base = (size_t)b * M * np + i;
-    const float *s = in + base;
-    float *o = out + base;
-    float m = -INFINITY;
-    for (int l = 0; l < M; l++) m = fmaxf(m, s[(size_t)l * np]);
-    float sum = 0.f;
-    for (int l = 0; l < M; l++) {
-        const float v = expf(__fsub_rn(s[(size_t)l * np], m));
-        o[(size_t)l * np] = v;
-        sum = __fadd_rn(sum, v);
-    }
-    for (int l = 0; l < M; l++) o[(size_t)l * np] = __fdiv_rn(o[(size_t)l * np], sum);
+__global__ void __launch_bounds__(kThreads) k_post_sel_row(LabelRow row, int32_t *sel, int M) {
+    for (int k = threadIdx.x; k < M; k += blockDim.x) sel[k] = row.id[k];
 }
 
 // Per (pixel, image b = blockIdx.y): np.argmax (first maximum) over image b's selected labels, result = the label's
@@ -333,7 +178,7 @@ k_post_argmax_batch(const float *q, int32_t *out, int N, int M, long long ls, lo
     for (int k = threadIdx.x; k < M; k += blockDim.x) s_id[k] = sel ? sel[(size_t)b * M + k] : k;
     __syncthreads();
     if (threadIdx.x == 0) {
-        int n = 0;
+        int n = sel ? 0 : M;  // without a selection there is no row to scan
         while (n < M && s_id[n] != -1) {
             if (s_id[n] < 0 || s_id[n] >= M) {
                 n = -1;
@@ -370,28 +215,29 @@ k_post_argmax_batch(const float *q, int32_t *out, int N, int M, long long ls, lo
 int crf_core_batch_for_post(Engine *e, int B, const float *unary_hwc, const uint8_t *images,
                             const dsrg_crf_params *p, cudaStream_t s);  // api.cu
 
+// sel: device rows as k_post_argmax_batch reads them, or NULL; row (B = 1): a selection written to st_sel by the pass
 static int predict_mask_batch_body(Engine *e, int B, int mode, const ZoomScales &sc, const uint8_t *images, float eps,
-                                   int smooth, const dsrg_crf_params *p, const int32_t *sel, int32_t *result,
-                                   float *probs_out, cudaStream_t s) {
+                                   int smooth, const dsrg_crf_params *p, const int32_t *sel, const LabelRow *row,
+                                   int32_t *result, float *probs_out, cudaStream_t s) {
     const int N = e->N, M = e->M;
     const long long n = (long long)B * N * M;
     float *unary = e->st_unary;                       // [B][H][W][M]
     float *clamped = smooth ? nullptr : (probs_out ? probs_out : e->st_out);
     if (mode == DSRG_POST_SUM_SCORES) {
-        DSRG_LAUNCH(e, T_POST, s, k_zoom_sum_batch<<<cdiv(n, kThreads), kThreads, 0, s>>>(sc, unary, B, M, e->H, e->W));
-        post_softmax<true>(e, unary, unary, clamped, B * N, 1, M, eps, s);  // NHWC is contiguous across the batch
+        zoom_sum(e, B, sc, unary, 0, s);
+        post_softmax<true>(e, unary, unary, clamped, B, N, 1, M, eps, s);
     } else {
         const int np = sc.h[0] * sc.w[0];
         float *small = e->st_cues;                    // [B][M][h][w] probabilities at network resolution
-        const int g = cdiv((long long)B * np, kThreads);
-        if (M > DSRG_MAX_LABELS)
-            DSRG_LAUNCH(e, T_POST, s, k_net_softmax_batch_wide<<<g, kThreads, 0, s>>>(sc.p[0], small, B, M, np));
-        else
-            DSRG_LAUNCH(e, T_POST, s, k_net_softmax_batch<<<g, kThreads, 0, s>>>(sc.p[0], small, B, M, np));
+        post_softmax<false>(e, sc.p[0], small, nullptr, B, np, np, 1, eps, s);
         ZoomScales zs = sc;
         zs.p[0] = small;
-        DSRG_LAUNCH(e, T_POST, s, k_zoom_sum_batch<<<cdiv(n, kThreads), kThreads, 0, s>>>(zs, unary, B, M, e->H, e->W));
+        zoom_sum(e, B, zs, unary, 0, s);
         DSRG_LAUNCH(e, T_POST, s, k_post_clamp_log<<<cdiv(n, kThreads), kThreads, 0, s>>>(unary, unary, clamped, n, eps));
+    }
+    if (row) {
+        DSRG_LAUNCH(e, T_POST, s, k_post_sel_row<<<1, kThreads, 0, s>>>(*row, e->st_sel, M));
+        sel = e->st_sel;
     }
     DSRG_CUDA_TRY(cudaGetLastError());
     const dim3 ga(cdiv(N, kThreads), B);
@@ -428,7 +274,8 @@ static int post_batch_check(const Engine *e, int mode, int n_scales, const float
 
 static int predict_mask_batch(Engine *e, int B, int mode, int n_scales, const float *const *scores, const int *hs,
                               const int *ws, const uint8_t *images, float eps, int smooth, const dsrg_crf_params *p,
-                              const int32_t *sel, int32_t *result, float *probs_out, cudaStream_t s) {
+                              const int32_t *sel, const LabelRow *row, int32_t *result, float *probs_out,
+                              cudaStream_t s) {
     int rc = post_batch_check(e, mode, n_scales, scores, hs, ws);
     if (rc || (rc = ensure_staging(e))) return rc;
     ZoomScales sc = {};
@@ -438,37 +285,109 @@ static int predict_mask_batch(Engine *e, int B, int mode, int n_scales, const fl
         sc.h[k] = hs[k];
         sc.w[k] = ws[k];
     }
-    // the selection is read by the pass, so its content is not part of the key: a replay follows what sel holds
+    // the pass reads sel, so its content is not part of the key: a replay follows what sel holds.  A row is a kernel
+    // parameter of the pass, so a replay writes the ids it was captured with: they are part of the key.
     const bool rebuild = smooth && post_pass_needs_spatial(e, p);
     GraphKey key;
     key.add(7).add(B).add(e->H).add(e->W).add(mode).add(n_scales).add(images).add(eps).add(smooth).add(sel)
-        .add(result).add(probs_out).add(rebuild);
+        .add(result).add(probs_out).add(rebuild).add(row != nullptr);
     for (int k = 0; k < n_scales; k++) key.add(scores[k]).add(hs[k]).add(ws[k]);
     if (smooth) key.add(*p);
+    if (row) key.add(*row);
     if (rebuild) e->sp_valid = false;
     rc = run_pass(e, s, key, true, [&]() {
-        return predict_mask_batch_body(e, B, mode, sc, images, eps, smooth, p, sel, result, probs_out, s);
+        return predict_mask_batch_body(e, B, mode, sc, images, eps, smooth, p, sel, row, result, probs_out, s);
     });
     if (smooth) post_pass_done(e, p, B, rc);
     return rc;
+}
+
+// The *_host entry points: the score maps, the images (when smoothing) and the selection rows in through the
+// engine's staging, the pass, the label maps (and probabilities) back.  sel: host [B][M] rows, or NULL.
+static int predict_mask_staged(Engine *e, int B, int mode, int n_scales, const float *const *scores, const int *hs,
+                               const int *ws, const uint8_t *images, float eps, int smooth, const dsrg_crf_params *p,
+                               const int32_t *sel, const LabelRow *row, int32_t *result_out, float *probs_out,
+                               cudaStream_t s) {
+    const int M = e->M;
+    if (int rc = post_batch_check(e, mode, n_scales, scores, hs, ws)) return rc;
+    for (int b = 0; sel && b < B; b++)
+        for (int k = 0; k < M && sel[(size_t)b * M + k] != -1; k++) {
+            const int v = sel[(size_t)b * M + k];
+            if (v < 0 || v >= M) {
+                set_error("image %d: selected label %d outside [0, %d)", b, v, M);
+                return DSRG_E_INVALID;
+            }
+        }
+    size_t total = 0;
+    for (int k = 0; k < n_scales; k++) total += (size_t)B * M * hs[k] * ws[k];
+    if (int rc = grow_staging(e, (void **)&e->st_raw, &e->st_raw_cap, total * sizeof(float))) return rc;
+    if (sel)
+        if (int rc = grow_staging(e, (void **)&e->st_idx, &e->st_idx_cap, (size_t)B * M * sizeof(int32_t)))
+            return rc;
+    const float *dptr[kPostMaxScales];
+    size_t at = 0;
+    for (int k = 0; k < n_scales; k++) {
+        const size_t n = (size_t)B * M * hs[k] * ws[k];
+        DSRG_CUDA_TRY(cudaMemcpyAsync(e->st_raw + at, scores[k], n * sizeof(float), cudaMemcpyHostToDevice, s));
+        dptr[k] = e->st_raw + at;
+        at += n;
+    }
+    if (smooth)
+        DSRG_CUDA_TRY(cudaMemcpyAsync(e->st_image, images, (size_t)B * e->N * 3, cudaMemcpyHostToDevice, s));
+    if (sel)
+        DSRG_CUDA_TRY(cudaMemcpyAsync(e->st_idx, sel, (size_t)B * M * sizeof(int32_t), cudaMemcpyHostToDevice, s));
+    if (int rc = predict_mask_batch(e, B, mode, n_scales, dptr, hs, ws, e->st_image, eps, smooth, p,
+                                    sel ? e->st_idx : nullptr, row, e->st_lmap, probs_out ? e->st_out : nullptr, s))
+        return rc;
+    DSRG_CUDA_TRY(cudaMemcpyAsync(result_out, e->st_lmap, (size_t)B * e->N * sizeof(int32_t),
+                                  cudaMemcpyDeviceToHost, s));
+    if (probs_out)
+        DSRG_CUDA_TRY(cudaMemcpyAsync(probs_out, e->st_out, (size_t)B * e->N * M * sizeof(float),
+                                      cudaMemcpyDeviceToHost, s));
+    return DSRG_OK;
+}
+
+// labels_sel / n_sel of the per-image entry points as one selection row: each id's first occurrence, in the caller's
+// order (the arg-max keeps the first strict maximum, so a repeated id never wins again), then -1
+static int label_row(const Engine *e, const int32_t *labels_sel, int n_sel, LabelRow *row) {
+    bool seen[DSRG_MAX_LABELS_WIDE] = {};
+    int n = 0;
+    for (int k = 0; k < n_sel; k++) {
+        const int v = labels_sel[k];
+        if (v < 0 || v >= e->M) {
+            set_error("selected label %d outside [0, %d)", v, e->M);
+            return DSRG_E_INVALID;
+        }
+        if (!seen[v]) {
+            seen[v] = true;
+            row->id[n++] = v;
+        }
+    }
+    for (int k = n; k < DSRG_MAX_LABELS_WIDE; k++) row->id[k] = -1;
+    return DSRG_OK;
 }
 
 }  // namespace dsrg
 
 using namespace dsrg;
 
-// a predict_mask call's pointers: the score maps, hs / ws and the result always; the image and the CRF parameters
-// when it smooths; the label selection when it has one
-static bool post_args_ok(const float *const *scores, const int *hs, const int *ws, const uint8_t *image, int smooth,
-                         const dsrg_crf_params *params, const int32_t *labels_sel, int n_sel, const int32_t *result) {
-    return scores && hs && ws && result && (!smooth || (image && params)) && (n_sel <= 0 || labels_sel);
+// a predict_mask call's arguments: 1 to kPostMaxScales score maps, their pointers, hs / ws and the result always;
+// the image and the CRF parameters when it smooths; the label selection when it has one
+static bool post_args_ok(int n_scales, const float *const *scores, const int *hs, const int *ws, const uint8_t *image,
+                         int smooth, const dsrg_crf_params *params, const int32_t *labels_sel, int n_sel,
+                         const int32_t *result) {
+    return n_scales >= 1 && n_scales <= kPostMaxScales && scores && hs && ws && result &&
+           (!smooth || (image && params)) && n_sel >= 0 && n_sel <= DSRG_MAX_LABELS_WIDE && (n_sel == 0 || labels_sel);
 }
 
 extern "C" int dsrg_zoom_scores_dev(dsrg_engine *h, const float *scores_dev, int hi, int wi, float *out_dev,
                                     int accumulate, void *stream) {
     const cudaStream_t s = (cudaStream_t)stream;
-    return dev_call(h, 1, s, scores_dev && out_dev && hi >= 1 && wi >= 1,
-                    [&](Engine *e) { return zoom_scores(e, scores_dev, hi, wi, out_dev, accumulate, s); });
+    return dev_call(h, 1, s, scores_dev && out_dev && hi >= 1 && wi >= 1, [&](Engine *e) {
+        zoom_sum(e, 1, {{scores_dev}, {hi}, {wi}, 1}, out_dev, accumulate, s);
+        DSRG_CUDA_TRY(cudaGetLastError());
+        return DSRG_OK;
+    });
 }
 
 extern "C" int dsrg_zoom_scores_host(dsrg_engine *h, const float *scores, int hi, int wi, float *out,
@@ -479,7 +398,8 @@ extern "C" int dsrg_zoom_scores_host(dsrg_engine *h, const float *scores, int hi
         DSRG_CUDA_TRY(cudaMemcpyAsync(e->st_raw, scores, nin * sizeof(float), cudaMemcpyHostToDevice, s));
         if (accumulate)
             DSRG_CUDA_TRY(cudaMemcpyAsync(e->st_unary, out, nout * sizeof(float), cudaMemcpyHostToDevice, s));
-        if (int rc = zoom_scores(e, e->st_raw, hi, wi, e->st_unary, accumulate, s)) return rc;
+        zoom_sum(e, 1, {{e->st_raw}, {hi}, {wi}, 1}, e->st_unary, accumulate, s);
+        DSRG_CUDA_TRY(cudaGetLastError());
         DSRG_CUDA_TRY(cudaMemcpyAsync(out, e->st_unary, nout * sizeof(float), cudaMemcpyDeviceToHost, s));
         return DSRG_OK;
     });
@@ -490,10 +410,13 @@ extern "C" int dsrg_predict_mask_dev(dsrg_engine *h, int mode, int n_scales, con
                                      int smooth, const dsrg_crf_params *params, const int32_t *labels_sel,
                                      int n_sel, int32_t *result_out_dev, float *probs_out_dev, void *stream) {
     const cudaStream_t s = (cudaStream_t)stream;
-    const bool ok = post_args_ok(scores_dev, hs, ws, image_dev, smooth, params, labels_sel, n_sel, result_out_dev);
+    const bool ok = post_args_ok(n_scales, scores_dev, hs, ws, image_dev, smooth, params, labels_sel, n_sel,
+                                 result_out_dev);
     return dev_call(h, 1, s, ok, [&](Engine *e) {
-        return predict_mask(e, mode, n_scales, scores_dev, hs, ws, image_dev, eps, smooth, params, labels_sel, n_sel,
-                            result_out_dev, probs_out_dev, s);
+        LabelRow row;
+        if (int rc = label_row(e, labels_sel, n_sel, &row)) return rc;
+        return predict_mask_batch(e, 1, mode, n_scales, scores_dev, hs, ws, image_dev, eps, smooth, params, nullptr,
+                                  n_sel ? &row : nullptr, result_out_dev, probs_out_dev, s);
     });
 }
 
@@ -501,36 +424,12 @@ extern "C" int dsrg_predict_mask_host(dsrg_engine *h, int mode, int n_scales, co
                                       const int *hs, const int *ws, const uint8_t *image, float eps, int smooth,
                                       const dsrg_crf_params *params, const int32_t *labels_sel, int n_sel,
                                       int32_t *result_out, float *probs_out) {
-    const bool ok = n_scales >= 1 && n_scales <= 16 &&
-                    post_args_ok(scores, hs, ws, image, smooth, params, labels_sel, n_sel, result_out);
+    const bool ok = post_args_ok(n_scales, scores, hs, ws, image, smooth, params, labels_sel, n_sel, result_out);
     return host_call(h, 1, ok, false, [&](Engine *e, cudaStream_t s) {
-        size_t total = 0;
-        for (int k = 0; k < n_scales; k++) {
-            if (!scores[k] || hs[k] < 1 || ws[k] < 1) {
-                set_error("score map %d: bad pointer or size", k);
-                return DSRG_E_INVALID;
-            }
-            total += (size_t)e->M * hs[k] * ws[k];
-        }
-        if (int rc = grow_staging(e, (void **)&e->st_raw, &e->st_raw_cap, total * sizeof(float))) return rc;
-        const float *dptr[16];
-        size_t at = 0;
-        for (int k = 0; k < n_scales; k++) {
-            const size_t n = (size_t)e->M * hs[k] * ws[k];
-            DSRG_CUDA_TRY(cudaMemcpyAsync(e->st_raw + at, scores[k], n * sizeof(float), cudaMemcpyHostToDevice, s));
-            dptr[k] = e->st_raw + at;
-            at += n;
-        }
-        if (smooth)
-            DSRG_CUDA_TRY(cudaMemcpyAsync(e->st_image, image, (size_t)e->N * 3, cudaMemcpyHostToDevice, s));
-        if (int rc = predict_mask(e, mode, n_scales, dptr, hs, ws, e->st_image, eps, smooth, params, labels_sel, n_sel,
-                                  e->st_lmap, probs_out ? e->st_out : nullptr, s))
-            return rc;
-        DSRG_CUDA_TRY(cudaMemcpyAsync(result_out, e->st_lmap, (size_t)e->N * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
-        if (probs_out)
-            DSRG_CUDA_TRY(cudaMemcpyAsync(probs_out, e->st_out, (size_t)e->N * e->M * sizeof(float),
-                                          cudaMemcpyDeviceToHost, s));
-        return DSRG_OK;
+        LabelRow row;
+        if (int rc = label_row(e, labels_sel, n_sel, &row)) return rc;
+        return predict_mask_staged(e, 1, mode, n_scales, scores, hs, ws, image, eps, smooth, params, nullptr,
+                                   n_sel ? &row : nullptr, result_out, probs_out, s);
     });
 }
 
@@ -540,11 +439,10 @@ extern "C" int dsrg_predict_mask_batch_dev(dsrg_engine *h, const float *const *s
                                            const int32_t *sel_dev, int32_t *result_out_dev, float *probs_out_dev,
                                            void *stream) {
     const cudaStream_t s = (cudaStream_t)stream;
-    const bool ok = n_scales >= 1 && n_scales <= kPostMaxScales &&
-                    post_args_ok(scores_dev, hs, ws, images_dev, smooth, params, nullptr, 0, result_out_dev);
+    const bool ok = post_args_ok(n_scales, scores_dev, hs, ws, images_dev, smooth, params, nullptr, 0, result_out_dev);
     return dev_call(h, B, s, ok, [&](Engine *e) {
         return predict_mask_batch(e, B, mode, n_scales, scores_dev, hs, ws, images_dev, eps, smooth, params, sel_dev,
-                                  result_out_dev, probs_out_dev, s);
+                                  nullptr, result_out_dev, probs_out_dev, s);
     });
 }
 
@@ -552,45 +450,9 @@ extern "C" int dsrg_predict_mask_batch_host(dsrg_engine *h, const float *const *
                                             int n_scales, int B, int mode, const uint8_t *images, float eps,
                                             int smooth, const dsrg_crf_params *params, const int32_t *sel,
                                             int32_t *result_out, float *probs_out) {
-    const bool ok = n_scales >= 1 && n_scales <= kPostMaxScales &&
-                    post_args_ok(scores, hs, ws, images, smooth, params, nullptr, 0, result_out);
+    const bool ok = post_args_ok(n_scales, scores, hs, ws, images, smooth, params, nullptr, 0, result_out);
     return host_call(h, B, ok, false, [&](Engine *e, cudaStream_t s) {
-        const int M = e->M;
-        if (int rc = post_batch_check(e, mode, n_scales, scores, hs, ws)) return rc;
-        for (int b = 0; sel && b < B; b++)
-            for (int k = 0; k < M && sel[(size_t)b * M + k] != -1; k++) {
-                const int v = sel[(size_t)b * M + k];
-                if (v < 0 || v >= M) {
-                    set_error("image %d: selected label %d outside [0, %d)", b, v, M);
-                    return DSRG_E_INVALID;
-                }
-            }
-        size_t total = 0;
-        for (int k = 0; k < n_scales; k++) total += (size_t)B * M * hs[k] * ws[k];
-        if (int rc = grow_staging(e, (void **)&e->st_raw, &e->st_raw_cap, total * sizeof(float))) return rc;
-        if (sel)
-            if (int rc = grow_staging(e, (void **)&e->st_idx, &e->st_idx_cap, (size_t)B * M * sizeof(int32_t)))
-                return rc;
-        const float *dptr[kPostMaxScales];
-        size_t at = 0;
-        for (int k = 0; k < n_scales; k++) {
-            const size_t n = (size_t)B * M * hs[k] * ws[k];
-            DSRG_CUDA_TRY(cudaMemcpyAsync(e->st_raw + at, scores[k], n * sizeof(float), cudaMemcpyHostToDevice, s));
-            dptr[k] = e->st_raw + at;
-            at += n;
-        }
-        if (smooth)
-            DSRG_CUDA_TRY(cudaMemcpyAsync(e->st_image, images, (size_t)B * e->N * 3, cudaMemcpyHostToDevice, s));
-        if (sel)
-            DSRG_CUDA_TRY(cudaMemcpyAsync(e->st_idx, sel, (size_t)B * M * sizeof(int32_t), cudaMemcpyHostToDevice, s));
-        if (int rc = predict_mask_batch(e, B, mode, n_scales, dptr, hs, ws, e->st_image, eps, smooth, params,
-                                        sel ? e->st_idx : nullptr, e->st_lmap, probs_out ? e->st_out : nullptr, s))
-            return rc;
-        DSRG_CUDA_TRY(cudaMemcpyAsync(result_out, e->st_lmap, (size_t)B * e->N * sizeof(int32_t),
-                                      cudaMemcpyDeviceToHost, s));
-        if (probs_out)
-            DSRG_CUDA_TRY(cudaMemcpyAsync(probs_out, e->st_out, (size_t)B * e->N * M * sizeof(float),
-                                          cudaMemcpyDeviceToHost, s));
-        return DSRG_OK;
+        return predict_mask_staged(e, B, mode, n_scales, scores, hs, ws, images, eps, smooth, params, sel, nullptr,
+                                   result_out, probs_out, s);
     });
 }

@@ -262,11 +262,13 @@ int dsrg_prepare_net_input_batch_host(dsrg_engine *e, const uint8_t *const *imag
  *                         softmax over labels; clamp at eps; CRF(im, log(probs)); argmax
  *   DSRG_POST_ZOOM_PROBS  training/tools/generate_train_gt.py:76-104: softmax at network resolution;
  *                         zoom(probs, order=1); clamp at eps; CRF(im, log(probs)); argmax over `labels_sel`
- *   scores     : n_scales pointers to [M][h_k][w_k] float32 (net.blobs['fc8-SEC'].data[0]); the array of
- *                pointers and hs / ws live on the host in both variants
+ * These two are dsrg_predict_mask_batch_* below at B = 1, with the selection taken from host memory.
+ *   scores     : n_scales pointers (1 <= n_scales <= 16) to [M][h_k][w_k] float32 (net.blobs['fc8-SEC'].data[0]);
+ *                the array of pointers and hs / ws live on the host in both variants
  *   image      : [H][W][3] uint8 as handed to krahenbuhl2013.CRF (may be NULL when smooth == 0)
  *   smooth     : 0 skips the CRF (the tools' `smooth=False`)
- *   labels_sel : n_sel label ids ([0] + image tags in generate_train_gt.py:96-97); n_sel == 0 = all labels
+ *   labels_sel : n_sel (<= 255) label ids in [0, M), on the host in both variants ([0] + image tags in
+ *                generate_train_gt.py:96-97); n_sel == 0 = all labels.  Read during the call only
  *   result_out : [H][W] int32 label map;  probs_out : optional [H][W][M] float32 (CRF marginals, or the
  *                clamped probabilities when smooth == 0)
  * dsrg_zoom_scores_* is the zoom step alone ([M][h][w] -> [H][W][M], scipy.ndimage.zoom order=1 semantics,
@@ -299,8 +301,9 @@ int dsrg_predict_mask_host(dsrg_engine *e, int mode, int n_scales, const float *
  *               selects every label.  In _dev it is device memory read when the pass runs (its content is not
  *               part of a cached graph's key)
  *   result_out: [B][H][W] int32;  probs_out : optional [B][H][W][M] float32
- * With smooth == 0 every image's result and probs_out are bit-identical to dsrg_predict_mask_* on that image alone;
- * with smooth == 1 the CRF marginals follow the batched CRF's 1e-4 bound.
+ * dsrg_predict_mask_* runs this pass at B = 1, so with smooth == 0 every image's result and probs_out are
+ * bit-identical to dsrg_predict_mask_* on that image alone: the same kernels compute every image the same way.
+ * With smooth == 1 the CRF marginals follow the batched CRF's 1e-4 bound.
  * A sel entry outside [0, M) before the row's -1:
  *   _host: DSRG_E_INVALID before any copy or launch.
  *   _dev : the row is not read past it, and every pixel of that image's result is -1 (a prediction that

@@ -164,6 +164,16 @@ def test_predict_mask_argument_errors(torch_cuda):
         eng.predict_mask_host([blob], im, labels_sel=[0, 21])
     with pytest.raises(api.DsrgError):
         eng.predict_mask_host([blob], None, smooth=True)
+    # at most 16 score maps, in both entry points, refused before any launch
+    torch = torch_cuda
+    d_blob, d_im = torch.from_numpy(blob).cuda(), torch.from_numpy(im).cuda()
+    res = torch.empty((40, 40), dtype=torch.int32, device="cuda")
+    eng.take_launch_count()
+    with pytest.raises(api.DsrgError):
+        eng.predict_mask_host([blob] * 17, im)
+    with pytest.raises(api.DsrgError):
+        eng.predict_mask_dev([d_blob] * 17, d_im, res)
+    assert eng.take_launch_count() == 0
     assert eng.predict_mask_host([blob], None, smooth=False).shape == (40, 40)
 
 
@@ -185,7 +195,7 @@ def test_crf_function_many_sizes_one_engine(torch_cuda):
 
 def test_per_image_callers_replay_graphs_across_sizes(torch_cuda):
     """The evaluation tools meet the same image sizes again and again: the post-processing of one image and a
-    DenseCRF object's inference are replayed as CUDA graphs per size (post.cu:predict_mask, api.cu:densecrf_run),
+    DenseCRF object's inference are replayed as CUDA graphs per size (post.cu:predict_mask_batch, api.cu:densecrf_run),
     also when another size ran on the shared engine in between (the replayed graph then contains the rebuild of
     the shared spatial lattice).  Results equal the plain launches up to the float atomics' noise."""
     import fake_caffe
