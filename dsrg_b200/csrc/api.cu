@@ -157,7 +157,7 @@ int check_device_flag(Engine *e, cudaStream_t s) {
     return DSRG_OK;
 }
 
-// (re)build lattices for this call: spatial only when its sigmas changed, bilateral always
+// (re)build lattices for this call: spatial only when crf_pass found it due, bilateral always
 static int prepare_lattices(Engine *e, int B, const uint8_t *image, const dsrg_crf_params &p,
                             cudaStream_t s) {
     if (!(p.theta_gamma_x > 0 && p.theta_gamma_y > 0 && p.theta_alpha_x > 0 && p.theta_alpha_y > 0 &&
@@ -165,7 +165,7 @@ static int prepare_lattices(Engine *e, int B, const uint8_t *image, const dsrg_c
         set_error("CRF parameters must be positive");
         return DSRG_E_INVALID;
     }
-    if (!e->sp_valid || e->sp.sigma[0] != p.theta_gamma_x || e->sp.sigma[1] != p.theta_gamma_y) {
+    if (!e->sp_valid) {
         e->sp.sigma[0] = p.theta_gamma_x;
         e->sp.sigma[1] = p.theta_gamma_y;
         if (!key_range_ok(e->sp, e->W, e->H)) {
@@ -175,7 +175,6 @@ static int prepare_lattices(Engine *e, int B, const uint8_t *image, const dsrg_c
         }
         int rc = lattice_build(e, e->sp, B, nullptr, s);
         if (rc) return rc;
-        e->sp_valid = true;
     }
     e->bi.sigma[0] = p.theta_alpha_x;
     e->bi.sigma[1] = p.theta_alpha_y;
@@ -204,31 +203,25 @@ int check_batch(Engine *e, int B) {
     return DSRG_OK;
 }
 
-// a pass may be captured / replayed as a graph only when it does not have to (re)build the shared spatial lattice
-static bool spatial_ready(const Engine *e, const dsrg_crf_params *p) {
-    return p && e->sp_valid && e->sp.sigma[0] == p->theta_gamma_x && e->sp.sigma[1] == p->theta_gamma_y;
+bool crf_pass_begin(Engine *e, const dsrg_crf_params &p) {
+    if (e->sp_valid && e->sp.sigma[0] == p.theta_gamma_x && e->sp.sigma[1] == p.theta_gamma_y) return false;
+    e->sp_valid = false;  // prepare_lattices rebuilds it, in the pass and so in its graph
+    return true;
 }
 
-// after a replayed pass the host-side notes a live pass would have left must be there too
-static int crf_pass_done(Engine *e, int B, int rc) {
-    if (rc == DSRG_OK) {
-        e->Qcur = e->Q0;
-        e->last_crf_B = B;
-    } else {
+void crf_pass_end(Engine *e, const dsrg_crf_params &p, int B, int rc) {
+    if (rc != DSRG_OK) {
         e->last_crf_B = 0;
+        return;
     }
-    return rc;
+    e->sp.sigma[0] = p.theta_gamma_x;
+    e->sp.sigma[1] = p.theta_gamma_y;
+    e->sp_valid = true;
+    e->last_crf_B = B;
 }
 
-static GraphKey pass_key(const Engine *e, int entry, int B, const dsrg_crf_params *p) {
-    GraphKey k;
-    k.add(entry).add(B).add(e->H).add(e->W);
-    if (p) k.add(*p);
-    return k;
-}
-
-static int crf_core(Engine *e, int B, const float *unary, int layout, bool clamp, float *unary_rw,
-                    const uint8_t *image, const dsrg_crf_params *p, cudaStream_t s) {
+int crf_core(Engine *e, int B, const float *unary, int layout, bool clamp, float *unary_rw, const uint8_t *image,
+             const dsrg_crf_params *p, cudaStream_t s) {
     if (layout != DSRG_LAYOUT_NHWC && layout != DSRG_LAYOUT_NCHW) {
         set_error("bad layout %d", layout);
         return DSRG_E_INVALID;
@@ -238,23 +231,42 @@ static int crf_core(Engine *e, int B, const float *unary, int layout, bool clamp
     return meanfield_run(e, B, unary, layout, clamp, unary_rw, *p, s);
 }
 
-int crf_core_batch_for_post(Engine *e, int B, const float *unary_hwc, const uint8_t *images,
-                            const dsrg_crf_params *p, cudaStream_t s) {
-    return crf_core(e, B, unary_hwc, DSRG_LAYOUT_NHWC, false, nullptr, images, p, s);
+static int crf_batch_pass(Engine *e, int B, const float *unary, int unary_layout, const uint8_t *image,
+                          const dsrg_crf_params *params, float *out, int out_layout, cudaStream_t s) {
+    GraphKey args;
+    args.add(unary).add(unary_layout).add(image).add(out).add(out_layout);
+    return crf_pass(e, s, PassKind::crf, B, params, args, [&]() {
+        int r = crf_core(e, B, unary, unary_layout, false, nullptr, image, params, s);
+        if (r) return r;
+        return meanfield_export(e, B, out, out_layout, s);
+    });
 }
 
-// Graph replay for the per-image callers (inference post-processing, DenseCRF objects), whose image size changes
-// from call to call: when the shared spatial lattice is not the one this call needs, the pass that rebuilds it is
-// captured as such (`rebuild` is part of the key), so its graph is self-contained and valid whatever the engine
-// worked on in between; `after` restores the host-side notes a replay skips.
-bool post_pass_needs_spatial(const Engine *e, const dsrg_crf_params *p) { return !spatial_ready(e, p); }
-void post_pass_done(Engine *e, const dsrg_crf_params *p, int B, int rc) {
-    if (rc == DSRG_OK && p) {
-        e->sp.sigma[0] = p->theta_gamma_x;
-        e->sp.sigma[1] = p->theta_gamma_y;
-        e->sp_valid = true;
-    }
-    crf_pass_done(e, B, rc);
+static int crflayer_pass(Engine *e, int B, float *probs, const uint8_t *image, const dsrg_crf_params *params,
+                         float *log_out, float *result, cudaStream_t s) {
+    GraphKey args;
+    args.add(probs).add(image).add(log_out).add(result);
+    return crf_pass(e, s, PassKind::crflayer, B, params, args, [&]() {
+        int r = crf_core(e, B, probs, DSRG_LAYOUT_NCHW, true, probs, image, params, s);
+        if (r) return r;
+        return meanfield_export_renorm(e, B, result, log_out, s);
+    });
+}
+
+// the full pass; cues / seeds as float planes or (host pipeline, wire.cu) in the 1-bit wire format
+int dsrg_forward_core(Engine *e, int B, const float *labels, float *probs, const float *cues, const uint32_t *cue_bits,
+                      const uint8_t *image, const dsrg_crf_params *params, double th1, double th2, float *seeds_out,
+                      uint32_t *seed_bits, float *crf_out, cudaStream_t s) {
+    GraphKey args;
+    args.add(labels).add(probs).add(cues).add(cue_bits).add(image).add(th1).add(th2).add(seeds_out).add(seed_bits).add(crf_out);
+    return crf_pass(e, s, PassKind::forward, B, params, args, [&]() {
+        // refinement (pylayers.py:310-331): in-place clamp, unary = probs (NCHW), CRF
+        int r = crf_core(e, B, probs, DSRG_LAYOUT_NCHW, true, probs, image, params, s);
+        if (r) return r;
+        if (crf_out && (r = meanfield_export(e, B, crf_out, DSRG_LAYOUT_NCHW, s))) return r;
+        // SRG on the raw marginals with the float64 clamp + renormalisation fused in (renorm = 1)
+        return srg_run(e, B, labels, e->Q0, cues, th1, th2, 1, seeds_out, nullptr, s, cue_bits, seed_bits);
+    });
 }
 
 int ensure_staging(Engine *e) {
@@ -301,7 +313,7 @@ using namespace dsrg;
 
 extern "C" {
 
-int dsrg_version(void) { return 109; }
+int dsrg_version(void) { return 110; }
 
 const char *dsrg_last_error(void) { return g_err; }
 
@@ -459,7 +471,6 @@ dsrg_engine *dsrg_engine_create(int device, int max_batch, int H, int W, int M) 
         dsrg_engine_destroy((dsrg_engine *)e);
         return nullptr;
     }
-    e->Qcur = e->Q0;
     return (dsrg_engine *)e;
 }
 
@@ -614,20 +625,7 @@ int dsrg_crf_batch_dev(dsrg_engine *h, int B, const float *unary, int unary_layo
                        int out_layout, void *stream) {
     const cudaStream_t s = (cudaStream_t)stream;
     return dev_call(h, B, s, unary && image && params && out && layout_ok(out_layout), [&](Engine *e) {
-        GraphKey key = pass_key(e, 1, B, params);
-        key.add(unary).add(unary_layout).add(image).add(out).add(out_layout);
-        // krahenbuhl2013.CRF runs on this entry point with a size that changes from call to call: like the other
-        // per-image callers its graph carries the rebuild of the shared spatial lattice when one is due
-        const bool rebuild = post_pass_needs_spatial(e, params);
-        key.add(rebuild);
-        if (rebuild) e->sp_valid = false;
-        const int rc = run_pass(e, s, key, true, [&]() {
-            int r = crf_core(e, B, unary, unary_layout, false, nullptr, image, params, s);
-            if (r) return r;
-            return meanfield_export(e, B, out, out_layout, s);
-        });
-        post_pass_done(e, params, B, rc);
-        return rc;
+        return crf_batch_pass(e, B, unary, unary_layout, image, params, out, out_layout, s);
     });
 }
 
@@ -636,24 +634,24 @@ int dsrg_crf_map_batch_dev(dsrg_engine *h, int B, const float *unary, int unary_
                            void *stream) {
     const cudaStream_t s = (cudaStream_t)stream;
     return dev_call(h, B, s, unary && image && params && labels_out, [&](Engine *e) {
-        GraphKey key = pass_key(e, 2, B, params);
-        key.add(unary).add(unary_layout).add(image).add(labels_out);
-        return crf_pass_done(e, B, run_pass(e, s, key, spatial_ready(e, params), [&]() {
+        GraphKey args;
+        args.add(unary).add(unary_layout).add(image).add(labels_out);
+        return crf_pass(e, s, PassKind::crf_map, B, params, args, [&]() {
             int r = crf_core(e, B, unary, unary_layout, false, nullptr, image, params, s);
             if (r) return r;
             return meanfield_export_map(e, B, labels_out, s);
-        }));
+        });
     });
 }
 
 int dsrg_crf_batch_host(dsrg_engine *h, int B, const float *unary, int unary_layout,
                         const uint8_t *image, const dsrg_crf_params *params, float *out,
                         int out_layout) {
-    return host_call(h, B, unary && image && params && out, true, [&](Engine *e, cudaStream_t s) {
+    return host_call(h, B, unary && image && params && out && layout_ok(out_layout), true, [&](Engine *e, cudaStream_t s) {
         const size_t n = (size_t)B * e->M * e->N;
         DSRG_CUDA_TRY(cudaMemcpyAsync(e->st_unary, unary, n * sizeof(float), cudaMemcpyHostToDevice, s));
         DSRG_CUDA_TRY(cudaMemcpyAsync(e->st_image, image, (size_t)B * e->N * 3, cudaMemcpyHostToDevice, s));
-        if (int rc = dsrg_crf_batch_dev(h, B, e->st_unary, unary_layout, e->st_image, params, e->st_out, out_layout, s))
+        if (int rc = crf_batch_pass(e, B, e->st_unary, unary_layout, e->st_image, params, e->st_out, out_layout, s))
             return rc;
         DSRG_CUDA_TRY(cudaMemcpyAsync(out, e->st_out, n * sizeof(float), cudaMemcpyDeviceToHost, s));
         return DSRG_OK;
@@ -673,28 +671,6 @@ int dsrg_srg_batch_dev(dsrg_engine *h, int B, const float *labels, const float *
     });
 }
 
-}  // extern "C"
-
-namespace dsrg {
-// the full pass; cues / seeds as float planes or (host pipeline, wire.cu) in the 1-bit wire format
-int dsrg_forward_core(Engine *e, int B, const float *labels, float *probs, const float *cues, const uint32_t *cue_bits,
-                      const uint8_t *image, const dsrg_crf_params *params, double th1, double th2, float *seeds_out,
-                      uint32_t *seed_bits, float *crf_out, cudaStream_t s) {
-    GraphKey key = pass_key(e, 3, B, params);
-    key.add(labels).add(probs).add(cues).add(cue_bits).add(image).add(th1).add(th2).add(seeds_out).add(seed_bits).add(crf_out);
-    return crf_pass_done(e, B, run_pass(e, s, key, spatial_ready(e, params), [&]() {
-        // refinement (pylayers.py:310-331): in-place clamp, unary = probs (NCHW), CRF
-        int r = crf_core(e, B, probs, DSRG_LAYOUT_NCHW, true, probs, image, params, s);
-        if (r) return r;
-        if (crf_out && (r = meanfield_export(e, B, crf_out, DSRG_LAYOUT_NCHW, s))) return r;
-        // SRG on the raw marginals with the float64 clamp + renormalisation fused in (renorm = 1)
-        return srg_run(e, B, labels, e->Qcur, cues, th1, th2, 1, seeds_out, nullptr, s, cue_bits, seed_bits);
-    }));
-}
-}  // namespace dsrg
-
-extern "C" {
-
 int dsrg_dsrg_forward_dev(dsrg_engine *h, int B, const float *labels, float *probs,
                           const float *cues, const uint8_t *image, const dsrg_crf_params *params,
                           double th1, double th2, float *seeds_out, float *crf_out, void *stream) {
@@ -710,13 +686,7 @@ int dsrg_crflayer_forward_dev(dsrg_engine *h, int B, float *probs, const uint8_t
                               void *stream) {
     const cudaStream_t s = (cudaStream_t)stream;
     return dev_call(h, B, s, probs && image && params && log_out, [&](Engine *e) {
-        GraphKey key = pass_key(e, 4, B, params);
-        key.add(probs).add(image).add(log_out).add(result);
-        return crf_pass_done(e, B, run_pass(e, s, key, spatial_ready(e, params), [&]() {
-            int r = crf_core(e, B, probs, DSRG_LAYOUT_NCHW, true, probs, image, params, s);
-            if (r) return r;
-            return meanfield_export_renorm(e, B, result, log_out, s);
-        }));
+        return crflayer_pass(e, B, probs, image, params, log_out, result, s);
     });
 }
 
@@ -728,7 +698,7 @@ int dsrg_srg_last_crf_host(dsrg_engine *h, int B, const float *labels, const flo
         DSRG_CUDA_TRY(cudaMemcpyAsync(e->st_labels, labels, (size_t)B * e->M * sizeof(float), cudaMemcpyHostToDevice, s));
         DSRG_CUDA_TRY(cudaMemcpyAsync(e->st_cues, cues, n * sizeof(float), cudaMemcpyHostToDevice, s));
         // SRG on the raw marginals of the last pass, float64 clamp + renormalisation fused in (pylayers.py:328-344)
-        if (int rc = srg_run(e, B, e->st_labels, e->Qcur, e->st_cues, th1, th2, 1, e->st_out, nullptr, s)) return rc;
+        if (int rc = srg_run(e, B, e->st_labels, e->Q0, e->st_cues, th1, th2, 1, e->st_out, nullptr, s)) return rc;
         DSRG_CUDA_TRY(cudaMemcpyAsync(seeds_out, e->st_out, n * sizeof(float), cudaMemcpyDeviceToHost, s));
         return DSRG_OK;
     }, last_crf_held);
@@ -740,7 +710,7 @@ int dsrg_srg_last_crf_dev(dsrg_engine *h, const float *labels, const float *cues
     return dev_call(h, B, s, labels && cues && seeds_out, [&](Engine *e) {
         if (int rc = last_crf_held(e, B)) return rc;
         // the device twin of the host entry point above: same kernels, queued behind the pass on the caller's stream
-        return srg_run(e, B, labels, e->Qcur, cues, th1, th2, 1, seeds_out, nullptr, s);
+        return srg_run(e, B, labels, e->Q0, cues, th1, th2, 1, seeds_out, nullptr, s);
     });
 }
 
@@ -758,8 +728,7 @@ int dsrg_crflayer_forward_host(dsrg_engine *h, int B, float *probs, const uint8_
         const size_t n = (size_t)B * e->M * e->N;
         DSRG_CUDA_TRY(cudaMemcpyAsync(e->st_unary, probs, n * sizeof(float), cudaMemcpyHostToDevice, s));
         DSRG_CUDA_TRY(cudaMemcpyAsync(e->st_image, image, (size_t)B * e->N * 3, cudaMemcpyHostToDevice, s));
-        if (int rc = dsrg_crflayer_forward_dev(h, B, e->st_unary, e->st_image, params, e->st_out,
-                                               result ? e->st_cues : nullptr, s))
+        if (int rc = crflayer_pass(e, B, e->st_unary, e->st_image, params, e->st_out, result ? e->st_cues : nullptr, s))
             return rc;
         DSRG_CUDA_TRY(cudaMemcpyAsync(log_out, e->st_out, n * sizeof(float), cudaMemcpyDeviceToHost, s));
         DSRG_CUDA_TRY(cudaMemcpyAsync(probs, e->st_unary, n * sizeof(float), cudaMemcpyDeviceToHost, s));
@@ -949,15 +918,9 @@ static int densecrf_run(dsrg_densecrf *c, int n_iters, Engine *e, cudaStream_t s
         return meanfield_run(e, 1, e->st_unary, DSRG_LAYOUT_NHWC, false, nullptr, p0, s);
     }
     DSRG_CUDA_TRY(cudaMemcpyAsync(e->st_image, c->image.data(), c->image.size(), cudaMemcpyHostToDevice, s));
-    const bool rebuild = post_pass_needs_spatial(e, &c->params);
-    GraphKey key = pass_key(e, 7, 1, &c->params);
-    key.add(rebuild);
-    if (rebuild) e->sp_valid = false;
-    rc = run_pass(e, s, key, true, [&]() {
+    return crf_pass(e, s, PassKind::densecrf, 1, &c->params, GraphKey(), [&]() {
         return crf_core(e, 1, e->st_unary, DSRG_LAYOUT_NHWC, false, nullptr, e->st_image, &c->params, s);
     });
-    post_pass_done(e, &c->params, 1, rc);
-    return rc;
 }
 
 int dsrg_densecrf_inference(dsrg_densecrf *c, int n_iters, float *probs_out) {

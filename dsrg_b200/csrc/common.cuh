@@ -161,12 +161,12 @@ int meanfield_export_renorm(Engine *e, int B, float *result_out, float *log_out,
 int srg_run(Engine *e, int B, const float *labels, const float *probs, const float *cues,
             double th1, double th2, int renorm, float *seeds_out, int32_t *label_map_out,
             cudaStream_t s, const uint32_t *cue_bits = nullptr, uint32_t *seed_bits = nullptr);
-// ---- api.cu: the full pass with optional 1-bit cue / seed planes (wire.cu) ----
+// ---- api.cu: the full pass with optional 1-bit cue / seed planes (wire.cu), and the CRF of a pass's body ----
 int dsrg_forward_core(Engine *e, int B, const float *labels, float *probs, const float *cues, const uint32_t *cue_bits,
                       const uint8_t *image, const dsrg_crf_params *params, double th1, double th2, float *seeds_out,
                       uint32_t *seed_bits, float *crf_out, cudaStream_t s);
-bool post_pass_needs_spatial(const Engine *e, const dsrg_crf_params *p);
-void post_pass_done(Engine *e, const dsrg_crf_params *p, int B, int rc);
+int crf_core(Engine *e, int B, const float *unary, int layout, bool clamp, float *unary_rw, const uint8_t *image,
+             const dsrg_crf_params *p, cudaStream_t s);
 // ---- sec_loss.cu ----
 constexpr int kSecPlainChunks = 16;  // CTAs per image of SeedLossLayer's sums (fixed, so is their order)
 
@@ -184,8 +184,7 @@ struct Engine {
 
     // mean-field state, planar [B][M][N]
     float *U = nullptr, *Q0 = nullptr;
-    float *Qcur = nullptr;  // where the current marginals live
-    int last_crf_B = 0;     // images whose raw marginals of the last mean-field pass are still in Qcur (0: none)
+    int last_crf_B = 0;    // images whose raw marginals of the last mean-field pass are still in Q0 (0: none)
     // lattice value buffers [rows][MP]
     float *spA = nullptr, *spB = nullptr, *spC = nullptr, *biA = nullptr, *biB = nullptr, *biC = nullptr;
     int tiles_x = 0, tiles_y = 0, ntiles = 0;  // tiles of tile_w x 8 pixels
@@ -399,8 +398,15 @@ cudaError_t numa_host_alloc(void **p, size_t bytes, int device);
 // launches from the stream into a graph, instantiate, launch.  Afterwards: one cudaGraphLaunch.  Falls back to
 // plain launches on the legacy default stream, inside somebody else's capture, while per-kernel profiling is on,
 // or if capture fails.  `body` issues the launches on `s` and returns a DSRG_* code.
+enum class PassKind : int { crf, crf_map, forward, crflayer, densecrf, post };
 struct GraphKey {
     std::string bytes;
+    GraphKey() = default;
+    // the key of a pass: its kind, its batch and the image size, then the call's own arguments
+    GraphKey(PassKind kind, int B, const Engine *e, const GraphKey &args) {
+        add(kind).add(B).add(e->H).add(e->W);
+        bytes += args.bytes;
+    }
     template <typename T>
     GraphKey &add(const T &v) {
         bytes.append(reinterpret_cast<const char *>(&v), sizeof(T));
@@ -425,6 +431,26 @@ inline int run_pass(Engine *e, cudaStream_t s, const GraphKey &key, bool allow_g
         e->launches = l0;
         rc = body();
     }
+    return rc;
+}
+
+// ---- api.cu: the host side of crf_pass ----
+bool crf_pass_begin(Engine *e, const dsrg_crf_params &p);  // true: the pass rebuilds the shared spatial lattice
+void crf_pass_end(Engine *e, const dsrg_crf_params &p, int B, int rc);
+
+// Every mean-field pass runs through here; `args` are the call's own arguments.  The shared spatial lattice is rebuilt
+// when the image size or its sigmas changed since it was built, and that rebuild is captured with the pass (`rebuild`
+// is part of the key), so a graph is valid whatever the engine ran in between: the per-image callers alternate sizes
+// and would otherwise never replay.  A replay skips the host code of `body`, so the notes it leaves (the spatial
+// lattice's sigmas, the batch whose marginals Q0 holds) are written here, after the pass.
+template <typename F>
+inline int crf_pass(Engine *e, cudaStream_t s, PassKind kind, int B, const dsrg_crf_params *p, const GraphKey &args,
+                    F body) {
+    const bool rebuild = crf_pass_begin(e, *p);
+    GraphKey key(kind, B, e, args);
+    key.add(*p).add(rebuild);
+    const int rc = run_pass(e, s, key, true, body);
+    crf_pass_end(e, *p, B, rc);
     return rc;
 }
 

@@ -873,8 +873,6 @@ static int run_impl(Engine *e, int B, const float *unary, int layout, bool clamp
         DSRG_LAUNCH(e, T_MF_INIT, s,
                     k_mf_init<MP><<<gp, kThreads, 0, s>>>(unary, unary_rw, layout, clamp ? 1 : 0, e->U,
                                                           T == 0 ? e->Q0 : nullptr, M, N));
-    e->Qcur = e->Q0;
-    e->last_crf_B = B;  // host-side bookkeeping for dsrg_srg_last_crf_host (the launches below are already ordered on s)
     if (T == 0) return DSRG_OK;
     const float alpha_sp = 1.0f / (1 + powf(2, -e->sp.d));  // permutohedral.cpp:571
     const float alpha_bi = 1.0f / (1 + powf(2, -e->bi.d));
@@ -962,21 +960,21 @@ int meanfield_run(Engine *e, int B, const float *unary, int unary_layout, bool c
 
 int meanfield_export(Engine *e, int B, float *out, int layout, cudaStream_t s) {
     dim3 gp(cdiv(e->N, kThreads), B);
-    DSRG_LAUNCH(e, T_MF_EXPORT, s, k_mf_export<<<gp, kThreads, 0, s>>>(e->Qcur, out, layout, e->M, e->N));
+    DSRG_LAUNCH(e, T_MF_EXPORT, s, k_mf_export<<<gp, kThreads, 0, s>>>(e->Q0, out, layout, e->M, e->N));
     DSRG_CUDA_TRY(cudaGetLastError());
     return DSRG_OK;
 }
 
 int meanfield_export_map(Engine *e, int B, int32_t *labels, cudaStream_t s) {
     dim3 gp(cdiv(e->N, kThreads), B);
-    DSRG_LAUNCH(e, T_MF_EXPORT, s, k_mf_export_map<<<gp, kThreads, 0, s>>>(e->Qcur, labels, e->M, e->N));
+    DSRG_LAUNCH(e, T_MF_EXPORT, s, k_mf_export_map<<<gp, kThreads, 0, s>>>(e->Q0, labels, e->M, e->N));
     DSRG_CUDA_TRY(cudaGetLastError());
     return DSRG_OK;
 }
 
 int meanfield_export_renorm(Engine *e, int B, float *result_out, float *log_out, cudaStream_t s) {
     dim3 gp(cdiv(e->N, kThreads), B);
-    DSRG_LAUNCH(e, T_MF_EXPORT, s, k_mf_export_renorm<<<gp, kThreads, 0, s>>>(e->Qcur, result_out, log_out, e->M, e->N));
+    DSRG_LAUNCH(e, T_MF_EXPORT, s, k_mf_export_renorm<<<gp, kThreads, 0, s>>>(e->Q0, result_out, log_out, e->M, e->N));
     DSRG_CUDA_TRY(cudaGetLastError());
     return DSRG_OK;
 }

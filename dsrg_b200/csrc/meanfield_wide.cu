@@ -174,8 +174,6 @@ int meanfield_run_wide(Engine *e, int B, const float *unary, int layout, bool cl
     const int M = e->M, N = e->N, CH = e->MP / 4, T = p.n_iters;
     dim3 gp(cdiv(N, kThreads), B), gq(cdiv(N, kThreads), CH, B);
     DSRG_LAUNCH(e, T_MF_INIT, s, k_wide_init<<<gp, kThreads, 0, s>>>(unary, unary_rw, layout, clamp ? 1 : 0, e->U, e->Q0, M, N));
-    e->Qcur = e->Q0;
-    e->last_crf_B = B;
     if (T == 0) return DSRG_OK;
     const float alpha_sp = 1.0f / (1 + powf(2, -e->sp.d)), alpha_bi = 1.0f / (1 + powf(2, -e->bi.d));  // permutohedral.cpp:571
     const float c_sp = p.w2 * alpha_sp, c_bi = p.w1 * alpha_bi;

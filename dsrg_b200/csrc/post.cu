@@ -212,9 +212,6 @@ k_post_argmax_batch(const float *q, int32_t *out, int N, int M, long long ls, lo
     out[(size_t)b * N + i] = arg;
 }
 
-int crf_core_batch_for_post(Engine *e, int B, const float *unary_hwc, const uint8_t *images,
-                            const dsrg_crf_params *p, cudaStream_t s);  // api.cu
-
 // sel: device rows as k_post_argmax_batch reads them, or NULL; row (B = 1): a selection written to st_sel by the pass
 static int predict_mask_batch_body(Engine *e, int B, int mode, const ZoomScales &sc, const uint8_t *images, float eps,
                                    int smooth, const dsrg_crf_params *p, const int32_t *sel, const LabelRow *row,
@@ -242,10 +239,10 @@ static int predict_mask_batch_body(Engine *e, int B, int mode, const ZoomScales 
     DSRG_CUDA_TRY(cudaGetLastError());
     const dim3 ga(cdiv(N, kThreads), B);
     if (smooth) {
-        if (int rc = crf_core_batch_for_post(e, B, unary, images, p, s)) return rc;
+        if (int rc = crf_core(e, B, unary, DSRG_LAYOUT_NHWC, false, nullptr, images, p, s)) return rc;
         if (probs_out)
             if (int rc = meanfield_export(e, B, probs_out, DSRG_LAYOUT_NHWC, s)) return rc;
-        DSRG_LAUNCH(e, T_POST, s, k_post_argmax_batch<<<ga, kThreads, 0, s>>>(e->Qcur, result, N, M, N, 1, sel));
+        DSRG_LAUNCH(e, T_POST, s, k_post_argmax_batch<<<ga, kThreads, 0, s>>>(e->Q0, result, N, M, N, 1, sel));
     } else {
         DSRG_LAUNCH(e, T_POST, s, k_post_argmax_batch<<<ga, kThreads, 0, s>>>(clamped, result, N, M, 1, M, sel));
     }
@@ -286,20 +283,18 @@ static int predict_mask_batch(Engine *e, int B, int mode, int n_scales, const fl
         sc.w[k] = ws[k];
     }
     // the pass reads sel, so its content is not part of the key: a replay follows what sel holds.  A row is a kernel
-    // parameter of the pass, so a replay writes the ids it was captured with: they are part of the key.
-    const bool rebuild = smooth && post_pass_needs_spatial(e, p);
-    GraphKey key;
-    key.add(7).add(B).add(e->H).add(e->W).add(mode).add(n_scales).add(images).add(eps).add(smooth).add(sel)
-        .add(result).add(probs_out).add(rebuild).add(row != nullptr);
-    for (int k = 0; k < n_scales; k++) key.add(scores[k]).add(hs[k]).add(ws[k]);
-    if (smooth) key.add(*p);
-    if (row) key.add(*row);
-    if (rebuild) e->sp_valid = false;
-    rc = run_pass(e, s, key, true, [&]() {
+    // parameter of the pass, so a replay writes the ids it was captured with: they are part of the key.  `smooth`
+    // comes first, so a pass with the CRF and one without never share a key.
+    GraphKey args;
+    args.add(smooth).add(mode).add(n_scales).add(images).add(eps).add(sel).add(result).add(probs_out)
+        .add(row != nullptr);
+    for (int k = 0; k < n_scales; k++) args.add(scores[k]).add(hs[k]).add(ws[k]);
+    if (row) args.add(*row);
+    auto body = [&]() {
         return predict_mask_batch_body(e, B, mode, sc, images, eps, smooth, p, sel, row, result, probs_out, s);
-    });
-    if (smooth) post_pass_done(e, p, B, rc);
-    return rc;
+    };
+    if (smooth) return crf_pass(e, s, PassKind::post, B, p, args, body);
+    return run_pass(e, s, GraphKey(PassKind::post, B, e, args), true, body);
 }
 
 // The *_host entry points: the score maps, the images (when smoothing) and the selection rows in through the

@@ -374,9 +374,12 @@ static int host_pass_impl(Engine *e, int B, const float *labels, float *probs, c
         if (srg_only)
             rc = srg_run(e, nb, e->st_labels + (size_t)b0 * e->M, e->st_unary + o, e->st_cues + o, th1, th2, renorm,
                          e->st_out + o, label_map_out ? e->st_lmap + (size_t)b0 * e->N : nullptr, s, cbits, sbits);
-        else
+        else {
             rc = dsrg_forward_core(e, nb, e->st_labels + (size_t)b0 * e->M, e->st_unary + o, e->st_cues + o, cbits,
                                    e->st_image + (size_t)b0 * e->N * 3, params, th1, th2, e->st_out + o, sbits, nullptr, s);
+            // Q0 holds this chunk's marginals only: a batch cut into chunks leaves no result for the *_last_* calls
+            if (nchunks > 1) e->last_crf_B = 0;
+        }
         if (rc) return rc;
         if (crf_out) {  // raw marginals of this chunk, parked in the (now consumed) cues staging area
             if ((rc = meanfield_export(e, nb, e->st_cues + o, DSRG_LAYOUT_NCHW, s))) return rc;

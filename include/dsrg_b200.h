@@ -470,7 +470,8 @@ int dsrg_crflayer_backward_dev(dsrg_engine *e, const float *result_dev, const fl
  *                                  synchronisation; labels [B][M], cues / seeds_out [B][M][H][W]); the batch
  *                                  size follows the arrays it describes
  *   dsrg_crf_last_marginals_host : the raw float32 marginals themselves
- * All return DSRG_E_STATE unless the engine's last pass was a CRF over exactly B images.
+ * All return DSRG_E_STATE unless the engine's last pass was a CRF over exactly B images.  A dsrg_dsrg_forward_host
+ * call that its pipeline cuts into several chunks holds no such result: only one that runs as a single chunk does.
  */
 int dsrg_srg_last_crf_host(dsrg_engine *e, int B, const float *labels_host, const float *cues_host, double th1,
                            double th2, float *seeds_out_host);
