@@ -756,6 +756,20 @@ class Engine(object):
         check(self._L.dsrg_engine_copy_norm(self.h, 1, B, _hptr(nb, np.float32)))
         return ns, nb
 
+    def lattice_bary(self, which, b):
+        """Image b's barycentric weights of the last CRF call (d+1, N), in the layout of lattice_tables' off."""
+        d = 2 if which == 0 else 5
+        bary = np.zeros((d + 1, self.H * self.W), np.float32)
+        check(self._L.dsrg_engine_lattice_bary(self.h, which, b, _hptr(bary, np.float32)))
+        return bary
+
+    def lattice_idle(self, which):
+        """(non-empty hash slots, hval entries not -1, vkey entries not kNoKey) of a lattice family, over its whole
+        allocation: all 0 between passes.  Synchronises."""
+        counts = np.zeros(3, np.int64)
+        check(self._L.dsrg_engine_lattice_idle(self.h, which, _hptr(counts, np.int64)))
+        return tuple(int(c) for c in counts)
+
 
 def _pred_host(pred, K):
     """pred as a flat C-contiguous uint8 or int32 array.  Other integer predictions (np.argmax gives int64) are

@@ -84,6 +84,15 @@ static void engine_shape(Engine *e, int H, int W) {
     e->sp_valid = false;
 }
 
+// The renumbering key of an incidence, pos * (d+1) + r (lattice.cu: k_lattice_insert), is an int below kNoKey.  pos
+// runs to ntiles * kTileThreads (the phantom lanes' position), so the bilateral lattice's largest key is
+// ntiles * kTileThreads * 6 + 5.  Narrow images have few pixels per tile (one column: 8 of 256), and from
+// 11 140 945 x 1 on the key would reach kNoKey.  set_size keeps the tile count at or below the capacity's.
+static bool renum_keys_fit(int H, int W) {
+    const long long tiles_x = (W + kTileW - 1) / kTileW, tiles_y = (H + kTileH - 1) / kTileH;
+    return tiles_x * tiles_y * kTileThreads * 6 + 5 < (long long)kNoKey;
+}
+
 static int lattice_alloc(Engine *e, Lattice &L, int d, int shared) {
     L.d = d;
     L.shared = shared;
@@ -100,6 +109,8 @@ static int lattice_alloc(Engine *e, Lattice &L, int d, int shared) {
     rc |= dalloc(e, &L.vcount, n);
     rc |= dalloc(e, &L.aslot, n * L.capv);
     rc |= dalloc(e, &L.vkey, n * L.capv);
+    L.slots_alloc = (long long)n * L.cap;
+    L.verts_alloc = (long long)n * L.capv;
     const long long rn_words = renum_words(e->ntiles, d + 1);  // the capacity shape has the most tiles
     rc |= dalloc(e, &L.rn_words, n * rn_words);
     rc |= dalloc(e, &L.rn_chunk, n * (rn_words / kRenumChunk));
@@ -313,7 +324,7 @@ using namespace dsrg;
 
 extern "C" {
 
-int dsrg_version(void) { return 110; }
+int dsrg_version(void) { return 111; }
 
 const char *dsrg_last_error(void) { return g_err; }
 
@@ -384,9 +395,9 @@ void dsrg_crf_params_default(dsrg_crf_params *p, float scale_factor, float color
 
 dsrg_engine *dsrg_engine_create(int device, int max_batch, int H, int W, int M) {
     if (max_batch < 1 || H < 1 || W < 1 || M < 1 || M > DSRG_MAX_LABELS_WIDE ||
-        (long long)H * W > (1ll << 24)) {
-        set_error("bad engine shape (max_batch=%d H=%d W=%d M=%d; M <= %d)", max_batch, H, W, M,
-                  DSRG_MAX_LABELS_WIDE);
+        (long long)H * W > (1ll << 24) || !renum_keys_fit(H, W)) {
+        set_error("bad engine shape (max_batch=%d H=%d W=%d M=%d; M <= %d, H*W <= 2^24, lattice renumbering keys "
+                  "below %d)", max_batch, H, W, M, DSRG_MAX_LABELS_WIDE, kNoKey);
         return nullptr;
     }
     int ndev = 0;
@@ -785,6 +796,49 @@ int dsrg_engine_copy_norm(dsrg_engine *h, int which, int B, float *norm_out) {
         DSRG_CUDA_TRY(cudaMemcpy(norm_out, e->sp.norm, sizeof(float) * e->N, cudaMemcpyDeviceToHost));
     else
         DSRG_CUDA_TRY(cudaMemcpy(norm_out, e->bi.norm, sizeof(float) * (size_t)B * e->N, cudaMemcpyDeviceToHost));
+    return DSRG_OK;
+}
+
+int dsrg_engine_lattice_bary(dsrg_engine *h, int which, int b, float *bary_out) {
+    Engine *e = (Engine *)h;
+    DeviceScope dev_scope(e);
+    int rc = check_entry(e, 1, e && bary_out && (which == 0 || which == 1) && b >= 0 && b < e->maxB);
+    if (rc) return rc;
+    const Lattice &L = which == 0 ? e->sp : e->bi;
+    const size_t n = (size_t)(L.d + 1) * L.N;
+    DSRG_CUDA_TRY(cudaDeviceSynchronize());
+    DSRG_CUDA_TRY(cudaMemcpy(bary_out, L.bary + (L.shared ? 0 : b) * n, sizeof(float) * n, cudaMemcpyDeviceToHost));
+    return DSRG_OK;
+}
+
+int dsrg_engine_lattice_idle(dsrg_engine *h, int which, long long *counts_out) {
+    Engine *e = (Engine *)h;
+    DeviceScope dev_scope(e);
+    int rc = check_entry(e, 1, counts_out && (which == 0 || which == 1));
+    if (rc) return rc;
+    return lattice_idle(e, which == 0 ? e->sp : e->bi, counts_out);
+}
+
+int dsrg_engine_tile_views(dsrg_engine *h, int which, int b, int *nloc_out, uint8_t *hy_out, int *hdr_out,
+                           uint16_t *loc_out, float *wn_out) {
+    Engine *e = (Engine *)h;
+    DeviceScope dev_scope(e);
+    int rc = check_entry(e, 1, e && wn_out && (which == 0 || which == 1) && b >= 0 && b < e->maxB);
+    if (rc) return rc;
+    if (e->MP > DSRG_MAX_LABELS && (nloc_out || hy_out || hdr_out || loc_out)) {
+        set_error("the tile-local views are not built for %d labels (more than %d)", e->M, DSRG_MAX_LABELS);
+        return DSRG_E_STATE;
+    }
+    const Lattice &L = which == 0 ? e->sp : e->bi;
+    const size_t sb = L.shared ? 0 : b, n = (size_t)(L.d + 1) * L.N, nt = e->ntiles;
+    DSRG_CUDA_TRY(cudaDeviceSynchronize());
+    DSRG_CUDA_TRY(cudaMemcpy(wn_out, L.wn + sb * n, sizeof(float) * n, cudaMemcpyDeviceToHost));
+    if (nloc_out) DSRG_CUDA_TRY(cudaMemcpy(nloc_out, L.tl_nloc + sb * nt, sizeof(int32_t) * nt, cudaMemcpyDeviceToHost));
+    if (hy_out) DSRG_CUDA_TRY(cudaMemcpy(hy_out, L.tl_hy + sb * nt, nt, cudaMemcpyDeviceToHost));
+    if (hdr_out)
+        DSRG_CUDA_TRY(cudaMemcpy(hdr_out, L.tl_hdr + sb * nt * L.maxloc, sizeof(int2) * nt * L.maxloc,
+                                 cudaMemcpyDeviceToHost));
+    if (loc_out) DSRG_CUDA_TRY(cudaMemcpy(loc_out, L.tl_loc + sb * n, sizeof(uint16_t) * n, cudaMemcpyDeviceToHost));
     return DSRG_OK;
 }
 

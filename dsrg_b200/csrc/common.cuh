@@ -44,6 +44,7 @@ struct Lattice {
     int cap = 0;            // hash slots per structure
     int capv = 0;           // max vertices per structure = (N+P)*(d+1)
     long long rows_cap = 0; // rows in the value buffers (all images)
+    long long slots_alloc = 0, verts_alloc = 0;  // hkeys / hval and vkey entries allocated (capacity shape, all structures)
     int32_t *off = nullptr;     // [nimg][d+1][N] local row (1-based; 0 = zero row)
     float *bary = nullptr;      // [nimg][d+1][N]
     float *norm = nullptr;      // [nimg][N]
@@ -90,6 +91,9 @@ int lattice_build(Engine *e, Lattice &L, int B, const uint8_t *image_dev, cudaSt
 constexpr int kNoKey = 0x7F7F7F7F;  // renumbering key of no incidence yet (a byte pattern, for cudaMemset)
 constexpr int kRenumChunk = 4 * kThreads;  // bitmap words per renumbering chunk: 4 per thread of k_renum_scan
 long long renum_words(int ntiles, int dp1);  // bitmap words per image, a whole number of chunks
+// what a build must leave for the next one, over every structure's whole allocation: counts[0] hash slots that are
+// not kEmptyKey, [1] hval entries that are not -1, [2] vkey entries that are not kNoKey (synchronises the device)
+int lattice_idle(Engine *e, const Lattice &L, long long *counts);
 // ---- tiles.cu ----
 constexpr int kTileW = 32, kTileH = 8;   // one thread per pixel, one warp per tile row
 constexpr int kTileThreads = kTileW * kTileH;

@@ -512,6 +512,38 @@ static int build_impl(Engine *e, Lattice &L, int nb, const uint8_t *image, cudaS
     return DSRG_OK;
 }
 
+// Read-out for the tests (dsrg_engine_lattice_idle): the build-to-build state is all-empty hash slots, hval -1 and
+// vkey kNoKey; counts what differs from it
+__global__ void __launch_bounds__(kThreads)
+k_lattice_idle(const uint64_t *hkeys, const int32_t *hval, long long nslots, const int32_t *vkey, long long nverts,
+               unsigned long long *counts) {
+    unsigned long long c[3] = {0, 0, 0};
+    const long long stride = (long long)gridDim.x * blockDim.x;
+    for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < nslots; i += stride) {
+        c[0] += hkeys[i] != kEmptyKey;
+        c[1] += hval[i] != -1;
+    }
+    for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < nverts; i += stride) c[2] += vkey[i] != kNoKey;
+#pragma unroll
+    for (int k = 0; k < 3; k++)
+        if (c[k]) atomicAdd(counts + k, c[k]);
+}
+
+int lattice_idle(Engine *e, const Lattice &L, long long *counts) {
+    DSRG_CUDA_TRY(cudaDeviceSynchronize());
+    unsigned long long *d = nullptr;
+    DSRG_CUDA_TRY(cudaMalloc(&d, 3 * sizeof(unsigned long long)));
+    cudaError_t err = cudaMemset(d, 0, 3 * sizeof(unsigned long long));
+    if (err == cudaSuccess) {  // a read-out, not part of any pass: not counted in the engine's launches
+        k_lattice_idle<<<4 * e->sm_count, kThreads>>>(L.hkeys, L.hval, L.slots_alloc, L.vkey, L.verts_alloc, d);
+        err = cudaGetLastError();
+    }
+    if (err == cudaSuccess) err = cudaMemcpy(counts, d, 3 * sizeof(long long), cudaMemcpyDeviceToHost);
+    cudaFree(d);
+    DSRG_CUDA_TRY(err);
+    return DSRG_OK;
+}
+
 // Build the lattices of `B` images (or the single shared one), then their norm vectors.
 int lattice_build(Engine *e, Lattice &L, int B, const uint8_t *image_dev, cudaStream_t s) {
     const int nb = L.shared ? 1 : B;

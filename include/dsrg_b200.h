@@ -555,6 +555,22 @@ int dsrg_engine_lattice_tables(dsrg_engine *e, int which, int b, int *off_out, i
 /* Per-pixel symmetric normalisation vectors (DenseKernel::norm_, pairwise.cpp:54-57) of the
  * last CRF call: which = 0 spatial [N] (shared by the batch), 1 bilateral [B][N]. */
 int dsrg_engine_copy_norm(dsrg_engine *e, int which, int B, float *norm_out_host);
+/* Image b's barycentric weights of the last CRF call, [d+1][N] in the layout of dsrg_engine_lattice_tables' off:
+ * the weight of (r, pixel) on the vertex off[r][pixel].  For tests. */
+int dsrg_engine_lattice_bary(dsrg_engine *e, int which, int b, float *bary_out);
+/* What a lattice build leaves behind for the next one, over the whole allocation of the family (which = 0 spatial,
+ * 1 bilateral): counts_out[0] hash slots that are not empty, [1] slot-to-vertex entries that are not -1, [2]
+ * renumbering keys that are not the no-key value.  All three are 0 between passes.  Synchronises.  For tests. */
+int dsrg_engine_lattice_idle(dsrg_engine *e, int which, long long *counts_out);
+/* Image b's tile-local views of the last CRF call, as the mean-field kernels read them (tiles.cu), for the engine's
+ * ntiles tiles of the current size: nloc_out [ntiles] local vertices of each tile (| 1 << 16: hybrid tile; -1:
+ * overflow tile without a list), hy_out [ntiles] 1 for a hybrid tile, hdr_out [ntiles][maxloc][2] per local vertex
+ * (first entry | count << 16, row), maxloc = DSRG_MAXLOC_SP (spatial) or DSRG_MAXLOC_HY (bilateral), loc_out
+ * [d+1][N] the local vertex of every (r, pixel) (0xFFFF: not in its tile's list), wn_out [d+1][N] the weights
+ * bary * norm.  wn_out is required; the others may be NULL and are refused (DSRG_E_STATE) above DSRG_MAX_LABELS
+ * labels, where the views are not built.  For tests. */
+int dsrg_engine_tile_views(dsrg_engine *e, int which, int b, int *nloc_out, uint8_t *hy_out, int *hdr_out,
+                           uint16_t *loc_out, float *wn_out);
 
 /* ------------------------------------------------------------------------------------------
  * Per-object API with the exact surface of the reference's C++ class DenseCRFWrapper

@@ -419,6 +419,51 @@ def _hybrid_cover_ok(counts, npix, k):
     return covered * 100 >= npix * 6 * k["DSRG_HY_MIN_COVER"]
 
 
+def tile_of_pixels(H, W):
+    """The tile index and the thread index in the tile of every pixel (row-major), tiles.cu's geometry."""
+    k = csrc_constants()
+    tiles_x, tile_w, _ = tile_geometry(H, W)
+    ys, xs = np.mgrid[0:H, 0:W]
+    ty, tx = ys // k["kTileH"], xs // tile_w
+    return (ty * tiles_x + tx).ravel(), ((ys - ty * k["kTileH"]) * k["kTileW"] + xs - tx * tile_w).ravel()
+
+
+def lattice_tile_kinds(off, H, W, which, hybrid_on):
+    """k_tile_build's kind of every tile of one lattice (before k_tile_demote), from the oracle's offsets (N, d+1)."""
+    k = csrc_constants()
+    tiles_x, _, tiles_y = tile_geometry(H, W)
+    ntiles = tiles_x * tiles_y
+    tile_of, _ = tile_of_pixels(H, W)
+    npix = np.bincount(tile_of, minlength=ntiles)
+    maxa = k["DSRG_MAXLOC_SP"] if which == 0 else k["DSRG_MAXLOC_BI"]
+    off = off.astype(np.int64)
+    keys = tile_of[:, None] * (int(off.max()) + 1) + off
+    uniq, cnt = np.unique(keys.ravel(), return_counts=True)
+    utile = uniq // (int(off.max()) + 1)
+    nvert = np.bincount(utile, minlength=ntiles)
+    kinds = np.where(nvert > maxa, "direct", "smem").astype(object)
+    if which == 1 and hybrid_on:
+        for t in np.nonzero(nvert > maxa)[0]:
+            if _hybrid_cover_ok(cnt[utile == t], npix[t], k):
+                kinds[t] = "hybrid"
+    return kinds
+
+
+def hybrid_tiles_on(H, W, B, sm_count):
+    """common.cuh: hybrid_tiles_on (for label counts of the fused path)."""
+    tiles_x, _, tiles_y = tile_geometry(H, W)
+    return tiles_x * tiles_y * B >= 16 * sm_count
+
+
+def demote_hybrid_tiles(bi_kinds, sm_count):
+    """k_tile_demote on the bilateral kinds (B, ntiles), in place; returns the hybrid-tile count the engine reports."""
+    nhy = int((bi_kinds == "hybrid").sum())
+    if nhy < csrc_constants()["DSRG_HY_MIN_TILES"] * sm_count:
+        bi_kinds[bi_kinds == "hybrid"] = "direct"
+        nhy = 0
+    return nhy
+
+
 def predict_tile_paths(images, sf, sm_count, cf=13):
     """What tiles.cu does to each tile of a mean-field pass over `images` (B,H,W,3) with crf_params(sf, cf), from the
     oracle's own lattices.  Returns {"sp": kinds (ntiles,), "bi": kinds (B, ntiles), "hybrid_tiles": n}; a kind is
@@ -426,38 +471,233 @@ def predict_tile_paths(images, sf, sm_count, cf=13):
     path) or "hybrid" (k_mf_tile_hy).  Only the bilateral lattice has hybrid tiles; `hybrid_tiles` is the count the
     engine reports after k_tile_demote."""
     from oracle import crf_oracle
-    k = csrc_constants()
     B, H, W = images.shape[:3]
-    tiles_x, tile_w, tiles_y = tile_geometry(H, W)
-    ntiles = tiles_x * tiles_y
-    ys, xs = np.mgrid[0:H, 0:W]
-    tile_of = ((ys // k["kTileH"]) * tiles_x + xs // tile_w).ravel()
-    npix = np.bincount(tile_of, minlength=ntiles)
-    gate = ntiles * B >= 16 * sm_count                             # common.cuh: hybrid_tiles_on
-    sp_kinds, bi_kinds = None, np.empty((B, ntiles), object)
+    gate = hybrid_tiles_on(H, W, B, sm_count)
+    sp_kinds, bi_kinds = None, np.empty((B, tile_geometry(H, W)[0] * tile_geometry(H, W)[2]), object)
     for b in range(B):
         c = crf_oracle.DenseCRF(W, H, 1)
         c.set_unary_energy(np.zeros(H * W, np.float32))
         c.add_pairwise_energy(10, 80 / sf, 80 / sf, cf, cf, cf, 3, 3 / sf, 3 / sf, images[b].ravel())
-        for lat, maxa in ((0, k["DSRG_MAXLOC_SP"]), (1, k["DSRG_MAXLOC_BI"])):
-            if lat == 0 and b > 0:
-                continue                                           # one spatial lattice serves the batch
-            off = c.lattice(lat).offset.astype(np.int64)          # (N, d+1): the vertex of every (pixel, r)
-            keys = tile_of[:, None] * (int(off.max()) + 1) + off
-            uniq, cnt = np.unique(keys.ravel(), return_counts=True)
-            utile = uniq // (int(off.max()) + 1)
-            nvert = np.bincount(utile, minlength=ntiles)
-            kinds = np.where(nvert > maxa, "direct", "smem").astype(object)
-            if lat == 1 and gate:
-                for t in np.nonzero(nvert > maxa)[0]:
-                    if _hybrid_cover_ok(cnt[utile == t], npix[t], k):
-                        kinds[t] = "hybrid"
-            if lat == 0:
-                sp_kinds = kinds
-            else:
-                bi_kinds[b] = kinds
-    nhy = int((bi_kinds == "hybrid").sum())
-    if nhy < k["DSRG_HY_MIN_TILES"] * sm_count:                    # k_tile_demote
-        bi_kinds[bi_kinds == "hybrid"] = "direct"
-        nhy = 0
+        if b == 0:                                                 # one spatial lattice serves the batch
+            sp_kinds = lattice_tile_kinds(c.lattice(0).offset, H, W, 0, gate)
+        bi_kinds[b] = lattice_tile_kinds(c.lattice(1).offset, H, W, 1, gate)
+    nhy = demote_hybrid_tiles(bi_kinds, sm_count)
     return {"sp": sp_kinds, "bi": bi_kinds, "hybrid_tiles": nhy}
+
+
+# ---- the lattice build, table by table: the cases of test_gpu_lattice_exact.py (checked on the CPU by
+# test_lattice_exact_cpu.py) ----
+def tile_major_pos(H, W):
+    """Position of every pixel (row-major order) in tile-major order: tile index, then thread index in the tile."""
+    k = csrc_constants()
+    tile_of, tid = tile_of_pixels(H, W)
+    return tile_of * k["kTileW"] * k["kTileH"] + tid
+
+
+def check_order(off, H, W):
+    """ids follow the first tile-major incidence; vertices without one (the phantom lanes') come last.
+    Returns the number of vertices that pixels touch."""
+    dp1 = off.shape[0]
+    ids = off - 1
+    key = tile_major_pos(H, W)[None, :] * dp1 + np.arange(dp1)[:, None]
+    V_pix = int(ids.max()) + 1
+    first = np.full(V_pix, np.iinfo(np.int64).max)
+    np.minimum.at(first, ids.ravel(), key.ravel())
+    assert (first < np.iinfo(np.int64).max).all(), "ids touched by pixels are not contiguous from 0"
+    assert (np.diff(first) > 0).all(), "ids do not increase with the first tile-major incidence"
+    return V_pix
+
+
+def check_against_oracle(off, nbr, lat, V_pix):
+    """The engine's tables are the oracle's lattice renamed: one-to-one vertex mapping, same neighbours.  Returns the
+    mapping (oracle id -> engine id, -1 for the vertices only the phantom lanes touch)."""
+    dp1, V = off.shape[0], nbr.shape[1] - 1
+    assert V == lat.M
+    o = lat.offset.T                                   # (d+1, N) oracle ids
+    m = np.full(lat.M, -1, np.int64)
+    m[o.ravel()] = off.ravel() - 1
+    assert np.array_equal(m[o], off - 1), "a vertex maps to two ids"
+    seen = m >= 0
+    assert np.unique(m[seen]).size == seen.sum() == V_pix
+    assert (nbr[:, 0] == 0).all(), "the zero row must point at itself"
+    for j in range(dp1):
+        for on, col in ((lat.n1[j], 0), (lat.n2[j], 1)):
+            got = nbr[j, m[seen] + 1, col]
+            tgt = on[seen]
+            want = np.where(tgt < 0, 0, m[np.maximum(tgt, 0)] + 1)
+            mapped = (tgt < 0) | (m[np.maximum(tgt, 0)] >= 0)
+            assert np.array_equal(got[mapped], want[mapped]), "axis %d neighbour %d" % (j, col)
+            # a neighbour that no pixel touches is one of the phantom lanes' vertices, numbered last
+            assert (got[~mapped] > V_pix).all()
+    return m
+
+
+def phantom_lanes(N):
+    """api.cu:lattice_shape: the tail of the last 4-pixel block (permutohedral.cpp:196)."""
+    return (4 - N % 4) % 4
+
+
+def lattice_scales(d):
+    """api.cu:lattice_scales (permutohedral.cpp:179-182)."""
+    inv_std_dev = np.float32(np.sqrt(2.0 / 3.0) * (d + 1))
+    return np.array([1.0 / np.sqrt((i + 2) * (i + 1)) * np.float64(inv_std_dev) for i in range(d)], np.float32)
+
+
+def key_range_ok(sigma, H, W):
+    """api.cu:key_range_ok for a lattice with the feature sigmas `sigma` (x, y[, c0, c1, c2], float32 values)."""
+    d = len(sigma)
+    sig = [float(np.float32(s)) for s in sigma]
+    scale = lattice_scales(d)
+    fmax = [(W - 1) / sig[0], (H - 1) / sig[1]] + [255.0 / sig[i] for i in range(2, d)]
+    total = big = 0.0
+    for i in range(d):
+        cf = abs(fmax[i]) * float(scale[i])
+        total += cf
+        if (i + 1) * cf > big:
+            big = (i + 1) * cf
+    bound = total + big + 3.0 * (d + 1) + 2
+    return bool(bound < float((1 << ((16 if d == 2 else 12) - 1)) - 1) and np.isfinite(bound))
+
+
+def lattice_sigmas(params, which):
+    """The feature sigmas of lattice `which` (0 spatial, 1 bilateral) under a dsrg_crf_params."""
+    if which == 0:
+        return [params.theta_gamma_x, params.theta_gamma_y]
+    return [params.theta_alpha_x, params.theta_alpha_y, params.theta_beta_r, params.theta_beta_g, params.theta_beta_b]
+
+
+def lattice_features(image, sigma):
+    """(N + phantom lanes, d) float32 features of an (H, W, 3) image, as k_lattice_insert forms them (x / sigma_x,
+    y / sigma_y, colour / sigma_c, each one float32 division); the phantom lanes' rows are 0."""
+    H, W = image.shape[:2]
+    d = len(sigma)
+    ys, xs = np.mgrid[0:H, 0:W]
+    cols = [xs.ravel().astype(np.float32) / np.float32(sigma[0]), ys.ravel().astype(np.float32) / np.float32(sigma[1])]
+    px = image.reshape(-1, 3)
+    cols += [px[:, c].astype(np.float32) / np.float32(sigma[2 + c]) for c in range(d - 2)]
+    f = np.stack(cols, 1)
+    return np.concatenate([f, np.zeros((phantom_lanes(H * W), d), np.float32)])
+
+
+def lattice_insert(f):
+    """k_lattice_insert's arithmetic restated in float32 (one rounding per operation, no contraction) on features
+    (n, d): elevate, the closest 0-coloured simplex, the rank, the barycentric weights and the d+1 vertex keys.
+    Returns keys (n, d+1, d) int64 and bary (n, d+1) float32."""
+    f32 = np.float32
+    n, d = f.shape
+    dp1 = f32(d + 1)
+    scale = lattice_scales(d)
+    el = np.zeros((n, d + 1), f32)
+    sm = np.zeros(n, f32)
+    for j in range(d, 0, -1):
+        cf = f[:, j - 1] * scale[j - 1]
+        el[:, j] = sm - f32(j) * cf
+        sm = sm + cf
+    el[:, 0] = sm
+    inv = f32(1.0) / dp1
+    v = np.rint(inv * el)
+    rem0 = v * dp1
+    isum = v.astype(np.int64).sum(1)
+    rank = np.zeros((n, d + 1), np.int64)
+    for k in range(d):
+        di = el[:, k] - rem0[:, k]
+        for j in range(k + 1, d + 1):
+            lt = di < (el[:, j] - rem0[:, j])
+            rank[:, k] += lt
+            rank[:, j] += ~lt
+    rank += isum[:, None]
+    low, high = rank < 0, rank >= d + 1
+    rank[low] += d + 1
+    rem0[low] = rem0[low] + dp1
+    rank[high] -= d + 1
+    rem0[high] = rem0[high] - dp1
+    bc = np.zeros((n, d + 2), f32)
+    ar = np.arange(n)
+    for k in range(d + 1):
+        val = (el[:, k] - rem0[:, k]) * inv
+        p = d - rank[:, k]
+        bc[ar, p] = bc[ar, p] + val
+        bc[ar, p + 1] = bc[ar, p + 1] - val
+    bc[:, 0] = bc[:, 0] + (f32(1.0) + bc[:, d + 1])
+    keys = np.empty((n, d + 1, d), np.int64)
+    for r in range(d + 1):
+        canon = np.where(rank[:, :d] <= d - r, r, r - (d + 1))
+        keys[:, r] = rem0[:, :d].astype(np.int64) + canon
+    return keys, bc[:, :d + 1]
+
+
+def max_abs_key(image, sigma):
+    return int(np.abs(lattice_insert(lattice_features(image, sigma))[0]).max())
+
+
+def renum_key_limit(H, W):
+    """The largest renumbering key of an engine of H x W (lattice.cu: pos * (d+1) + r of the bilateral lattice, pos
+    up to the phantom lanes' ntiles * kTileThreads), which api.cu keeps below kNoKey."""
+    k = csrc_constants()
+    tiles_x, _, tiles_y = tile_geometry(H, W)
+    return tiles_x * tiles_y * k["kTileW"] * k["kTileH"] * 6 + 5
+
+
+K_NO_KEY = 0x7F7F7F7F                                  # common.cuh: kNoKey
+RENUM_MAX_H_W1 = 11140944                              # the tallest one-pixel-wide engine whose keys stay below it
+
+# A float32 sigma at which api.cu:key_range_ok only just passes: the smallest one (the others fixed), so that the next
+# float32 below it is refused
+EDGE_SHAPE, EDGE_B = (96, 128), 2
+# bilateral: per-axis sigmas that give each feature about the share of the bound that maximises the largest key
+# (cf_i ~ 1/(i+1)); alpha_x is the one at the edge
+EDGE_BI = (0.71240306, 0.616, 1.753, 1.81, 1.848)
+EDGE_SP = (0.016331082, 0.016331082)                   # spatial: both at the edge
+EDGE_MAX_KEY = {0: 19287, 1: 1412}                     # the largest |key| coordinate the edge images reach
+
+
+def edge_params(spatial=EDGE_SP, bilateral=EDGE_BI):
+    from dsrg_b200 import api
+    p = api.crf_params(1.0, maxiter=1)
+    p.theta_gamma_x, p.theta_gamma_y = spatial
+    (p.theta_alpha_x, p.theta_alpha_y, p.theta_beta_r, p.theta_beta_g, p.theta_beta_b) = bilateral
+    return p
+
+
+def extreme_image(rng, H, W):
+    """Colours 0 and 255 only; the first and last eight pixels of the first and last rows run through all eight
+    colour corners, so the largest features meet at the image's corners."""
+    im = (rng.randint(0, 2, (H, W, 3)) * 255).astype(np.uint8)
+    corners = ((np.arange(8)[:, None] >> np.arange(3)) & 1).astype(np.uint8) * 255
+    n = min(8, W)
+    for y in {0, H - 1}:
+        im[y, :n] = corners[:n]
+        im[y, W - n:] = corners[8 - n:]
+    return im
+
+
+# name -> (H, W, B, image kind, sf, M, phantom lanes, tile_w).  Kinds: synth's, "constant", "binary" (0 and 255 only),
+# "repeat" (one synth photo B times).  M > 32 takes the label-chunked path.
+EXACT_CASES = {
+    "1x1": (1, 1, 2, "noise", 1.0, 21, 3, 1),
+    "1x38": (1, 38, 2, "noise", 1.0, 21, 2, 19),
+    "39x1": (39, 1, 2, "noise", 1.0, 21, 1, 1),
+    "2x2": (2, 2, 2, "noise", 1.0, 21, 0, 2),
+    "21x33": (21, 33, 2, "photo", 1.0, 21, 3, 17),
+    "constant": (41, 41, 2, "constant", 1.0, 21, 3, 21),
+    "binary": (45, 52, 2, "binary", 1.0, 21, 0, 26),
+    "repeat": (37, 45, 4, "repeat", 12.0, 21, 3, 23),
+    "513x513": (513, 513, 2, "smooth", 1.0, 21, 3, 31),
+    "coco481x640": (481, 640, 1, "photo", 1.0, 81, 0, 32),
+}
+EXACT_BENCH = (321, 321, 64)                           # bench.py's batch, distinct images
+EXACT_BENCH_CONFIGS = [(img, sf) for img in ("smooth", "photo", "noise") for sf in (12.0, 1.0)]
+EXACT_BENCH_FULL = (0, 31, 63)                         # images whose full tables are compared
+EXACT_SEED = 500
+
+
+def exact_images(kind, H, W, B, seed=EXACT_SEED):
+    rng = np.random.RandomState(seed)
+    if kind == "constant":
+        return np.broadcast_to(np.array([90, 140, 200], np.uint8), (B, H, W, 3)).copy()
+    if kind == "binary":
+        return np.stack([extreme_image(rng, H, W) for _ in range(B)])
+    if kind == "repeat":
+        return np.stack([synth.make_image(rng, H, W, "photo")] * B)
+    return np.stack([small_image(rng, H, W, kind) if H * W < 4096 else synth.make_image(rng, H, W, kind)
+                     for _ in range(B)])

@@ -61,6 +61,11 @@ class Ctx(object):
         self.dptrs = (C.c_void_p * 1)(self.dsc[0].data_ptr())
         self.sel = np.array([0, 3, 5], np.int32)
         self.stream = C.c_void_p(torch.cuda.current_stream().cuda_stream)
+        # outputs of the lattice read-outs (tile views: 3 tiles of up to 256 local vertices)
+        self.counts = np.zeros(3, np.int64)
+        self.tl = [np.zeros(4, np.int32), np.zeros(4, np.uint8), np.zeros(4 * 256 * 2, np.int32),
+                   np.zeros(6 * H * W, np.uint16)]
+        self.off = np.zeros(6 * H * W, np.int32)
 
     def calls(self):
         """name -> (argument list with "B" for the batch size, required pointer positions)."""
@@ -111,6 +116,9 @@ class Ctx(object):
             "dsrg_expandloss_backward_host": ([e, "B", 2, f[0], lab, 0.996, 0.999, f[2]], [3, 4, 7]),
             "dsrg_engine_lattice_sizes": ([e, "B", _p(self.hi32[0]), _p(self.hi32[1])], []),
             "dsrg_engine_copy_norm": ([e, 1, "B", f[3]], [3]),
+            "dsrg_engine_lattice_bary": ([e, 1, MAXB - 1, f[3]], [3]),
+            "dsrg_engine_lattice_idle": ([e, 1, _p(self.counts)], [2]),
+            "dsrg_engine_tile_views": ([e, 1, MAXB - 1] + [_p(a) for a in self.tl] + [f[3]], [7]),
             "dsrg_zoom_scores_dev": ([e, _p(self.dsc[0]), SH, SW, d[3], 0, s], [1, 4]),
             "dsrg_zoom_scores_host": ([e, _p(self.hsc[0]), SH, SW, f[3], 0], [1, 4]),
             "dsrg_predict_mask_dev": ([e, _lib.POST_SUM_SCORES, 1, _p(self.dptrs), _p(self.hs), _p(self.ws), dimg,
@@ -176,6 +184,23 @@ def test_null_arguments_are_refused_before_any_launch(ctx, torch_cuda):
         rc = ctx.call(name, args, MAXB)
         assert rc == _lib.OK, (name, rc, ctx.L.dsrg_last_error().decode())
     torch.cuda.synchronize()
+
+
+def test_lattice_read_outs_refuse_bad_indices(ctx, torch_cuda):
+    """which outside {0, 1} and an image index outside [0, max_batch) are refused like a NULL output."""
+    calls = ctx.calls()
+    ctx.eng.take_launch_count()
+    for name in ("dsrg_engine_lattice_tables", "dsrg_engine_lattice_bary", "dsrg_engine_lattice_idle",
+                 "dsrg_engine_tile_views"):
+        args = calls[name][0] if name in calls else [C.c_void_p(ctx.eng.h), 1, MAXB - 1, _p(ctx.off), None]
+        bad = [(1, v) for v in (-1, 2)] + ([(2, v) for v in (-1, MAXB)] if name != "dsrg_engine_lattice_idle" else [])
+        for k, v in bad:
+            a = list(args)
+            a[k] = v
+            assert ctx.call(name, a, MAXB) == _lib.E_INVALID, (name, k, v)
+            assert "bad argument" in ctx.L.dsrg_last_error().decode(), (name, k, v)
+        assert ctx.call(name, args, MAXB) == _lib.OK, name
+    assert ctx.eng.take_launch_count() == 0
 
 
 def _batch(B=2, Hh=41, Ww=41):
