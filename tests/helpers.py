@@ -243,10 +243,36 @@ def parse_wire_log(text):
     return calls
 
 
-def mf64_problem_params(sf, zero=None, n_iters=10):
-    """api.crf_params(sf) for an n_iters run, with w1 ("w1") or w2 ("w2") set to 0 to isolate one lattice."""
+def as_params(params, cf=13, n_iters=10):
+    """A copy of a dsrg_crf_params, or api.crf_params(sf, cf, n_iters) for a scale factor sf."""
     from dsrg_b200 import api
-    p = api.crf_params(sf, maxiter=n_iters)
+    if isinstance(params, api.CrfParams):
+        return api.CrfParams.from_buffer_copy(params)
+    return api.crf_params(params, cf, n_iters)
+
+
+def pairwise_args(params):
+    """The nine pairwise values of a dsrg_crf_params in add_pairwise_energy's order (wrapper.pyx)."""
+    p = params
+    return (p.w1, p.theta_alpha_x, p.theta_alpha_y, p.theta_beta_r, p.theta_beta_g, p.theta_beta_b, p.w2,
+            p.theta_gamma_x, p.theta_gamma_y)
+
+
+def oracle_lattices(image, params):
+    """The oracle's DenseCRF of one (H,W,3) image under `params` (sf or dsrg_crf_params); .lattice(k) and .norm(k)."""
+    from oracle import crf_oracle
+    H, W = image.shape[:2]
+    c = crf_oracle.DenseCRF(W, H, 1)
+    c.set_unary_energy(np.zeros(H * W, np.float32))
+    c.add_pairwise_energy(*pairwise_args(as_params(params)), np.ascontiguousarray(image).ravel())
+    return c
+
+
+def mf64_problem_params(sf, zero=None, n_iters=10):
+    """api.crf_params(sf) (or a copy of the dsrg_crf_params `sf`) for an n_iters run, with w1 ("w1") or w2 ("w2") set
+    to 0 to isolate one lattice."""
+    p = as_params(sf)
+    p.n_iters = n_iters
     if zero:
         setattr(p, zero, 0.0)
     return p
@@ -300,6 +326,21 @@ def mf64_truth_and_bar(problem, unary, iters=MF64_ITERS, extra=()):
     return q64, bar, spread, [{n: r[n] for n in iters} for r in runs[1 + len(BAR_MODELS):]]
 
 
+
+class Truth(object):
+    """The float64 marginals and the bar of the compared images of a batch, each image's lattices built once."""
+
+    def __init__(self, image, params, images):
+        from oracle import meanfield64
+        self.images = list(images)
+        self.problems = {b: meanfield64.Problem(image[b], params) for b in self.images}
+
+    def __call__(self, unary):
+        q64, bars = {}, {}
+        for b in self.images:
+            q64[b], bars[b], _, _ = mf64_truth_and_bar(self.problems[b], unary[b])
+        return q64, bars
+
 def seeded_images(H, W, kinds, seed):
     return np.stack([synth.make_image(np.random.RandomState(seed + b), H, W, k) for b, k in enumerate(kinds)])
 
@@ -326,13 +367,9 @@ def blur_branch(H, W, vb):
 
 
 def bilateral_vertices(image, sf=1.0, cf=13):
-    """The oracle's bilateral lattice size of one (H,W,3) image (phantom lanes included, as the engine counts)."""
-    from oracle import crf_oracle
-    H, W = image.shape[:2]
-    c = crf_oracle.DenseCRF(W, H, 1)
-    c.set_unary_energy(np.zeros(H * W, np.float32))
-    c.add_pairwise_energy(10, 80 / sf, 80 / sf, cf, cf, cf, 3, 3 / sf, 3 / sf, image.ravel())
-    return int(c.lattice(1).M)
+    """The oracle's bilateral lattice size of one (H,W,3) image (phantom lanes included, as the engine counts) under
+    crf_params(sf, cf) or the dsrg_crf_params `sf`."""
+    return int(oracle_lattices(image, as_params(sf, cf)).lattice(1).M)
 
 
 def padded(M):
@@ -465,19 +502,17 @@ def demote_hybrid_tiles(bi_kinds, sm_count):
 
 
 def predict_tile_paths(images, sf, sm_count, cf=13):
-    """What tiles.cu does to each tile of a mean-field pass over `images` (B,H,W,3) with crf_params(sf, cf), from the
-    oracle's own lattices.  Returns {"sp": kinds (ntiles,), "bi": kinds (B, ntiles), "hybrid_tiles": n}; a kind is
-    "smem" (the tile's distinct vertices fit the shared-memory list), "direct" (overflow tile on k_mf_tile's direct
-    path) or "hybrid" (k_mf_tile_hy).  Only the bilateral lattice has hybrid tiles; `hybrid_tiles` is the count the
-    engine reports after k_tile_demote."""
-    from oracle import crf_oracle
+    """What tiles.cu does to each tile of a mean-field pass over `images` (B,H,W,3) with crf_params(sf, cf) or the
+    dsrg_crf_params `sf`, from the oracle's own lattices.  Returns {"sp": kinds (ntiles,), "bi": kinds (B, ntiles),
+    "hybrid_tiles": n}; a kind is "smem" (the tile's distinct vertices fit the shared-memory list), "direct" (overflow
+    tile on k_mf_tile's direct path) or "hybrid" (k_mf_tile_hy).  Only the bilateral lattice has hybrid tiles;
+    `hybrid_tiles` is the count the engine reports after k_tile_demote."""
     B, H, W = images.shape[:3]
+    params = as_params(sf, cf)
     gate = hybrid_tiles_on(H, W, B, sm_count)
     sp_kinds, bi_kinds = None, np.empty((B, tile_geometry(H, W)[0] * tile_geometry(H, W)[2]), object)
     for b in range(B):
-        c = crf_oracle.DenseCRF(W, H, 1)
-        c.set_unary_energy(np.zeros(H * W, np.float32))
-        c.add_pairwise_energy(10, 80 / sf, 80 / sf, cf, cf, cf, 3, 3 / sf, 3 / sf, images[b].ravel())
+        c = oracle_lattices(images[b], params)
         if b == 0:                                                 # one spatial lattice serves the batch
             sp_kinds = lattice_tile_kinds(c.lattice(0).offset, H, W, 0, gate)
         bi_kinds[b] = lattice_tile_kinds(c.lattice(1).offset, H, W, 1, gate)
@@ -659,6 +694,26 @@ def edge_params(spatial=EDGE_SP, bilateral=EDGE_BI):
     return p
 
 
+def check_restatement(image, params):
+    """The restated insert gives the oracle's barycentric weights bit for bit and its vertices one to one (real
+    pixels and phantom lanes); returns the largest |key| per lattice."""
+    c = oracle_lattices(image, params)
+    N = image.shape[0] * image.shape[1]
+    out = {}
+    for which in (0, 1):
+        lat = c.lattice(which)
+        keys, bary = lattice_insert(lattice_features(image, lattice_sigmas(params, which)))
+        assert np.array_equal(bary[:N].view(np.uint32), lat.bary.view(np.uint32)), which
+        d = keys.shape[2]
+        _, ids = np.unique(keys.reshape(-1, d), axis=0, return_inverse=True)
+        ids = ids.reshape(-1, d + 1)[:N]
+        pairs = np.unique(np.stack([ids.ravel(), lat.offset.ravel()]), axis=1)
+        assert pairs.shape[1] == np.unique(ids).size == np.unique(lat.offset).size, which
+        assert np.unique(keys.reshape(-1, d), axis=0).shape[0] == lat.M, which     # phantom lanes' vertices too
+        out[which] = int(np.abs(keys).max())
+    return out
+
+
 def extreme_image(rng, H, W):
     """Colours 0 and 255 only; the first and last eight pixels of the first and last rows run through all eight
     colour corners, so the largest features meet at the image's corners."""
@@ -701,3 +756,81 @@ def exact_images(kind, H, W, B, seed=EXACT_SEED):
         return np.stack([synth.make_image(rng, H, W, "photo")] * B)
     return np.stack([small_image(rng, H, W, kind) if H * W < 4096 else synth.make_image(rng, H, W, kind)
                      for _ in range(B)])
+
+
+# ---- pairwise parameters other than CRF()'s: the cases of test_gpu_crf_params.py (checked on the CPU by
+# test_crf_params_cpu.py) ----
+# name -> ((w1, theta_alpha x, y, theta_beta r, g, b, w2, theta_gamma x, y), n_iters, image kind, (H, W), B, the
+# tile paths the pass must reach as (spatial, bilateral), or None).  Every image is non-square, so an x / y mix-up
+# cannot hide behind symmetry.  Kinds: "smooth" and "photo" are synth's, "channels" a smooth red, a textured green and
+# a constant blue channel, "binary" helpers.extreme_image.
+PARAM_SETS = {
+    "aniso_xy": ((10, 50, 120, 13, 13, 13, 3, 2, 5), 10, "smooth", (37, 53), 2, None),
+    "aniso_xy_inv": ((10, 120, 50, 13, 13, 13, 3, 5, 2), 10, "smooth", (37, 53), 2, None),   # same images
+    "aniso_rgb": ((10, 80, 80, 7, 13, 31, 3, 3, 3), 10, "channels", (37, 53), 2, None),
+    "weights": ((4.5, 80, 80, 13, 13, 13, 7, 3, 3), 10, "smooth", (37, 53), 2, None),
+    "weights_neg": ((10, 80, 80, 13, 13, 13, -1.5, 3, 3), 10, "smooth", (37, 53), 2, None),
+    "decoupled_sp_direct_bi_smem": ((10, 80, 80, 13, 13, 13, 3, 1.0, 1.2), 10, "smooth", (37, 53), 2,
+                                    ("direct", "smem")),
+    "decoupled_sp_smem_bi_direct": ((10, 3, 4, 2, 2, 2, 3, 3, 3), 10, "smooth", (37, 53), 2, ("smem", "direct")),
+    "decoupled_sp_direct_bi_hybrid": ((10, 80, 80, 13, 13, 13, 3, 0.5, 0.6), 10, "photo", (321, 353), 5,
+                                      ("direct", "hybrid")),
+    "degenerate_x": ((10, 1e4, 80, 13, 13, 13, 3, 1e4, 3), 10, "smooth", (37, 53), 2, None),
+    "degenerate_g": ((10, 80, 80, 13, 1e4, 13, 3, 3, 3), 10, "channels", (37, 53), 2, None),
+}
+PARAM_M, PARAM_WIDE_M = 21, 81
+PARAM_WIDE_SETS = ("aniso_xy", "aniso_rgb")            # also run on the label-chunked path
+PARAM_TINY = (3, 7)                                    # N % 4 = 1: three phantom lanes
+PARAM_SEED = 300
+# A strip on which the x terms of both lattices sit at the packed-key limit: the smallest float32 theta_gamma_x
+# (theta_alpha_x) that api.cu:key_range_ok passes with theta_gamma_y (theta_alpha_y) fixed.  y is smaller than x,
+# so with the two swapped the x term is (W-1)/y and the set is refused.
+KEY_EDGE_SHAPE, KEY_EDGE_B = (31, 700), 2
+KEY_EDGE_SP = (0.07747016102075577, 0.02)
+KEY_EDGE_BI = (2.5485446453094482, 1.0, 13.0, 13.0, 13.0)
+KEY_EDGE_MAX_KEY = {0: 17129, 1: 1079}                 # the largest |key| coordinate the strip's images reach
+
+
+def make_params(values, n_iters=10):
+    """A dsrg_crf_params from the nine pairwise values (add_pairwise_energy's order) and n_iters."""
+    from dsrg_b200 import api
+    p = api.CrfParams()
+    (p.w1, p.theta_alpha_x, p.theta_alpha_y, p.theta_beta_r, p.theta_beta_g, p.theta_beta_b, p.w2, p.theta_gamma_x,
+     p.theta_gamma_y) = values
+    p.n_iters = n_iters
+    return p
+
+
+def set_params(name):
+    values, n_iters = PARAM_SETS[name][:2]
+    return make_params(values, n_iters)
+
+
+def set_images(kind, H, W, B, seed=PARAM_SEED):
+    if kind == "channels":
+        out = []
+        for b in range(B):
+            rng = np.random.RandomState(seed + b)
+            im = small_image(rng, H, W, "smooth").copy()
+            im[..., 1] = synth.make_image(rng, H, W, "noise")[..., 1]
+            im[..., 2] = 90
+            out.append(im)
+        return np.stack(out)
+    if kind == "photo":
+        return synth.make_batch(B, H, W, image="photo", start=seed)["image"]
+    if kind == "binary":
+        return exact_images("binary", H, W, B, seed)
+    return np.stack([small_image(np.random.RandomState(seed + b), H, W, kind) for b in range(B)])
+
+
+def param_set_images(name):
+    _, _, kind, (H, W), B, _ = PARAM_SETS[name]
+    return set_images(kind, H, W, B)
+
+
+def tile_pairing(pred):
+    """(spatial, bilateral) path of a predict_tile_paths result: "direct" when a tile overflows, "hybrid" when the
+    engine runs hybrid tiles, else "smem"."""
+    sp = "direct" if (pred["sp"] == "direct").any() else "smem"
+    bi = "hybrid" if pred["hybrid_tiles"] else "direct" if (pred["bi"] == "direct").any() else "smem"
+    return sp, bi

@@ -18,11 +18,9 @@ import pytest
 import helpers
 from helpers import (FUSED_CONFIGS, FUSED_ITER_M, GATE2_SEED, GATE2_SHAPE, HYBRID_M, MF64_GATE2_M, MF64_ITERS,
                      MF64_PATH_CONFIG, MF64_TINY, MF64_TINY_M, MF64_TINY_SEED, MF64_WIDE_M, MF64_ZERO_W,
-                     MF64_ZERO_W_M, SWITCH_CASES, crf_both_layouts, fused_images, hybrid_images, log_unary,
-                     mf64_problem_params, mf64_truth_and_bar, predict_tile_paths, seeded_images, small_image,
-                     wide_images)
+                     MF64_ZERO_W_M, SWITCH_CASES, Truth, crf_both_layouts, fused_images, hybrid_images, log_unary,
+                     mf64_problem_params, predict_tile_paths, seeded_images, small_image, wide_images)
 from dsrg_b200 import api
-from oracle import meanfield64
 
 pytestmark = pytest.mark.gpu
 ROWS = []          # (case, path, n_iters, device error, bar)
@@ -49,20 +47,6 @@ def check(case, path, got, q64, bar, n, images):
     ROWS.append((case, path, n, err, b_bar))
     for b, (e, bb) in zip(images, rows):
         assert e <= bb, (case, path, n, b, e, bb)
-
-
-class Truth(object):
-    """The float64 marginals and the bar of the compared images of a batch, each image's lattices built once."""
-
-    def __init__(self, image, params, images):
-        self.images = list(images)
-        self.problems = {b: meanfield64.Problem(image[b], params) for b in self.images}
-
-    def __call__(self, unary):
-        q64, bars = {}, {}
-        for b in self.images:
-            q64[b], bars[b], _, _ = mf64_truth_and_bar(self.problems[b], unary[b])
-        return q64, bars
 
 
 def run_case(torch, case, path, image, unary, params, truth, eng=None):

@@ -11,40 +11,9 @@ import pytest
 import helpers
 from conftest import ROOT
 from helpers import (EDGE_B, EDGE_BI, EDGE_MAX_KEY, EDGE_SHAPE, EDGE_SP, EXACT_BENCH, EXACT_CASES, K_NO_KEY,
-                     RENUM_MAX_H_W1, edge_params, exact_images, key_range_ok, lattice_features, lattice_insert,
-                     lattice_sigmas, phantom_lanes, renum_key_limit, tile_geometry)
+                     RENUM_MAX_H_W1, check_restatement, edge_params, exact_images, key_range_ok, lattice_sigmas,
+                     phantom_lanes, renum_key_limit, tile_geometry)
 from dsrg_b200 import _lib, api
-
-
-def oracle_lattices(image, params):
-    from oracle import crf_oracle
-    H, W = image.shape[:2]
-    c = crf_oracle.DenseCRF(W, H, 1)
-    c.set_unary_energy(np.zeros(H * W, np.float32))
-    c.add_pairwise_energy(params.w1, params.theta_alpha_x, params.theta_alpha_y, params.theta_beta_r,
-                          params.theta_beta_g, params.theta_beta_b, params.w2, params.theta_gamma_x,
-                          params.theta_gamma_y, np.ascontiguousarray(image).ravel())
-    return c
-
-
-def check_restatement(image, params):
-    """The restated insert gives the oracle's barycentric weights bit for bit and its vertices one to one (real
-    pixels and phantom lanes); returns the largest |key| per lattice."""
-    c = oracle_lattices(image, params)
-    N = image.shape[0] * image.shape[1]
-    out = {}
-    for which in (0, 1):
-        lat = c.lattice(which)
-        keys, bary = lattice_insert(lattice_features(image, lattice_sigmas(params, which)))
-        assert np.array_equal(bary[:N].view(np.uint32), lat.bary.view(np.uint32)), which
-        d = keys.shape[2]
-        _, ids = np.unique(keys.reshape(-1, d), axis=0, return_inverse=True)
-        ids = ids.reshape(-1, d + 1)[:N]
-        pairs = np.unique(np.stack([ids.ravel(), lat.offset.ravel()]), axis=1)
-        assert pairs.shape[1] == np.unique(ids).size == np.unique(lat.offset).size, which
-        assert np.unique(keys.reshape(-1, d), axis=0).shape[0] == lat.M, which     # phantom lanes' vertices too
-        out[which] = int(np.abs(keys).max())
-    return out
 
 
 @pytest.mark.parametrize("kind,sf", [("photo", 1.0), ("noise", 12.0), ("binary", 1.0)])
