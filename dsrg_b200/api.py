@@ -143,6 +143,23 @@ class Engine(object):
                                          _dptr(out), out_layout, _stream(stream)))
         return out
 
+    def crf_forward_train_dev(self, unary, image, params, q_hist, potts=None, stream=None):
+        """The CRF forward that keeps Q_0..Q_T for the backward: unary (B, M, H, W), image (B, H, W, 3) uint8,
+        q_hist (T+1, B, M, H, W) with q_hist[T] the marginals; potts an optional device float32 [2] {w1, w2} read in
+        place of params.w1 / w2."""
+        B = unary.shape[0]
+        check(self._L.dsrg_crf_forward_train_dev(self.h, _dptr(unary), B, _dptr(image), C.byref(params), _dptr(potts),
+                                                 _dptr(q_hist), _stream(stream)))
+        return q_hist
+
+    def crf_backward_dev(self, q_hist, image, params, grad_q, grad_unary, grad_potts=None, potts=None, stream=None):
+        """DenseCRF::gradient for grad_q = dL/dQ_T (B, M, H, W): grad_unary = dL/dunary (B, M, H, W) and, if given,
+        grad_potts (B, 2) = {dL/dw1, dL/dw2} per image.  image, params and potts as in the forward."""
+        B = grad_q.shape[0]
+        check(self._L.dsrg_crf_backward_dev(self.h, _dptr(q_hist), B, _dptr(image), C.byref(params), _dptr(potts),
+                                            _dptr(grad_q), _dptr(grad_unary), _dptr(grad_potts), _stream(stream)))
+        return grad_unary
+
     def crf_map_dev(self, unary, image, params, labels_out, unary_layout=LAYOUT_NHWC, stream=None):
         B = image.shape[0]
         check(self._L.dsrg_crf_map_batch_dev(self.h, B, _dptr(unary), unary_layout, _dptr(image), C.byref(params),

@@ -324,7 +324,7 @@ using namespace dsrg;
 
 extern "C" {
 
-int dsrg_version(void) { return 111; }
+int dsrg_version(void) { return 112; }
 
 const char *dsrg_last_error(void) { return g_err; }
 
@@ -468,6 +468,7 @@ dsrg_engine *dsrg_engine_create(int device, int max_batch, int H, int W, int M) 
     rc |= dalloc(e, &e->sec_w, (size_t)2 * e->sec_wcap);
     rc |= dalloc(e, &e->dev_err, 1);
     rc |= dalloc(e, &e->hy_list, (size_t)max_batch * e->ntiles);
+    rc |= dalloc(e, &e->potts_part, (size_t)max_batch * e->ntiles);
     rc |= dalloc(e, &e->hy_count, 1);
     if (!rc && cudaMemset(e->hy_count, 0, sizeof(int)) != cudaSuccess) rc = DSRG_E_CUDA;
     if (!rc && cudaMemset(e->dev_err, 0, sizeof(int)) != cudaSuccess) rc = DSRG_E_CUDA;
@@ -495,7 +496,7 @@ void dsrg_engine_destroy(dsrg_engine *h) {
     lattice_free(e->bi);
     void *ptrs[] = {e->U, e->Q0, e->spA, e->spB, e->spC, e->biA, e->biB, e->biC, e->nvA, e->nvB, e->lmap,
                     e->lflag, e->parent, e->hc, e->loss_acc, e->sec_rec, e->sec_img, e->sec_part, e->sec_w, e->dev_err,
-                    e->hy_list, e->hy_count, e->st_unary, e->st_out, e->st_cues, e->st_labels, e->st_image, e->st_lmap, e->st_raw, e->st_idx,
+                    e->hy_list, e->hy_count, e->potts_part, e->st_unary, e->st_out, e->st_cues, e->st_labels, e->st_image, e->st_lmap, e->st_raw, e->st_idx,
                     e->st_prep, e->st_sel};
     for (void *p : ptrs) cudaFree(p);
     if (e->own_stream) cudaStreamDestroy(e->own_stream);
@@ -637,6 +638,50 @@ int dsrg_crf_batch_dev(dsrg_engine *h, int B, const float *unary, int unary_layo
     const cudaStream_t s = (cudaStream_t)stream;
     return dev_call(h, B, s, unary && image && params && out && layout_ok(out_layout), [&](Engine *e) {
         return crf_batch_pass(e, B, unary, unary_layout, image, params, out, out_layout, s);
+    });
+}
+
+// the CRF gradient runs on the fused kernels only
+static int grad_labels_ok(const Engine *e) {
+    if (e->MP <= DSRG_MAX_LABELS) return DSRG_OK;
+    set_error("the CRF gradient supports at most %d labels (got %d); the label-chunked path above that has no backward",
+              DSRG_MAX_LABELS, e->M);
+    return DSRG_E_INVALID;
+}
+
+int dsrg_crf_forward_train_dev(dsrg_engine *h, const float *unary, int B, const uint8_t *image,
+                               const dsrg_crf_params *params, const float *potts, float *q_hist, void *stream) {
+    const cudaStream_t s = (cudaStream_t)stream;
+    return dev_call(h, B, s, unary && image && params && q_hist, [&](Engine *e) {
+        if (int rc = grad_labels_ok(e)) return rc;
+        GraphKey args;
+        args.add(unary).add(image).add(potts).add(q_hist);
+        const int rc = crf_pass(e, s, PassKind::crf_train, B, params, args, [&]() {
+            int r = prepare_lattices(e, B, image, *params, s);
+            if (r) return r;
+            return meanfield_run_train(e, B, unary, q_hist, potts, *params, s);
+        });
+        e->last_crf_B = 0;  // the marginals are q_hist[T], not the engine's: the *_last_* entry points refuse
+        return rc;
+    });
+}
+
+int dsrg_crf_backward_dev(dsrg_engine *h, const float *q_hist, int B, const uint8_t *image,
+                          const dsrg_crf_params *params, const float *potts, const float *grad_q, float *grad_unary,
+                          float *grad_potts, void *stream) {
+    const cudaStream_t s = (cudaStream_t)stream;
+    return dev_call(h, B, s, q_hist && image && params && grad_q && grad_unary, [&](Engine *e) {
+        if (int rc = grad_labels_ok(e)) return rc;
+        GraphKey args;
+        args.add(q_hist).add(image).add(potts).add(grad_q).add(grad_unary).add(grad_potts);
+        const int rc = crf_pass(e, s, PassKind::crf_backward, B, params, args, [&]() {
+            // the lattices are rebuilt: autograd may have run other passes on this engine since the forward
+            int r = prepare_lattices(e, B, image, *params, s);
+            if (r) return r;
+            return meanfield_backward(e, B, q_hist, potts, grad_q, grad_unary, grad_potts, *params, s);
+        });
+        e->last_crf_B = 0;
+        return rc;
     });
 }
 

@@ -89,7 +89,11 @@ struct TileLat {
     int shared;
 };
 
-enum { MODE_FIRST = 0, MODE_MID = 1, MODE_LAST = 2 };
+// MODE & 3 is the iteration's place in the loop.  MODE_HIST (the training forward, dsrg_crf_forward_train_dev) also
+// stores every iteration's Q_t to the caller's history for the backward, never clamps the unary, and reads the Potts
+// weights from device memory when the U_rw argument (unused without the clamp) carries them: {w1, w2}, with c_sp /
+// c_bi then passed as alpha alone.  Without MODE_HIST the instantiations are the inference kernels, unchanged.
+enum { MODE_FIRST = 0, MODE_MID = 1, MODE_LAST = 2, MODE_HIST = 4 };
 
 // exp(x) for x <= 0 via ex2.approx with the rounding error of x*log2(e) folded back in
 // (relative error ~2^-22, independent of |x|)
@@ -383,7 +387,8 @@ __device__ __forceinline__ const float4 *tile_park(TileSmem<MP, MAXBI> &smt, con
     return qs;
 }
 
-// Q = softmax(t) in place (expAndNormalize, densecrf.cpp:98-106); the last iteration stores it to Qout
+// Q = softmax(t) in place (expAndNormalize, densecrf.cpp:98-106); the last iteration (every one with MODE_HIST) stores
+// it to Qout
 template <int MP, int MODE>
 __device__ __forceinline__ void tile_update(float *t, int M, int N, float *__restrict__ Qout, int b, int pix, bool in) {
     float mx = -INFINITY;
@@ -399,7 +404,7 @@ __device__ __forceinline__ void tile_update(float *t, int M, int N, float *__res
     const float inv = __frcp_rn(s);
 #pragma unroll
     for (int k = 0; k < MP; k++) t[k] *= inv;
-    if (MODE == MODE_LAST) {
+    if ((MODE & 3) == MODE_LAST || (MODE & MODE_HIST)) {
         if (in) {
             float *Qb = Qout + (size_t)b * M * N + pix;
 #pragma unroll
@@ -424,8 +429,8 @@ __device__ __forceinline__ void tile_load_pixel(const float *U, float *U_rw, int
 #pragma unroll
         for (int k = 0; k < MP; k++) {
             float v = 0.0f;
-            if (in && k < M) v = (MODE == MODE_FIRST) ? *Ub : __ldg(Ub);  // read-only path once nothing writes U
-            if (MODE == MODE_FIRST) {  // later iterations read the values this one wrote back
+            if (in && k < M) v = ((MODE & 3) == MODE_FIRST) ? *Ub : __ldg(Ub);  // read-only path once nothing writes U
+            if ((MODE & 3) == MODE_FIRST && !(MODE & MODE_HIST)) {  // later iterations read the values this one wrote back
                 if (clamp && in && k < M && v < kMinProb) {
                     v = kMinProb;
                     U_rw[ub + (size_t)k * N] = v;
@@ -459,6 +464,10 @@ k_mf_tile(const float *U, float *U_rw, int clamp, float *__restrict__ Qout, Tile
     // same test on the tile's vertex count, wherever it was placed, made ptxas allocate this kernel's 64 registers
     // differently (more spill traffic in the splat loop, also on images that have no such tile at all).
     if (bi.tl_hy[(size_t)blockIdx.y * ntiles + blockIdx.x]) return;
+    if ((MODE & MODE_HIST) && U_rw) {
+        c_sp *= __ldg(U_rw + 1);
+        c_bi *= __ldg(U_rw);
+    }
     const int tile = blockIdx.x, b = blockIdx.y, tid = threadIdx.x;
     const int tx = tile % tiles_x, ty = tile / tiles_x;
     const int x = tx * tile_w + (tid & 31), y = ty * kTileH + (tid >> 5);
@@ -479,7 +488,7 @@ k_mf_tile(const float *U, float *U_rw, int clamp, float *__restrict__ Qout, Tile
 
     // ---- asynchronous staging: every local vertex's value row (96 B) and the two CSR entry blocks
     // are pulled into shared memory by the bulk-copy engine while the threads load their per-pixel data
-    const int n_copies = (MODE != MODE_FIRST ? n_sp + n_bi : 0) + (MODE != MODE_LAST ? (n_sp > 0) + (n_bi > 0) : 0);
+    const int n_copies = ((MODE & 3) != MODE_FIRST ? n_sp + n_bi : 0) + ((MODE & 3) != MODE_LAST ? (n_sp > 0) + (n_bi > 0) : 0);
     if (tid == 0) {
         mbar_init(&sm.bar, n_copies > 0 ? n_copies : 1);
         smt.wtab[kEntZero] = 0.0f;
@@ -491,12 +500,12 @@ k_mf_tile(const float *U, float *U_rw, int clamp, float *__restrict__ Qout, Tile
         const int lv = is_sp ? i : i - n_sp;
         const int2 h = __ldg((is_sp ? hdr_sp : hdr_bi) + lv);
         const int row = (is_sp ? base_sp : base_bi) + h.y;
-        if (MODE != MODE_FIRST) {
+        if ((MODE & 3) != MODE_FIRST) {
             mbar_arrive_expect_tx(&sm.bar, kRowBytes);
             bulk_g2s((is_sp ? vs_sp : vs_bi) + lv * CHP, (is_sp ? sp.val_in : bi.val_in) + (size_t)row * MP,
                      kRowBytes, &sm.bar);
         }
-        if (MODE != MODE_LAST && lv == (is_sp ? n_sp : n_bi) - 1) {  // the last segment tells the block's length
+        if ((MODE & 3) != MODE_LAST && lv == (is_sp ? n_sp : n_bi) - 1) {  // the last segment tells the block's length
             const uint32_t bytes = ent_block_bytes(h);
             mbar_arrive_expect_tx(&sm.bar, bytes);
             bulk_g2s(is_sp ? ent_sp : ent_bi,
@@ -516,7 +525,7 @@ k_mf_tile(const float *U, float *U_rw, int clamp, float *__restrict__ Qout, Tile
 #else
     const bool tail1 = (M == MP - 3);
 #endif
-    if (MODE != MODE_FIRST && in) {
+    if ((MODE & 3) != MODE_FIRST && in) {
         if (!fb_sp)
             tile_slice_smem<MP, 3>(vs_sp, sp.tl_loc + px_sp, strideN, w_sp, c_sp, t, tail1);
         else
@@ -529,7 +538,7 @@ k_mf_tile(const float *U, float *U_rw, int clamp, float *__restrict__ Qout, Tile
                                      base_bi, w_bi, c_bi, t);
     }
     tile_update<MP, MODE>(t, M, N, Qout, b, pix, in);
-    if (MODE == MODE_LAST) return;
+    if ((MODE & 3) == MODE_LAST) return;
     const float4 *qs = tile_park(smt, t, w_sp, w_bi);
     // ---- splat ----
     float4 *vout_sp = reinterpret_cast<float4 *>(sp.val_out), *vout_bi = reinterpret_cast<float4 *>(bi.val_out);
@@ -557,6 +566,10 @@ k_mf_tile_hy(const float *U, float *U_rw, int clamp, float *__restrict__ Qout, T
     ST &sm = smt.st;
     const int tid = threadIdx.x;
     const int nhy = *hy_count;
+    if ((MODE & MODE_HIST) && U_rw) {
+        c_sp *= __ldg(U_rw + 1);
+        c_bi *= __ldg(U_rw);
+    }
     const size_t strideN = (size_t)N;
     float4 *vs_sp = sm.buf, *vs_bi = sm.buf + kMaxLocSp * CHP;
     uint16_t *ent_sp = sm.ent, *ent_bi = sm.ent + ST::kEntSp;
@@ -580,7 +593,7 @@ k_mf_tile_hy(const float *U, float *U_rw, int clamp, float *__restrict__ Qout, T
         const size_t px_sp = (size_t)sb_sp * 3 * N + pix, px_bi = (size_t)sb_bi * 6 * N + pix;
 
         // ---- asynchronous staging of the local vertices' rows and the CSR entry blocks (as in k_mf_tile) ----
-        const int n_copies = (MODE != MODE_FIRST ? n_sp + n_bi : 0) + (MODE != MODE_LAST ? (n_sp > 0) + (n_bi > 0) : 0);
+        const int n_copies = ((MODE & 3) != MODE_FIRST ? n_sp + n_bi : 0) + ((MODE & 3) != MODE_LAST ? (n_sp > 0) + (n_bi > 0) : 0);
         if (tid == 0) {
             mbar_init(&sm.bar, n_copies > 0 ? n_copies : 1);
             asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
@@ -594,12 +607,12 @@ k_mf_tile_hy(const float *U, float *U_rw, int clamp, float *__restrict__ Qout, T
             const int lv = is_sp ? i : i - n_sp;
             const int2 h = __ldg((is_sp ? hdr_sp : hdr_bi) + lv);
             const int row = (is_sp ? base_sp : base_bi) + h.y;
-            if (MODE != MODE_FIRST) {
+            if ((MODE & 3) != MODE_FIRST) {
                 mbar_arrive_expect_tx(&sm.bar, kRowBytes);
                 bulk_g2s((is_sp ? vs_sp : vs_bi) + lv * CHP, (is_sp ? sp.val_in : bi.val_in) + (size_t)row * MP,
                          kRowBytes, &sm.bar);
             }
-            if (MODE != MODE_LAST && lv == (is_sp ? n_sp : n_bi) - 1) {  // the last segment tells the block's length
+            if ((MODE & 3) != MODE_LAST && lv == (is_sp ? n_sp : n_bi) - 1) {  // the last segment tells the block's length
                 const uint32_t bytes = ent_block_bytes(h);
                 mbar_arrive_expect_tx(&sm.bar, bytes);
                 bulk_g2s(is_sp ? ent_sp : ent_bi,
@@ -616,7 +629,7 @@ k_mf_tile_hy(const float *U, float *U_rw, int clamp, float *__restrict__ Qout, T
         // ---- slice + update ----
         unsigned rm_sp = 0, rm_bi = 0;  // this pixel's incidences that go direct
         if (in) {
-            if (MODE != MODE_FIRST) {
+            if ((MODE & 3) != MODE_FIRST) {
                 rm_sp = tile_slice_mixed<MP, 3>(vs_sp, sp.tl_loc + px_sp, reinterpret_cast<const float4 *>(sp.val_in),
                                                 sp.off + px_sp, strideN, base_sp, w_sp, c_sp, t);
                 rm_bi = tile_slice_mixed<MP, 6>(vs_bi, bi.tl_loc + px_bi, reinterpret_cast<const float4 *>(bi.val_in),
@@ -627,7 +640,7 @@ k_mf_tile_hy(const float *U, float *U_rw, int clamp, float *__restrict__ Qout, T
             }
         }
         tile_update<MP, MODE>(t, M, N, Qout, b, pix, in);
-        if (MODE != MODE_LAST) {
+        if ((MODE & 3) != MODE_LAST) {
             // ---- splat: remote incidences straight from the registers, the local vertices through the CSR ----
             if (rm_sp) tile_splat_remote<MP, 3>(vout_sp, rm_sp, sp.off + px_sp, strideN, base_sp, w_sp, t);
             if (rm_bi) tile_splat_remote<MP, 6>(vout_bi, rm_bi, bi.off + px_bi, strideN, base_bi, w_bi, t);
@@ -637,6 +650,218 @@ k_mf_tile_hy(const float *U, float *U_rw, int clamp, float *__restrict__ Qout, T
         }
         __syncthreads();  // the tile is done with the shared buffers and the barrier
         if (tid == 0) asm volatile("mbarrier.inval.shared::cta.b64 [%0];" ::"r"(smem_u32(&sm.bar)) : "memory");
+    }
+}
+
+// ---------------------------------------------------------------------------------------------
+// The backward of the mean field (DenseCRF::gradient, densecrf.cpp:238-297), one launch per iteration, run from T
+// down to 0 on the forward's tile-local views.  With G = dL/dQ_T and F(X) = norm K(norm X) (alpha folded in):
+//   FIRST : g_T = Q_T (G - <G, Q_T>);  grad_U = g_T;  splat wn g_T
+//   MID   : S_sp = F_sp^T(g_{t+1}), S_bi = F_bi^T(g_{t+1})   (slice of the reverse-blurred splat)
+//           dL/dw2 += <S_sp, Q_t>, dL/dw1 += <S_bi, Q_t>;  G_t = w2 S_sp + w1 S_bi
+//           g_t = Q_t (G_t - <G_t, Q_t>);  grad_U += g_t;  splat wn g_t
+//   LAST  : MID without the splat (t = 0)
+// F^T is the same splat and slice around the transposed blur (blur_all with reverse), so only the blur differs from
+// the forward.  The Potts terms use <g, F(Q)> = <F^T(g), Q>, which needs no forward filter of Q_t (the reference
+// filters Q_t, pairwise.cpp:190-195: equal in exact arithmetic).  Each thread owns its pixel's grad_U row; each CTA
+// adds its tile's two Potts partials to part[b][tile] (FIRST writes zeros), so the sums are deterministic.
+// Every tile kind runs here: hybrid tiles take the direct global path for the bilateral lattice, like overflow tiles.
+// A pixel holds Q_t, G_t and one slice (3 MP floats): above 12 labels that takes more than 128 registers, so those
+// instantiations run one CTA per SM rather than spill.
+// ---------------------------------------------------------------------------------------------
+template <int MP, int MODE>
+__global__ void __launch_bounds__(kTileThreads, MP > 12 ? 1 : 2)
+k_mf_tile_bwd(const float *__restrict__ G, const float *__restrict__ Qt, float *__restrict__ gU, TileLat sp,
+              TileLat bi, float a_sp, float a_bi, const float *potts, float w1, float w2, float2 *part, int M, int N,
+              int W, int H, int tiles_x, int ntiles, int tile_w) {
+    constexpr int kRowBytes = MP * 4;
+    using SM = TileSmem<MP>;
+    using ST = TileStage<MP>;
+    extern __shared__ __align__(128) unsigned char smem_raw[];
+    __shared__ float2 red[kTileThreads / 32];
+    SM &smt = *reinterpret_cast<SM *>(smem_raw);
+    ST &sm = smt.st;
+    const int tile = blockIdx.x, b = blockIdx.y, tid = threadIdx.x;
+    if (potts) {
+        w1 = __ldg(potts);
+        w2 = __ldg(potts + 1);
+    }
+    const int tx = tile % tiles_x, ty = tile / tiles_x;
+    const int x = tx * tile_w + (tid & 31), y = ty * kTileH + (tid >> 5);
+    const bool in = (tid & 31) < tile_w && x < W && y < H;
+    const int pix = in ? y * W + x : 0;
+    const int sb_sp = sp.shared ? 0 : b, sb_bi = bi.shared ? 0 : b;
+    const size_t ti_sp = (size_t)sb_sp * ntiles + tile, ti_bi = (size_t)sb_bi * ntiles + tile;
+    const int nl_sp = sp.tl_nloc[ti_sp], nl_bi = bi.tl_nloc[ti_bi];
+    const bool fb_sp = nl_sp < 0, fb_bi = nl_bi < 0 || bi.tl_hy[ti_bi];
+    const int n_sp = fb_sp ? 0 : nl_sp, n_bi = fb_bi ? 0 : nl_bi;
+    const int base_sp = sp.rowbase[b], base_bi = bi.rowbase[b];
+    constexpr int CHP = ST::CHP;
+    float4 *vs_sp = sm.buf, *vs_bi = sm.buf + kMaxLocSp * CHP;
+    const int2 *hdr_sp = sp.tl_hdr + ti_sp * kMaxLocSp, *hdr_bi = bi.tl_hdr + ti_bi * kMaxLocHy;
+    uint16_t *ent_sp = sm.ent, *ent_bi = sm.ent + ST::kEntSp;
+    const size_t strideN = (size_t)N;
+    const size_t px_sp = (size_t)sb_sp * 3 * N + pix, px_bi = (size_t)sb_bi * 6 * N + pix;
+
+    // ---- asynchronous staging, as in k_mf_tile ----
+    const int n_copies = (MODE != MODE_FIRST ? n_sp + n_bi : 0) + (MODE != MODE_LAST ? (n_sp > 0) + (n_bi > 0) : 0);
+    if (tid == 0) {
+        mbar_init(&sm.bar, n_copies > 0 ? n_copies : 1);
+        smt.wtab[kEntZero] = 0.0f;
+        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    }
+    __syncthreads();
+    for (int i = tid; i < n_sp + n_bi; i += kTileThreads) {
+        const bool is_sp = i < n_sp;
+        const int lv = is_sp ? i : i - n_sp;
+        const int2 h = __ldg((is_sp ? hdr_sp : hdr_bi) + lv);
+        const int row = (is_sp ? base_sp : base_bi) + h.y;
+        if (MODE != MODE_FIRST) {
+            mbar_arrive_expect_tx(&sm.bar, kRowBytes);
+            bulk_g2s((is_sp ? vs_sp : vs_bi) + lv * CHP, (is_sp ? sp.val_in : bi.val_in) + (size_t)row * MP,
+                     kRowBytes, &sm.bar);
+        }
+        if (MODE != MODE_LAST && lv == (is_sp ? n_sp : n_bi) - 1) {
+            const uint32_t bytes = ent_block_bytes(h);
+            mbar_arrive_expect_tx(&sm.bar, bytes);
+            bulk_g2s(is_sp ? ent_sp : ent_bi,
+                     is_sp ? sp.tl_pack + ti_sp * sp.entcap : bi.tl_pack + ti_bi * bi.entcap, bytes, &sm.bar);
+        }
+    }
+    if (n_copies == 0 && tid == 0) mbar_arrive_expect_tx(&sm.bar, 0);
+
+    // ---- per-pixel data: Q_t, the weights, and G (FIRST) ----
+    const size_t ub = (size_t)b * M * N + pix;
+    float q[MP], t[MP], w_sp[3], w_bi[6];
+#pragma unroll
+    for (int k = 0; k < MP; k++) {
+        q[k] = (in && k < M) ? __ldg(Qt + ub + (size_t)k * N) : 0.0f;
+        t[k] = (MODE == MODE_FIRST && in && k < M) ? __ldg(G + ub + (size_t)k * N) : 0.0f;
+    }
+#pragma unroll
+    for (int r = 0; r < 3; r++) w_sp[r] = in ? __ldg(sp.wn + px_sp + r * strideN) : 0.0f;
+#pragma unroll
+    for (int r = 0; r < 6; r++) w_bi[r] = in ? __ldg(bi.wn + px_bi + r * strideN) : 0.0f;
+    mbar_wait(&sm.bar, 0);
+
+    // ---- slice both lattices separately: the Potts partials, then G_t ----
+#ifdef DSRG_NO_TAIL1
+    const bool tail1 = false;
+#else
+    const bool tail1 = (M == MP - 3);
+#endif
+    float p_sp = 0.0f, p_bi = 0.0f;
+    if (MODE != MODE_FIRST && in) {
+        float sl[MP];
+#pragma unroll
+        for (int k = 0; k < MP; k++) sl[k] = 0.0f;
+        if (!fb_sp)
+            tile_slice_smem<MP, 3>(vs_sp, sp.tl_loc + px_sp, strideN, w_sp, a_sp, sl, tail1);
+        else
+            tile_slice_global<MP, 3>(reinterpret_cast<const float4 *>(sp.val_in), sp.off + px_sp, strideN, base_sp,
+                                     w_sp, a_sp, sl);
+#pragma unroll
+        for (int k = 0; k < MP; k++) {
+            p_sp = fmaf(sl[k], q[k], p_sp);
+            t[k] = w2 * sl[k];
+            sl[k] = 0.0f;
+        }
+        if (!fb_bi)
+            tile_slice_smem<MP, 6>(vs_bi, bi.tl_loc + px_bi, strideN, w_bi, a_bi, sl, tail1);
+        else
+            tile_slice_global<MP, 6>(reinterpret_cast<const float4 *>(bi.val_in), bi.off + px_bi, strideN, base_bi,
+                                     w_bi, a_bi, sl);
+#pragma unroll
+        for (int k = 0; k < MP; k++) {
+            p_bi = fmaf(sl[k], q[k], p_bi);
+            t[k] = fmaf(w1, sl[k], t[k]);
+        }
+    }
+    // ---- g = Q (G - <G, Q>)  (sumAndNormalize, densecrf.cpp:107-114, with the opposite sign) ----
+    float dot = 0.0f;
+#pragma unroll
+    for (int k = 0; k < MP; k++) dot = fmaf(t[k], q[k], dot);
+#pragma unroll
+    for (int k = 0; k < MP; k++) t[k] = q[k] * (t[k] - dot);
+    if (in) {
+        float *gb = gU + ub;
+#pragma unroll
+        for (int k = 0; k < MP; k++) {
+            if (k < M) *gb = (MODE == MODE_FIRST) ? t[k] : *gb + t[k];
+            gb += N;
+        }
+    }
+    // ---- the tile's Potts partials, in a fixed order ----
+    if (MODE != MODE_FIRST) {
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) {
+            p_sp += __shfl_down_sync(0xffffffffu, p_sp, o);
+            p_bi += __shfl_down_sync(0xffffffffu, p_bi, o);
+        }
+        if ((tid & 31) == 0) red[tid >> 5] = make_float2(p_sp, p_bi);
+    }
+    if (MODE == MODE_LAST) {
+        __syncthreads();
+    } else {
+        // ---- splat g (tile_park's barriers also publish red[]) ----
+        const float4 *qs = tile_park(smt, t, w_sp, w_bi);
+        float4 *vout_sp = reinterpret_cast<float4 *>(sp.val_out), *vout_bi = reinterpret_cast<float4 *>(bi.val_out);
+        if (fb_sp && in) tile_splat_direct<MP, 3>(vout_sp, sp.off + px_sp, strideN, base_sp, w_sp, t);
+        if (fb_bi && in) tile_splat_direct<MP, 6>(vout_bi, bi.off + px_bi, strideN, base_bi, w_bi, t);
+        tile_splat_csr<MP>(vout_sp, vout_bi, n_sp, n_bi, hdr_sp, hdr_bi, base_sp, base_bi, ent_sp, ent_bi, qs,
+                           smt.wtab);
+    }
+    if (tid == 0) {
+        float2 *pp = part + (size_t)b * ntiles + tile;
+        if (MODE == MODE_FIRST) {
+            *pp = make_float2(0.0f, 0.0f);
+        } else {
+            float2 a = *pp;
+#pragma unroll
+            for (int w = 0; w < kTileThreads / 32; w++) {
+                a.x += red[w].x;
+                a.y += red[w].y;
+            }
+            *pp = a;
+        }
+    }
+}
+
+// dL/dU = g_0 alone (T = 0: Q_0 = softmax(U))
+__global__ void __launch_bounds__(kThreads)
+k_mf_softmax_vjp(const float *G, const float *Q, float *gU, int M, int N) {
+    const int b = blockIdx.y;
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= N) return;
+    const size_t at = (size_t)b * M * N + i;
+    float dot = 0.0f;
+    for (int k = 0; k < M; k++) dot = fmaf(G[at + (size_t)k * N], Q[at + (size_t)k * N], dot);
+    for (int k = 0; k < M; k++) gU[at + (size_t)k * N] = Q[at + (size_t)k * N] * (G[at + (size_t)k * N] - dot);
+}
+
+// per image: the Potts partials of its tiles, summed in a fixed order -> out[b] = {dL/dw1, dL/dw2}
+__global__ void __launch_bounds__(kThreads)
+k_mf_potts_reduce(const float2 *part, float *out, int ntiles) {
+    __shared__ float2 acc[kThreads];
+    const int b = blockIdx.x;
+    float2 a = make_float2(0.0f, 0.0f);
+    for (int i = threadIdx.x; i < ntiles; i += kThreads) {
+        const float2 v = part[(size_t)b * ntiles + i];
+        a.x += v.x;
+        a.y += v.y;
+    }
+    acc[threadIdx.x] = a;
+    __syncthreads();
+    for (int o = kThreads / 2; o > 0; o >>= 1) {
+        if (threadIdx.x < o) {
+            acc[threadIdx.x].x += acc[threadIdx.x + o].x;
+            acc[threadIdx.x].y += acc[threadIdx.x + o].y;
+        }
+        __syncthreads();
+    }
+    if (threadIdx.x == 0) {
+        out[2 * b] = acc[0].y;       // bilateral: w1
+        out[2 * b + 1] = acc[0].x;   // spatial: w2
     }
 }
 
@@ -827,27 +1052,36 @@ static TileLat make_tile_view(const Lattice &L, const float *val_in, float *val_
 // three-axis spatial pass (27 rows) was slower than pair + single.  Re-measured on the tile-major vertex numbering
 // (lattice.cu), same card and limit: three-axis passes (spatial one pass, bilateral two, 2 CTAs per SM) took 6.1 ms
 // against 4.6 for this grouping.  Bilateral pair passes pick their occupancy by the lattice's size (k_mf_blur).
+//
+// `reverse` applies the transposed blur K^T of the backward (DenseKernel::filter(..., transpose=true),
+// pairwise.cpp:63-80; permutohedral.cpp:556 with reverse: axes d..0): the same passes in the opposite order, each pair
+// with its two axes swapped (a negative neighbour stride), so the bilateral lattice runs (5,4) (3,2) (1,0) and the
+// spatial one 2 then (1,0).  Each axis' blur is symmetric on the real rows (a missing neighbour is the zero row, which
+// stays zero), so K^T is the product of the same axis blurs in the opposite order.
 template <int MP>
 static float *blur_all(Engine *e, const Lattice &L, float *buf, float *tmp, float *dead, int B, int tag, int grid,
-                       cudaStream_t s) {
+                       cudaStream_t s, bool reverse = false) {
     float *src = buf, *dst = tmp;
-    for (int j = 0; j <= L.d; j += 2) {
+    const int npass = L.d / 2 + 1;
+    for (int p = 0; p < npass; p++) {
+        const int j = 2 * (reverse ? npass - 1 - p : p);  // the pass's lowest axis
         const float4 *in = (const float4 *)src;
-        const int2 *nbr = L.nbr + (size_t)j * L.nbr_stride;
-        float4 *zero = j == 0 ? (float4 *)dead : nullptr;
+        const long long nst = reverse ? -L.nbr_stride : L.nbr_stride;
+        const int2 *nbr = L.nbr + (size_t)(reverse && j < L.d ? j + 1 : j) * L.nbr_stride;
+        float4 *zero = p == 0 ? (float4 *)dead : nullptr;
         if (j == L.d) {
-            DSRG_LAUNCH(e, tag, s, (k_mf_blur<MP, 1, 8><<<grid, kThreads, 0, s>>>(in, (float4 *)dst, nbr, L.nbr_stride,
+            DSRG_LAUNCH(e, tag, s, (k_mf_blur<MP, 1, 8><<<grid, kThreads, 0, s>>>(in, (float4 *)dst, nbr, nst,
                                                                                 L.rowbase, B, L.shared, zero, 0)));
         } else if (L.shared) {  // the spatial lattice: ~13.5 k rows per image at 321², always cached
-            DSRG_LAUNCH(e, tag, s, (k_mf_blur<MP, 2, 4><<<grid, kThreads, 0, s>>>(in, (float4 *)dst, nbr, L.nbr_stride,
+            DSRG_LAUNCH(e, tag, s, (k_mf_blur<MP, 2, 4><<<grid, kThreads, 0, s>>>(in, (float4 *)dst, nbr, nst,
                                                                                 L.rowbase, B, L.shared, zero, 0)));
         } else if (L.capv <= kBlurCachedRows) {  // no image of this size can have more rows
             DSRG_LAUNCH(e, tag, s, (k_mf_blur<MP, 2, blur_cached_ctas(MP)><<<grid, kThreads, 0, s>>>(
-                                       in, (float4 *)dst, nbr, L.nbr_stride, L.rowbase, B, L.shared, zero, 0)));
+                                       in, (float4 *)dst, nbr, nst, L.rowbase, B, L.shared, zero, 0)));
         } else {
-            DSRG_LAUNCH(e, tag, s, (k_mf_blur<MP, 2, blur_cached_ctas(MP)><<<grid, kThreads, 0, s>>>(in, (float4 *)dst, nbr, L.nbr_stride,
+            DSRG_LAUNCH(e, tag, s, (k_mf_blur<MP, 2, blur_cached_ctas(MP)><<<grid, kThreads, 0, s>>>(in, (float4 *)dst, nbr, nst,
                                                                                 L.rowbase, B, L.shared, zero, 1)));
-            DSRG_LAUNCH(e, tag, s, (k_mf_blur<MP, 2, 4><<<grid, kThreads, 0, s>>>(in, (float4 *)dst, nbr, L.nbr_stride,
+            DSRG_LAUNCH(e, tag, s, (k_mf_blur<MP, 2, 4><<<grid, kThreads, 0, s>>>(in, (float4 *)dst, nbr, nst,
                                                                                 L.rowbase, B, L.shared, zero, 2)));
         }
         float *t = src;
@@ -857,12 +1091,16 @@ static float *blur_all(Engine *e, const Lattice &L, float *buf, float *tmp, floa
     return src;
 }
 
+// q_hist != nullptr: the training forward (MODE_HIST), Q_t of every iteration to q_hist[t] ([T+1][B][M][N]), with
+// the Potts weights read from `potts` ({w1, w2}, device) when it is given
 template <int MP>
 static int run_impl(Engine *e, int B, const float *unary, int layout, bool clamp, float *unary_rw,
-                    const dsrg_crf_params &p, cudaStream_t s) {
+                    const dsrg_crf_params &p, cudaStream_t s, float *q_hist = nullptr, const float *potts = nullptr) {
     const int M = e->M, N = e->N;
     dim3 gp(cdiv(N, kThreads), B);
     const int T = p.n_iters;
+    const bool hist = q_hist != nullptr;
+    const size_t slab = (size_t)B * M * N;
     // planar (NCHW) callers are read in place by the tile kernel; NHWC callers (and T == 0) go
     // through the layout-converting init kernel
     const bool direct = (layout == DSRG_LAYOUT_NCHW) && T > 0;
@@ -872,11 +1110,13 @@ static int run_impl(Engine *e, int B, const float *unary, int layout, bool clamp
     if (!direct)
         DSRG_LAUNCH(e, T_MF_INIT, s,
                     k_mf_init<MP><<<gp, kThreads, 0, s>>>(unary, unary_rw, layout, clamp ? 1 : 0, e->U,
-                                                          T == 0 ? e->Q0 : nullptr, M, N));
+                                                          T == 0 ? (hist ? q_hist : e->Q0) : nullptr, M, N));
     if (T == 0) return DSRG_OK;
     const float alpha_sp = 1.0f / (1 + powf(2, -e->sp.d));  // permutohedral.cpp:571
     const float alpha_bi = 1.0f / (1 + powf(2, -e->bi.d));
-    const float c_sp = p.w2 * alpha_sp, c_bi = p.w1 * alpha_bi;
+    // device-resident weights: the kernels multiply alpha by them (MODE_HIST)
+    const float c_sp = potts ? alpha_sp : p.w2 * alpha_sp, c_bi = potts ? alpha_bi : p.w1 * alpha_bi;
+    float *urw = hist ? const_cast<float *>(potts) : Urw;
     const size_t smem = sizeof(TileSmem<MP>);
     const size_t smem_hy = sizeof(TileSmem<MP, kMaxLocHy>);
     static bool attr_done[64] = {false};   // function attributes are per device
@@ -888,6 +1128,12 @@ static int run_impl(Engine *e, int B, const float *unary, int layout, bool clamp
         DSRG_CUDA_TRY(cudaFuncSetAttribute(k_mf_tile_hy<MP, MODE_FIRST>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_hy));
         DSRG_CUDA_TRY(cudaFuncSetAttribute(k_mf_tile_hy<MP, MODE_MID>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_hy));
         DSRG_CUDA_TRY(cudaFuncSetAttribute(k_mf_tile_hy<MP, MODE_LAST>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_hy));
+        DSRG_CUDA_TRY(cudaFuncSetAttribute(k_mf_tile<MP, MODE_FIRST | MODE_HIST>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        DSRG_CUDA_TRY(cudaFuncSetAttribute(k_mf_tile<MP, MODE_MID | MODE_HIST>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        DSRG_CUDA_TRY(cudaFuncSetAttribute(k_mf_tile<MP, MODE_LAST | MODE_HIST>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        DSRG_CUDA_TRY(cudaFuncSetAttribute(k_mf_tile_hy<MP, MODE_FIRST | MODE_HIST>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_hy));
+        DSRG_CUDA_TRY(cudaFuncSetAttribute(k_mf_tile_hy<MP, MODE_MID | MODE_HIST>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_hy));
+        DSRG_CUDA_TRY(cudaFuncSetAttribute(k_mf_tile_hy<MP, MODE_LAST | MODE_HIST>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_hy));
         attr_done[dv] = true;
     }
 #ifndef DSRG_BLUR_GRID
@@ -911,23 +1157,35 @@ static int run_impl(Engine *e, int B, const float *unary, int layout, bool clamp
         if (hy_on)                                                                                                    \
             DSRG_LAUNCH(e, T_MF_TILE_HY, s,                                                                           \
                         (k_mf_tile_hy<MP, MODEV><<<hgrid, kTileThreads, smem_hy, s>>>(                                \
-                            Usrc, Urw, tclamp, QOUT, vsp, vbi, c_sp, c_bi, M, N, e->W, e->H, e->tiles_x, e->ntiles,   \
+                            Usrc, urw, tclamp, QOUT, vsp, vbi, c_sp, c_bi, M, N, e->W, e->H, e->tiles_x, e->ntiles,   \
                             e->tile_w, e->hy_list, e->hy_count)));                                                    \
         DSRG_LAUNCH(e, T_MF_TILE, s,                                                                                  \
-                    (k_mf_tile<MP, MODEV><<<gt, kTileThreads, smem, s>>>(Usrc, Urw, tclamp, QOUT, vsp, vbi, c_sp,     \
+                    (k_mf_tile<MP, MODEV><<<gt, kTileThreads, smem, s>>>(Usrc, urw, tclamp, QOUT, vsp, vbi, c_sp,     \
                                                                         c_bi, M, N, e->W, e->H, e->tiles_x,           \
                                                                         e->ntiles, e->tile_w)));                      \
     } while (0)
     for (int it = 0; it <= T; it++) {
         TileLat vsp = make_tile_view(e->sp, spX, spY), vbi = make_tile_view(e->bi, biX, biY);
-        if (it == T) {
-            DSRG_TILE_LAUNCH(MODE_LAST, e->Q0);
-            break;
+        if (hist) {
+            float *qt = q_hist + (size_t)it * slab;
+            if (it == T) {
+                DSRG_TILE_LAUNCH(MODE_LAST | MODE_HIST, qt);
+                break;
+            }
+            if (it == 0)
+                DSRG_TILE_LAUNCH(MODE_FIRST | MODE_HIST, qt);
+            else
+                DSRG_TILE_LAUNCH(MODE_MID | MODE_HIST, qt);
+        } else {
+            if (it == T) {
+                DSRG_TILE_LAUNCH(MODE_LAST, e->Q0);
+                break;
+            }
+            if (it == 0)
+                DSRG_TILE_LAUNCH(MODE_FIRST, nullptr);
+            else
+                DSRG_TILE_LAUNCH(MODE_MID, nullptr);
         }
-        if (it == 0)
-            DSRG_TILE_LAUNCH(MODE_FIRST, nullptr);
-        else
-            DSRG_TILE_LAUNCH(MODE_MID, nullptr);
         // the old X is dead: the first blur pass clears it and it becomes the next splat target
         float *sp_res = blur_all<MP>(e, e->sp, spY, spZ, spX, B, T_MF_BLUR_SP, bgrid, s);
         float *bi_res = blur_all<MP>(e, e->bi, biY, biZ, biX, B, T_MF_BLUR_BI, bgrid, s);
@@ -939,6 +1197,90 @@ static int run_impl(Engine *e, int B, const float *unary, int layout, bool clamp
 #undef DSRG_TILE_LAUNCH
     DSRG_CUDA_TRY(cudaGetLastError());
     return DSRG_OK;
+}
+
+// The backward of a training forward (DenseCRF::gradient, densecrf.cpp:238-297) on the lattices the pass just built:
+// k_mf_tile_bwd from T down to 0 with the transposed blur in between, then the per-image Potts sums.
+template <int MP>
+static int bwd_impl(Engine *e, int B, const float *q_hist, const float *potts, const float *G, float *gU,
+                    float *g_potts, const dsrg_crf_params &p, cudaStream_t s) {
+    const int M = e->M, N = e->N, T = p.n_iters;
+    const size_t slab = (size_t)B * M * N;
+    if (T == 0) {
+        DSRG_LAUNCH(e, T_MF_INIT, s,
+                    k_mf_softmax_vjp<<<dim3(cdiv(N, kThreads), B), kThreads, 0, s>>>(G, q_hist, gU, M, N));
+        if (g_potts) DSRG_CUDA_TRY(cudaMemsetAsync(g_potts, 0, sizeof(float) * 2 * B, s));
+        DSRG_CUDA_TRY(cudaGetLastError());
+        return DSRG_OK;
+    }
+    static bool attr_done[64] = {false};
+    const int dv = e->device & 63;
+    const size_t smem = sizeof(TileSmem<MP>);
+    if (!attr_done[dv]) {
+        DSRG_CUDA_TRY(cudaFuncSetAttribute(k_mf_tile_bwd<MP, MODE_FIRST>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        DSRG_CUDA_TRY(cudaFuncSetAttribute(k_mf_tile_bwd<MP, MODE_MID>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        DSRG_CUDA_TRY(cudaFuncSetAttribute(k_mf_tile_bwd<MP, MODE_LAST>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        attr_done[dv] = true;
+    }
+    const float a_sp = 1.0f / (1 + powf(2, -e->sp.d)), a_bi = 1.0f / (1 + powf(2, -e->bi.d));
+    const int bgrid = DSRG_BLUR_GRID * e->sm_count;
+    const dim3 gt(e->ntiles, B);
+    float *spX = e->spA, *spY = e->spB, *spZ = e->spC;
+    float *biX = e->biA, *biY = e->biB, *biZ = e->biC;
+    DSRG_LAUNCH(e, T_MF_ZERO, s,
+                k_mf_zero<MP><<<bgrid, kThreads, 0, s>>>((float4 *)spY, e->sp.rowbase, (float4 *)biY, e->bi.rowbase, B));
+#define DSRG_BWD_LAUNCH(MODEV)                                                                                        \
+    DSRG_LAUNCH(e, T_MF_TILE, s,                                                                                      \
+                (k_mf_tile_bwd<MP, MODEV><<<gt, kTileThreads, smem, s>>>(G, qt, gU, vsp, vbi, a_sp, a_bi, potts, p.w1, \
+                                                                        p.w2, e->potts_part, M, N, e->W, e->H,        \
+                                                                        e->tiles_x, e->ntiles, e->tile_w)))
+    for (int it = T; it >= 0; it--) {
+        const TileLat vsp = make_tile_view(e->sp, spX, spY), vbi = make_tile_view(e->bi, biX, biY);
+        const float *qt = q_hist + (size_t)it * slab;
+        if (it == 0) {
+            DSRG_BWD_LAUNCH(MODE_LAST);
+            break;
+        }
+        if (it == T)
+            DSRG_BWD_LAUNCH(MODE_FIRST);
+        else
+            DSRG_BWD_LAUNCH(MODE_MID);
+        float *sp_res = blur_all<MP>(e, e->sp, spY, spZ, spX, B, T_MF_BLUR_SP, bgrid, s, true);
+        float *bi_res = blur_all<MP>(e, e->bi, biY, biZ, biX, B, T_MF_BLUR_BI, bgrid, s, true);
+        float *sp_other = (sp_res == spY) ? spZ : spY, *bi_other = (bi_res == biY) ? biZ : biY;
+        float *nspY = spX, *nbiY = biX;
+        spX = sp_res; spY = nspY; spZ = sp_other;
+        biX = bi_res; biY = nbiY; biZ = bi_other;
+    }
+#undef DSRG_BWD_LAUNCH
+    if (g_potts)
+        DSRG_LAUNCH(e, T_MF_EXPORT, s, k_mf_potts_reduce<<<B, kThreads, 0, s>>>(e->potts_part, g_potts, e->ntiles));
+    DSRG_CUDA_TRY(cudaGetLastError());
+    return DSRG_OK;
+}
+
+int meanfield_run_train(Engine *e, int B, const float *unary, float *q_hist, const float *potts,
+                        const dsrg_crf_params &p, cudaStream_t s) {
+    switch (e->MP) {
+#define DSRG_CASE(MPV) \
+    case MPV: return run_impl<MPV>(e, B, unary, DSRG_LAYOUT_NCHW, false, nullptr, p, s, q_hist, potts);
+        DSRG_CASE(4) DSRG_CASE(8) DSRG_CASE(12) DSRG_CASE(16) DSRG_CASE(20) DSRG_CASE(24) DSRG_CASE(28) DSRG_CASE(32)
+#undef DSRG_CASE
+    }
+    set_error("unsupported label count %d", e->M);
+    return DSRG_E_INVALID;
+}
+
+int meanfield_backward(Engine *e, int B, const float *q_hist, const float *potts, const float *grad_q,
+                       float *grad_unary, float *grad_potts, const dsrg_crf_params &p, cudaStream_t s) {
+    switch (e->MP) {
+#define DSRG_CASE(MPV) \
+    case MPV: return bwd_impl<MPV>(e, B, q_hist, potts, grad_q, grad_unary, grad_potts, p, s);
+        DSRG_CASE(4) DSRG_CASE(8) DSRG_CASE(12) DSRG_CASE(16) DSRG_CASE(20) DSRG_CASE(24) DSRG_CASE(28) DSRG_CASE(32)
+#undef DSRG_CASE
+    }
+    set_error("unsupported label count %d", e->M);
+    return DSRG_E_INVALID;
 }
 
 int meanfield_run(Engine *e, int B, const float *unary, int unary_layout, bool clamp_inplace,

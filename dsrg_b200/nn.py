@@ -16,6 +16,9 @@ Semantics follow the drop-in Caffe layers (dsrg_b200/dropin/pylayers):
   Caffe layers ignore.
 * ``DSRGHead`` runs one mean-field pass per step: the DSRG seeds grow on the marginals the CRF layer has just
   computed (``dsrg_srg_last_crf_dev``), where the composition ``crf_layer`` + ``dsrg_seeds`` runs two.
+* ``dense_crf`` is the CRF alone with its exact gradient (DenseCRF::gradient, densecrf.cpp:238-297): the mean field
+  run backwards to the unaries and, when they are tensors, the two Potts weights.  ``crf_layer`` and ``DSRGHead``
+  keep the reference's ``(1 - result) * top_diff``.
 
 Engines are cached per (labels, height, width, device) and recreated when a larger batch arrives.  Autograd runs
 a backward on the forward's stream and device, so one engine is never driven from two threads at once.
@@ -335,6 +338,79 @@ class _ExpandLoss(torch.autograd.Function):
         _engine_for(probs).expandloss_backward_dev(probs, labels, grad, n_global=probs.shape[0], q_fg=ctx.q[0],
                                                    q_bg=ctx.q[1], stream=_stream(probs))
         return _scaled(grad, g), None, None, None
+
+
+FUSED_LABELS = 32   # DSRG_MAX_LABELS: the CRF gradient runs on the fused kernels only
+_POTTS_DEFAULT = (10.0, 3.0)   # CRF.py:31-32: w1 (bilateral), w2 (spatial)
+
+
+def _potts_weight(w, name, ref):
+    if w is None:
+        return None
+    if not isinstance(w, torch.Tensor) or w.dim() != 0 or not w.is_floating_point() or w.device != ref.device:
+        raise ValueError("%s must be None or a 0-dim floating-point tensor on %s (got %r)"
+                         % (name, ref.device, w if not isinstance(w, torch.Tensor) else (w.dtype, tuple(w.shape), w.device)))
+    return w
+
+
+class _DenseCrf(torch.autograd.Function):
+    @staticmethod
+    @_fwd
+    def forward(ctx, unary, image, w1, w2, scale_factor, color_factor, maxiter):
+        eng = _engine_for(unary)
+        s = _stream(unary)
+        params = api.crf_params(scale_factor, color_factor, maxiter)
+        potts = None
+        if w1 is not None or w2 is not None:   # the kernels read both weights from here (no host synchronisation)
+            potts = torch.empty(2, dtype=torch.float32, device=unary.device)
+            for i, (w, d) in enumerate(zip((w1, w2), _POTTS_DEFAULT)):
+                if w is None:
+                    potts[i].fill_(d)
+                else:
+                    potts[i].copy_(w.detach())
+        q_hist = torch.empty((maxiter + 1,) + tuple(unary.shape), dtype=torch.float32, device=unary.device)
+        eng.crf_forward_train_dev(unary, image, params, q_hist, potts=potts, stream=s)
+        ctx.save_for_backward(q_hist, image, potts)
+        ctx.params = params
+        return q_hist[maxiter].clone()
+
+    @staticmethod
+    @_bwd
+    def backward(ctx, g):
+        q_hist, image, potts = ctx.saved_tensors
+        grad_u = torch.empty(q_hist.shape[1:], dtype=torch.float32, device=q_hist.device)
+        grad_potts = None
+        if potts is not None and (ctx.needs_input_grad[2] or ctx.needs_input_grad[3]):
+            grad_potts = torch.empty((q_hist.shape[1], 2), dtype=torch.float32, device=q_hist.device)
+        _engine_for(grad_u).crf_backward_dev(q_hist, image, ctx.params, g.contiguous(), grad_u, grad_potts=grad_potts,
+                                             potts=potts, stream=_stream(grad_u))
+        gw1 = grad_potts[:, 0].sum() if grad_potts is not None and ctx.needs_input_grad[2] else None
+        gw2 = grad_potts[:, 1].sum() if grad_potts is not None and ctx.needs_input_grad[3] else None
+        return grad_u, None, gw1, gw2, None, None, None
+
+
+def dense_crf(unary, image, scale_factor=1.0, color_factor=13, maxiter=10, w1=None, w2=None):
+    """The dense CRF of CRF() (CRF/krahenbuhl2013/CRF.py:4-37) as a differentiable layer: unary (N, M, H, W) float32,
+    M <= 32, the values CRF(image, unary) takes (energy = -unary); image (N, H, W, 3) uint8 at the map size ->
+    marginals (N, M, H, W) after `maxiter` mean-field iterations.  The backward is the exact gradient of the
+    marginals (the mean field run backwards, DenseCRF::gradient): to `unary` and, when given as 0-dim CUDA tensors,
+    to the Potts weights w1 (bilateral) and w2 (spatial), whose gradient is the sum over the batch.  None means
+    CRF()'s 10 and 3, without a gradient.  The forward keeps every iteration's marginals for the backward:
+    (maxiter + 1) * N * M * H * W * 4 bytes of device memory."""
+    if torch.is_autocast_enabled("cuda"):   # what custom_fwd(cast_inputs=float32) does, before the checks
+        unary = unary.float() if isinstance(unary, torch.Tensor) and unary.is_floating_point() else unary
+    u = _maps(unary, "unary")
+    N, M, H, W = u.shape
+    if M > FUSED_LABELS:
+        raise ValueError("dense_crf supports at most %d labels (got %d)" % (FUSED_LABELS, M))
+    if (not isinstance(image, torch.Tensor) or image.dtype != torch.uint8 or tuple(image.shape) != (N, H, W, 3)
+            or image.device != u.device):
+        raise ValueError("image must be a (%d, %d, %d, 3) uint8 tensor on %s" % (N, H, W, u.device))
+    _cuda(u, "unary")
+    w1, w2 = _potts_weight(w1, "w1", u), _potts_weight(w2, "w2", u)
+    if int(maxiter) < 0:
+        raise ValueError("maxiter must be >= 0 (got %d)" % maxiter)
+    return _DenseCrf.apply(u, image.contiguous(), w1, w2, float(scale_factor), float(color_factor), int(maxiter))
 
 
 def softmax(fc8):

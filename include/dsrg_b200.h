@@ -136,6 +136,29 @@ int dsrg_crf_batch_dev(dsrg_engine *e, int B, const float *unary_dev, int unary_
 int dsrg_crf_batch_host(dsrg_engine *e, int B, const float *unary_host, int unary_layout,
                         const uint8_t *image_host, const dsrg_crf_params *params, float *out_host,
                         int out_layout);
+/*
+ * The CRF as a differentiable layer: the forward keeps every iteration's marginals and the backward runs the mean
+ * field backwards through them (DenseCRF::gradient, densecrf.cpp:238-297, with the objective's gradient given).
+ * Label counts up to DSRG_MAX_LABELS; more return DSRG_E_INVALID.
+ *   unary  : [B][M][H][W] (NCHW) values as passed to CRF(image, unary), energy = -unary; not clamped
+ *   potts  : optional device float[2] {w1, w2} read by the kernels in place of params->w1 / w2, so that a caller can
+ *            learn the Potts weights without a host synchronisation.  Its address is part of a cached graph's key,
+ *            its values are not
+ *   q_hist : [T+1][B][M][H][W] float32 with T = params->n_iters: Q_0 = softmax(unary), ..., q_hist[T] = the marginals
+ *            (dsrg_crf_batch_dev's result within its bound).  (T+1)*B*M*H*W*4 bytes of HBM: 31 MB at batch 20 @ 41x41
+ *            with 21 labels and T = 10, 6.1 GB at batch 64 @ 321x321
+ * dsrg_crf_backward_dev takes grad_q = dL/dQ_T [B][M][H][W] and writes
+ *   grad_unary : dL/dunary [B][M][H][W] (the reference's unary_grad is taken w.r.t. the energy: its negation, [N][M])
+ *   grad_potts : optional [B][2] {dL/dw1, dL/dw2} per image (the reference's lbl_cmp_grad lists w2 first)
+ * with the same image, params and potts as the forward.  It rebuilds the lattices, so other passes may run on the
+ * engine in between.  Neither call leaves marginals for the *_last_* entry points: they return DSRG_E_STATE after it.
+ * The batch size follows the array it describes (unary, q_hist), as in dsrg_crflayer_backward_dev.
+ */
+int dsrg_crf_forward_train_dev(dsrg_engine *e, const float *unary_dev, int B, const uint8_t *image_dev,
+                               const dsrg_crf_params *params, const float *potts_dev, float *q_hist_dev, void *stream);
+int dsrg_crf_backward_dev(dsrg_engine *e, const float *q_hist_dev, int B, const uint8_t *image_dev,
+                          const dsrg_crf_params *params, const float *potts_dev, const float *grad_q_dev,
+                          float *grad_unary_dev, float *grad_potts_dev, void *stream);
 /* arg-max labelling after inference: DenseCRFWrapper::map, densecrf_wrapper.cpp:39-43 */
 int dsrg_crf_map_batch_dev(dsrg_engine *e, int B, const float *unary_dev, int unary_layout,
                            const uint8_t *image_dev, const dsrg_crf_params *params,

@@ -1,0 +1,98 @@
+"""Time the differentiable CRF against the plain forward, per step:
+
+  forward   dsrg_crf_batch_dev: the mean field alone (inference)
+  train     dsrg_crf_forward_train_dev + dsrg_crf_backward_dev: the forward that keeps Q_0..Q_T, then the exact
+            backward to the unaries and the Potts weights (what nn.dense_crf runs per training step)
+
+on three workloads: train-s's shape (batch 20, 41 x 41 maps, 21 labels, scale_factor 12, smooth images) and batch 64
+at 321 x 321 with scale_factor 1 on smooth and on photo-like images; 10 mean-field iterations.  The legs run on a side
+stream (the engine's CUDA graphs need one), are warmed up, and are alternated in rounds within one session; each
+window is timed with CUDA events.  Prints one JSON line per workload with the median ms per step of each leg, and the
+card's name, power limit and SM clocks read in the same run.
+
+usage: python tools/bench_crf_grad.py [--steps 20] [--warmup 3] [--rounds 5] [--workloads train_s,b64_smooth,b64_photo]
+"""
+import argparse
+import json
+import os
+import sys
+
+import numpy as np
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+sys.path.insert(0, os.path.join(ROOT, "tools"))
+
+from bench_torch_step import card  # noqa: E402
+
+WORKLOADS = {   # name -> (B, H, W, M, scale factor, image)
+    "train_s": (20, 41, 41, 21, 12.0, "smooth"),
+    "b64_smooth": (64, 321, 321, 21, 1.0, "smooth"),
+    "b64_photo": (64, 321, 321, 21, 1.0, "photo"),
+}
+T = 10
+
+
+def run(name, steps, warmup, rounds):
+    import torch
+    from dsrg_b200 import api, synth
+    B, H, W, M, sf, img = WORKLOADS[name]
+    batch = synth.make_batch(B, H, W, C=M, image=img, start=3, unique=8)
+    unary = torch.from_numpy(np.log(np.maximum(batch["probs"], 1e-5)).astype(np.float32)).cuda()
+    image = torch.from_numpy(batch["image"]).cuda()
+    G = torch.randn_like(unary)
+    p = api.crf_params(sf, 13, T)
+    eng = api.Engine(B, H, W, M)
+    out = torch.empty_like(unary)
+    q_hist = torch.empty((T + 1,) + tuple(unary.shape), device="cuda")
+    gu, gw = torch.empty_like(unary), torch.empty((B, 2), device="cuda")
+    s = torch.cuda.Stream()
+    legs = {
+        "forward": lambda: eng.crf_dev(unary, image, p, out, unary_layout=api.LAYOUT_NCHW,
+                                       out_layout=api.LAYOUT_NCHW, stream=s.cuda_stream),
+        "train": lambda: (eng.crf_forward_train_dev(unary, image, p, q_hist, stream=s.cuda_stream),
+                          eng.crf_backward_dev(q_hist, image, p, G, gu, grad_potts=gw, stream=s.cuda_stream)),
+    }
+    times = {k: [] for k in legs}
+    with torch.cuda.stream(s):
+        for fn in legs.values():
+            for _ in range(warmup):
+                fn()
+        torch.cuda.synchronize()
+        for _ in range(rounds):
+            for k, fn in legs.items():
+                a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+                a.record(s)
+                for _ in range(steps):
+                    fn()
+                b.record(s)
+                b.synchronize()
+                times[k].append(a.elapsed_time(b) / steps)
+    eng.close()
+    med = {k: float(np.median(v)) for k, v in times.items()}
+    return dict(workload=name, B=B, H=H, W=W, M=M, scale_factor=sf, image=img, n_iters=T,
+                ms_per_step={k: round(v, 3) for k, v in med.items()},
+                spread_ms={k: [round(min(v), 3), round(max(v), 3)] for k, v in times.items()},
+                train_over_forward=round(med["train"] / med["forward"], 2),
+                q_hist_bytes=(T + 1) * B * M * H * W * 4)
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--steps", type=int, default=20)
+    ap.add_argument("--warmup", type=int, default=3)
+    ap.add_argument("--rounds", type=int, default=5)
+    ap.add_argument("--workloads", default=",".join(WORKLOADS))
+    a = ap.parse_args()
+    import torch
+    if not torch.cuda.is_available():
+        sys.exit("bench_crf_grad.py needs a CUDA device")
+    info = card()
+    for name in a.workloads.split(","):
+        r = run(name, a.steps, a.warmup, a.rounds)
+        r.update(info)
+        print(json.dumps(r), flush=True)
+
+
+if __name__ == "__main__":
+    main()
