@@ -160,6 +160,24 @@ class Engine(object):
                                             _dptr(grad_q), _dptr(grad_unary), _dptr(grad_potts), _stream(stream)))
         return grad_unary
 
+    def crf_forward_train_compat_dev(self, unary, image, params, compat, q_hist, stream=None):
+        """crf_forward_train_dev with label-compatibility matrices in place of the Potts weights: compat a device
+        float32 (2, M, M) {mu_bi, mu_sp}, t = unary - mu_sp F_sp(Q) - mu_bi F_bi(Q); params.w1 / w2 are ignored."""
+        B = unary.shape[0]
+        check(self._L.dsrg_crf_forward_train_compat_dev(self.h, _dptr(unary), B, _dptr(image), C.byref(params),
+                                                        _dptr(compat), _dptr(q_hist), _stream(stream)))
+        return q_hist
+
+    def crf_backward_compat_dev(self, q_hist, image, params, compat, grad_q, grad_unary, grad_compat=None,
+                                stream=None):
+        """The backward of crf_forward_train_compat_dev: grad_unary (B, M, H, W) and, if given, grad_compat
+        (B, 2, M, M) = dL/d{mu_bi, mu_sp} per image."""
+        B = grad_q.shape[0]
+        check(self._L.dsrg_crf_backward_compat_dev(self.h, _dptr(q_hist), B, _dptr(image), C.byref(params),
+                                                   _dptr(compat), _dptr(grad_q), _dptr(grad_unary),
+                                                   _dptr(grad_compat), _stream(stream)))
+        return grad_unary
+
     def crf_map_dev(self, unary, image, params, labels_out, unary_layout=LAYOUT_NHWC, stream=None):
         B = image.shape[0]
         check(self._L.dsrg_crf_map_batch_dev(self.h, B, _dptr(unary), unary_layout, _dptr(image), C.byref(params),

@@ -496,7 +496,7 @@ void dsrg_engine_destroy(dsrg_engine *h) {
     lattice_free(e->bi);
     void *ptrs[] = {e->U, e->Q0, e->spA, e->spB, e->spC, e->biA, e->biB, e->biC, e->nvA, e->nvB, e->lmap,
                     e->lflag, e->parent, e->hc, e->loss_acc, e->sec_rec, e->sec_img, e->sec_part, e->sec_w, e->dev_err,
-                    e->hy_list, e->hy_count, e->potts_part, e->st_unary, e->st_out, e->st_cues, e->st_labels, e->st_image, e->st_lmap, e->st_raw, e->st_idx,
+                    e->hy_list, e->hy_count, e->potts_part, e->compat_part, e->st_unary, e->st_out, e->st_cues, e->st_labels, e->st_image, e->st_lmap, e->st_raw, e->st_idx,
                     e->st_prep, e->st_sel};
     for (void *p : ptrs) cudaFree(p);
     if (e->own_stream) cudaStreamDestroy(e->own_stream);
@@ -659,7 +659,7 @@ int dsrg_crf_forward_train_dev(dsrg_engine *h, const float *unary, int B, const 
         const int rc = crf_pass(e, s, PassKind::crf_train, B, params, args, [&]() {
             int r = prepare_lattices(e, B, image, *params, s);
             if (r) return r;
-            return meanfield_run_train(e, B, unary, q_hist, potts, *params, s);
+            return meanfield_run_train(e, B, unary, q_hist, potts, nullptr, *params, s);
         });
         e->last_crf_B = 0;  // the marginals are q_hist[T], not the engine's: the *_last_* entry points refuse
         return rc;
@@ -678,7 +678,57 @@ int dsrg_crf_backward_dev(dsrg_engine *h, const float *q_hist, int B, const uint
             // the lattices are rebuilt: autograd may have run other passes on this engine since the forward
             int r = prepare_lattices(e, B, image, *params, s);
             if (r) return r;
-            return meanfield_backward(e, B, q_hist, potts, grad_q, grad_unary, grad_potts, *params, s);
+            return meanfield_backward(e, B, q_hist, potts, grad_q, grad_unary, grad_potts, nullptr, nullptr, *params, s);
+        });
+        e->last_crf_B = 0;
+        return rc;
+    });
+}
+
+int dsrg_crf_forward_train_compat_dev(dsrg_engine *h, const float *unary, int B, const uint8_t *image,
+                                      const dsrg_crf_params *params, const float *compat, float *q_hist, void *stream) {
+    const cudaStream_t s = (cudaStream_t)stream;
+    return dev_call(h, B, s, unary && image && params && compat && q_hist, [&](Engine *e) {
+        if (int rc = grad_labels_ok(e)) return rc;
+        GraphKey args;
+        args.add(unary).add(image).add(compat).add(q_hist);
+        const int rc = crf_pass(e, s, PassKind::crf_train_compat, B, params, args, [&]() {
+            int r = prepare_lattices(e, B, image, *params, s);
+            if (r) return r;
+            return meanfield_run_train(e, B, unary, q_hist, nullptr, compat, *params, s);
+        });
+        e->last_crf_B = 0;
+        return rc;
+    });
+}
+
+// The compatibility backward's per-tile partials, B * ntiles * 2 * M^2 floats, on its first call: an engine that never
+// learns matrices keeps its footprint.  Sized for the capacity's tile count (set_size never exceeds it).  The call may
+// sit inside a caller's stream capture, where an allocation is allowed in relaxed mode only.
+static int ensure_compat_part(Engine *e) {
+    if (e->compat_part) return DSRG_OK;
+    const size_t tiles = (size_t)((e->Wcap + kTileW - 1) / kTileW) * ((e->Hcap + kTileH - 1) / kTileH);
+    cudaStreamCaptureMode mode = cudaStreamCaptureModeRelaxed;
+    DSRG_CUDA_TRY(cudaThreadExchangeStreamCaptureMode(&mode));
+    const int rc = dalloc(e, &e->compat_part, (size_t)e->maxB * tiles * 2 * e->M * e->M);
+    DSRG_CUDA_TRY(cudaThreadExchangeStreamCaptureMode(&mode));
+    return rc;
+}
+
+int dsrg_crf_backward_compat_dev(dsrg_engine *h, const float *q_hist, int B, const uint8_t *image,
+                                 const dsrg_crf_params *params, const float *compat, const float *grad_q,
+                                 float *grad_unary, float *grad_compat, void *stream) {
+    const cudaStream_t s = (cudaStream_t)stream;
+    return dev_call(h, B, s, q_hist && image && params && compat && grad_q && grad_unary, [&](Engine *e) {
+        if (int rc = grad_labels_ok(e)) return rc;
+        if (int rc = ensure_compat_part(e)) return rc;
+        GraphKey args;
+        args.add(q_hist).add(image).add(compat).add(grad_q).add(grad_unary).add(grad_compat);
+        const int rc = crf_pass(e, s, PassKind::crf_backward_compat, B, params, args, [&]() {
+            int r = prepare_lattices(e, B, image, *params, s);   // as in dsrg_crf_backward_dev
+            if (r) return r;
+            return meanfield_backward(e, B, q_hist, nullptr, grad_q, grad_unary, nullptr, compat, grad_compat, *params,
+                                      s);
         });
         e->last_crf_B = 0;
         return rc;

@@ -155,10 +155,13 @@ inline bool hybrid_tiles_on(const Engine *e, int B);
 int meanfield_run(Engine *e, int B, const float *unary, int unary_layout, bool clamp_inplace,
                   float *unary_rw, const dsrg_crf_params &p, cudaStream_t s);
 // the training forward (NCHW unary, Q_0..Q_T to q_hist) and its backward; at most DSRG_MAX_LABELS labels
-int meanfield_run_train(Engine *e, int B, const float *unary, float *q_hist, const float *potts,
+// (with `compat` = {mu_bi, mu_sp} [2][M][M] in place of the Potts weights: the compatibility-matrix variant, whose
+// backward needs e->compat_part, ensure_compat_part)
+int meanfield_run_train(Engine *e, int B, const float *unary, float *q_hist, const float *potts, const float *compat,
                         const dsrg_crf_params &p, cudaStream_t s);
 int meanfield_backward(Engine *e, int B, const float *q_hist, const float *potts, const float *grad_q,
-                       float *grad_unary, float *grad_potts, const dsrg_crf_params &p, cudaStream_t s);
+                       float *grad_unary, float *grad_potts, const float *compat, float *grad_compat,
+                       const dsrg_crf_params &p, cudaStream_t s);
 // ---- meanfield_wide.cu: label counts above DSRG_MAX_LABELS ----
 int meanfield_run_wide(Engine *e, int B, const float *unary, int unary_layout, bool clamp_inplace,
                        float *unary_rw, const dsrg_crf_params &p, cudaStream_t s);
@@ -200,6 +203,9 @@ struct Engine {
     int tile_w = 32;  // <= 32: the image width is split evenly so that no sliver tiles remain
     int2 *hy_list = nullptr;   // [maxB * ntiles] (tile, image) of the hybrid tiles of the current lattices
     float2 *potts_part = nullptr;  // [maxB * ntiles] the CRF backward's per-tile Potts partials (spatial, bilateral)
+    // [maxB * ntiles][2][M][M] the compatibility backward's per-tile partials (bilateral, spatial); allocated by its
+    // first call (ensure_compat_part)
+    float *compat_part = nullptr;
     int *hy_count = nullptr;   // their number (device-resident)
     // 1-channel buffers for the normalisation pass
     float *nvA = nullptr, *nvB = nullptr;
@@ -408,7 +414,8 @@ cudaError_t numa_host_alloc(void **p, size_t bytes, int device);
 // launches from the stream into a graph, instantiate, launch.  Afterwards: one cudaGraphLaunch.  Falls back to
 // plain launches on the legacy default stream, inside somebody else's capture, while per-kernel profiling is on,
 // or if capture fails.  `body` issues the launches on `s` and returns a DSRG_* code.
-enum class PassKind : int { crf, crf_map, forward, crflayer, densecrf, post, crf_train, crf_backward };
+enum class PassKind : int { crf, crf_map, forward, crflayer, densecrf, post, crf_train, crf_backward, crf_train_compat,
+                            crf_backward_compat };
 struct GraphKey {
     std::string bytes;
     GraphKey() = default;

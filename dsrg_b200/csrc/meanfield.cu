@@ -93,7 +93,10 @@ struct TileLat {
 // stores every iteration's Q_t to the caller's history for the backward, never clamps the unary, and reads the Potts
 // weights from device memory when the U_rw argument (unused without the clamp) carries them: {w1, w2}, with c_sp /
 // c_bi then passed as alpha alone.  Without MODE_HIST the instantiations are the inference kernels, unchanged.
-enum { MODE_FIRST = 0, MODE_MID = 1, MODE_LAST = 2, MODE_HIST = 4 };
+// MODE_COMPAT (with MODE_HIST: dsrg_crf_forward_train_compat_dev; in k_mf_tile_bwd: dsrg_crf_backward_compat_dev)
+// replaces the Potts messages by label-compatibility matrices, t = U - mu_sp F_sp(Q) - mu_bi F_bi(Q): U_rw (potts in
+// the backward) then carries {mu_bi, mu_sp} ([2][M][M], row l = the message to label l), c_sp / c_bi are alpha alone.
+enum { MODE_FIRST = 0, MODE_MID = 1, MODE_LAST = 2, MODE_HIST = 4, MODE_COMPAT = 8 };
 
 // exp(x) for x <= 0 via ex2.approx with the rounding error of x*log2(e) folded back in
 // (relative error ~2^-22, independent of |x|)
@@ -367,6 +370,59 @@ __device__ __forceinline__ void tile_splat_remote(float4 *vout, unsigned remote,
     }
 }
 
+// ---- label-compatibility matrices (MODE_COMPAT) ----
+// They sit in dynamic shared memory behind the kernel's TileSmem, zero-padded to [2][MP][MP] ({bi, sp}); every
+// thread of a warp reads the same element, so the reads are broadcasts.  The CTA stages them before its first barrier.
+template <int MP>
+constexpr size_t kCompatSmem = sizeof(float) * 2 * MP * MP;
+template <int MP>
+__device__ __forceinline__ const float *compat_stage(unsigned char *at, const float *mu, int M) {
+    float *s = reinterpret_cast<float *>(at);
+    for (int i = threadIdx.x; i < 2 * MP * MP; i += kTileThreads) {
+        const int k = i / (MP * MP), l = i / MP % MP, l2 = i % MP;
+        s[i] = (l < M && l2 < M) ? __ldg(mu + ((size_t)k * M + l) * M + l2) : 0.0f;
+    }
+    return s;
+}
+
+// The phantom lanes of a slice are set to zero: under tail1 the slice never reads them, elsewhere they hold whatever the
+// staged or global rows hold there, and the zero-padded columns of mu would turn a non-finite one into NaN (0 * inf).
+template <int MP>
+__device__ __forceinline__ void compat_clear_phantoms(float *sl, int M) {
+#pragma unroll
+    for (int k = 0; k < MP; k++)
+        if (k >= M) sl[k] = 0.0f;
+}
+
+// t -= mu sl (the forward's message) or, with TRANSPOSE, t -= mu^T sl (the backward's G_t), as fma chains over the
+// labels in ascending order.  The empty asm keeps each row's loads of mu next to that row's fmas, so that the
+// registers hold one row of mu at a time beside t and the slice.
+template <int MP, bool TRANSPOSE>
+__device__ __forceinline__ void compat_apply(const float *mu, const float *sl, float *t) {
+#pragma unroll
+    for (int l = 0; l < MP; l++) {
+#pragma unroll
+        for (int l2 = 0; l2 < MP; l2++) t[l] = fmaf(-mu[TRANSPOSE ? l2 * MP + l : l * MP + l2], sl[l2], t[l]);
+        asm volatile("" ::: "memory");
+    }
+}
+
+// tile_slice_smem / tile_slice_global one row at a time (the same fma chain): at 32 labels ptxas otherwise issued a
+// whole lattice's row loads ahead of the previous lattice's message and spilled
+template <int MP, int DP1>
+__device__ __forceinline__ void compat_slice(bool direct, const float4 *vs, const uint16_t *loc, const float4 *vin,
+                                             const int32_t *off, size_t stride, int base, const float *w, float coef,
+                                             float *sl, bool tail1) {
+#pragma unroll
+    for (int r = 0; r < DP1; r++) {
+        if (!direct)
+            tile_slice_smem<MP, 1>(vs, loc + r * stride, stride, w + r, coef, sl, tail1);
+        else
+            tile_slice_global<MP, 1>(vin, off + r * stride, stride, base, w + r, coef, sl);
+        asm volatile("" ::: "memory");
+    }
+}
+
 // ---- the per-tile steps both tile kernels share ----
 // The tile coordinates and the bulk-copy staging are still written out in each kernel: moved into a shared helper,
 // either one changed the SASS of some k_mf_tile / k_mf_tile_hy instantiations (register choice, loop offsets).
@@ -450,8 +506,10 @@ __device__ __forceinline__ void tile_load_pixel(const float *U, float *U_rw, int
     }
 }
 
+// MODE_COMPAT holds a slice beside t (2 MP floats): like k_mf_tile_bwd it runs one CTA per SM above 12 labels rather
+// than spill
 template <int MP, int MODE>
-__global__ void __launch_bounds__(kTileThreads, DSRG_TILE_CTAS)
+__global__ void __launch_bounds__(kTileThreads, (MODE & MODE_COMPAT) ? (MP > 12 ? 1 : 2) : DSRG_TILE_CTAS)
 k_mf_tile(const float *U, float *U_rw, int clamp, float *__restrict__ Qout, TileLat sp, TileLat bi, float c_sp,
           float c_bi, int M, int N, int W, int H, int tiles_x, int ntiles, int tile_w) {
     constexpr int kRowBytes = MP * 4;
@@ -464,7 +522,10 @@ k_mf_tile(const float *U, float *U_rw, int clamp, float *__restrict__ Qout, Tile
     // same test on the tile's vertex count, wherever it was placed, made ptxas allocate this kernel's 64 registers
     // differently (more spill traffic in the splat loop, also on images that have no such tile at all).
     if (bi.tl_hy[(size_t)blockIdx.y * ntiles + blockIdx.x]) return;
-    if ((MODE & MODE_HIST) && U_rw) {
+    const float *mu = nullptr;
+    if constexpr ((MODE & MODE_COMPAT) != 0) {
+        mu = compat_stage<MP>(smem_raw + sizeof(SM), U_rw, M);
+    } else if ((MODE & MODE_HIST) && U_rw) {
         c_sp *= __ldg(U_rw + 1);
         c_bi *= __ldg(U_rw);
     }
@@ -526,16 +587,33 @@ k_mf_tile(const float *U, float *U_rw, int clamp, float *__restrict__ Qout, Tile
     const bool tail1 = (M == MP - 3);
 #endif
     if ((MODE & 3) != MODE_FIRST && in) {
-        if (!fb_sp)
-            tile_slice_smem<MP, 3>(vs_sp, sp.tl_loc + px_sp, strideN, w_sp, c_sp, t, tail1);
-        else
-            tile_slice_global<MP, 3>(reinterpret_cast<const float4 *>(sp.val_in), sp.off + px_sp, strideN,
-                                     base_sp, w_sp, c_sp, t);
-        if (!fb_bi)
-            tile_slice_smem<MP, 6>(vs_bi, bi.tl_loc + px_bi, strideN, w_bi, c_bi, t, tail1);
-        else
-            tile_slice_global<MP, 6>(reinterpret_cast<const float4 *>(bi.val_in), bi.off + px_bi, strideN,
-                                     base_bi, w_bi, c_bi, t);
+        if constexpr ((MODE & MODE_COMPAT) != 0) {
+            // each lattice sliced into its own vector, then its matrix message
+            float sl[MP];
+#pragma unroll
+            for (int k = 0; k < MP; k++) sl[k] = 0.0f;
+            compat_slice<MP, 3>(fb_sp, vs_sp, sp.tl_loc + px_sp, reinterpret_cast<const float4 *>(sp.val_in),
+                                sp.off + px_sp, strideN, base_sp, w_sp, c_sp, sl, tail1);
+            compat_clear_phantoms<MP>(sl, M);
+            compat_apply<MP, false>(mu + MP * MP, sl, t);
+#pragma unroll
+            for (int k = 0; k < MP; k++) sl[k] = 0.0f;
+            compat_slice<MP, 6>(fb_bi, vs_bi, bi.tl_loc + px_bi, reinterpret_cast<const float4 *>(bi.val_in),
+                                bi.off + px_bi, strideN, base_bi, w_bi, c_bi, sl, tail1);
+            compat_clear_phantoms<MP>(sl, M);
+            compat_apply<MP, false>(mu, sl, t);
+        } else {
+            if (!fb_sp)
+                tile_slice_smem<MP, 3>(vs_sp, sp.tl_loc + px_sp, strideN, w_sp, c_sp, t, tail1);
+            else
+                tile_slice_global<MP, 3>(reinterpret_cast<const float4 *>(sp.val_in), sp.off + px_sp, strideN,
+                                         base_sp, w_sp, c_sp, t);
+            if (!fb_bi)
+                tile_slice_smem<MP, 6>(vs_bi, bi.tl_loc + px_bi, strideN, w_bi, c_bi, t, tail1);
+            else
+                tile_slice_global<MP, 6>(reinterpret_cast<const float4 *>(bi.val_in), bi.off + px_bi, strideN,
+                                         base_bi, w_bi, c_bi, t);
+        }
     }
     tile_update<MP, MODE>(t, M, N, Qout, b, pix, in);
     if ((MODE & 3) == MODE_LAST) return;
@@ -554,7 +632,7 @@ k_mf_tile(const float *U, float *U_rw, int clamp, float *__restrict__ Qout, Tile
 // memory straight from the registers.  Its own register / shared-memory budget (DSRG_HY_CTAS CTAs per SM) keeps
 // this code out of k_mf_tile's 64-register allocation.
 template <int MP, int MODE>
-__global__ void __launch_bounds__(kTileThreads, DSRG_HY_CTAS)
+__global__ void __launch_bounds__(kTileThreads, (MODE & MODE_COMPAT) ? (MP > 12 ? 1 : 2) : DSRG_HY_CTAS)
 k_mf_tile_hy(const float *U, float *U_rw, int clamp, float *__restrict__ Qout, TileLat sp, TileLat bi, float c_sp,
              float c_bi, int M, int N, int W, int H, int tiles_x, int ntiles, int tile_w, const int2 *hy_list,
              const int *hy_count) {
@@ -566,7 +644,10 @@ k_mf_tile_hy(const float *U, float *U_rw, int clamp, float *__restrict__ Qout, T
     ST &sm = smt.st;
     const int tid = threadIdx.x;
     const int nhy = *hy_count;
-    if ((MODE & MODE_HIST) && U_rw) {
+    const float *mu = nullptr;   // visible after the first tile's barriers
+    if constexpr ((MODE & MODE_COMPAT) != 0) {
+        mu = compat_stage<MP>(smem_raw + sizeof(TileSmem<MP, kMaxLocHy>), U_rw, M);
+    } else if ((MODE & MODE_HIST) && U_rw) {
         c_sp *= __ldg(U_rw + 1);
         c_bi *= __ldg(U_rw);
     }
@@ -629,7 +710,21 @@ k_mf_tile_hy(const float *U, float *U_rw, int clamp, float *__restrict__ Qout, T
         // ---- slice + update ----
         unsigned rm_sp = 0, rm_bi = 0;  // this pixel's incidences that go direct
         if (in) {
-            if ((MODE & 3) != MODE_FIRST) {
+            if ((MODE & 3) != MODE_FIRST && (MODE & MODE_COMPAT)) {
+                float sl[MP];
+#pragma unroll
+                for (int k = 0; k < MP; k++) sl[k] = 0.0f;
+                rm_sp = tile_slice_mixed<MP, 3>(vs_sp, sp.tl_loc + px_sp, reinterpret_cast<const float4 *>(sp.val_in),
+                                                sp.off + px_sp, strideN, base_sp, w_sp, c_sp, sl);
+                compat_clear_phantoms<MP>(sl, M);
+                compat_apply<MP, false>(mu + MP * MP, sl, t);
+#pragma unroll
+                for (int k = 0; k < MP; k++) sl[k] = 0.0f;
+                rm_bi = tile_slice_mixed<MP, 6>(vs_bi, bi.tl_loc + px_bi, reinterpret_cast<const float4 *>(bi.val_in),
+                                                bi.off + px_bi, strideN, base_bi, w_bi, c_bi, sl);
+                compat_clear_phantoms<MP>(sl, M);
+                compat_apply<MP, false>(mu, sl, t);
+            } else if ((MODE & 3) != MODE_FIRST) {
                 rm_sp = tile_slice_mixed<MP, 3>(vs_sp, sp.tl_loc + px_sp, reinterpret_cast<const float4 *>(sp.val_in),
                                                 sp.off + px_sp, strideN, base_sp, w_sp, c_sp, t);
                 rm_bi = tile_slice_mixed<MP, 6>(vs_bi, bi.tl_loc + px_bi, reinterpret_cast<const float4 *>(bi.val_in),
@@ -667,14 +762,26 @@ k_mf_tile_hy(const float *U, float *U_rw, int clamp, float *__restrict__ Qout, T
 // adds its tile's two Potts partials to part[b][tile] (FIRST writes zeros), so the sums are deterministic.
 // Every tile kind runs here: hybrid tiles take the direct global path for the bilateral lattice, like overflow tiles.
 // A pixel holds Q_t, G_t and one slice (3 MP floats): above 12 labels that takes more than 128 registers, so those
-// instantiations run one CTA per SM rather than spill.
+// instantiations run one CTA per SM rather than spill (MODE_COMPAT: above 8, for its outer products).
+//
+// MODE_COMPAT (potts = {mu_bi, mu_sp}, part = the [B][ntiles][2][M][M] float partials): G_t = -(mu_sp^T S_sp +
+// mu_bi^T S_bi), and dL/dmu_k += -sum_i S_k,i (x) Q_t,i, again by <g, F(Q)> = <F^T(g), Q> per label pair.  Each pixel
+// parks S_bi, S_sp and Q_t in shared memory (behind mu, rows of an odd stride so that the parking is conflict free);
+// after the splat each thread owns fixed (l, l') entries and sums them over the tile's pixels in pixel order.
 // ---------------------------------------------------------------------------------------------
+// rows of the parked S_bi / S_sp / Q_t: an odd stride >= M
+__host__ __device__ constexpr int compat_park_stride(int m) { return m | 1; }
+template <int MP>
+constexpr size_t kCompatParkSmem = sizeof(float) * 3 * kTileThreads * compat_park_stride(MP);
+
 template <int MP, int MODE>
-__global__ void __launch_bounds__(kTileThreads, MP > 12 ? 1 : 2)
+__global__ void __launch_bounds__(kTileThreads, MP > ((MODE & MODE_COMPAT) ? 8 : 12) ? 1 : 2)
 k_mf_tile_bwd(const float *__restrict__ G, const float *__restrict__ Qt, float *__restrict__ gU, TileLat sp,
               TileLat bi, float a_sp, float a_bi, const float *potts, float w1, float w2, float2 *part, int M, int N,
               int W, int H, int tiles_x, int ntiles, int tile_w) {
     constexpr int kRowBytes = MP * 4;
+    constexpr int PH = MODE & 3;   // the iteration's place in the loop
+    constexpr bool kCompat = (MODE & MODE_COMPAT) != 0;
     using SM = TileSmem<MP>;
     using ST = TileStage<MP>;
     extern __shared__ __align__(128) unsigned char smem_raw[];
@@ -682,7 +789,12 @@ k_mf_tile_bwd(const float *__restrict__ G, const float *__restrict__ Qt, float *
     SM &smt = *reinterpret_cast<SM *>(smem_raw);
     ST &sm = smt.st;
     const int tile = blockIdx.x, b = blockIdx.y, tid = threadIdx.x;
-    if (potts) {
+    const float *mu = nullptr;
+    float *park = nullptr;
+    if constexpr (kCompat) {
+        mu = compat_stage<MP>(smem_raw + sizeof(SM), potts, M);
+        park = reinterpret_cast<float *>(smem_raw + sizeof(SM) + kCompatSmem<MP>);
+    } else if (potts) {
         w1 = __ldg(potts);
         w2 = __ldg(potts + 1);
     }
@@ -704,7 +816,7 @@ k_mf_tile_bwd(const float *__restrict__ G, const float *__restrict__ Qt, float *
     const size_t px_sp = (size_t)sb_sp * 3 * N + pix, px_bi = (size_t)sb_bi * 6 * N + pix;
 
     // ---- asynchronous staging, as in k_mf_tile ----
-    const int n_copies = (MODE != MODE_FIRST ? n_sp + n_bi : 0) + (MODE != MODE_LAST ? (n_sp > 0) + (n_bi > 0) : 0);
+    const int n_copies = (PH != MODE_FIRST ? n_sp + n_bi : 0) + (PH != MODE_LAST ? (n_sp > 0) + (n_bi > 0) : 0);
     if (tid == 0) {
         mbar_init(&sm.bar, n_copies > 0 ? n_copies : 1);
         smt.wtab[kEntZero] = 0.0f;
@@ -716,12 +828,12 @@ k_mf_tile_bwd(const float *__restrict__ G, const float *__restrict__ Qt, float *
         const int lv = is_sp ? i : i - n_sp;
         const int2 h = __ldg((is_sp ? hdr_sp : hdr_bi) + lv);
         const int row = (is_sp ? base_sp : base_bi) + h.y;
-        if (MODE != MODE_FIRST) {
+        if (PH != MODE_FIRST) {
             mbar_arrive_expect_tx(&sm.bar, kRowBytes);
             bulk_g2s((is_sp ? vs_sp : vs_bi) + lv * CHP, (is_sp ? sp.val_in : bi.val_in) + (size_t)row * MP,
                      kRowBytes, &sm.bar);
         }
-        if (MODE != MODE_LAST && lv == (is_sp ? n_sp : n_bi) - 1) {
+        if (PH != MODE_LAST && lv == (is_sp ? n_sp : n_bi) - 1) {
             const uint32_t bytes = ent_block_bytes(h);
             mbar_arrive_expect_tx(&sm.bar, bytes);
             bulk_g2s(is_sp ? ent_sp : ent_bi,
@@ -736,7 +848,7 @@ k_mf_tile_bwd(const float *__restrict__ G, const float *__restrict__ Qt, float *
 #pragma unroll
     for (int k = 0; k < MP; k++) {
         q[k] = (in && k < M) ? __ldg(Qt + ub + (size_t)k * N) : 0.0f;
-        t[k] = (MODE == MODE_FIRST && in && k < M) ? __ldg(G + ub + (size_t)k * N) : 0.0f;
+        t[k] = (PH == MODE_FIRST && in && k < M) ? __ldg(G + ub + (size_t)k * N) : 0.0f;
     }
 #pragma unroll
     for (int r = 0; r < 3; r++) w_sp[r] = in ? __ldg(sp.wn + px_sp + r * strideN) : 0.0f;
@@ -751,7 +863,48 @@ k_mf_tile_bwd(const float *__restrict__ G, const float *__restrict__ Qt, float *
     const bool tail1 = (M == MP - 3);
 #endif
     float p_sp = 0.0f, p_bi = 0.0f;
-    if (MODE != MODE_FIRST && in) {
+    if constexpr (kCompat) {
+        if (PH != MODE_FIRST) {
+            // S_sp, then S_bi, each sliced into sl (zero outside the image), its mu^T message into G_t and its row
+            // parked; Q_t parked beside them
+            constexpr int kRow = compat_park_stride(MP);
+            const int rs = compat_park_stride(M);
+            float *pk_bi = park + tid * rs, *pk_sp = pk_bi + kTileThreads * kRow, *pk_q = pk_sp + kTileThreads * kRow;
+            float sl[MP];
+#pragma unroll
+            for (int k = 0; k < MP; k++) sl[k] = 0.0f;
+            if (in) {
+                if (!fb_sp)
+                    tile_slice_smem<MP, 3>(vs_sp, sp.tl_loc + px_sp, strideN, w_sp, a_sp, sl, tail1);
+                else
+                    tile_slice_global<MP, 3>(reinterpret_cast<const float4 *>(sp.val_in), sp.off + px_sp, strideN,
+                                             base_sp, w_sp, a_sp, sl);
+            }
+            compat_clear_phantoms<MP>(sl, M);
+            compat_apply<MP, true>(mu + MP * MP, sl, t);
+#pragma unroll
+            for (int k = 0; k < MP; k++) {
+                if (k < M) pk_sp[k] = sl[k];
+                sl[k] = 0.0f;
+            }
+            if (in) {
+                if (!fb_bi)
+                    tile_slice_smem<MP, 6>(vs_bi, bi.tl_loc + px_bi, strideN, w_bi, a_bi, sl, tail1);
+                else
+                    tile_slice_global<MP, 6>(reinterpret_cast<const float4 *>(bi.val_in), bi.off + px_bi, strideN,
+                                             base_bi, w_bi, a_bi, sl);
+            }
+            compat_clear_phantoms<MP>(sl, M);
+            compat_apply<MP, true>(mu, sl, t);
+#pragma unroll
+            for (int k = 0; k < MP; k++) {
+                if (k < M) {
+                    pk_bi[k] = sl[k];
+                    pk_q[k] = q[k];
+                }
+            }
+        }
+    } else if (PH != MODE_FIRST && in) {
         float sl[MP];
 #pragma unroll
         for (int k = 0; k < MP; k++) sl[k] = 0.0f;
@@ -787,12 +940,12 @@ k_mf_tile_bwd(const float *__restrict__ G, const float *__restrict__ Qt, float *
         float *gb = gU + ub;
 #pragma unroll
         for (int k = 0; k < MP; k++) {
-            if (k < M) *gb = (MODE == MODE_FIRST) ? t[k] : *gb + t[k];
+            if (k < M) *gb = (PH == MODE_FIRST) ? t[k] : *gb + t[k];
             gb += N;
         }
     }
     // ---- the tile's Potts partials, in a fixed order ----
-    if (MODE != MODE_FIRST) {
+    if (!kCompat && PH != MODE_FIRST) {
 #pragma unroll
         for (int o = 16; o > 0; o >>= 1) {
             p_sp += __shfl_down_sync(0xffffffffu, p_sp, o);
@@ -800,7 +953,7 @@ k_mf_tile_bwd(const float *__restrict__ G, const float *__restrict__ Qt, float *
         }
         if ((tid & 31) == 0) red[tid >> 5] = make_float2(p_sp, p_bi);
     }
-    if (MODE == MODE_LAST) {
+    if (PH == MODE_LAST) {
         __syncthreads();
     } else {
         // ---- splat g (tile_park's barriers also publish red[]) ----
@@ -811,9 +964,30 @@ k_mf_tile_bwd(const float *__restrict__ G, const float *__restrict__ Qt, float *
         tile_splat_csr<MP>(vout_sp, vout_bi, n_sp, n_bi, hdr_sp, hdr_bi, base_sp, base_bi, ent_sp, ent_bi, qs,
                            smt.wtab);
     }
-    if (tid == 0) {
+    if constexpr (kCompat) {
+        // ---- the tile's two outer-product partials (the barriers above published the parked rows) ----
+        float *pp = reinterpret_cast<float *>(part) + ((size_t)b * ntiles + tile) * 2 * M * M;
+        const int rs = compat_park_stride(M);
+        constexpr int kRow = compat_park_stride(MP);
+        const float *pk_bi = park, *pk_sp = park + kTileThreads * kRow, *pk_q = pk_sp + kTileThreads * kRow;
+        for (int e = tid; e < M * M; e += kTileThreads) {
+            float a_b = 0.0f, a_s = 0.0f;
+            if (PH != MODE_FIRST) {
+                const int l = e / M, l2 = e - l * M;
+                for (int i = 0; i < kTileThreads; i++) {
+                    const float qv = pk_q[i * rs + l2];
+                    a_b = fmaf(pk_bi[i * rs + l], qv, a_b);
+                    a_s = fmaf(pk_sp[i * rs + l], qv, a_s);
+                }
+                a_b += pp[e];
+                a_s += pp[M * M + e];
+            }
+            pp[e] = a_b;
+            pp[M * M + e] = a_s;
+        }
+    } else if (tid == 0) {
         float2 *pp = part + (size_t)b * ntiles + tile;
-        if (MODE == MODE_FIRST) {
+        if (PH == MODE_FIRST) {
             *pp = make_float2(0.0f, 0.0f);
         } else {
             float2 a = *pp;
@@ -863,6 +1037,17 @@ k_mf_potts_reduce(const float2 *part, float *out, int ntiles) {
         out[2 * b] = acc[0].y;       // bilateral: w1
         out[2 * b + 1] = acc[0].x;   // spatial: w2
     }
+}
+
+// per image: the compatibility partials of its tiles, summed in tile order -> out[b] = -sum ([2][M][M], {bi, sp})
+__global__ void __launch_bounds__(kThreads)
+k_mf_compat_reduce(const float *part, float *out, int ntiles, int mm2) {
+    const int b = blockIdx.y;
+    const int e = blockIdx.x * kThreads + threadIdx.x;
+    if (e >= mm2) return;
+    float a = 0.0f;
+    for (int i = 0; i < ntiles; i++) a += part[((size_t)b * ntiles + i) * mm2 + e];
+    out[(size_t)b * mm2 + e] = -a;
 }
 
 // zero the splat targets of both lattices for the B images of the pass (row counts are device-resident)
@@ -1092,10 +1277,12 @@ static float *blur_all(Engine *e, const Lattice &L, float *buf, float *tmp, floa
 }
 
 // q_hist != nullptr: the training forward (MODE_HIST), Q_t of every iteration to q_hist[t] ([T+1][B][M][N]), with
-// the Potts weights read from `potts` ({w1, w2}, device) when it is given
+// the Potts weights read from `potts` ({w1, w2}, device) when it is given, or the compatibility matrices `compat`
+// ({mu_bi, mu_sp}, device) in their place (MODE_COMPAT)
 template <int MP>
 static int run_impl(Engine *e, int B, const float *unary, int layout, bool clamp, float *unary_rw,
-                    const dsrg_crf_params &p, cudaStream_t s, float *q_hist = nullptr, const float *potts = nullptr) {
+                    const dsrg_crf_params &p, cudaStream_t s, float *q_hist = nullptr, const float *potts = nullptr,
+                    const float *compat = nullptr) {
     const int M = e->M, N = e->N;
     dim3 gp(cdiv(N, kThreads), B);
     const int T = p.n_iters;
@@ -1115,10 +1302,11 @@ static int run_impl(Engine *e, int B, const float *unary, int layout, bool clamp
     const float alpha_sp = 1.0f / (1 + powf(2, -e->sp.d));  // permutohedral.cpp:571
     const float alpha_bi = 1.0f / (1 + powf(2, -e->bi.d));
     // device-resident weights: the kernels multiply alpha by them (MODE_HIST)
-    const float c_sp = potts ? alpha_sp : p.w2 * alpha_sp, c_bi = potts ? alpha_bi : p.w1 * alpha_bi;
+    const float c_sp = (potts || compat) ? alpha_sp : p.w2 * alpha_sp, c_bi = (potts || compat) ? alpha_bi : p.w1 * alpha_bi;
     float *urw = hist ? const_cast<float *>(potts) : Urw;
     const size_t smem = sizeof(TileSmem<MP>);
     const size_t smem_hy = sizeof(TileSmem<MP, kMaxLocHy>);
+    const size_t smem_c = smem + kCompatSmem<MP>, smem_hy_c = smem_hy + kCompatSmem<MP>;
     static bool attr_done[64] = {false};   // function attributes are per device
     const int dv = e->device & 63;
     if (!attr_done[dv]) {
@@ -1134,6 +1322,10 @@ static int run_impl(Engine *e, int B, const float *unary, int layout, bool clamp
         DSRG_CUDA_TRY(cudaFuncSetAttribute(k_mf_tile_hy<MP, MODE_FIRST | MODE_HIST>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_hy));
         DSRG_CUDA_TRY(cudaFuncSetAttribute(k_mf_tile_hy<MP, MODE_MID | MODE_HIST>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_hy));
         DSRG_CUDA_TRY(cudaFuncSetAttribute(k_mf_tile_hy<MP, MODE_LAST | MODE_HIST>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_hy));
+        DSRG_CUDA_TRY(cudaFuncSetAttribute(k_mf_tile<MP, MODE_MID | MODE_HIST | MODE_COMPAT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_c));
+        DSRG_CUDA_TRY(cudaFuncSetAttribute(k_mf_tile<MP, MODE_LAST | MODE_HIST | MODE_COMPAT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_c));
+        DSRG_CUDA_TRY(cudaFuncSetAttribute(k_mf_tile_hy<MP, MODE_MID | MODE_HIST | MODE_COMPAT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_hy_c));
+        DSRG_CUDA_TRY(cudaFuncSetAttribute(k_mf_tile_hy<MP, MODE_LAST | MODE_HIST | MODE_COMPAT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_hy_c));
         attr_done[dv] = true;
     }
 #ifndef DSRG_BLUR_GRID
@@ -1152,21 +1344,35 @@ static int run_impl(Engine *e, int B, const float *unary, int layout, bool clamp
     float *biX = e->biA, *biY = e->biB, *biZ = e->biC;
     DSRG_LAUNCH(e, T_MF_ZERO, s,
                 k_mf_zero<MP><<<bgrid, kThreads, 0, s>>>((float4 *)spY, e->sp.rowbase, (float4 *)biY, e->bi.rowbase, B));
-#define DSRG_TILE_LAUNCH(MODEV, QOUT)                                                                                 \
+#define DSRG_TILE_LAUNCH_AT(MODEV, QOUT, URW, SMEM, SMEM_HY)                                                          \
     do {                                                                                                              \
         if (hy_on)                                                                                                    \
             DSRG_LAUNCH(e, T_MF_TILE_HY, s,                                                                           \
-                        (k_mf_tile_hy<MP, MODEV><<<hgrid, kTileThreads, smem_hy, s>>>(                                \
-                            Usrc, urw, tclamp, QOUT, vsp, vbi, c_sp, c_bi, M, N, e->W, e->H, e->tiles_x, e->ntiles,   \
+                        (k_mf_tile_hy<MP, MODEV><<<hgrid, kTileThreads, SMEM_HY, s>>>(                                \
+                            Usrc, URW, tclamp, QOUT, vsp, vbi, c_sp, c_bi, M, N, e->W, e->H, e->tiles_x, e->ntiles,   \
                             e->tile_w, e->hy_list, e->hy_count)));                                                    \
         DSRG_LAUNCH(e, T_MF_TILE, s,                                                                                  \
-                    (k_mf_tile<MP, MODEV><<<gt, kTileThreads, smem, s>>>(Usrc, urw, tclamp, QOUT, vsp, vbi, c_sp,     \
+                    (k_mf_tile<MP, MODEV><<<gt, kTileThreads, SMEM, s>>>(Usrc, URW, tclamp, QOUT, vsp, vbi, c_sp,     \
                                                                         c_bi, M, N, e->W, e->H, e->tiles_x,           \
                                                                         e->ntiles, e->tile_w)));                      \
     } while (0)
+#define DSRG_TILE_LAUNCH(MODEV, QOUT) DSRG_TILE_LAUNCH_AT(MODEV, QOUT, urw, smem, smem_hy)
+#define DSRG_TILE_LAUNCH_COMPAT(MODEV, QOUT)                                                                          \
+    DSRG_TILE_LAUNCH_AT(MODEV | MODE_HIST | MODE_COMPAT, QOUT, const_cast<float *>(compat), smem_c, smem_hy_c)
     for (int it = 0; it <= T; it++) {
         TileLat vsp = make_tile_view(e->sp, spX, spY), vbi = make_tile_view(e->bi, biX, biY);
-        if (hist) {
+        if (compat) {
+            // the first iteration slices nothing: the plain training kernel, without weights
+            float *qt = q_hist + (size_t)it * slab;
+            if (it == T) {
+                DSRG_TILE_LAUNCH_COMPAT(MODE_LAST, qt);
+                break;
+            }
+            if (it == 0)
+                DSRG_TILE_LAUNCH_AT(MODE_FIRST | MODE_HIST, qt, nullptr, smem, smem_hy);
+            else
+                DSRG_TILE_LAUNCH_COMPAT(MODE_MID, qt);
+        } else if (hist) {
             float *qt = q_hist + (size_t)it * slab;
             if (it == T) {
                 DSRG_TILE_LAUNCH(MODE_LAST | MODE_HIST, qt);
@@ -1194,32 +1400,40 @@ static int run_impl(Engine *e, int B, const float *unary, int layout, bool clamp
         spX = sp_res; spY = nspY; spZ = sp_other;
         biX = bi_res; biY = nbiY; biZ = bi_other;
     }
+#undef DSRG_TILE_LAUNCH_COMPAT
 #undef DSRG_TILE_LAUNCH
+#undef DSRG_TILE_LAUNCH_AT
     DSRG_CUDA_TRY(cudaGetLastError());
     return DSRG_OK;
 }
 
 // The backward of a training forward (DenseCRF::gradient, densecrf.cpp:238-297) on the lattices the pass just built:
-// k_mf_tile_bwd from T down to 0 with the transposed blur in between, then the per-image Potts sums.
+// k_mf_tile_bwd from T down to 0 with the transposed blur in between, then the per-image Potts sums -- or, with
+// `compat` ({mu_bi, mu_sp}), the MODE_COMPAT kernels and the per-image compatibility sums to g_compat ([B][2][M][M]).
 template <int MP>
 static int bwd_impl(Engine *e, int B, const float *q_hist, const float *potts, const float *G, float *gU,
-                    float *g_potts, const dsrg_crf_params &p, cudaStream_t s) {
+                    float *g_potts, const float *compat, float *g_compat, const dsrg_crf_params &p, cudaStream_t s) {
     const int M = e->M, N = e->N, T = p.n_iters;
     const size_t slab = (size_t)B * M * N;
     if (T == 0) {
         DSRG_LAUNCH(e, T_MF_INIT, s,
                     k_mf_softmax_vjp<<<dim3(cdiv(N, kThreads), B), kThreads, 0, s>>>(G, q_hist, gU, M, N));
         if (g_potts) DSRG_CUDA_TRY(cudaMemsetAsync(g_potts, 0, sizeof(float) * 2 * B, s));
+        if (g_compat) DSRG_CUDA_TRY(cudaMemsetAsync(g_compat, 0, sizeof(float) * 2 * M * M * B, s));
         DSRG_CUDA_TRY(cudaGetLastError());
         return DSRG_OK;
     }
     static bool attr_done[64] = {false};
     const int dv = e->device & 63;
     const size_t smem = sizeof(TileSmem<MP>);
+    const size_t smem_c = smem + kCompatSmem<MP> + kCompatParkSmem<MP>;
     if (!attr_done[dv]) {
         DSRG_CUDA_TRY(cudaFuncSetAttribute(k_mf_tile_bwd<MP, MODE_FIRST>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         DSRG_CUDA_TRY(cudaFuncSetAttribute(k_mf_tile_bwd<MP, MODE_MID>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         DSRG_CUDA_TRY(cudaFuncSetAttribute(k_mf_tile_bwd<MP, MODE_LAST>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        DSRG_CUDA_TRY(cudaFuncSetAttribute(k_mf_tile_bwd<MP, MODE_FIRST | MODE_COMPAT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_c));
+        DSRG_CUDA_TRY(cudaFuncSetAttribute(k_mf_tile_bwd<MP, MODE_MID | MODE_COMPAT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_c));
+        DSRG_CUDA_TRY(cudaFuncSetAttribute(k_mf_tile_bwd<MP, MODE_LAST | MODE_COMPAT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_c));
         attr_done[dv] = true;
     }
     const float a_sp = 1.0f / (1 + powf(2, -e->sp.d)), a_bi = 1.0f / (1 + powf(2, -e->bi.d));
@@ -1229,22 +1443,34 @@ static int bwd_impl(Engine *e, int B, const float *q_hist, const float *potts, c
     float *biX = e->biA, *biY = e->biB, *biZ = e->biC;
     DSRG_LAUNCH(e, T_MF_ZERO, s,
                 k_mf_zero<MP><<<bgrid, kThreads, 0, s>>>((float4 *)spY, e->sp.rowbase, (float4 *)biY, e->bi.rowbase, B));
-#define DSRG_BWD_LAUNCH(MODEV)                                                                                        \
+#define DSRG_BWD_LAUNCH_AT(MODEV, WP, PART, SMEM)                                                                     \
     DSRG_LAUNCH(e, T_MF_TILE, s,                                                                                      \
-                (k_mf_tile_bwd<MP, MODEV><<<gt, kTileThreads, smem, s>>>(G, qt, gU, vsp, vbi, a_sp, a_bi, potts, p.w1, \
-                                                                        p.w2, e->potts_part, M, N, e->W, e->H,        \
+                (k_mf_tile_bwd<MP, MODEV><<<gt, kTileThreads, SMEM, s>>>(G, qt, gU, vsp, vbi, a_sp, a_bi, WP, p.w1,    \
+                                                                        p.w2, PART, M, N, e->W, e->H,                 \
                                                                         e->tiles_x, e->ntiles, e->tile_w)))
+#define DSRG_BWD_LAUNCH(MODEV) DSRG_BWD_LAUNCH_AT(MODEV, potts, e->potts_part, smem)
+#define DSRG_BWD_LAUNCH_COMPAT(MODEV)                                                                                 \
+    DSRG_BWD_LAUNCH_AT(MODEV | MODE_COMPAT, compat, reinterpret_cast<float2 *>(e->compat_part), smem_c)
     for (int it = T; it >= 0; it--) {
         const TileLat vsp = make_tile_view(e->sp, spX, spY), vbi = make_tile_view(e->bi, biX, biY);
         const float *qt = q_hist + (size_t)it * slab;
-        if (it == 0) {
+        if (compat) {
+            if (it == 0) {
+                DSRG_BWD_LAUNCH_COMPAT(MODE_LAST);
+                break;
+            }
+            if (it == T)
+                DSRG_BWD_LAUNCH_COMPAT(MODE_FIRST);
+            else
+                DSRG_BWD_LAUNCH_COMPAT(MODE_MID);
+        } else if (it == 0) {
             DSRG_BWD_LAUNCH(MODE_LAST);
             break;
-        }
-        if (it == T)
+        } else if (it == T) {
             DSRG_BWD_LAUNCH(MODE_FIRST);
-        else
+        } else {
             DSRG_BWD_LAUNCH(MODE_MID);
+        }
         float *sp_res = blur_all<MP>(e, e->sp, spY, spZ, spX, B, T_MF_BLUR_SP, bgrid, s, true);
         float *bi_res = blur_all<MP>(e, e->bi, biY, biZ, biX, B, T_MF_BLUR_BI, bgrid, s, true);
         float *sp_other = (sp_res == spY) ? spZ : spY, *bi_other = (bi_res == biY) ? biZ : biY;
@@ -1252,18 +1478,26 @@ static int bwd_impl(Engine *e, int B, const float *q_hist, const float *potts, c
         spX = sp_res; spY = nspY; spZ = sp_other;
         biX = bi_res; biY = nbiY; biZ = bi_other;
     }
+#undef DSRG_BWD_LAUNCH_COMPAT
 #undef DSRG_BWD_LAUNCH
+#undef DSRG_BWD_LAUNCH_AT
+    if (g_compat) {
+        const int mm2 = 2 * M * M;
+        DSRG_LAUNCH(e, T_MF_EXPORT, s,
+                    k_mf_compat_reduce<<<dim3(cdiv(mm2, kThreads), B), kThreads, 0, s>>>(e->compat_part, g_compat,
+                                                                                         e->ntiles, mm2));
+    }
     if (g_potts)
         DSRG_LAUNCH(e, T_MF_EXPORT, s, k_mf_potts_reduce<<<B, kThreads, 0, s>>>(e->potts_part, g_potts, e->ntiles));
     DSRG_CUDA_TRY(cudaGetLastError());
     return DSRG_OK;
 }
 
-int meanfield_run_train(Engine *e, int B, const float *unary, float *q_hist, const float *potts,
+int meanfield_run_train(Engine *e, int B, const float *unary, float *q_hist, const float *potts, const float *compat,
                         const dsrg_crf_params &p, cudaStream_t s) {
     switch (e->MP) {
 #define DSRG_CASE(MPV) \
-    case MPV: return run_impl<MPV>(e, B, unary, DSRG_LAYOUT_NCHW, false, nullptr, p, s, q_hist, potts);
+    case MPV: return run_impl<MPV>(e, B, unary, DSRG_LAYOUT_NCHW, false, nullptr, p, s, q_hist, potts, compat);
         DSRG_CASE(4) DSRG_CASE(8) DSRG_CASE(12) DSRG_CASE(16) DSRG_CASE(20) DSRG_CASE(24) DSRG_CASE(28) DSRG_CASE(32)
 #undef DSRG_CASE
     }
@@ -1272,10 +1506,11 @@ int meanfield_run_train(Engine *e, int B, const float *unary, float *q_hist, con
 }
 
 int meanfield_backward(Engine *e, int B, const float *q_hist, const float *potts, const float *grad_q,
-                       float *grad_unary, float *grad_potts, const dsrg_crf_params &p, cudaStream_t s) {
+                       float *grad_unary, float *grad_potts, const float *compat, float *grad_compat,
+                       const dsrg_crf_params &p, cudaStream_t s) {
     switch (e->MP) {
 #define DSRG_CASE(MPV) \
-    case MPV: return bwd_impl<MPV>(e, B, q_hist, potts, grad_q, grad_unary, grad_potts, p, s);
+    case MPV: return bwd_impl<MPV>(e, B, q_hist, potts, grad_q, grad_unary, grad_potts, compat, grad_compat, p, s);
         DSRG_CASE(4) DSRG_CASE(8) DSRG_CASE(12) DSRG_CASE(16) DSRG_CASE(20) DSRG_CASE(24) DSRG_CASE(28) DSRG_CASE(32)
 #undef DSRG_CASE
     }

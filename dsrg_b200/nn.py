@@ -389,14 +389,58 @@ class _DenseCrf(torch.autograd.Function):
         return grad_u, None, gw1, gw2, None, None, None
 
 
-def dense_crf(unary, image, scale_factor=1.0, color_factor=13, maxiter=10, w1=None, w2=None):
+class _DenseCrfCompat(torch.autograd.Function):
+    """dense_crf with compatibility matrices: compat (2, M, M) float32 {mu_bi, mu_sp}."""
+
+    @staticmethod
+    @_fwd
+    def forward(ctx, unary, image, compat, scale_factor, color_factor, maxiter):
+        eng = _engine_for(unary)
+        params = api.crf_params(scale_factor, color_factor, maxiter)
+        q_hist = torch.empty((maxiter + 1,) + tuple(unary.shape), dtype=torch.float32, device=unary.device)
+        eng.crf_forward_train_compat_dev(unary, image, params, compat, q_hist, stream=_stream(unary))
+        ctx.save_for_backward(q_hist, image, compat)
+        ctx.params = params
+        return q_hist[maxiter].clone()
+
+    @staticmethod
+    @_bwd
+    def backward(ctx, g):
+        q_hist, image, compat = ctx.saved_tensors
+        grad_u = torch.empty(q_hist.shape[1:], dtype=torch.float32, device=q_hist.device)
+        grad_c = None
+        if ctx.needs_input_grad[2]:
+            M = compat.shape[-1]
+            grad_c = torch.empty((q_hist.shape[1], 2, M, M), dtype=torch.float32, device=q_hist.device)
+        _engine_for(grad_u).crf_backward_compat_dev(q_hist, image, ctx.params, compat, g.contiguous(), grad_u,
+                                                    grad_compat=grad_c, stream=_stream(grad_u))
+        return grad_u, None, None if grad_c is None else grad_c.sum(0), None, None, None
+
+
+def _compat_matrix(mu, name, ref, M):
+    if not isinstance(mu, torch.Tensor) or tuple(mu.shape) != (M, M) or not mu.is_floating_point() \
+            or mu.device != ref.device:
+        raise ValueError("%s must be None or an (%d, %d) floating-point tensor on %s (got %r)"
+                         % (name, M, M, ref.device,
+                            mu if not isinstance(mu, torch.Tensor) else (mu.dtype, tuple(mu.shape), mu.device)))
+    return mu.float()
+
+
+def dense_crf(unary, image, scale_factor=1.0, color_factor=13, maxiter=10, w1=None, w2=None, compat_bi=None,
+              compat_sp=None):
     """The dense CRF of CRF() (CRF/krahenbuhl2013/CRF.py:4-37) as a differentiable layer: unary (N, M, H, W) float32,
     M <= 32, the values CRF(image, unary) takes (energy = -unary); image (N, H, W, 3) uint8 at the map size ->
     marginals (N, M, H, W) after `maxiter` mean-field iterations.  The backward is the exact gradient of the
     marginals (the mean field run backwards, DenseCRF::gradient): to `unary` and, when given as 0-dim CUDA tensors,
     to the Potts weights w1 (bilateral) and w2 (spatial), whose gradient is the sum over the batch.  None means
     CRF()'s 10 and 3, without a gradient.  The forward keeps every iteration's marginals for the backward:
-    (maxiter + 1) * N * M * H * W * 4 bytes of device memory."""
+    (maxiter + 1) * N * M * H * W * 4 bytes of device memory.
+
+    compat_bi / compat_sp: (M, M) label-compatibility matrices of the bilateral / spatial kernel, learnable in place
+    of w1 / w2 (not together with them): the message to label l is -sum_l' mu[l, l'] F(Q)[l'], so Potts(w) is
+    -w * I, the reference's MatrixCompatibility(m) is (m + m.T) / 2 and its DiagonalCompatibility(v) is diag(v).
+    A matrix left None is -w * I of its weight (w1 / w2, or CRF()'s 10 / 3).  Their gradients are summed over the
+    batch."""
     if torch.is_autocast_enabled("cuda"):   # what custom_fwd(cast_inputs=float32) does, before the checks
         unary = unary.float() if isinstance(unary, torch.Tensor) and unary.is_floating_point() else unary
     u = _maps(unary, "unary")
@@ -410,7 +454,20 @@ def dense_crf(unary, image, scale_factor=1.0, color_factor=13, maxiter=10, w1=No
     w1, w2 = _potts_weight(w1, "w1", u), _potts_weight(w2, "w2", u)
     if int(maxiter) < 0:
         raise ValueError("maxiter must be >= 0 (got %d)" % maxiter)
-    return _DenseCrf.apply(u, image.contiguous(), w1, w2, float(scale_factor), float(color_factor), int(maxiter))
+    if compat_bi is None and compat_sp is None:
+        return _DenseCrf.apply(u, image.contiguous(), w1, w2, float(scale_factor), float(color_factor), int(maxiter))
+    mats = []
+    for mu, w, d, name, wname in ((compat_bi, w1, _POTTS_DEFAULT[0], "compat_bi", "w1"),
+                                  (compat_sp, w2, _POTTS_DEFAULT[1], "compat_sp", "w2")):
+        if mu is None:   # Potts: -w I, through which autograd carries w's gradient
+            eye = torch.eye(M, dtype=torch.float32, device=u.device)
+            mats.append(-(w.float() if w is not None else d) * eye)
+        elif w is not None:
+            raise ValueError("%s and %s are two forms of one term: give one of them" % (name, wname))
+        else:
+            mats.append(_compat_matrix(mu, name, u, M))
+    return _DenseCrfCompat.apply(u, image.contiguous(), torch.stack(mats), float(scale_factor), float(color_factor),
+                                 int(maxiter))
 
 
 def softmax(fc8):

@@ -159,6 +159,24 @@ int dsrg_crf_forward_train_dev(dsrg_engine *e, const float *unary_dev, int B, co
 int dsrg_crf_backward_dev(dsrg_engine *e, const float *q_hist_dev, int B, const uint8_t *image_dev,
                           const dsrg_crf_params *params, const float *potts_dev, const float *grad_q_dev,
                           float *grad_unary_dev, float *grad_potts_dev, void *stream);
+/*
+ * The same layer with a learnable label-compatibility matrix per kernel in place of the Potts weights (the
+ * reference's MatrixCompatibility, labelcompatibility.cpp:64-108, applied as given, not symmetrised):
+ *   t = unary - mu_sp F_sp(Q) - mu_bi F_bi(Q);  Q = softmax(t)
+ * so Potts(w) is mu = -w I, the reference's MatrixCompatibility(m) is mu = (m + m^T) / 2 and its
+ * DiagonalCompatibility(v) is mu = diag(v).
+ *   compat      : device float [2][M][M] {mu_bi, mu_sp}; row l, column l' is the weight of label l' in the message to
+ *                 label l.  params->w1 / w2 are ignored.  Its address is part of a cached graph's key, its values are not
+ *   grad_compat : optional [B][2][M][M] dL/dmu per image, in the same order
+ * Everything else as dsrg_crf_forward_train_dev / dsrg_crf_backward_dev.  The first backward allocates the per-tile
+ * partials: maxB * tiles * 2 * M^2 * 4 bytes, 102 MB at batch 64 @ 321x321 (451 tiles) with 21 labels.
+ */
+int dsrg_crf_forward_train_compat_dev(dsrg_engine *e, const float *unary_dev, int B, const uint8_t *image_dev,
+                                      const dsrg_crf_params *params, const float *compat_dev, float *q_hist_dev,
+                                      void *stream);
+int dsrg_crf_backward_compat_dev(dsrg_engine *e, const float *q_hist_dev, int B, const uint8_t *image_dev,
+                                 const dsrg_crf_params *params, const float *compat_dev, const float *grad_q_dev,
+                                 float *grad_unary_dev, float *grad_compat_dev, void *stream);
 /* arg-max labelling after inference: DenseCRFWrapper::map, densecrf_wrapper.cpp:39-43 */
 int dsrg_crf_map_batch_dev(dsrg_engine *e, int B, const float *unary_dev, int unary_layout,
                            const uint8_t *image_dev, const dsrg_crf_params *params,

@@ -3,6 +3,8 @@
   forward   dsrg_crf_batch_dev: the mean field alone (inference)
   train     dsrg_crf_forward_train_dev + dsrg_crf_backward_dev: the forward that keeps Q_0..Q_T, then the exact
             backward to the unaries and the Potts weights (what nn.dense_crf runs per training step)
+  compat    (--compat) dsrg_crf_forward_train_compat_dev + dsrg_crf_backward_compat_dev: the same step with a
+            compatibility matrix per kernel (random, not symmetric) and its gradient
 
 on three workloads: train-s's shape (batch 20, 41 x 41 maps, 21 labels, scale_factor 12, smooth images) and batch 64
 at 321 x 321 with scale_factor 1 on smooth and on photo-like images; 10 mean-field iterations.  The legs run on a side
@@ -11,6 +13,7 @@ window is timed with CUDA events.  Prints one JSON line per workload with the me
 card's name, power limit and SM clocks read in the same run.
 
 usage: python tools/bench_crf_grad.py [--steps 20] [--warmup 3] [--rounds 5] [--workloads train_s,b64_smooth,b64_photo]
+                                     [--compat]
 """
 import argparse
 import json
@@ -33,7 +36,7 @@ WORKLOADS = {   # name -> (B, H, W, M, scale factor, image)
 T = 10
 
 
-def run(name, steps, warmup, rounds):
+def run(name, steps, warmup, rounds, compat=False):
     import torch
     from dsrg_b200 import api, synth
     B, H, W, M, sf, img = WORKLOADS[name]
@@ -47,12 +50,19 @@ def run(name, steps, warmup, rounds):
     q_hist = torch.empty((T + 1,) + tuple(unary.shape), device="cuda")
     gu, gw = torch.empty_like(unary), torch.empty((B, 2), device="cuda")
     s = torch.cuda.Stream()
+    if compat:
+        mu = (torch.randn((2, M, M), generator=torch.Generator().manual_seed(5)) - 2 * torch.eye(M)).cuda()
+        gmu = torch.empty((B, 2, M, M), device="cuda")
     legs = {
         "forward": lambda: eng.crf_dev(unary, image, p, out, unary_layout=api.LAYOUT_NCHW,
                                        out_layout=api.LAYOUT_NCHW, stream=s.cuda_stream),
         "train": lambda: (eng.crf_forward_train_dev(unary, image, p, q_hist, stream=s.cuda_stream),
                           eng.crf_backward_dev(q_hist, image, p, G, gu, grad_potts=gw, stream=s.cuda_stream)),
     }
+    if compat:
+        legs["compat"] = lambda: (eng.crf_forward_train_compat_dev(unary, image, p, mu, q_hist, stream=s.cuda_stream),
+                                  eng.crf_backward_compat_dev(q_hist, image, p, mu, G, gu, grad_compat=gmu,
+                                                              stream=s.cuda_stream))
     times = {k: [] for k in legs}
     with torch.cuda.stream(s):
         for fn in legs.values():
@@ -70,7 +80,8 @@ def run(name, steps, warmup, rounds):
                 times[k].append(a.elapsed_time(b) / steps)
     eng.close()
     med = {k: float(np.median(v)) for k, v in times.items()}
-    return dict(workload=name, B=B, H=H, W=W, M=M, scale_factor=sf, image=img, n_iters=T,
+    extra = dict(compat_over_train=round(med["compat"] / med["train"], 2)) if compat else {}
+    return dict(**extra, workload=name, B=B, H=H, W=W, M=M, scale_factor=sf, image=img, n_iters=T,
                 ms_per_step={k: round(v, 3) for k, v in med.items()},
                 spread_ms={k: [round(min(v), 3), round(max(v), 3)] for k, v in times.items()},
                 train_over_forward=round(med["train"] / med["forward"], 2),
@@ -83,13 +94,14 @@ def main():
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--rounds", type=int, default=5)
     ap.add_argument("--workloads", default=",".join(WORKLOADS))
+    ap.add_argument("--compat", action="store_true", help="also time the compatibility-matrix step")
     a = ap.parse_args()
     import torch
     if not torch.cuda.is_available():
         sys.exit("bench_crf_grad.py needs a CUDA device")
     info = card()
     for name in a.workloads.split(","):
-        r = run(name, a.steps, a.warmup, a.rounds)
+        r = run(name, a.steps, a.warmup, a.rounds, a.compat)
         r.update(info)
         print(json.dumps(r), flush=True)
 
