@@ -178,6 +178,25 @@ class Engine(object):
                                                    _dptr(grad_compat), _stream(stream)))
         return grad_unary
 
+    def crf_backward_theta_dev(self, q_hist, image, params, grad_q, grad_unary, grad_theta, grad_potts=None,
+                               potts=None, stream=None):
+        """crf_backward_dev that also writes grad_theta (B, 7) = dL/dtheta per image in dsrg_crf_params' order
+        (theta_alpha_x, theta_alpha_y, theta_beta_r, theta_beta_g, theta_beta_b, theta_gamma_x, theta_gamma_y)."""
+        B = grad_q.shape[0]
+        check(self._L.dsrg_crf_backward_theta_dev(self.h, _dptr(q_hist), B, _dptr(image), C.byref(params),
+                                                  _dptr(potts), _dptr(grad_q), _dptr(grad_unary), _dptr(grad_potts),
+                                                  _dptr(grad_theta), _stream(stream)))
+        return grad_unary
+
+    def crf_backward_compat_theta_dev(self, q_hist, image, params, compat, grad_q, grad_unary, grad_theta,
+                                      grad_compat=None, stream=None):
+        """crf_backward_compat_dev that also writes grad_theta (B, 7) as crf_backward_theta_dev does."""
+        B = grad_q.shape[0]
+        check(self._L.dsrg_crf_backward_compat_theta_dev(self.h, _dptr(q_hist), B, _dptr(image), C.byref(params),
+                                                         _dptr(compat), _dptr(grad_q), _dptr(grad_unary),
+                                                         _dptr(grad_compat), _dptr(grad_theta), _stream(stream)))
+        return grad_unary
+
     def crf_map_dev(self, unary, image, params, labels_out, unary_layout=LAYOUT_NHWC, stream=None):
         B = image.shape[0]
         check(self._L.dsrg_crf_map_batch_dev(self.h, B, _dptr(unary), unary_layout, _dptr(image), C.byref(params),

@@ -324,7 +324,7 @@ using namespace dsrg;
 
 extern "C" {
 
-int dsrg_version(void) { return 112; }
+int dsrg_version(void) { return 113; }
 
 const char *dsrg_last_error(void) { return g_err; }
 
@@ -496,7 +496,8 @@ void dsrg_engine_destroy(dsrg_engine *h) {
     lattice_free(e->bi);
     void *ptrs[] = {e->U, e->Q0, e->spA, e->spB, e->spC, e->biA, e->biB, e->biC, e->nvA, e->nvB, e->lmap,
                     e->lflag, e->parent, e->hc, e->loss_acc, e->sec_rec, e->sec_img, e->sec_part, e->sec_w, e->dev_err,
-                    e->hy_list, e->hy_count, e->potts_part, e->compat_part, e->st_unary, e->st_out, e->st_cues, e->st_labels, e->st_image, e->st_lmap, e->st_raw, e->st_idx,
+                    e->hy_list, e->hy_count, e->potts_part, e->compat_part, e->kg_g, e->kg_csum, e->kg_part, e->kg_sp[0],
+                    e->kg_sp[1], e->kg_bi[0], e->kg_bi[1], e->st_unary, e->st_out, e->st_cues, e->st_labels, e->st_image, e->st_lmap, e->st_raw, e->st_idx,
                     e->st_prep, e->st_sel};
     for (void *p : ptrs) cudaFree(p);
     if (e->own_stream) cudaStreamDestroy(e->own_stream);
@@ -562,7 +563,8 @@ long long dsrg_engine_take_launch_count(dsrg_engine *h) {
 static const char *kTagNames[T_COUNT] = {
     "lattice_insert", "lattice_misc", "lattice_norm", "mf_init", "mf_zero", "mf_blur_spatial",
     "mf_blur_bilateral", "mf_tile", "mf_export", "srg_label", "srg_merge", "srg_flag", "srg_emit",
-    "seedloss", "wire_bits", "prepare_image", "postprocess", "annotation", "mf_tile_hybrid"};
+    "seedloss", "wire_bits", "prepare_image", "postprocess", "annotation", "mf_tile_hybrid",
+    "kernel_grad"};
 
 int dsrg_profile_tag_count(void) { return T_COUNT; }
 
@@ -729,6 +731,65 @@ int dsrg_crf_backward_compat_dev(dsrg_engine *h, const float *q_hist, int B, con
             if (r) return r;
             return meanfield_backward(e, B, q_hist, nullptr, grad_q, grad_unary, nullptr, compat, grad_compat, *params,
                                       s);
+        });
+        e->last_crf_B = 0;
+        return rc;
+    });
+}
+
+// The kernel-bandwidth backward's buffers on its first call (as ensure_compat_part): g_t and c per pixel, the per-block
+// sums and two value buffers per lattice, sized for the engine's capacity.
+static int ensure_kgrad(Engine *e) {
+    if (e->kg_g) return DSRG_OK;
+    cudaStreamCaptureMode mode = cudaStreamCaptureModeRelaxed;
+    DSRG_CUDA_TRY(cudaThreadExchangeStreamCaptureMode(&mode));
+    int rc = 0;
+    rc |= dalloc(e, &e->kg_g, (size_t)e->maxB * e->M * e->Ncap);
+    rc |= dalloc(e, &e->kg_csum, (size_t)2 * e->maxB * e->Ncap);
+    rc |= dalloc(e, &e->kg_part, (size_t)e->maxB * ((e->Ncap + kThreads - 1) / kThreads) * 8);
+    for (int i = 0; i < 2; i++) {
+        rc |= dalloc(e, &e->kg_sp[i], (size_t)e->sp.rows_cap * e->MP);
+        rc |= dalloc(e, &e->kg_bi[i], (size_t)e->bi.rows_cap * e->MP);
+    }
+    DSRG_CUDA_TRY(cudaThreadExchangeStreamCaptureMode(&mode));
+    return rc ? DSRG_E_NOMEM : DSRG_OK;
+}
+
+int dsrg_crf_backward_theta_dev(dsrg_engine *h, const float *q_hist, int B, const uint8_t *image,
+                                const dsrg_crf_params *params, const float *potts, const float *grad_q,
+                                float *grad_unary, float *grad_potts, float *grad_theta, void *stream) {
+    const cudaStream_t s = (cudaStream_t)stream;
+    return dev_call(h, B, s, q_hist && image && params && grad_q && grad_unary && grad_theta, [&](Engine *e) {
+        if (int rc = grad_labels_ok(e)) return rc;
+        if (int rc = ensure_kgrad(e)) return rc;
+        GraphKey args;
+        args.add(q_hist).add(image).add(potts).add(grad_q).add(grad_unary).add(grad_potts).add(grad_theta);
+        const int rc = crf_pass(e, s, PassKind::crf_backward_theta, B, params, args, [&]() {
+            int r = prepare_lattices(e, B, image, *params, s);   // as in dsrg_crf_backward_dev
+            if (r) return r;
+            return meanfield_backward(e, B, q_hist, potts, grad_q, grad_unary, grad_potts, nullptr, nullptr, *params, s,
+                                      grad_theta, image);
+        });
+        e->last_crf_B = 0;
+        return rc;
+    });
+}
+
+int dsrg_crf_backward_compat_theta_dev(dsrg_engine *h, const float *q_hist, int B, const uint8_t *image,
+                                       const dsrg_crf_params *params, const float *compat, const float *grad_q,
+                                       float *grad_unary, float *grad_compat, float *grad_theta, void *stream) {
+    const cudaStream_t s = (cudaStream_t)stream;
+    return dev_call(h, B, s, q_hist && image && params && compat && grad_q && grad_unary && grad_theta, [&](Engine *e) {
+        if (int rc = grad_labels_ok(e)) return rc;
+        if (int rc = ensure_compat_part(e)) return rc;
+        if (int rc = ensure_kgrad(e)) return rc;
+        GraphKey args;
+        args.add(q_hist).add(image).add(compat).add(grad_q).add(grad_unary).add(grad_compat).add(grad_theta);
+        const int rc = crf_pass(e, s, PassKind::crf_backward_compat_theta, B, params, args, [&]() {
+            int r = prepare_lattices(e, B, image, *params, s);
+            if (r) return r;
+            return meanfield_backward(e, B, q_hist, nullptr, grad_q, grad_unary, nullptr, compat, grad_compat, *params,
+                                      s, grad_theta, image);
         });
         e->last_crf_B = 0;
         return rc;

@@ -83,7 +83,7 @@ struct Engine;
 enum KTag {
     T_LAT_INSERT = 0, T_LAT_MISC, T_LAT_NORM, T_MF_INIT, T_MF_ZERO, T_MF_BLUR_SP,
     T_MF_BLUR_BI, T_MF_TILE, T_MF_EXPORT, T_SRG_LABEL, T_SRG_MERGE, T_SRG_FLAG, T_SRG_EMIT,
-    T_LOSS, T_WIRE, T_PREP, T_POST, T_ANNOT, T_MF_TILE_HY, T_COUNT
+    T_LOSS, T_WIRE, T_PREP, T_POST, T_ANNOT, T_MF_TILE_HY, T_KGRAD, T_COUNT
 };
 
 // ---- lattice.cu ----
@@ -159,9 +159,12 @@ int meanfield_run(Engine *e, int B, const float *unary, int unary_layout, bool c
 // backward needs e->compat_part, ensure_compat_part)
 int meanfield_run_train(Engine *e, int B, const float *unary, float *q_hist, const float *potts, const float *compat,
                         const dsrg_crf_params &p, cudaStream_t s);
+// grad_theta ([B][7], with the batch's image): the kernel-bandwidth gradient too, which needs the kg_* buffers
+// (ensure_kgrad)
 int meanfield_backward(Engine *e, int B, const float *q_hist, const float *potts, const float *grad_q,
                        float *grad_unary, float *grad_potts, const float *compat, float *grad_compat,
-                       const dsrg_crf_params &p, cudaStream_t s);
+                       const dsrg_crf_params &p, cudaStream_t s, float *grad_theta = nullptr,
+                       const uint8_t *image = nullptr);
 // ---- meanfield_wide.cu: label counts above DSRG_MAX_LABELS ----
 int meanfield_run_wide(Engine *e, int B, const float *unary, int unary_layout, bool clamp_inplace,
                        float *unary_rw, const dsrg_crf_params &p, cudaStream_t s);
@@ -206,6 +209,10 @@ struct Engine {
     // [maxB * ntiles][2][M][M] the compatibility backward's per-tile partials (bilateral, spatial); allocated by its
     // first call (ensure_compat_part)
     float *compat_part = nullptr;
+    // the kernel-bandwidth backward's buffers, allocated by its first call (ensure_kgrad): g_t [maxB][M][N], c per
+    // pixel [2][maxB][N], per-block sums [maxB][blocks][8], and two value buffers per lattice [rows][MP]
+    float *kg_g = nullptr, *kg_csum = nullptr, *kg_part = nullptr;
+    float *kg_sp[2] = {nullptr, nullptr}, *kg_bi[2] = {nullptr, nullptr};
     int *hy_count = nullptr;   // their number (device-resident)
     // 1-channel buffers for the normalisation pass
     float *nvA = nullptr, *nvB = nullptr;
@@ -415,7 +422,7 @@ cudaError_t numa_host_alloc(void **p, size_t bytes, int device);
 // plain launches on the legacy default stream, inside somebody else's capture, while per-kernel profiling is on,
 // or if capture fails.  `body` issues the launches on `s` and returns a DSRG_* code.
 enum class PassKind : int { crf, crf_map, forward, crflayer, densecrf, post, crf_train, crf_backward, crf_train_compat,
-                            crf_backward_compat };
+                            crf_backward_compat, crf_backward_theta, crf_backward_compat_theta };
 struct GraphKey {
     std::string bytes;
     GraphKey() = default;

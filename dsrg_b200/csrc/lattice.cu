@@ -15,6 +15,7 @@
 // keys.  Lattice neighbours then sit a few ids apart for the spatial lattice and mostly so for the bilateral one,
 // each tile's rows are a few contiguous runs, and the numbering is deterministic.
 #include "common.cuh"
+#include "simplex.cuh"
 
 namespace dsrg {
 
@@ -137,61 +138,13 @@ __global__ void __launch_bounds__(kThreads) k_lattice_insert(BuildArgs a) {
     if (real) {
         const int x = i % a.W, y = i / a.W;
         pos = tile_major_pos(x, y, a.tile_w, a.tiles_x);
-        f[0] = __fdiv_rn((float)x, a.sigma[0]);  // densecrf.cpp:65-66 / :74-75
-        f[1] = __fdiv_rn((float)y, a.sigma[1]);
-        if (D == 5) {
-            const uint8_t *px = a.image + ((size_t)b * a.N + i) * 3;  // densecrf.cpp:76-78
-            f[2] = __fdiv_rn((float)px[0], a.sigma[2]);
-            f[3] = __fdiv_rn((float)px[1], a.sigma[3]);
-            f[4] = __fdiv_rn((float)px[2], a.sigma[4]);
-        }
+        lattice_features<D>(x, y, a.image, b, a.N, i, a.sigma, f);
     }
-    // elevate (:201-207)
-    float el[D + 1];
-    float sm = 0.0f;
-#pragma unroll
-    for (int j = D; j > 0; j--) {
-        float cf = __fmul_rn(f[j - 1], a.scale[j - 1]);
-        el[j] = __fsub_rn(sm, __fmul_rn((float)j, cf));
-        sm = __fadd_rn(sm, cf);
-    }
-    el[0] = sm;
-    // closest 0-coloured simplex (:210-220); cvtps_epi32 under MXCSR-nearest == rintf
-    const float inv = __fdiv_rn(1.0f, (float)(D + 1));
-    const float dp1 = (float)(D + 1);
-    float rem0[D + 1];
-    int isum = 0;
-#pragma unroll
-    for (int k = 0; k <= D; k++) {
-        float v = rintf(__fmul_rn(inv, el[k]));
-        rem0[k] = __fmul_rn(v, dp1);
-        isum += (int)v;
-    }
-    // rank (:223-233): strict <, ties increment the later coordinate
+    // elevate, simplex, rank (simplex.cuh)
+    float el[D + 1], rem0[D + 1];
     int rank[D + 1];
-#pragma unroll
-    for (int k = 0; k <= D; k++) rank[k] = 0;
-#pragma unroll
-    for (int k = 0; k < D; k++) {
-        float di = __fsub_rn(el[k], rem0[k]);
-#pragma unroll
-        for (int j = k + 1; j <= D; j++) {
-            float dj = __fsub_rn(el[j], rem0[j]);
-            if (di < dj) rank[k]++; else rank[j]++;
-        }
-    }
-    // back onto the plane (:236-242)
-#pragma unroll
-    for (int k = 0; k <= D; k++) {
-        rank[k] += isum;
-        if (rank[k] < 0) {
-            rank[k] += D + 1;
-            rem0[k] = __fadd_rn(rem0[k], dp1);
-        } else if (rank[k] >= D + 1) {
-            rank[k] -= D + 1;
-            rem0[k] = __fsub_rn(rem0[k], dp1);
-        }
-    }
+    lattice_simplex<D>(f, a.scale, el, rem0, rank);
+    const float inv = __fdiv_rn(1.0f, (float)(D + 1));
     // barycentric (:245-263), same accumulation order as the reference
     float bc[D + 2];
 #pragma unroll

@@ -9,6 +9,7 @@
 // lattice value rows are [rows][MP] float32 with MP = M rounded up to a multiple of 4
 // (the reference pads 21 -> 24 the same way, permutohedral.cpp:531).
 #include "common.cuh"
+#include "simplex.cuh"
 
 namespace dsrg {
 
@@ -96,7 +97,7 @@ struct TileLat {
 // MODE_COMPAT (with MODE_HIST: dsrg_crf_forward_train_compat_dev; in k_mf_tile_bwd: dsrg_crf_backward_compat_dev)
 // replaces the Potts messages by label-compatibility matrices, t = U - mu_sp F_sp(Q) - mu_bi F_bi(Q): U_rw (potts in
 // the backward) then carries {mu_bi, mu_sp} ([2][M][M], row l = the message to label l), c_sp / c_bi are alpha alone.
-enum { MODE_FIRST = 0, MODE_MID = 1, MODE_LAST = 2, MODE_HIST = 4, MODE_COMPAT = 8 };
+enum { MODE_FIRST = 0, MODE_MID = 1, MODE_LAST = 2, MODE_HIST = 4, MODE_COMPAT = 8, MODE_GSTORE = 16 };
 
 // exp(x) for x <= 0 via ex2.approx with the rounding error of x*log2(e) folded back in
 // (relative error ~2^-22, independent of |x|)
@@ -768,6 +769,9 @@ k_mf_tile_hy(const float *U, float *U_rw, int clamp, float *__restrict__ Qout, T
 // mu_bi^T S_bi), and dL/dmu_k += -sum_i S_k,i (x) Q_t,i, again by <g, F(Q)> = <F^T(g), Q> per label pair.  Each pixel
 // parks S_bi, S_sp and Q_t in shared memory (behind mu, rows of an odd stride so that the parking is conflict free);
 // after the splat each thread owns fixed (l, l') entries and sums them over the tile's pixels in pixel order.
+//
+// MODE_GSTORE (the kernel-bandwidth backward) also stores g_t, the vector the launch splats, to gstore ([B][M][N]):
+// k_kg_pass of iteration t - 1 reads it before the next launch overwrites it.
 // ---------------------------------------------------------------------------------------------
 // rows of the parked S_bi / S_sp / Q_t: an odd stride >= M
 __host__ __device__ constexpr int compat_park_stride(int m) { return m | 1; }
@@ -778,7 +782,7 @@ template <int MP, int MODE>
 __global__ void __launch_bounds__(kTileThreads, MP > ((MODE & MODE_COMPAT) ? 8 : 12) ? 1 : 2)
 k_mf_tile_bwd(const float *__restrict__ G, const float *__restrict__ Qt, float *__restrict__ gU, TileLat sp,
               TileLat bi, float a_sp, float a_bi, const float *potts, float w1, float w2, float2 *part, int M, int N,
-              int W, int H, int tiles_x, int ntiles, int tile_w) {
+              int W, int H, int tiles_x, int ntiles, int tile_w, float *gstore) {
     constexpr int kRowBytes = MP * 4;
     constexpr int PH = MODE & 3;   // the iteration's place in the loop
     constexpr bool kCompat = (MODE & MODE_COMPAT) != 0;
@@ -944,6 +948,13 @@ k_mf_tile_bwd(const float *__restrict__ G, const float *__restrict__ Qt, float *
             gb += N;
         }
     }
+    if constexpr ((MODE & MODE_GSTORE) != 0) {   // g_t for the kernel-bandwidth pass of iteration t - 1
+        if (in) {
+#pragma unroll
+            for (int k = 0; k < MP; k++)
+                if (k < M) gstore[ub + (size_t)k * N] = t[k];
+        }
+    }
     // ---- the tile's Potts partials, in a fixed order ----
     if (!kCompat && PH != MODE_FIRST) {
 #pragma unroll
@@ -1048,6 +1059,275 @@ k_mf_compat_reduce(const float *part, float *out, int ntiles, int mm2) {
     float a = 0.0f;
     for (int i = 0; i < ntiles; i++) a += part[((size_t)b * ntiles + i) * mm2 + e];
     out[(size_t)b * mm2 + e] = -a;
+}
+
+// ---------------------------------------------------------------------------------------------
+// The kernel-bandwidth gradient (DenseCRF::gradient's kernel_grad under DIAG_KERNEL and NORMALIZE_SYMMETRIC,
+// pairwise.cpp:87-97, :175-185).  Per lattice, with x_t = -mu^T g_{t+1}, u_t = -mu Q_t (Potts: w g_{t+1}, w Q_t):
+//
+//   dL/df = sum_t d^K <n x_t, K (n Q_t)>  -  d^K <c, K 1>,   c = sum_t 1/2 n^3 sum_l (x_t K(n Q_t) + K^T(n x_t) Q_t)
+//
+// d^K is the derivative through the barycentric weights with simplices, vertices and neighbours held
+// (Permutohedral::gradient).  At a pixel's incidence r it needs s_r = n (x . Vy[r] + u . Vg[r]) with
+// Vy = B S(n Q_t) (a new splat and forward blur per iteration, k_kg_splatq) and Vg = B^T S(n g_{t+1}), the
+// reverse-blurred buffer k_mf_tile_bwd slices at iteration t: mu^T acts label-wise, so B^T S(n x) = -mu^T Vg and
+// its dot with n Q is u . Vg.  c at the pixel is 1/2 n^2 alpha sum_r bary_r s_r, so the normalisation term needs
+// one splat of the summed c and of ones after the loop (k_kg_splat1, k_kg_norm).  The derivative goes to the
+// features through the pixel's ranks (recomputed with the build's arithmetic, simplex.cuh) and the transposed
+// elevation matrix, and to the DIAG parameters as dL/dp_i = sum f_i (dL/df)_i.  Each 256-pixel block keeps its seven
+// sums in part[b][block] (the first pass writes them), and k_kg_reduce adds the blocks in order: no float atomics.
+// ---------------------------------------------------------------------------------------------
+struct KgLat {
+    const int32_t *off;      // [nimg][d+1][N]
+    const float *bary, *wn;  // [nimg][d+1][N]
+    const float *norm;       // [nimg][N]
+    const int32_t *rowbase;
+    int shared;
+    float alpha;
+    float sigma[5], scale[5];
+};
+struct KgArgs {
+    KgLat sp, bi;
+    const uint8_t *image;  // [B][N][3]
+    const float *potts;    // {w1, w2} on the device, or nullptr: w1, w2
+    float w1, w2;
+    float *part;           // [B][nblk][8] per-block sums of dL/dp in theta order
+    float *csum;           // [2][B][N] c per pixel: spatial, bilateral
+    int M, N, W, nblk;
+};
+
+// per-incidence s_r of one lattice -> the pixel's dL/dp over that lattice's features (added to dp), scaled by sign
+template <int D>
+__device__ __forceinline__ void kg_features(const KgLat &L, int x, int y, const uint8_t *image, int b, int N,
+                                            int i, const float *s, float sign, float *dp) {
+    float f[D], el[D + 1], rem0[D + 1];
+    int rank[D + 1];
+    lattice_features<D>(x, y, image, b, N, i, L.sigma, f);
+    lattice_simplex<D>(f, L.scale, el, rem0, rank);
+    const float c = sign * L.alpha / (float)(D + 1);
+    float gel[D + 1];
+#pragma unroll
+    for (int j = 0; j <= D; j++) {
+        const int r0 = D - rank[j], r1 = r0 == D ? 0 : r0 + 1;
+        float a = 0.0f, b = 0.0f;
+#pragma unroll
+        for (int r = 0; r <= D; r++) {
+            if (r == r0) a = s[r];
+            if (r == r1) b = s[r];
+        }
+        gel[j] = c * (a - b);
+    }
+    float sm = gel[0];
+#pragma unroll
+    for (int j = 1; j <= D; j++) {
+        dp[j - 1] = fmaf(f[j - 1], L.scale[j - 1] * (sm - (float)j * gel[j]), dp[j - 1]);
+        sm += gel[j];
+    }
+}
+
+// s_r = n * w * (x . Vy[r] + u . Vg[r]) at every incidence of one lattice; c = 1/2 n^2 alpha sum_r bary_r s_r
+template <int MP, int D>
+__device__ __forceinline__ float kg_incidences(const KgLat &L, int b, int i, int N, const float *x, const float *u,
+                                               float w, const float4 *vy, const float4 *vg, float *s) {
+    constexpr int CH = MP / 4;
+    const size_t at = (size_t)(L.shared ? 0 : b) * (D + 1) * N + i;
+    const int base = L.rowbase[b];
+    const float n = __ldg(L.norm + (size_t)(L.shared ? 0 : b) * N + i);
+    float cs = 0.0f;
+#pragma unroll
+    for (int r = 0; r <= D; r++) {
+        const size_t row = (size_t)(base + __ldg(L.off + at + (size_t)r * N)) * CH;
+        float acc = 0.0f;
+#pragma unroll
+        for (int c = 0; c < CH; c++) {
+            const float4 a = vy[row + c], g = vg[row + c];
+            acc = fmaf(x[4 * c], a.x, acc);
+            acc = fmaf(x[4 * c + 1], a.y, acc);
+            acc = fmaf(x[4 * c + 2], a.z, acc);
+            acc = fmaf(x[4 * c + 3], a.w, acc);
+            acc = fmaf(u[4 * c], g.x, acc);
+            acc = fmaf(u[4 * c + 1], g.y, acc);
+            acc = fmaf(u[4 * c + 2], g.z, acc);
+            acc = fmaf(u[4 * c + 3], g.w, acc);
+        }
+        s[r] = n * w * acc;
+        cs = fmaf(__ldg(L.bary + at + (size_t)r * N), s[r], cs);
+    }
+    return 0.5f * n * n * L.alpha * cs;
+}
+
+// the block's seven sums into part[b][block] (written when `first`, else added), in a fixed order
+__device__ __forceinline__ void kg_block_sum(const KgArgs &a, int b, const float *dp, bool first) {
+    __shared__ float red[kThreads / 32][7];
+    float v[7];
+#pragma unroll
+    for (int k = 0; k < 7; k++) {
+        v[k] = dp[k];
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) v[k] += __shfl_down_sync(0xffffffffu, v[k], o);
+    }
+    if ((threadIdx.x & 31) == 0) {
+#pragma unroll
+        for (int k = 0; k < 7; k++) red[threadIdx.x >> 5][k] = v[k];
+    }
+    __syncthreads();
+    if (threadIdx.x < 7) {
+        float acc = 0.0f;
+        for (int w = 0; w < kThreads / 32; w++) acc += red[w][threadIdx.x];
+        float *pp = a.part + ((size_t)b * a.nblk + blockIdx.x) * 8 + threadIdx.x;
+        *pp = first ? acc : *pp + acc;
+    }
+}
+
+// splat wn Q_t into both lattices' zeroed targets (the forward's splat, straight to global rows)
+template <int MP>
+__global__ void __launch_bounds__(kThreads)
+k_kg_splatq(KgArgs a, const float *Qt, float4 *vsp, float4 *vbi) {
+    const int b = blockIdx.y, i = blockIdx.x * kThreads + threadIdx.x;
+    if (i >= a.N) return;
+    float q[MP], w[6];
+#pragma unroll
+    for (int k = 0; k < MP; k++) q[k] = k < a.M ? __ldg(Qt + ((size_t)b * a.M + k) * a.N + i) : 0.0f;
+    const size_t px_sp = (size_t)(a.sp.shared ? 0 : b) * 3 * a.N + i, px_bi = (size_t)(a.bi.shared ? 0 : b) * 6 * a.N + i;
+#pragma unroll
+    for (int r = 0; r < 3; r++) w[r] = __ldg(a.sp.wn + px_sp + (size_t)r * a.N);
+    tile_splat_direct<MP, 3>(vsp, a.sp.off + px_sp, a.N, a.sp.rowbase[b], w, q);
+#pragma unroll
+    for (int r = 0; r < 6; r++) w[r] = __ldg(a.bi.wn + px_bi + (size_t)r * a.N);
+    tile_splat_direct<MP, 6>(vbi, a.bi.off + px_bi, a.N, a.bi.rowbase[b], w, q);
+}
+
+// iteration t's lattice terms: g = g_{t+1}, Qt = Q_t, vy_* = B S(n Q_t), vg_* = B^T S(n g_{t+1}); COMPAT: a.potts is
+// {mu_bi, mu_sp} ([2][M][M])
+template <int MP, bool COMPAT>
+__global__ void __launch_bounds__(kThreads)
+k_kg_pass(KgArgs a, const float *g, const float *Qt, const float4 *vy_sp, const float4 *vy_bi, const float4 *vg_sp,
+          const float4 *vg_bi, int first) {
+    __shared__ float mus[COMPAT ? 2 * MP * MP : 1];
+    const int b = blockIdx.y, i = blockIdx.x * kThreads + threadIdx.x;
+    const bool in = i < a.N;
+    if constexpr (COMPAT) {
+        for (int e = threadIdx.x; e < 2 * MP * MP; e += kThreads) {
+            const int k = e / (MP * MP), l = e / MP % MP, l2 = e % MP;
+            mus[e] = (l < a.M && l2 < a.M) ? __ldg(a.potts + ((size_t)k * a.M + l) * a.M + l2) : 0.0f;
+        }
+        __syncthreads();
+    }
+    float dp[7];
+#pragma unroll
+    for (int k = 0; k < 7; k++) dp[k] = 0.0f;
+    if (in) {
+        const int x = i % a.W, y = i / a.W;
+        float gv[MP], qv[MP];
+#pragma unroll
+        for (int k = 0; k < MP; k++) {
+            gv[k] = k < a.M ? __ldg(g + ((size_t)b * a.M + k) * a.N + i) : 0.0f;
+            qv[k] = k < a.M ? __ldg(Qt + ((size_t)b * a.M + k) * a.N + i) : 0.0f;
+        }
+        float s[6];
+        float *csum_sp = a.csum + (size_t)b * a.N + i, *csum_bi = csum_sp + (size_t)gridDim.y * a.N;
+        float c_sp, c_bi;
+        if constexpr (COMPAT) {
+            // x = -mu^T g, u = -mu Q per lattice (mus: {mu_bi, mu_sp})
+            float xv[MP], uv[MP];
+#pragma unroll
+            for (int kk = 0; kk < 2; kk++) {
+                const float *mu = mus + (kk == 0 ? MP * MP : 0);
+#pragma unroll
+                for (int l = 0; l < MP; l++) {
+                    float xa = 0.0f, ua = 0.0f;
+#pragma unroll
+                    for (int l2 = 0; l2 < MP; l2++) {
+                        xa = fmaf(-mu[l2 * MP + l], gv[l2], xa);
+                        ua = fmaf(-mu[l * MP + l2], qv[l2], ua);
+                    }
+                    xv[l] = xa;
+                    uv[l] = ua;
+                }
+                if (kk == 0) {
+                    c_sp = kg_incidences<MP, 2>(a.sp, b, i, a.N, xv, uv, 1.0f, vy_sp, vg_sp, s);
+                    kg_features<2>(a.sp, x, y, a.image, b, a.N, i, s, 1.0f, dp + 5);
+                } else {
+                    c_bi = kg_incidences<MP, 5>(a.bi, b, i, a.N, xv, uv, 1.0f, vy_bi, vg_bi, s);
+                    kg_features<5>(a.bi, x, y, a.image, b, a.N, i, s, 1.0f, dp);
+                }
+            }
+        } else {
+            const float w1 = a.potts ? __ldg(a.potts) : a.w1, w2 = a.potts ? __ldg(a.potts + 1) : a.w2;
+            c_sp = kg_incidences<MP, 2>(a.sp, b, i, a.N, gv, qv, w2, vy_sp, vg_sp, s);
+            kg_features<2>(a.sp, x, y, a.image, b, a.N, i, s, 1.0f, dp + 5);
+            c_bi = kg_incidences<MP, 5>(a.bi, b, i, a.N, gv, qv, w1, vy_bi, vg_bi, s);
+            kg_features<5>(a.bi, x, y, a.image, b, a.N, i, s, 1.0f, dp);
+        }
+        *csum_sp = first ? c_sp : *csum_sp + c_sp;
+        *csum_bi = first ? c_bi : *csum_bi + c_bi;
+    }
+    kg_block_sum(a, b, dp, first != 0);
+}
+
+// the normalisation term's splats, one channel each in 4-wide rows: bary into fw_* (channel 0, blurred in K's order)
+// and bary * c into rv_* (channel 1, blurred in K^T's order)
+__global__ void __launch_bounds__(kThreads)
+k_kg_splat1(KgArgs a, float *fw_sp, float *rv_sp, float *fw_bi, float *rv_bi) {
+    const int b = blockIdx.y, i = blockIdx.x * kThreads + threadIdx.x;
+    if (i >= a.N) return;
+#pragma unroll
+    for (int k = 0; k < 2; k++) {
+        const KgLat &L = k ? a.bi : a.sp;
+        const int dp1 = k ? 6 : 3;
+        const float c = a.csum[((size_t)k * gridDim.y + b) * a.N + i];
+        const size_t at = (size_t)(L.shared ? 0 : b) * dp1 * a.N + i;
+        float *fw = k ? fw_bi : fw_sp, *rv = k ? rv_bi : rv_sp;
+        for (int r = 0; r < dp1; r++) {
+            const size_t row = (size_t)(L.rowbase[b] + __ldg(L.off + at + (size_t)r * a.N)) * 4;
+            const float w = __ldg(L.bary + at + (size_t)r * a.N);
+            atomicAdd(fw + row, w);
+            atomicAdd(rv + row + 1, w * c);
+        }
+    }
+}
+
+// -d^K <c, K 1> = -(c . B S 1 + 1 . B^T S c) at each incidence, rotated to the features
+__global__ void __launch_bounds__(kThreads)
+k_kg_norm(KgArgs a, const float4 *v1_sp, const float4 *vc_sp, const float4 *v1_bi, const float4 *vc_bi) {
+    const int b = blockIdx.y, i = blockIdx.x * kThreads + threadIdx.x;
+    float dp[7];
+#pragma unroll
+    for (int k = 0; k < 7; k++) dp[k] = 0.0f;
+    if (i < a.N) {
+        const int x = i % a.W, y = i / a.W;
+        float s[6];
+#pragma unroll
+        for (int k = 0; k < 2; k++) {
+            const KgLat &L = k ? a.bi : a.sp;
+            const int dp1 = k ? 6 : 3;
+            const float c = a.csum[((size_t)k * gridDim.y + b) * a.N + i];
+            const size_t at = (size_t)(L.shared ? 0 : b) * dp1 * a.N + i;
+            const float4 *v1 = k ? v1_bi : v1_sp, *vc = k ? vc_bi : vc_sp;
+#pragma unroll
+            for (int r = 0; r < 6; r++) {
+                if (r < dp1) {
+                    const size_t row = (size_t)(L.rowbase[b] + __ldg(L.off + at + (size_t)r * a.N));
+                    s[r] = fmaf(c, v1[row].x, vc[row].y);
+                }
+            }
+            if (k)
+                kg_features<5>(L, x, y, a.image, b, a.N, i, s, -1.0f, dp);
+            else
+                kg_features<2>(L, x, y, a.image, b, a.N, i, s, -1.0f, dp + 5);
+        }
+    }
+    kg_block_sum(a, b, dp, false);
+}
+
+// per image: the blocks' sums in block order -> grad_theta[b] = -dL/dp / theta (theta order)
+__global__ void k_kg_reduce(const float *part, int nblk, float *out, KgArgs a) {
+    const int b = blockIdx.x, k = threadIdx.x;
+    if (k >= 7) return;
+    float acc = 0.0f;
+    for (int i = 0; i < nblk; i++) acc += part[((size_t)b * nblk + i) * 8 + k];
+    const float th = k < 5 ? a.bi.sigma[k] : a.sp.sigma[k - 5];
+    out[(size_t)b * 7 + k] = -acc / th;
 }
 
 // zero the splat targets of both lattices for the B images of the pass (row counts are device-resident)
@@ -1410,9 +1690,73 @@ static int run_impl(Engine *e, int B, const float *unary, int layout, bool clamp
 // The backward of a training forward (DenseCRF::gradient, densecrf.cpp:238-297) on the lattices the pass just built:
 // k_mf_tile_bwd from T down to 0 with the transposed blur in between, then the per-image Potts sums -- or, with
 // `compat` ({mu_bi, mu_sp}), the MODE_COMPAT kernels and the per-image compatibility sums to g_compat ([B][2][M][M]).
+static KgLat kg_lat(const Lattice &L) {
+    KgLat k;
+    k.off = L.off;
+    k.bary = L.bary;
+    k.wn = L.wn;
+    k.norm = L.norm;
+    k.rowbase = L.rowbase;
+    k.shared = L.shared;
+    k.alpha = 1.0f / (1 + powf(2, -L.d));
+    for (int i = 0; i < 5; i++) {
+        k.sigma[i] = L.sigma[i];
+        k.scale[i] = L.scale[i];
+    }
+    return k;
+}
+
+// Iteration t's kernel-bandwidth terms (before k_mf_tile_bwd of iteration t overwrites e->kg_g = g_{t+1}): splat
+// n Q_t, blur it in K's order into the kernel-gradient buffers, and k_kg_pass against spX / biX = B^T S(n g_{t+1}).
+template <int MP>
+static void kg_iter(Engine *e, const KgArgs &ka, bool compat, int B, const float *qt, const float *spX,
+                    const float *biX, bool first, int bgrid, cudaStream_t s) {
+    const dim3 gp(ka.nblk, B);
+    DSRG_LAUNCH(e, T_KGRAD, s,
+                k_mf_zero<MP><<<bgrid, kThreads, 0, s>>>((float4 *)e->kg_sp[0], e->sp.rowbase, (float4 *)e->kg_bi[0],
+                                                         e->bi.rowbase, B));
+    DSRG_LAUNCH(e, T_KGRAD, s,
+                k_kg_splatq<MP><<<gp, kThreads, 0, s>>>(ka, qt, (float4 *)e->kg_sp[0], (float4 *)e->kg_bi[0]));
+    const float *vy_sp = blur_all<MP>(e, e->sp, e->kg_sp[0], e->kg_sp[1], nullptr, B, T_KGRAD, bgrid, s);
+    const float *vy_bi = blur_all<MP>(e, e->bi, e->kg_bi[0], e->kg_bi[1], nullptr, B, T_KGRAD, bgrid, s);
+    if (compat)
+        DSRG_LAUNCH(e, T_KGRAD, s,
+                    (k_kg_pass<MP, true><<<gp, kThreads, 0, s>>>(ka, e->kg_g, qt, (const float4 *)vy_sp,
+                                                                (const float4 *)vy_bi, (const float4 *)spX,
+                                                                (const float4 *)biX, first)));
+    else
+        DSRG_LAUNCH(e, T_KGRAD, s,
+                    (k_kg_pass<MP, false><<<gp, kThreads, 0, s>>>(ka, e->kg_g, qt, (const float4 *)vy_sp,
+                                                                 (const float4 *)vy_bi, (const float4 *)spX,
+                                                                 (const float4 *)biX, first)));
+}
+
+// (every launch of the kernel-bandwidth passes is timed under T_KGRAD)
+// After the loop: the normalisation term from the summed c, then the per-image sums.  The mean-field buffers are free
+// by now: spA / biA take the reverse-blurred splat of c, the kernel-gradient buffers the forward-blurred one of ones.
+static void kg_finish(Engine *e, const KgArgs &ka, int B, float *g_theta, int bgrid, cudaStream_t s) {
+    const dim3 gp(ka.nblk, B);
+    DSRG_LAUNCH(e, T_KGRAD, s,
+                k_mf_zero<4><<<bgrid, kThreads, 0, s>>>((float4 *)e->kg_sp[0], e->sp.rowbase, (float4 *)e->kg_bi[0],
+                                                        e->bi.rowbase, B));
+    DSRG_LAUNCH(e, T_KGRAD, s,
+                k_mf_zero<4><<<bgrid, kThreads, 0, s>>>((float4 *)e->spA, e->sp.rowbase, (float4 *)e->biA,
+                                                        e->bi.rowbase, B));
+    DSRG_LAUNCH(e, T_KGRAD, s, k_kg_splat1<<<gp, kThreads, 0, s>>>(ka, e->kg_sp[0], e->spA, e->kg_bi[0], e->biA));
+    const float *v1_sp = blur_all<4>(e, e->sp, e->kg_sp[0], e->kg_sp[1], nullptr, B, T_KGRAD, bgrid, s);
+    const float *v1_bi = blur_all<4>(e, e->bi, e->kg_bi[0], e->kg_bi[1], nullptr, B, T_KGRAD, bgrid, s);
+    const float *vc_sp = blur_all<4>(e, e->sp, e->spA, e->spB, nullptr, B, T_KGRAD, bgrid, s, true);
+    const float *vc_bi = blur_all<4>(e, e->bi, e->biA, e->biB, nullptr, B, T_KGRAD, bgrid, s, true);
+    DSRG_LAUNCH(e, T_KGRAD, s,
+                k_kg_norm<<<gp, kThreads, 0, s>>>(ka, (const float4 *)v1_sp, (const float4 *)vc_sp,
+                                                  (const float4 *)v1_bi, (const float4 *)vc_bi));
+    DSRG_LAUNCH(e, T_KGRAD, s, k_kg_reduce<<<B, 32, 0, s>>>(ka.part, ka.nblk, g_theta, ka));
+}
+
 template <int MP>
 static int bwd_impl(Engine *e, int B, const float *q_hist, const float *potts, const float *G, float *gU,
-                    float *g_potts, const float *compat, float *g_compat, const dsrg_crf_params &p, cudaStream_t s) {
+                    float *g_potts, const float *compat, float *g_compat, float *g_theta, const uint8_t *image,
+                    const dsrg_crf_params &p, cudaStream_t s) {
     const int M = e->M, N = e->N, T = p.n_iters;
     const size_t slab = (size_t)B * M * N;
     if (T == 0) {
@@ -1420,6 +1764,7 @@ static int bwd_impl(Engine *e, int B, const float *q_hist, const float *potts, c
                     k_mf_softmax_vjp<<<dim3(cdiv(N, kThreads), B), kThreads, 0, s>>>(G, q_hist, gU, M, N));
         if (g_potts) DSRG_CUDA_TRY(cudaMemsetAsync(g_potts, 0, sizeof(float) * 2 * B, s));
         if (g_compat) DSRG_CUDA_TRY(cudaMemsetAsync(g_compat, 0, sizeof(float) * 2 * M * M * B, s));
+        if (g_theta) DSRG_CUDA_TRY(cudaMemsetAsync(g_theta, 0, sizeof(float) * 7 * B, s));
         DSRG_CUDA_TRY(cudaGetLastError());
         return DSRG_OK;
     }
@@ -1434,6 +1779,10 @@ static int bwd_impl(Engine *e, int B, const float *q_hist, const float *potts, c
         DSRG_CUDA_TRY(cudaFuncSetAttribute(k_mf_tile_bwd<MP, MODE_FIRST | MODE_COMPAT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_c));
         DSRG_CUDA_TRY(cudaFuncSetAttribute(k_mf_tile_bwd<MP, MODE_MID | MODE_COMPAT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_c));
         DSRG_CUDA_TRY(cudaFuncSetAttribute(k_mf_tile_bwd<MP, MODE_LAST | MODE_COMPAT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_c));
+        DSRG_CUDA_TRY(cudaFuncSetAttribute(k_mf_tile_bwd<MP, MODE_FIRST | MODE_GSTORE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        DSRG_CUDA_TRY(cudaFuncSetAttribute(k_mf_tile_bwd<MP, MODE_MID | MODE_GSTORE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        DSRG_CUDA_TRY(cudaFuncSetAttribute(k_mf_tile_bwd<MP, MODE_FIRST | MODE_COMPAT | MODE_GSTORE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_c));
+        DSRG_CUDA_TRY(cudaFuncSetAttribute(k_mf_tile_bwd<MP, MODE_MID | MODE_COMPAT | MODE_GSTORE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_c));
         attr_done[dv] = true;
     }
     const float a_sp = 1.0f / (1 + powf(2, -e->sp.d)), a_bi = 1.0f / (1 + powf(2, -e->bi.d));
@@ -1443,29 +1792,58 @@ static int bwd_impl(Engine *e, int B, const float *q_hist, const float *potts, c
     float *biX = e->biA, *biY = e->biB, *biZ = e->biC;
     DSRG_LAUNCH(e, T_MF_ZERO, s,
                 k_mf_zero<MP><<<bgrid, kThreads, 0, s>>>((float4 *)spY, e->sp.rowbase, (float4 *)biY, e->bi.rowbase, B));
+    // the kernel-bandwidth gradient (g_theta): g_t stored by the launches (MODE_GSTORE), k_kg_pass per iteration
+    KgArgs ka{};
+    if (g_theta) {
+        ka.sp = kg_lat(e->sp);
+        ka.bi = kg_lat(e->bi);
+        ka.image = image;
+        ka.potts = compat ? compat : potts;
+        ka.w1 = p.w1;
+        ka.w2 = p.w2;
+        ka.part = e->kg_part;
+        ka.csum = e->kg_csum;
+        ka.M = M;
+        ka.N = N;
+        ka.W = e->W;
+        ka.nblk = cdiv(N, kThreads);
+    }
 #define DSRG_BWD_LAUNCH_AT(MODEV, WP, PART, SMEM)                                                                     \
     DSRG_LAUNCH(e, T_MF_TILE, s,                                                                                      \
                 (k_mf_tile_bwd<MP, MODEV><<<gt, kTileThreads, SMEM, s>>>(G, qt, gU, vsp, vbi, a_sp, a_bi, WP, p.w1,    \
                                                                         p.w2, PART, M, N, e->W, e->H,                 \
-                                                                        e->tiles_x, e->ntiles, e->tile_w)))
+                                                                        e->tiles_x, e->ntiles, e->tile_w,             \
+                                                                        ((MODEV) & MODE_GSTORE) ? e->kg_g : nullptr)))
 #define DSRG_BWD_LAUNCH(MODEV) DSRG_BWD_LAUNCH_AT(MODEV, potts, e->potts_part, smem)
 #define DSRG_BWD_LAUNCH_COMPAT(MODEV)                                                                                 \
     DSRG_BWD_LAUNCH_AT(MODEV | MODE_COMPAT, compat, reinterpret_cast<float2 *>(e->compat_part), smem_c)
     for (int it = T; it >= 0; it--) {
         const TileLat vsp = make_tile_view(e->sp, spX, spY), vbi = make_tile_view(e->bi, biX, biY);
         const float *qt = q_hist + (size_t)it * slab;
+        if (g_theta && it < T) kg_iter<MP>(e, ka, compat != nullptr, B, qt, spX, biX, it == T - 1, bgrid, s);
         if (compat) {
             if (it == 0) {
                 DSRG_BWD_LAUNCH_COMPAT(MODE_LAST);
                 break;
             }
-            if (it == T)
+            if (g_theta) {
+                if (it == T)
+                    DSRG_BWD_LAUNCH_COMPAT(MODE_FIRST | MODE_GSTORE);
+                else
+                    DSRG_BWD_LAUNCH_COMPAT(MODE_MID | MODE_GSTORE);
+            } else if (it == T) {
                 DSRG_BWD_LAUNCH_COMPAT(MODE_FIRST);
-            else
+            } else {
                 DSRG_BWD_LAUNCH_COMPAT(MODE_MID);
+            }
         } else if (it == 0) {
             DSRG_BWD_LAUNCH(MODE_LAST);
             break;
+        } else if (g_theta) {
+            if (it == T)
+                DSRG_BWD_LAUNCH(MODE_FIRST | MODE_GSTORE);
+            else
+                DSRG_BWD_LAUNCH(MODE_MID | MODE_GSTORE);
         } else if (it == T) {
             DSRG_BWD_LAUNCH(MODE_FIRST);
         } else {
@@ -1489,6 +1867,7 @@ static int bwd_impl(Engine *e, int B, const float *q_hist, const float *potts, c
     }
     if (g_potts)
         DSRG_LAUNCH(e, T_MF_EXPORT, s, k_mf_potts_reduce<<<B, kThreads, 0, s>>>(e->potts_part, g_potts, e->ntiles));
+    if (g_theta) kg_finish(e, ka, B, g_theta, bgrid, s);
     DSRG_CUDA_TRY(cudaGetLastError());
     return DSRG_OK;
 }
@@ -1507,10 +1886,12 @@ int meanfield_run_train(Engine *e, int B, const float *unary, float *q_hist, con
 
 int meanfield_backward(Engine *e, int B, const float *q_hist, const float *potts, const float *grad_q,
                        float *grad_unary, float *grad_potts, const float *compat, float *grad_compat,
-                       const dsrg_crf_params &p, cudaStream_t s) {
+                       const dsrg_crf_params &p, cudaStream_t s, float *grad_theta, const uint8_t *image) {
     switch (e->MP) {
-#define DSRG_CASE(MPV) \
-    case MPV: return bwd_impl<MPV>(e, B, q_hist, potts, grad_q, grad_unary, grad_potts, compat, grad_compat, p, s);
+#define DSRG_CASE(MPV)                                                                                        \
+    case MPV:                                                                                                 \
+        return bwd_impl<MPV>(e, B, q_hist, potts, grad_q, grad_unary, grad_potts, compat, grad_compat, grad_theta, \
+                             image, p, s);
         DSRG_CASE(4) DSRG_CASE(8) DSRG_CASE(12) DSRG_CASE(16) DSRG_CASE(20) DSRG_CASE(24) DSRG_CASE(28) DSRG_CASE(32)
 #undef DSRG_CASE
     }

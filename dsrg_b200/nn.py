@@ -29,6 +29,7 @@ A step captured in a CUDA graph uses the cached engine's buffers.  Two rules fol
 * The engine orders its eager calls across streams, but a graph replay leaves no mark it can wait for.  Replays and
   eager steps on the same engine must run on one stream, or be ordered by the caller.
 """
+import math
 import threading
 
 import torch
@@ -417,6 +418,87 @@ class _DenseCrfCompat(torch.autograd.Function):
         return grad_u, None, None if grad_c is None else grad_c.sum(0), None, None, None
 
 
+class _DenseCrfTheta(torch.autograd.Function):
+    """dense_crf with learnable kernel bandwidths: theta_bi (5,), theta_sp (2,) (None: params' own values) beside
+    the Potts weights (w1, w2) or the matrices (compat (2, M, M) {mu_bi, mu_sp}); params carries the sigmas."""
+
+    @staticmethod
+    @_fwd
+    def forward(ctx, unary, image, w1, w2, compat, theta_bi, theta_sp, params):
+        eng = _engine_for(unary)
+        s = _stream(unary)
+        maxiter = params.n_iters
+        q_hist = torch.empty((maxiter + 1,) + tuple(unary.shape), dtype=torch.float32, device=unary.device)
+        potts = None
+        if compat is not None:
+            eng.crf_forward_train_compat_dev(unary, image, params, compat, q_hist, stream=s)
+        else:
+            if w1 is not None or w2 is not None:
+                potts = torch.empty(2, dtype=torch.float32, device=unary.device)
+                for i, (w, d) in enumerate(zip((w1, w2), _POTTS_DEFAULT)):
+                    if w is None:
+                        potts[i].fill_(d)
+                    else:
+                        potts[i].copy_(w.detach())
+            eng.crf_forward_train_dev(unary, image, params, q_hist, potts=potts, stream=s)
+        ctx.save_for_backward(q_hist, image, potts, compat)
+        ctx.params = params
+        ctx.theta = [(t.device, t.dtype) if t is not None else None for t in (theta_bi, theta_sp)]
+        return q_hist[maxiter].clone()
+
+    @staticmethod
+    @_bwd
+    def backward(ctx, g):
+        q_hist, image, potts, compat = ctx.saved_tensors
+        B = q_hist.shape[1]
+        grad_u = torch.empty(q_hist.shape[1:], dtype=torch.float32, device=q_hist.device)
+        grad_t = torch.empty((B, 7), dtype=torch.float32, device=q_hist.device)
+        eng, s = _engine_for(grad_u), _stream(grad_u)
+        gw1 = gw2 = gc = None
+        if compat is not None:
+            grad_c = None
+            if ctx.needs_input_grad[4]:
+                M = compat.shape[-1]
+                grad_c = torch.empty((B, 2, M, M), dtype=torch.float32, device=q_hist.device)
+            eng.crf_backward_compat_theta_dev(q_hist, image, ctx.params, compat, g.contiguous(), grad_u, grad_t,
+                                              grad_compat=grad_c, stream=s)
+            gc = None if grad_c is None else grad_c.sum(0)
+        else:
+            grad_potts = None
+            if potts is not None and (ctx.needs_input_grad[2] or ctx.needs_input_grad[3]):
+                grad_potts = torch.empty((B, 2), dtype=torch.float32, device=q_hist.device)
+            eng.crf_backward_theta_dev(q_hist, image, ctx.params, g.contiguous(), grad_u, grad_t,
+                                       grad_potts=grad_potts, potts=potts, stream=s)
+            gw1 = grad_potts[:, 0].sum() if grad_potts is not None and ctx.needs_input_grad[2] else None
+            gw2 = grad_potts[:, 1].sum() if grad_potts is not None and ctx.needs_input_grad[3] else None
+        gt = grad_t.sum(0)
+        out = []
+        for part, spec, need in ((gt[0:5], ctx.theta[0], ctx.needs_input_grad[5]),
+                                 (gt[5:7], ctx.theta[1], ctx.needs_input_grad[6])):
+            out.append(part.to(spec[0], spec[1]) if spec is not None and need else None)
+        return grad_u, None, gw1, gw2, gc, out[0], out[1], None
+
+
+def _theta_values(theta, name, n, ref):
+    """A learnable bandwidth vector's values as floats (one synchronising copy for a CUDA tensor)."""
+    if theta is None:
+        return None
+    if (not isinstance(theta, torch.Tensor) or tuple(theta.shape) != (n,) or not theta.is_floating_point()
+            or (theta.device.type != "cpu" and theta.device != ref.device)):
+        raise ValueError("%s must be None or a (%d,) floating-point tensor on the CPU or on %s (got %r)"
+                         % (name, n, ref.device,
+                            theta if not isinstance(theta, torch.Tensor) else (theta.dtype, tuple(theta.shape),
+                                                                               theta.device)))
+    if torch.cuda.is_available() and torch.cuda.is_current_stream_capturing():
+        # a CUDA theta is copied to the host here, and the backward copies a CPU theta's gradient back to the host
+        raise ValueError("%s is read on the host to build the lattices: it cannot be given inside CUDA-graph "
+                         "capture" % name)
+    v = [float(x) for x in theta.detach().to("cpu", torch.float64)]
+    if not all(math.isfinite(x) and x > 0 for x in v):
+        raise ValueError("%s must be positive and finite (got %r)" % (name, v))
+    return v
+
+
 def _compat_matrix(mu, name, ref, M):
     if not isinstance(mu, torch.Tensor) or tuple(mu.shape) != (M, M) or not mu.is_floating_point() \
             or mu.device != ref.device:
@@ -427,7 +509,7 @@ def _compat_matrix(mu, name, ref, M):
 
 
 def dense_crf(unary, image, scale_factor=1.0, color_factor=13, maxiter=10, w1=None, w2=None, compat_bi=None,
-              compat_sp=None):
+              compat_sp=None, theta_bi=None, theta_sp=None):
     """The dense CRF of CRF() (CRF/krahenbuhl2013/CRF.py:4-37) as a differentiable layer: unary (N, M, H, W) float32,
     M <= 32, the values CRF(image, unary) takes (energy = -unary); image (N, H, W, 3) uint8 at the map size ->
     marginals (N, M, H, W) after `maxiter` mean-field iterations.  The backward is the exact gradient of the
@@ -440,7 +522,15 @@ def dense_crf(unary, image, scale_factor=1.0, color_factor=13, maxiter=10, w1=No
     of w1 / w2 (not together with them): the message to label l is -sum_l' mu[l, l'] F(Q)[l'], so Potts(w) is
     -w * I, the reference's MatrixCompatibility(m) is (m + m.T) / 2 and its DiagonalCompatibility(v) is diag(v).
     A matrix left None is -w * I of its weight (w1 / w2, or CRF()'s 10 / 3).  Their gradients are summed over the
-    batch."""
+    batch.
+
+    theta_bi (5,) = (theta_alpha_x, theta_alpha_y, theta_beta_r, theta_beta_g, theta_beta_b) and theta_sp (2,) =
+    (theta_gamma_x, theta_gamma_y): learnable kernel bandwidths, floating-point tensors on the CPU or on unary's
+    device, in place of the values scale_factor / color_factor give (a None one keeps those).  Their gradient is the
+    exact derivative of the function the device computes with every pixel's simplex held, summed over the batch and
+    returned on the tensor's own device and dtype; it works with the Potts weights and with the matrices.  The
+    lattice build takes the sigmas as host values, so the forward reads a given theta on the host: one synchronising
+    copy for a CUDA tensor, which is why a given theta is refused inside CUDA-graph capture."""
     if torch.is_autocast_enabled("cuda"):   # what custom_fwd(cast_inputs=float32) does, before the checks
         unary = unary.float() if isinstance(unary, torch.Tensor) and unary.is_floating_point() else unary
     u = _maps(unary, "unary")
@@ -450,12 +540,31 @@ def dense_crf(unary, image, scale_factor=1.0, color_factor=13, maxiter=10, w1=No
     if (not isinstance(image, torch.Tensor) or image.dtype != torch.uint8 or tuple(image.shape) != (N, H, W, 3)
             or image.device != u.device):
         raise ValueError("image must be a (%d, %d, %d, 3) uint8 tensor on %s" % (N, H, W, u.device))
+    th_bi, th_sp = _theta_values(theta_bi, "theta_bi", 5, u), _theta_values(theta_sp, "theta_sp", 2, u)
     _cuda(u, "unary")
     w1, w2 = _potts_weight(w1, "w1", u), _potts_weight(w2, "w2", u)
     if int(maxiter) < 0:
         raise ValueError("maxiter must be >= 0 (got %d)" % maxiter)
+    if th_bi is not None or th_sp is not None:
+        params = api.crf_params(float(scale_factor), float(color_factor), int(maxiter))
+        if th_bi is not None:
+            (params.theta_alpha_x, params.theta_alpha_y, params.theta_beta_r, params.theta_beta_g,
+             params.theta_beta_b) = th_bi
+        if th_sp is not None:
+            params.theta_gamma_x, params.theta_gamma_y = th_sp
+        compat = None
+        if compat_bi is not None or compat_sp is not None:
+            compat = _compat_stack(u, M, w1, w2, compat_bi, compat_sp)
+            w1 = w2 = None
+        return _DenseCrfTheta.apply(u, image.contiguous(), w1, w2, compat, theta_bi, theta_sp, params)
     if compat_bi is None and compat_sp is None:
         return _DenseCrf.apply(u, image.contiguous(), w1, w2, float(scale_factor), float(color_factor), int(maxiter))
+    return _DenseCrfCompat.apply(u, image.contiguous(), _compat_stack(u, M, w1, w2, compat_bi, compat_sp),
+                                 float(scale_factor), float(color_factor), int(maxiter))
+
+
+def _compat_stack(u, M, w1, w2, compat_bi, compat_sp):
+    """(2, M, M) {mu_bi, mu_sp}, a missing matrix built as -w I of its weight."""
     mats = []
     for mu, w, d, name, wname in ((compat_bi, w1, _POTTS_DEFAULT[0], "compat_bi", "w1"),
                                   (compat_sp, w2, _POTTS_DEFAULT[1], "compat_sp", "w2")):
@@ -466,8 +575,7 @@ def dense_crf(unary, image, scale_factor=1.0, color_factor=13, maxiter=10, w1=No
             raise ValueError("%s and %s are two forms of one term: give one of them" % (name, wname))
         else:
             mats.append(_compat_matrix(mu, name, u, M))
-    return _DenseCrfCompat.apply(u, image.contiguous(), torch.stack(mats), float(scale_factor), float(color_factor),
-                                 int(maxiter))
+    return torch.stack(mats)
 
 
 def softmax(fc8):

@@ -177,6 +177,26 @@ int dsrg_crf_forward_train_compat_dev(dsrg_engine *e, const float *unary_dev, in
 int dsrg_crf_backward_compat_dev(dsrg_engine *e, const float *q_hist_dev, int B, const uint8_t *image_dev,
                                  const dsrg_crf_params *params, const float *compat_dev, const float *grad_q_dev,
                                  float *grad_unary_dev, float *grad_compat_dev, void *stream);
+/*
+ * The two backwards with the gradient to the kernel bandwidths too (DenseCRF::gradient's kernel_grad under the
+ * reference's default DIAG_KERNEL and NORMALIZE_SYMMETRIC, exact for the function the device computes as long as no
+ * pixel changes simplex):
+ *   grad_theta : [B][7] dL/dtheta per image in the struct's order: theta_alpha_x, theta_alpha_y, theta_beta_r,
+ *                theta_beta_g, theta_beta_b, theta_gamma_x, theta_gamma_y
+ * The reference's kernel_grad is dL/dp for the DIAG parameters p (features p * f at p = 1) in the order the kernels are
+ * added: spatial x, y, then bilateral x, y, r, g, b.  With f = raw / theta, dL/dtheta_i = -dL/dp_i / theta_i.
+ * The derivative differs from the reference's, whose Permutohedral::gradient differentiates K^T where K is meant
+ * (DESIGN.md section 1).  Everything else as dsrg_crf_backward_dev / dsrg_crf_backward_compat_dev.  The first call
+ * allocates g_t, the c term and two value buffers per lattice: 12.0 GB for an engine of batch 64 @ 321x321 with
+ * 21 labels, 61 MB at batch 20 @ 41x41 (measured with dsrg_engine_device_bytes).
+ */
+int dsrg_crf_backward_theta_dev(dsrg_engine *e, const float *q_hist_dev, int B, const uint8_t *image_dev,
+                                const dsrg_crf_params *params, const float *potts_dev, const float *grad_q_dev,
+                                float *grad_unary_dev, float *grad_potts_dev, float *grad_theta_dev, void *stream);
+int dsrg_crf_backward_compat_theta_dev(dsrg_engine *e, const float *q_hist_dev, int B, const uint8_t *image_dev,
+                                       const dsrg_crf_params *params, const float *compat_dev,
+                                       const float *grad_q_dev, float *grad_unary_dev, float *grad_compat_dev,
+                                       float *grad_theta_dev, void *stream);
 /* arg-max labelling after inference: DenseCRFWrapper::map, densecrf_wrapper.cpp:39-43 */
 int dsrg_crf_map_batch_dev(dsrg_engine *e, int B, const float *unary_dev, int unary_layout,
                            const uint8_t *image_dev, const dsrg_crf_params *params,

@@ -1,0 +1,29 @@
+"""Regenerate tests/golden/crf_kgrad_ref.npz: the reference CRF's own kernel_grad (DenseCRF::gradient's third output,
+built into oracle/_ref/libdensecrf_kgrad_ref.so by oracle/kgrad.mk) on a few images, with Potts and
+MatrixCompatibility terms, so that the kernel-gradient tests have a pin to the reference wherever oracle/_ref was not
+built.  Run from the repository root:  python tests/golden/make_crf_kgrad_golden.py
+"""
+import os
+import sys
+
+import numpy as np
+
+HERE = os.path.dirname(os.path.abspath(__file__))
+sys.path[:0] = [os.path.join(HERE, "..", ".."), os.path.join(HERE, "..")]
+
+from crf_kgrad_cases import GOLDEN, GOLDEN_CASES, golden_inputs  # noqa: E402
+from oracle import crf_kgrad_oracle  # noqa: E402
+
+
+def main():
+    if not crf_kgrad_oracle.ref_available():
+        sys.exit("oracle/_ref/libdensecrf_kgrad_ref.so is not built")
+    out = {}
+    for name in GOLDEN_CASES:
+        image, unary, G, p, mus = golden_inputs(name)
+        out[name + "/kernel_grad"] = crf_kgrad_oracle.ref_kernel_grad(image, unary, p, G, mus)
+    np.savez_compressed(os.path.join(HERE, GOLDEN), **out)
+
+
+if __name__ == "__main__":
+    main()

@@ -5,6 +5,10 @@
             backward to the unaries and the Potts weights (what nn.dense_crf runs per training step)
   compat    (--compat) dsrg_crf_forward_train_compat_dev + dsrg_crf_backward_compat_dev: the same step with a
             compatibility matrix per kernel (random, not symmetric) and its gradient
+  train_theta, compat_theta
+            (--kernel) the train (and with --compat the compat) step with the backward that also gives the gradient
+            to the seven kernel bandwidths (dsrg_crf_backward_theta_dev, dsrg_crf_backward_compat_theta_dev); the
+            line also reports the device memory the first such backward allocates (kgrad_bytes)
 
 on three workloads: train-s's shape (batch 20, 41 x 41 maps, 21 labels, scale_factor 12, smooth images) and batch 64
 at 321 x 321 with scale_factor 1 on smooth and on photo-like images; 10 mean-field iterations.  The legs run on a side
@@ -13,7 +17,7 @@ window is timed with CUDA events.  Prints one JSON line per workload with the me
 card's name, power limit and SM clocks read in the same run.
 
 usage: python tools/bench_crf_grad.py [--steps 20] [--warmup 3] [--rounds 5] [--workloads train_s,b64_smooth,b64_photo]
-                                     [--compat]
+                                     [--compat] [--kernel]
 """
 import argparse
 import json
@@ -36,7 +40,7 @@ WORKLOADS = {   # name -> (B, H, W, M, scale factor, image)
 T = 10
 
 
-def run(name, steps, warmup, rounds, compat=False):
+def run(name, steps, warmup, rounds, compat=False, kernel=False):
     import torch
     from dsrg_b200 import api, synth
     B, H, W, M, sf, img = WORKLOADS[name]
@@ -63,6 +67,23 @@ def run(name, steps, warmup, rounds, compat=False):
         legs["compat"] = lambda: (eng.crf_forward_train_compat_dev(unary, image, p, mu, q_hist, stream=s.cuda_stream),
                                   eng.crf_backward_compat_dev(q_hist, image, p, mu, G, gu, grad_compat=gmu,
                                                               stream=s.cuda_stream))
+    extra = {}
+    if kernel:
+        from dsrg_b200 import _lib
+        gt = torch.empty((B, 7), device="cuda")
+        before = _lib.lib().dsrg_engine_device_bytes(eng.h)
+        legs["train_theta"] = lambda: (eng.crf_forward_train_dev(unary, image, p, q_hist, stream=s.cuda_stream),
+                                       eng.crf_backward_theta_dev(q_hist, image, p, G, gu, gt, grad_potts=gw,
+                                                                  stream=s.cuda_stream))
+        if compat:
+            legs["compat_theta"] = lambda: (
+                eng.crf_forward_train_compat_dev(unary, image, p, mu, q_hist, stream=s.cuda_stream),
+                eng.crf_backward_compat_theta_dev(q_hist, image, p, mu, G, gu, gt, grad_compat=gmu,
+                                                  stream=s.cuda_stream))
+        with torch.cuda.stream(s):
+            legs["train_theta"]()
+        torch.cuda.synchronize()
+        extra["kgrad_bytes"] = int(_lib.lib().dsrg_engine_device_bytes(eng.h) - before)
     times = {k: [] for k in legs}
     with torch.cuda.stream(s):
         for fn in legs.values():
@@ -80,7 +101,12 @@ def run(name, steps, warmup, rounds, compat=False):
                 times[k].append(a.elapsed_time(b) / steps)
     eng.close()
     med = {k: float(np.median(v)) for k, v in times.items()}
-    extra = dict(compat_over_train=round(med["compat"] / med["train"], 2)) if compat else {}
+    if compat:
+        extra["compat_over_train"] = round(med["compat"] / med["train"], 2)
+    if kernel:
+        extra["train_theta_over_train"] = round(med["train_theta"] / med["train"], 2)
+        if compat:
+            extra["compat_theta_over_compat"] = round(med["compat_theta"] / med["compat"], 2)
     return dict(**extra, workload=name, B=B, H=H, W=W, M=M, scale_factor=sf, image=img, n_iters=T,
                 ms_per_step={k: round(v, 3) for k, v in med.items()},
                 spread_ms={k: [round(min(v), 3), round(max(v), 3)] for k, v in times.items()},
@@ -95,13 +121,14 @@ def main():
     ap.add_argument("--rounds", type=int, default=5)
     ap.add_argument("--workloads", default=",".join(WORKLOADS))
     ap.add_argument("--compat", action="store_true", help="also time the compatibility-matrix step")
+    ap.add_argument("--kernel", action="store_true", help="also time the steps with the kernel-bandwidth gradient")
     a = ap.parse_args()
     import torch
     if not torch.cuda.is_available():
         sys.exit("bench_crf_grad.py needs a CUDA device")
     info = card()
     for name in a.workloads.split(","):
-        r = run(name, a.steps, a.warmup, a.rounds, a.compat)
+        r = run(name, a.steps, a.warmup, a.rounds, a.compat, a.kernel)
         r.update(info)
         print(json.dumps(r), flush=True)
 
