@@ -506,16 +506,21 @@ def predict_tile_paths(images, sf, sm_count, cf=13):
     dsrg_crf_params `sf`, from the oracle's own lattices.  Returns {"sp": kinds (ntiles,), "bi": kinds (B, ntiles),
     "hybrid_tiles": n}; a kind is "smem" (the tile's distinct vertices fit the shared-memory list), "direct" (overflow
     tile on k_mf_tile's direct path) or "hybrid" (k_mf_tile_hy).  Only the bilateral lattice has hybrid tiles;
-    `hybrid_tiles` is the count the engine reports after k_tile_demote."""
+    `hybrid_tiles` is the count the engine reports after k_tile_demote.  A batch that repeats an image builds its
+    lattices once."""
     B, H, W = images.shape[:3]
     params = as_params(sf, cf)
     gate = hybrid_tiles_on(H, W, B, sm_count)
     sp_kinds, bi_kinds = None, np.empty((B, tile_geometry(H, W)[0] * tile_geometry(H, W)[2]), object)
+    seen = {}
     for b in range(B):
-        c = oracle_lattices(images[b], params)
-        if b == 0:                                                 # one spatial lattice serves the batch
-            sp_kinds = lattice_tile_kinds(c.lattice(0).offset, H, W, 0, gate)
-        bi_kinds[b] = lattice_tile_kinds(c.lattice(1).offset, H, W, 1, gate)
+        key = digest(images[b])
+        if key not in seen:
+            c = oracle_lattices(images[b], params)
+            if b == 0:                                             # one spatial lattice serves the batch
+                sp_kinds = lattice_tile_kinds(c.lattice(0).offset, H, W, 0, gate)
+            seen[key] = lattice_tile_kinds(c.lattice(1).offset, H, W, 1, gate)
+        bi_kinds[b] = seen[key]
     nhy = demote_hybrid_tiles(bi_kinds, sm_count)
     return {"sp": sp_kinds, "bi": bi_kinds, "hybrid_tiles": nhy}
 
