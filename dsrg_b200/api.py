@@ -197,6 +197,35 @@ class Engine(object):
                                                          _dptr(grad_compat), _dptr(grad_theta), _stream(stream)))
         return grad_unary
 
+    def crf_forward_train_feat_dev(self, unary, features, params, q_hist, potts=None, compat=None, stream=None):
+        """crf_forward_train_dev with caller-given bilateral features: features (B, 5, H, W) float32 on the device
+        replace (x/theta_alpha, y/theta_alpha, rgb/theta_beta), taken as they are; params gives the spatial sigmas, the
+        iterations and (without potts / compat) the weights.  potts {w1, w2} or compat (2, M, M) {mu_bi, mu_sp}, not
+        both.  An image whose lattice keys leave the packed range gets NaN in every iterate (feature_range_flags)."""
+        B = unary.shape[0]
+        check(self._L.dsrg_crf_forward_train_feat_dev(self.h, _dptr(unary), B, _dptr(features), C.byref(params),
+                                                      _dptr(potts), _dptr(compat), _dptr(q_hist), _stream(stream)))
+        return q_hist
+
+    def crf_backward_feat_dev(self, q_hist, features, params, grad_q, grad_unary, grad_features, potts=None,
+                              compat=None, grad_potts=None, grad_compat=None, grad_theta_sp=None, stream=None):
+        """The backward of crf_forward_train_feat_dev: grad_unary (B, M, H, W), grad_features (B, 5, H, W) = dL/df per
+        pixel and, if given, grad_potts (B, 2) (Potts), grad_compat (B, 2, M, M) (matrices) and grad_theta_sp (B, 2) =
+        dL/d{theta_gamma_x, theta_gamma_y}.  A flagged image's gradients are NaN."""
+        B = grad_q.shape[0]
+        check(self._L.dsrg_crf_backward_feat_dev(self.h, _dptr(q_hist), B, _dptr(features), C.byref(params),
+                                                 _dptr(potts), _dptr(compat), _dptr(grad_q), _dptr(grad_unary),
+                                                 _dptr(grad_features), _dptr(grad_potts), _dptr(grad_compat),
+                                                 _dptr(grad_theta_sp), _stream(stream)))
+        return grad_unary
+
+    def feature_range_flags(self, B):
+        """(B,) bool: which images of the engine's last feature pass (a batch of B) had lattice keys outside the packed
+        range, and so NaN results.  Synchronises the device."""
+        out = np.zeros(B, np.int32)
+        check(self._L.dsrg_engine_feature_range_flags(self.h, B, _hptr(out, np.int32)))
+        return out.astype(bool)
+
     def crf_map_dev(self, unary, image, params, labels_out, unary_layout=LAYOUT_NHWC, stream=None):
         B = image.shape[0]
         check(self._L.dsrg_crf_map_batch_dev(self.h, B, _dptr(unary), unary_layout, _dptr(image), C.byref(params),

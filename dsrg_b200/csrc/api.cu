@@ -168,14 +168,8 @@ int check_device_flag(Engine *e, cudaStream_t s) {
     return DSRG_OK;
 }
 
-// (re)build lattices for this call: spatial only when crf_pass found it due, bilateral always
-static int prepare_lattices(Engine *e, int B, const uint8_t *image, const dsrg_crf_params &p,
-                            cudaStream_t s) {
-    if (!(p.theta_gamma_x > 0 && p.theta_gamma_y > 0 && p.theta_alpha_x > 0 && p.theta_alpha_y > 0 &&
-          p.theta_beta_r > 0 && p.theta_beta_g > 0 && p.theta_beta_b > 0) || p.n_iters < 0) {
-        set_error("CRF parameters must be positive");
-        return DSRG_E_INVALID;
-    }
+// the shared spatial lattice, when crf_pass found it due
+static int prepare_spatial(Engine *e, int B, const dsrg_crf_params &p, cudaStream_t s) {
     if (!e->sp_valid) {
         e->sp.sigma[0] = p.theta_gamma_x;
         e->sp.sigma[1] = p.theta_gamma_y;
@@ -187,6 +181,18 @@ static int prepare_lattices(Engine *e, int B, const uint8_t *image, const dsrg_c
         int rc = lattice_build(e, e->sp, B, nullptr, s);
         if (rc) return rc;
     }
+    return DSRG_OK;
+}
+
+// (re)build lattices for this call: spatial only when crf_pass found it due, bilateral always
+static int prepare_lattices(Engine *e, int B, const uint8_t *image, const dsrg_crf_params &p,
+                            cudaStream_t s) {
+    if (!(p.theta_gamma_x > 0 && p.theta_gamma_y > 0 && p.theta_alpha_x > 0 && p.theta_alpha_y > 0 &&
+          p.theta_beta_r > 0 && p.theta_beta_g > 0 && p.theta_beta_b > 0) || p.n_iters < 0) {
+        set_error("CRF parameters must be positive");
+        return DSRG_E_INVALID;
+    }
+    if (int rc = prepare_spatial(e, B, p, s)) return rc;
     e->bi.sigma[0] = p.theta_alpha_x;
     e->bi.sigma[1] = p.theta_alpha_y;
     e->bi.sigma[2] = p.theta_beta_r;
@@ -198,6 +204,18 @@ static int prepare_lattices(Engine *e, int B, const uint8_t *image, const dsrg_c
         return DSRG_E_KEYRANGE;
     }
     return lattice_build(e, e->bi, B, image, s);
+}
+
+// prepare_lattices with caller-given bilateral features ([B][5][N]): the bilateral sigmas of `p` are not used, and the
+// key range is checked per image on the device (e->feat_bad, which ensure_feat allocates)
+static int prepare_lattices_feat(Engine *e, int B, const float *feat, const dsrg_crf_params &p, cudaStream_t s) {
+    if (!(p.theta_gamma_x > 0 && p.theta_gamma_y > 0) || p.n_iters < 0) {
+        set_error("CRF parameters must be positive");
+        return DSRG_E_INVALID;
+    }
+    if (int rc = prepare_spatial(e, B, p, s)) return rc;
+    for (int i = 0; i < 5; i++) e->bi.sigma[i] = 1.0f;
+    return lattice_build(e, e->bi, B, nullptr, s, feat, e->feat_bad);
 }
 
 int check_batch(Engine *e, int B) {
@@ -324,7 +342,7 @@ using namespace dsrg;
 
 extern "C" {
 
-int dsrg_version(void) { return 113; }
+int dsrg_version(void) { return 114; }
 
 const char *dsrg_last_error(void) { return g_err; }
 
@@ -497,7 +515,7 @@ void dsrg_engine_destroy(dsrg_engine *h) {
     void *ptrs[] = {e->U, e->Q0, e->spA, e->spB, e->spC, e->biA, e->biB, e->biC, e->nvA, e->nvB, e->lmap,
                     e->lflag, e->parent, e->hc, e->loss_acc, e->sec_rec, e->sec_img, e->sec_part, e->sec_w, e->dev_err,
                     e->hy_list, e->hy_count, e->potts_part, e->compat_part, e->kg_g, e->kg_csum, e->kg_part, e->kg_sp[0],
-                    e->kg_sp[1], e->kg_bi[0], e->kg_bi[1], e->st_unary, e->st_out, e->st_cues, e->st_labels, e->st_image, e->st_lmap, e->st_raw, e->st_idx,
+                    e->kg_sp[1], e->kg_bi[0], e->kg_bi[1], e->feat_bad, e->st_unary, e->st_out, e->st_cues, e->st_labels, e->st_image, e->st_lmap, e->st_raw, e->st_idx,
                     e->st_prep, e->st_sel};
     for (void *p : ptrs) cudaFree(p);
     if (e->own_stream) cudaStreamDestroy(e->own_stream);
@@ -564,7 +582,7 @@ static const char *kTagNames[T_COUNT] = {
     "lattice_insert", "lattice_misc", "lattice_norm", "mf_init", "mf_zero", "mf_blur_spatial",
     "mf_blur_bilateral", "mf_tile", "mf_export", "srg_label", "srg_merge", "srg_flag", "srg_emit",
     "seedloss", "wire_bits", "prepare_image", "postprocess", "annotation", "mf_tile_hybrid",
-    "kernel_grad"};
+    "kernel_grad", "feature_grad"};
 
 int dsrg_profile_tag_count(void) { return T_COUNT; }
 
@@ -794,6 +812,91 @@ int dsrg_crf_backward_compat_theta_dev(dsrg_engine *h, const float *q_hist, int 
         e->last_crf_B = 0;
         return rc;
     });
+}
+
+// The feature passes' per-image key-range flags on their first call (as ensure_compat_part)
+static int ensure_feat(Engine *e) {
+    if (e->feat_bad) return DSRG_OK;
+    cudaStreamCaptureMode mode = cudaStreamCaptureModeRelaxed;
+    DSRG_CUDA_TRY(cudaThreadExchangeStreamCaptureMode(&mode));
+    const int rc = dalloc(e, &e->feat_bad, (size_t)e->maxB);
+    DSRG_CUDA_TRY(cudaThreadExchangeStreamCaptureMode(&mode));
+    return rc;
+}
+
+int dsrg_crf_forward_train_feat_dev(dsrg_engine *h, const float *unary, int B, const float *features,
+                                    const dsrg_crf_params *params, const float *potts, const float *compat,
+                                    float *q_hist, void *stream) {
+    const cudaStream_t s = (cudaStream_t)stream;
+    return dev_call(h, B, s, unary && features && params && q_hist && !(potts && compat), [&](Engine *e) {
+        if (int rc = grad_labels_ok(e)) return rc;
+        if (int rc = ensure_feat(e)) return rc;
+        GraphKey args;
+        args.add(unary).add(features).add(potts).add(compat).add(q_hist);
+        const int rc = crf_pass(e, s, PassKind::crf_train_feat, B, params, args, [&]() {
+            int r = prepare_lattices_feat(e, B, features, *params, s);
+            if (!r) r = meanfield_run_train(e, B, unary, q_hist, potts, compat, *params, s);
+            if (r) return r;
+            const long long mn = (long long)e->M * e->N;
+            nan_images(e, e->feat_bad, q_hist, B, mn, params->n_iters + 1, B * mn, s);   // every kept iterate
+            DSRG_CUDA_TRY(cudaGetLastError());
+            return DSRG_OK;
+        });
+        e->last_crf_B = 0;
+        e->feat_B = rc == DSRG_OK ? B : 0;
+        return rc;
+    });
+}
+
+int dsrg_crf_backward_feat_dev(dsrg_engine *h, const float *q_hist, int B, const float *features,
+                               const dsrg_crf_params *params, const float *potts, const float *compat,
+                               const float *grad_q, float *grad_unary, float *grad_features, float *grad_potts,
+                               float *grad_compat, float *grad_theta_sp, void *stream) {
+    const cudaStream_t s = (cudaStream_t)stream;
+    const bool ok = q_hist && features && params && grad_q && grad_unary && grad_features && !(potts && compat) &&
+                    !(grad_potts && compat) && !(grad_compat && !compat);
+    return dev_call(h, B, s, ok, [&](Engine *e) {
+        if (int rc = grad_labels_ok(e)) return rc;
+        if (compat)
+            if (int rc = ensure_compat_part(e)) return rc;
+        if (int rc = ensure_kgrad(e)) return rc;
+        if (int rc = ensure_feat(e)) return rc;
+        GraphKey args;
+        args.add(q_hist).add(features).add(potts).add(compat).add(grad_q).add(grad_unary).add(grad_features)
+            .add(grad_potts).add(grad_compat).add(grad_theta_sp);
+        const int rc = crf_pass(e, s, PassKind::crf_backward_feat, B, params, args, [&]() {
+            int r = prepare_lattices_feat(e, B, features, *params, s);   // as in dsrg_crf_backward_dev
+            if (!r)
+                r = meanfield_backward(e, B, q_hist, potts, grad_q, grad_unary, grad_potts, compat, grad_compat,
+                                       *params, s, nullptr, nullptr, features, grad_features, grad_theta_sp);
+            if (r) return r;
+            const long long M = e->M, N = e->N;
+            const std::pair<float *, long long> outs[] = {{grad_unary, M * N}, {grad_features, 5 * N},
+                                                          {grad_potts, 2}, {grad_compat, 2 * M * M},
+                                                          {grad_theta_sp, 2}};
+            for (const auto &o : outs)
+                if (o.first) nan_images(e, e->feat_bad, o.first, B, o.second, 1, 0, s);
+            DSRG_CUDA_TRY(cudaGetLastError());
+            return DSRG_OK;
+        });
+        e->last_crf_B = 0;
+        e->feat_B = rc == DSRG_OK ? B : 0;
+        return rc;
+    });
+}
+
+int dsrg_engine_feature_range_flags(dsrg_engine *h, int B, int32_t *flags_out) {
+    Engine *e = (Engine *)h;
+    if (!e) return no_engine();
+    if (!flags_out) return DSRG_E_INVALID;
+    DeviceScope dev_scope(e);
+    if (e->feat_B == 0 || B != e->feat_B) {
+        set_error("the engine's last feature pass was not a batch of %d (last: %d)", B, e->feat_B);
+        return DSRG_E_STATE;
+    }
+    DSRG_CUDA_TRY(cudaDeviceSynchronize());
+    DSRG_CUDA_TRY(cudaMemcpy(flags_out, e->feat_bad, sizeof(int32_t) * B, cudaMemcpyDeviceToHost));
+    return DSRG_OK;
 }
 
 int dsrg_crf_map_batch_dev(dsrg_engine *h, int B, const float *unary, int unary_layout,

@@ -83,11 +83,14 @@ struct Engine;
 enum KTag {
     T_LAT_INSERT = 0, T_LAT_MISC, T_LAT_NORM, T_MF_INIT, T_MF_ZERO, T_MF_BLUR_SP,
     T_MF_BLUR_BI, T_MF_TILE, T_MF_EXPORT, T_SRG_LABEL, T_SRG_MERGE, T_SRG_FLAG, T_SRG_EMIT,
-    T_LOSS, T_WIRE, T_PREP, T_POST, T_ANNOT, T_MF_TILE_HY, T_KGRAD, T_COUNT
+    T_LOSS, T_WIRE, T_PREP, T_POST, T_ANNOT, T_MF_TILE_HY, T_KGRAD, T_FGRAD, T_COUNT
 };
 
 // ---- lattice.cu ----
-int lattice_build(Engine *e, Lattice &L, int B, const uint8_t *image_dev, cudaStream_t s);
+// feat ([B][5][N], bilateral lattice only): caller-given features in place of the image's; a key outside the packed
+// range sets bad[b] (the engine's error flag is left alone)
+int lattice_build(Engine *e, Lattice &L, int B, const uint8_t *image_dev, cudaStream_t s, const float *feat = nullptr,
+                  int *bad = nullptr);
 constexpr int kNoKey = 0x7F7F7F7F;  // renumbering key of no incidence yet (a byte pattern, for cudaMemset)
 constexpr int kRenumChunk = 4 * kThreads;  // bitmap words per renumbering chunk: 4 per thread of k_renum_scan
 long long renum_words(int ntiles, int dp1);  // bitmap words per image, a whole number of chunks
@@ -160,11 +163,17 @@ int meanfield_run(Engine *e, int B, const float *unary, int unary_layout, bool c
 int meanfield_run_train(Engine *e, int B, const float *unary, float *q_hist, const float *potts, const float *compat,
                         const dsrg_crf_params &p, cudaStream_t s);
 // grad_theta ([B][7], with the batch's image): the kernel-bandwidth gradient too, which needs the kg_* buffers
-// (ensure_kgrad)
+// (ensure_kgrad).  With caller-given bilateral features `feat` (the lattice built on them) grad_feat [B][5][N] gets
+// the per-pixel dL/df of the bilateral lattice instead, and grad_theta_sp, if given, [B][2] dL/dtheta_gamma; this
+// needs the kg_* buffers too
 int meanfield_backward(Engine *e, int B, const float *q_hist, const float *potts, const float *grad_q,
                        float *grad_unary, float *grad_potts, const float *compat, float *grad_compat,
                        const dsrg_crf_params &p, cudaStream_t s, float *grad_theta = nullptr,
-                       const uint8_t *image = nullptr);
+                       const uint8_t *image = nullptr, const float *feat = nullptr, float *grad_feat = nullptr,
+                       float *grad_theta_sp = nullptr);
+// NaN into every image b of p (reps slabs rep_stride apart, per_image floats per image) with bad[b] set
+void nan_images(Engine *e, const int *bad, float *p, int B, long long per_image, int reps, long long rep_stride,
+                cudaStream_t s);
 // ---- meanfield_wide.cu: label counts above DSRG_MAX_LABELS ----
 int meanfield_run_wide(Engine *e, int B, const float *unary, int unary_layout, bool clamp_inplace,
                        float *unary_rw, const dsrg_crf_params &p, cudaStream_t s);
@@ -213,6 +222,9 @@ struct Engine {
     // pixel [2][maxB][N], per-block sums [maxB][blocks][8], and two value buffers per lattice [rows][MP]
     float *kg_g = nullptr, *kg_csum = nullptr, *kg_part = nullptr;
     float *kg_sp[2] = {nullptr, nullptr}, *kg_bi[2] = {nullptr, nullptr};
+    // the feature passes' per-image key-range flags [maxB] (allocated by the first one) and that pass's batch
+    int *feat_bad = nullptr;
+    int feat_B = 0;
     int *hy_count = nullptr;   // their number (device-resident)
     // 1-channel buffers for the normalisation pass
     float *nvA = nullptr, *nvB = nullptr;
@@ -422,7 +434,8 @@ cudaError_t numa_host_alloc(void **p, size_t bytes, int device);
 // plain launches on the legacy default stream, inside somebody else's capture, while per-kernel profiling is on,
 // or if capture fails.  `body` issues the launches on `s` and returns a DSRG_* code.
 enum class PassKind : int { crf, crf_map, forward, crflayer, densecrf, post, crf_train, crf_backward, crf_train_compat,
-                            crf_backward_compat, crf_backward_theta, crf_backward_compat_theta };
+                            crf_backward_compat, crf_backward_theta, crf_backward_compat_theta, crf_train_feat,
+                            crf_backward_feat };
 struct GraphKey {
     std::string bytes;
     GraphKey() = default;

@@ -110,6 +110,8 @@ struct BuildArgs {
     uint64_t *hkeys;
     int32_t *hval, *aslot, *vcount, *vkey;
     int *err;
+    const float *feat;  // k_lattice_insert<kFeatLattice>: the caller's features [B][5][N]
+    int *bad;           // ... and its per-image key-range flags [B]
 };
 
 // A pixel's position in tile-major order (tiles.cu: tile index, then the pixel's thread index in the tile); the
@@ -123,43 +125,54 @@ __device__ __forceinline__ int tile_major_pos(int x, int y, int tile_w, int tile
 // ---------------------------------------------------------------------------------------------
 // Kernel 1: one thread per pixel (plus the phantom tail lanes): features -> elevate -> simplex ->
 // rank -> barycentric -> d+1 vertex keys -> hash insert.  Follows permutohedral.cpp:191-276.
+// D = kFeatLattice: the bilateral lattice (d = 5) on the caller's features (a.feat [B][5][N], taken as they are), and a
+// key outside the packed range flags the image in a.bad[b] instead of the engine's error flag.
 // ---------------------------------------------------------------------------------------------
+constexpr int kFeatLattice = -5;
+
 template <int D>
 __global__ void __launch_bounds__(kThreads) k_lattice_insert(BuildArgs a) {
+    constexpr bool FEAT = D == kFeatLattice;
+    constexpr int DIM = FEAT ? 5 : D;
     const int b = blockIdx.y;
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     const bool valid = i < a.N + a.P;
     const bool real = i < a.N;
 
-    float f[D];
+    float f[DIM];
 #pragma unroll
-    for (int j = 0; j < D; j++) f[j] = 0.0f;  // phantom lanes carry feature 0 (:196)
+    for (int j = 0; j < DIM; j++) f[j] = 0.0f;  // phantom lanes carry feature 0 (:196)
     int pos = a.ntiles * kTileThreads;
     if (real) {
         const int x = i % a.W, y = i / a.W;
         pos = tile_major_pos(x, y, a.tile_w, a.tiles_x);
-        lattice_features<D>(x, y, a.image, b, a.N, i, a.sigma, f);
+        if constexpr (FEAT) {
+#pragma unroll
+            for (int j = 0; j < DIM; j++) f[j] = __ldg(a.feat + ((size_t)b * DIM + j) * a.N + i);
+        } else {
+            lattice_features<DIM>(x, y, a.image, b, a.N, i, a.sigma, f);
+        }
     }
     // elevate, simplex, rank (simplex.cuh)
-    float el[D + 1], rem0[D + 1];
-    int rank[D + 1];
-    lattice_simplex<D>(f, a.scale, el, rem0, rank);
-    const float inv = __fdiv_rn(1.0f, (float)(D + 1));
+    float el[DIM + 1], rem0[DIM + 1];
+    int rank[DIM + 1];
+    lattice_simplex<DIM>(f, a.scale, el, rem0, rank);
+    const float inv = __fdiv_rn(1.0f, (float)(DIM + 1));
     // barycentric (:245-263), same accumulation order as the reference
-    float bc[D + 2];
+    float bc[DIM + 2];
 #pragma unroll
-    for (int q = 0; q <= D + 1; q++) bc[q] = 0.0f;
+    for (int q = 0; q <= DIM + 1; q++) bc[q] = 0.0f;
 #pragma unroll
-    for (int k = 0; k <= D; k++) {
+    for (int k = 0; k <= DIM; k++) {
         float v = __fmul_rn(__fsub_rn(el[k], rem0[k]), inv);
-        int p = D - rank[k];
+        int p = DIM - rank[k];
 #pragma unroll
-        for (int q = 0; q <= D + 1; q++) {
+        for (int q = 0; q <= DIM + 1; q++) {
             if (q == p) bc[q] = __fadd_rn(bc[q], v);
             if (q == p + 1) bc[q] = __fsub_rn(bc[q], v);
         }
     }
-    bc[0] = __fadd_rn(bc[0], __fadd_rn(1.0f, bc[D + 1]));
+    bc[0] = __fadd_rn(bc[0], __fadd_rn(1.0f, bc[DIM + 1]));
 
     // vertices (:268-275)
     uint64_t *keys = a.hkeys + (size_t)b * a.cap;
@@ -170,21 +183,21 @@ __global__ void __launch_bounds__(kThreads) k_lattice_insert(BuildArgs a) {
     const unsigned lane = threadIdx.x & 31;
     bool range_bad = false;
 #pragma unroll
-    for (int r = 0; r <= D; r++) {
-        int key[D];
+    for (int r = 0; r <= DIM; r++) {
+        int key[DIM];
 #pragma unroll
-        for (int k = 0; k < D; k++) {
-            int canon = (rank[k] <= D - r) ? r : r - (D + 1);  // canonical simplex (:171-176)
+        for (int k = 0; k < DIM; k++) {
+            int canon = (rank[k] <= DIM - r) ? r : r - (DIM + 1);  // canonical simplex (:171-176)
             key[k] = (int)rem0[k] + canon;
-            if (key[k] < KeyBits<D>::lo || key[k] > KeyBits<D>::hi) range_bad = true;
+            if (key[k] < KeyBits<DIM>::lo || key[k] > KeyBits<DIM>::hi) range_bad = true;
         }
-        uint64_t pk = pack_key<D>(key);
+        uint64_t pk = pack_key<DIM>(key);
         // neighbouring pixels mostly share vertices: one insert per distinct key per warp
         unsigned peers = __match_any_sync(0xffffffffu, valid ? pk : (kEmptyKey - 1 - lane));
         int leader = __ffs(peers) - 1;
         int id = 0;
         // the first incidence of the vertex among the lanes, for the renumbering key (vkey is kNoKey between builds)
-        const int kmin = __reduce_min_sync(peers, valid ? pos * (D + 1) + r : kNoKey);
+        const int kmin = __reduce_min_sync(peers, valid ? pos * (DIM + 1) + r : kNoKey);
         if (valid && (int)lane == leader) {
             const int slot = hash_insert(keys, hval, aslot, vcount, a.cap, pk);
             // the slot's owner publishes the vertex id right after winning the CAS; owners of the
@@ -197,12 +210,16 @@ __global__ void __launch_bounds__(kThreads) k_lattice_insert(BuildArgs a) {
         }
         id = __shfl_sync(0xffffffffu, id, leader);
         if (real) {
-            size_t at = ((size_t)b * (D + 1) + r) * a.N + i;
+            size_t at = ((size_t)b * (DIM + 1) + r) * a.N + i;
             a.off[at] = id + 1;  // local row (row 0 of every image is its zero row)
             a.bary[at] = bc[r];
         }
     }
-    if (valid && range_bad) *a.err = DSRG_E_KEYRANGE;
+    if constexpr (FEAT) {
+        if (valid && range_bad) a.bad[b] = 1;
+    } else {
+        if (valid && range_bad) *a.err = DSRG_E_KEYRANGE;
+    }
 }
 
 // rowbase[b] = first value row of image b (its zero row); rowbase[B] = total rows
@@ -420,7 +437,8 @@ k_norm_slice(const int32_t *off, const float *bary, const int32_t *rowbase, cons
 }
 
 template <int D>
-static int build_impl(Engine *e, Lattice &L, int nb, const uint8_t *image, cudaStream_t s) {
+static int build_impl(Engine *e, Lattice &L, int nb, const uint8_t *image, const float *feat, int *bad,
+                      cudaStream_t s) {
     BuildArgs a;
     a.N = L.N;
     a.P = L.P;
@@ -443,12 +461,19 @@ static int build_impl(Engine *e, Lattice &L, int nb, const uint8_t *image, cudaS
     a.vcount = L.vcount;
     a.vkey = L.vkey;
     a.err = e->dev_err;
+    a.feat = feat;
+    a.bad = bad;
     DSRG_CUDA_TRY(cudaMemsetAsync(L.vcount, 0, sizeof(int32_t) * nb, s));
     const long long nwords = renum_words(e->ntiles, D + 1);
     const int nchunks = (int)(nwords / kRenumChunk);
     DSRG_CUDA_TRY(cudaMemsetAsync(L.rn_words, 0, sizeof(uint2) * nb * nwords, s));
     dim3 gp(cdiv(L.N + L.P, kThreads), nb);
-    DSRG_LAUNCH(e, T_LAT_INSERT, s, k_lattice_insert<D><<<gp, kThreads, 0, s>>>(a));
+    if (feat) {
+        DSRG_CUDA_TRY(cudaMemsetAsync(bad, 0, sizeof(int) * nb, s));
+        DSRG_LAUNCH(e, T_LAT_INSERT, s, k_lattice_insert<kFeatLattice><<<gp, kThreads, 0, s>>>(a));
+    } else {
+        DSRG_LAUNCH(e, T_LAT_INSERT, s, k_lattice_insert<D><<<gp, kThreads, 0, s>>>(a));
+    }
     DSRG_LAUNCH(e, T_LAT_MISC, s, k_rowbase<<<1, 32, 0, s>>>(L.vcount, L.rowbase, L.shared ? e->maxB : nb, L.shared));
     dim3 gv(2 * e->sm_count, nb);
     DSRG_LAUNCH(e, T_LAT_MISC, s, k_renum_mark<<<gv, kThreads, 0, s>>>(L.vcount, L.vkey, L.rn_words, L.capv, nwords));
@@ -497,10 +522,13 @@ int lattice_idle(Engine *e, const Lattice &L, long long *counts) {
     return DSRG_OK;
 }
 
-// Build the lattices of `B` images (or the single shared one), then their norm vectors.
-int lattice_build(Engine *e, Lattice &L, int B, const uint8_t *image_dev, cudaStream_t s) {
+// Build the lattices of `B` images (or the single shared one), then their norm vectors.  `feat` ([B][5][N], the
+// bilateral lattice only): the caller's features in place of the image's, with per-image range flags in `bad` [B].
+int lattice_build(Engine *e, Lattice &L, int B, const uint8_t *image_dev, cudaStream_t s, const float *feat,
+                  int *bad) {
     const int nb = L.shared ? 1 : B;
-    int rc = (L.d == 2) ? build_impl<2>(e, L, nb, image_dev, s) : build_impl<5>(e, L, nb, image_dev, s);
+    int rc = (L.d == 2) ? build_impl<2>(e, L, nb, image_dev, nullptr, nullptr, s)
+                        : build_impl<5>(e, L, nb, image_dev, feat, bad, s);
     if (rc) return rc;
     // norm pass on nb structures; value rows of the norm pass use the per-structure packing,
     // which for the shared lattice is simply image 0's rows [0, V+1).

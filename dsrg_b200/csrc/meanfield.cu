@@ -1096,13 +1096,21 @@ struct KgArgs {
     int M, N, W, nblk;
 };
 
-// per-incidence s_r of one lattice -> the pixel's dL/dp over that lattice's features (added to dp), scaled by sign
-template <int D>
+// per-incidence s_r of one lattice -> the pixel's dL/dp over that lattice's features (added to dp), scaled by sign.
+// FEAT: the features are the caller's (feat [B][D][N]), and the pixel's dL/df also goes to gfeat [B][D][N] (written
+// when `first`, else added).
+template <int D, bool FEAT = false>
 __device__ __forceinline__ void kg_features(const KgLat &L, int x, int y, const uint8_t *image, int b, int N,
-                                            int i, const float *s, float sign, float *dp) {
+                                            int i, const float *s, float sign, float *dp, const float *feat = nullptr,
+                                            float *gfeat = nullptr, bool first = false) {
     float f[D], el[D + 1], rem0[D + 1];
     int rank[D + 1];
-    lattice_features<D>(x, y, image, b, N, i, L.sigma, f);
+    if constexpr (FEAT) {
+#pragma unroll
+        for (int j = 0; j < D; j++) f[j] = __ldg(feat + ((size_t)b * D + j) * N + i);
+    } else {
+        lattice_features<D>(x, y, image, b, N, i, L.sigma, f);
+    }
     lattice_simplex<D>(f, L.scale, el, rem0, rank);
     const float c = sign * L.alpha / (float)(D + 1);
     float gel[D + 1];
@@ -1120,7 +1128,12 @@ __device__ __forceinline__ void kg_features(const KgLat &L, int x, int y, const 
     float sm = gel[0];
 #pragma unroll
     for (int j = 1; j <= D; j++) {
-        dp[j - 1] = fmaf(f[j - 1], L.scale[j - 1] * (sm - (float)j * gel[j]), dp[j - 1]);
+        const float df = L.scale[j - 1] * (sm - (float)j * gel[j]);   // dL/df_{j-1}
+        dp[j - 1] = fmaf(f[j - 1], df, dp[j - 1]);
+        if constexpr (FEAT) {
+            float *o = gfeat + ((size_t)b * D + j - 1) * N + i;
+            *o = first ? df : *o + df;
+        }
         sm += gel[j];
     }
 }
@@ -1198,11 +1211,11 @@ k_kg_splatq(KgArgs a, const float *Qt, float4 *vsp, float4 *vbi) {
 }
 
 // iteration t's lattice terms: g = g_{t+1}, Qt = Q_t, vy_* = B S(n Q_t), vg_* = B^T S(n g_{t+1}); COMPAT: a.potts is
-// {mu_bi, mu_sp} ([2][M][M])
-template <int MP, bool COMPAT>
-__global__ void __launch_bounds__(kThreads)
-k_kg_pass(KgArgs a, const float *g, const float *Qt, const float4 *vy_sp, const float4 *vy_bi, const float4 *vg_sp,
-          const float4 *vg_bi, int first) {
+// {mu_bi, mu_sp} ([2][M][M]); FEAT: the bilateral features from feat, their per-pixel dL/df to gfeat (kg_features)
+template <int MP, bool COMPAT, bool FEAT>
+__device__ __forceinline__ void kg_pass(const KgArgs &a, const float *g, const float *Qt, const float4 *vy_sp,
+                                        const float4 *vy_bi, const float4 *vg_sp, const float4 *vg_bi, int first,
+                                        const float *feat, float *gfeat) {
     __shared__ float mus[COMPAT ? 2 * MP * MP : 1];
     const int b = blockIdx.y, i = blockIdx.x * kThreads + threadIdx.x;
     const bool in = i < a.N;
@@ -1249,7 +1262,7 @@ k_kg_pass(KgArgs a, const float *g, const float *Qt, const float4 *vy_sp, const 
                     kg_features<2>(a.sp, x, y, a.image, b, a.N, i, s, 1.0f, dp + 5);
                 } else {
                     c_bi = kg_incidences<MP, 5>(a.bi, b, i, a.N, xv, uv, 1.0f, vy_bi, vg_bi, s);
-                    kg_features<5>(a.bi, x, y, a.image, b, a.N, i, s, 1.0f, dp);
+                    kg_features<5, FEAT>(a.bi, x, y, a.image, b, a.N, i, s, 1.0f, dp, feat, gfeat, first != 0);
                 }
             }
         } else {
@@ -1257,12 +1270,27 @@ k_kg_pass(KgArgs a, const float *g, const float *Qt, const float4 *vy_sp, const 
             c_sp = kg_incidences<MP, 2>(a.sp, b, i, a.N, gv, qv, w2, vy_sp, vg_sp, s);
             kg_features<2>(a.sp, x, y, a.image, b, a.N, i, s, 1.0f, dp + 5);
             c_bi = kg_incidences<MP, 5>(a.bi, b, i, a.N, gv, qv, w1, vy_bi, vg_bi, s);
-            kg_features<5>(a.bi, x, y, a.image, b, a.N, i, s, 1.0f, dp);
+            kg_features<5, FEAT>(a.bi, x, y, a.image, b, a.N, i, s, 1.0f, dp, feat, gfeat, first != 0);
         }
         *csum_sp = first ? c_sp : *csum_sp + c_sp;
         *csum_bi = first ? c_bi : *csum_bi + c_bi;
     }
     kg_block_sum(a, b, dp, first != 0);
+}
+
+template <int MP, bool COMPAT>
+__global__ void __launch_bounds__(kThreads)
+k_kg_pass(KgArgs a, const float *g, const float *Qt, const float4 *vy_sp, const float4 *vy_bi, const float4 *vg_sp,
+          const float4 *vg_bi, int first) {
+    kg_pass<MP, COMPAT, false>(a, g, Qt, vy_sp, vy_bi, vg_sp, vg_bi, first, nullptr, nullptr);
+}
+
+// k_kg_pass on caller-given bilateral features: feat [B][5][N] in, the pass's dL/df out to gfeat [B][5][N]
+template <int MP, bool COMPAT>
+__global__ void __launch_bounds__(kThreads)
+k_kgf_pass(KgArgs a, const float *g, const float *Qt, const float4 *vy_sp, const float4 *vy_bi, const float4 *vg_sp,
+           const float4 *vg_bi, int first, const float *feat, float *gfeat) {
+    kg_pass<MP, COMPAT, true>(a, g, Qt, vy_sp, vy_bi, vg_sp, vg_bi, first, feat, gfeat);
 }
 
 // the normalisation term's splats, one channel each in 4-wide rows: bary into fw_* (channel 0, blurred in K's order)
@@ -1288,8 +1316,9 @@ k_kg_splat1(KgArgs a, float *fw_sp, float *rv_sp, float *fw_bi, float *rv_bi) {
 }
 
 // -d^K <c, K 1> = -(c . B S 1 + 1 . B^T S c) at each incidence, rotated to the features
-__global__ void __launch_bounds__(kThreads)
-k_kg_norm(KgArgs a, const float4 *v1_sp, const float4 *vc_sp, const float4 *v1_bi, const float4 *vc_bi) {
+template <bool FEAT>
+__device__ __forceinline__ void kg_norm(const KgArgs &a, const float4 *v1_sp, const float4 *vc_sp,
+                                        const float4 *v1_bi, const float4 *vc_bi, const float *feat, float *gfeat) {
     const int b = blockIdx.y, i = blockIdx.x * kThreads + threadIdx.x;
     float dp[7];
 #pragma unroll
@@ -1312,12 +1341,24 @@ k_kg_norm(KgArgs a, const float4 *v1_sp, const float4 *vc_sp, const float4 *v1_b
                 }
             }
             if (k)
-                kg_features<5>(L, x, y, a.image, b, a.N, i, s, -1.0f, dp);
+                kg_features<5, FEAT>(L, x, y, a.image, b, a.N, i, s, -1.0f, dp, feat, gfeat, false);
             else
                 kg_features<2>(L, x, y, a.image, b, a.N, i, s, -1.0f, dp + 5);
         }
     }
     kg_block_sum(a, b, dp, false);
+}
+
+__global__ void __launch_bounds__(kThreads)
+k_kg_norm(KgArgs a, const float4 *v1_sp, const float4 *vc_sp, const float4 *v1_bi, const float4 *vc_bi) {
+    kg_norm<false>(a, v1_sp, vc_sp, v1_bi, vc_bi, nullptr, nullptr);
+}
+
+// k_kg_norm on caller-given bilateral features: adds the normalisation term's dL/df to gfeat
+__global__ void __launch_bounds__(kThreads)
+k_kgf_norm(KgArgs a, const float4 *v1_sp, const float4 *vc_sp, const float4 *v1_bi, const float4 *vc_bi,
+           const float *feat, float *gfeat) {
+    kg_norm<true>(a, v1_sp, vc_sp, v1_bi, vc_bi, feat, gfeat);
 }
 
 // per image: the blocks' sums in block order -> grad_theta[b] = -dL/dp / theta (theta order)
@@ -1328,6 +1369,25 @@ __global__ void k_kg_reduce(const float *part, int nblk, float *out, KgArgs a) {
     for (int i = 0; i < nblk; i++) acc += part[((size_t)b * nblk + i) * 8 + k];
     const float th = k < 5 ? a.bi.sigma[k] : a.sp.sigma[k - 5];
     out[(size_t)b * 7 + k] = -acc / th;
+}
+
+// k_kg_reduce for the spatial bandwidths alone (the feature backward): grad_theta_sp[b] = -dL/dp / theta_gamma
+__global__ void k_kgf_reduce_sp(const float *part, int nblk, float *out, KgArgs a) {
+    const int b = blockIdx.x, k = threadIdx.x;
+    if (k >= 2) return;
+    float acc = 0.0f;
+    for (int i = 0; i < nblk; i++) acc += part[((size_t)b * nblk + i) * 8 + 5 + k];
+    out[(size_t)b * 2 + k] = -acc / a.sp.sigma[k];
+}
+
+// the NaN policy of the feature passes (nan_images): every value of a flagged image's slabs becomes NaN
+__global__ void __launch_bounds__(kThreads)
+k_nan_images(const int *bad, float *p, long long per_image, long long rep_stride) {
+    const int b = blockIdx.y, r = blockIdx.z;
+    if (!bad[b]) return;
+    float *q = p + r * rep_stride + b * per_image;
+    for (long long k = blockIdx.x * (long long)kThreads + threadIdx.x; k < per_image; k += (long long)gridDim.x * kThreads)
+        q[k] = __int_as_float(0x7fc00000);
 }
 
 // zero the splat targets of both lattices for the B images of the pass (row counts are device-resident)
@@ -1708,17 +1768,32 @@ static KgLat kg_lat(const Lattice &L) {
 
 // Iteration t's kernel-bandwidth terms (before k_mf_tile_bwd of iteration t overwrites e->kg_g = g_{t+1}): splat
 // n Q_t, blur it in K's order into the kernel-gradient buffers, and k_kg_pass against spX / biX = B^T S(n g_{t+1}).
+// With caller-given bilateral features (`feat`) k_kgf_pass, which also writes (first) or adds the per-pixel dL/df to
+// gfeat; every launch is timed under `tag`.
 template <int MP>
 static void kg_iter(Engine *e, const KgArgs &ka, bool compat, int B, const float *qt, const float *spX,
-                    const float *biX, bool first, int bgrid, cudaStream_t s) {
+                    const float *biX, bool first, int bgrid, cudaStream_t s, const float *feat, float *gfeat, int tag) {
     const dim3 gp(ka.nblk, B);
-    DSRG_LAUNCH(e, T_KGRAD, s,
+    DSRG_LAUNCH(e, tag, s,
                 k_mf_zero<MP><<<bgrid, kThreads, 0, s>>>((float4 *)e->kg_sp[0], e->sp.rowbase, (float4 *)e->kg_bi[0],
                                                          e->bi.rowbase, B));
-    DSRG_LAUNCH(e, T_KGRAD, s,
+    DSRG_LAUNCH(e, tag, s,
                 k_kg_splatq<MP><<<gp, kThreads, 0, s>>>(ka, qt, (float4 *)e->kg_sp[0], (float4 *)e->kg_bi[0]));
-    const float *vy_sp = blur_all<MP>(e, e->sp, e->kg_sp[0], e->kg_sp[1], nullptr, B, T_KGRAD, bgrid, s);
-    const float *vy_bi = blur_all<MP>(e, e->bi, e->kg_bi[0], e->kg_bi[1], nullptr, B, T_KGRAD, bgrid, s);
+    const float *vy_sp = blur_all<MP>(e, e->sp, e->kg_sp[0], e->kg_sp[1], nullptr, B, tag, bgrid, s);
+    const float *vy_bi = blur_all<MP>(e, e->bi, e->kg_bi[0], e->kg_bi[1], nullptr, B, tag, bgrid, s);
+    if (feat) {
+        if (compat)
+            DSRG_LAUNCH(e, tag, s,
+                        (k_kgf_pass<MP, true><<<gp, kThreads, 0, s>>>(ka, e->kg_g, qt, (const float4 *)vy_sp,
+                                                                     (const float4 *)vy_bi, (const float4 *)spX,
+                                                                     (const float4 *)biX, first, feat, gfeat)));
+        else
+            DSRG_LAUNCH(e, tag, s,
+                        (k_kgf_pass<MP, false><<<gp, kThreads, 0, s>>>(ka, e->kg_g, qt, (const float4 *)vy_sp,
+                                                                      (const float4 *)vy_bi, (const float4 *)spX,
+                                                                      (const float4 *)biX, first, feat, gfeat)));
+        return;
+    }
     if (compat)
         DSRG_LAUNCH(e, T_KGRAD, s,
                     (k_kg_pass<MP, true><<<gp, kThreads, 0, s>>>(ka, e->kg_g, qt, (const float4 *)vy_sp,
@@ -1731,35 +1806,47 @@ static void kg_iter(Engine *e, const KgArgs &ka, bool compat, int B, const float
                                                                  (const float4 *)biX, first)));
 }
 
-// (every launch of the kernel-bandwidth passes is timed under T_KGRAD)
+// (every launch of the kernel-bandwidth passes is timed under T_KGRAD, of the feature passes under T_FGRAD)
 // After the loop: the normalisation term from the summed c, then the per-image sums.  The mean-field buffers are free
 // by now: spA / biA take the reverse-blurred splat of c, the kernel-gradient buffers the forward-blurred one of ones.
-static void kg_finish(Engine *e, const KgArgs &ka, int B, float *g_theta, int bgrid, cudaStream_t s) {
+// With `feat`: k_kgf_norm adds the term's dL/df to gfeat, and only the spatial sums are reduced (to g_theta [B][2],
+// when given).
+static void kg_finish(Engine *e, const KgArgs &ka, int B, float *g_theta, int bgrid, cudaStream_t s,
+                      const float *feat, float *gfeat, int tag) {
     const dim3 gp(ka.nblk, B);
-    DSRG_LAUNCH(e, T_KGRAD, s,
+    DSRG_LAUNCH(e, tag, s,
                 k_mf_zero<4><<<bgrid, kThreads, 0, s>>>((float4 *)e->kg_sp[0], e->sp.rowbase, (float4 *)e->kg_bi[0],
                                                         e->bi.rowbase, B));
-    DSRG_LAUNCH(e, T_KGRAD, s,
+    DSRG_LAUNCH(e, tag, s,
                 k_mf_zero<4><<<bgrid, kThreads, 0, s>>>((float4 *)e->spA, e->sp.rowbase, (float4 *)e->biA,
                                                         e->bi.rowbase, B));
-    DSRG_LAUNCH(e, T_KGRAD, s, k_kg_splat1<<<gp, kThreads, 0, s>>>(ka, e->kg_sp[0], e->spA, e->kg_bi[0], e->biA));
-    const float *v1_sp = blur_all<4>(e, e->sp, e->kg_sp[0], e->kg_sp[1], nullptr, B, T_KGRAD, bgrid, s);
-    const float *v1_bi = blur_all<4>(e, e->bi, e->kg_bi[0], e->kg_bi[1], nullptr, B, T_KGRAD, bgrid, s);
-    const float *vc_sp = blur_all<4>(e, e->sp, e->spA, e->spB, nullptr, B, T_KGRAD, bgrid, s, true);
-    const float *vc_bi = blur_all<4>(e, e->bi, e->biA, e->biB, nullptr, B, T_KGRAD, bgrid, s, true);
-    DSRG_LAUNCH(e, T_KGRAD, s,
+    DSRG_LAUNCH(e, tag, s, k_kg_splat1<<<gp, kThreads, 0, s>>>(ka, e->kg_sp[0], e->spA, e->kg_bi[0], e->biA));
+    const float *v1_sp = blur_all<4>(e, e->sp, e->kg_sp[0], e->kg_sp[1], nullptr, B, tag, bgrid, s);
+    const float *v1_bi = blur_all<4>(e, e->bi, e->kg_bi[0], e->kg_bi[1], nullptr, B, tag, bgrid, s);
+    const float *vc_sp = blur_all<4>(e, e->sp, e->spA, e->spB, nullptr, B, tag, bgrid, s, true);
+    const float *vc_bi = blur_all<4>(e, e->bi, e->biA, e->biB, nullptr, B, tag, bgrid, s, true);
+    if (feat) {
+        DSRG_LAUNCH(e, tag, s,
+                    k_kgf_norm<<<gp, kThreads, 0, s>>>(ka, (const float4 *)v1_sp, (const float4 *)vc_sp,
+                                                       (const float4 *)v1_bi, (const float4 *)vc_bi, feat, gfeat));
+        if (g_theta) DSRG_LAUNCH(e, tag, s, k_kgf_reduce_sp<<<B, 32, 0, s>>>(ka.part, ka.nblk, g_theta, ka));
+        return;
+    }
+    DSRG_LAUNCH(e, tag, s,
                 k_kg_norm<<<gp, kThreads, 0, s>>>(ka, (const float4 *)v1_sp, (const float4 *)vc_sp,
                                                   (const float4 *)v1_bi, (const float4 *)vc_bi));
-    DSRG_LAUNCH(e, T_KGRAD, s, k_kg_reduce<<<B, 32, 0, s>>>(ka.part, ka.nblk, g_theta, ka));
+    DSRG_LAUNCH(e, tag, s, k_kg_reduce<<<B, 32, 0, s>>>(ka.part, ka.nblk, g_theta, ka));
 }
 
 template <int MP>
 static int bwd_impl(Engine *e, int B, const float *q_hist, const float *potts, const float *G, float *gU,
                     float *g_potts, const float *compat, float *g_compat, float *g_theta, const uint8_t *image,
-                    const dsrg_crf_params &p, cudaStream_t s) {
+                    const float *feat, float *g_feat, float *g_theta_sp, const dsrg_crf_params &p, cudaStream_t s) {
     const int M = e->M, N = e->N, T = p.n_iters;
     const size_t slab = (size_t)B * M * N;
     if (T == 0) {
+        if (g_feat) DSRG_CUDA_TRY(cudaMemsetAsync(g_feat, 0, sizeof(float) * 5 * N * B, s));
+        if (g_theta_sp) DSRG_CUDA_TRY(cudaMemsetAsync(g_theta_sp, 0, sizeof(float) * 2 * B, s));
         DSRG_LAUNCH(e, T_MF_INIT, s,
                     k_mf_softmax_vjp<<<dim3(cdiv(N, kThreads), B), kThreads, 0, s>>>(G, q_hist, gU, M, N));
         if (g_potts) DSRG_CUDA_TRY(cudaMemsetAsync(g_potts, 0, sizeof(float) * 2 * B, s));
@@ -1792,9 +1879,13 @@ static int bwd_impl(Engine *e, int B, const float *q_hist, const float *potts, c
     float *biX = e->biA, *biY = e->biB, *biZ = e->biC;
     DSRG_LAUNCH(e, T_MF_ZERO, s,
                 k_mf_zero<MP><<<bgrid, kThreads, 0, s>>>((float4 *)spY, e->sp.rowbase, (float4 *)biY, e->bi.rowbase, B));
-    // the kernel-bandwidth gradient (g_theta): g_t stored by the launches (MODE_GSTORE), k_kg_pass per iteration
+    // the kernel-bandwidth gradient (g_theta): g_t stored by the launches (MODE_GSTORE), k_kg_pass per iteration;
+    // the feature gradient (g_feat) runs the same flow on the kgf kernels and keeps g_theta_sp for the spatial sums
+    if (g_feat) g_theta = g_theta_sp;
+    const bool kg = g_theta || g_feat;
+    const int kg_tag = g_feat ? T_FGRAD : T_KGRAD;
     KgArgs ka{};
-    if (g_theta) {
+    if (kg) {
         ka.sp = kg_lat(e->sp);
         ka.bi = kg_lat(e->bi);
         ka.image = image;
@@ -1820,13 +1911,14 @@ static int bwd_impl(Engine *e, int B, const float *q_hist, const float *potts, c
     for (int it = T; it >= 0; it--) {
         const TileLat vsp = make_tile_view(e->sp, spX, spY), vbi = make_tile_view(e->bi, biX, biY);
         const float *qt = q_hist + (size_t)it * slab;
-        if (g_theta && it < T) kg_iter<MP>(e, ka, compat != nullptr, B, qt, spX, biX, it == T - 1, bgrid, s);
+        if (kg && it < T)
+            kg_iter<MP>(e, ka, compat != nullptr, B, qt, spX, biX, it == T - 1, bgrid, s, feat, g_feat, kg_tag);
         if (compat) {
             if (it == 0) {
                 DSRG_BWD_LAUNCH_COMPAT(MODE_LAST);
                 break;
             }
-            if (g_theta) {
+            if (kg) {
                 if (it == T)
                     DSRG_BWD_LAUNCH_COMPAT(MODE_FIRST | MODE_GSTORE);
                 else
@@ -1839,7 +1931,7 @@ static int bwd_impl(Engine *e, int B, const float *q_hist, const float *potts, c
         } else if (it == 0) {
             DSRG_BWD_LAUNCH(MODE_LAST);
             break;
-        } else if (g_theta) {
+        } else if (kg) {
             if (it == T)
                 DSRG_BWD_LAUNCH(MODE_FIRST | MODE_GSTORE);
             else
@@ -1867,7 +1959,7 @@ static int bwd_impl(Engine *e, int B, const float *q_hist, const float *potts, c
     }
     if (g_potts)
         DSRG_LAUNCH(e, T_MF_EXPORT, s, k_mf_potts_reduce<<<B, kThreads, 0, s>>>(e->potts_part, g_potts, e->ntiles));
-    if (g_theta) kg_finish(e, ka, B, g_theta, bgrid, s);
+    if (kg) kg_finish(e, ka, B, g_theta, bgrid, s, feat, g_feat, kg_tag);
     DSRG_CUDA_TRY(cudaGetLastError());
     return DSRG_OK;
 }
@@ -1886,17 +1978,25 @@ int meanfield_run_train(Engine *e, int B, const float *unary, float *q_hist, con
 
 int meanfield_backward(Engine *e, int B, const float *q_hist, const float *potts, const float *grad_q,
                        float *grad_unary, float *grad_potts, const float *compat, float *grad_compat,
-                       const dsrg_crf_params &p, cudaStream_t s, float *grad_theta, const uint8_t *image) {
+                       const dsrg_crf_params &p, cudaStream_t s, float *grad_theta, const uint8_t *image,
+                       const float *feat, float *grad_feat, float *grad_theta_sp) {
     switch (e->MP) {
 #define DSRG_CASE(MPV)                                                                                        \
     case MPV:                                                                                                 \
         return bwd_impl<MPV>(e, B, q_hist, potts, grad_q, grad_unary, grad_potts, compat, grad_compat, grad_theta, \
-                             image, p, s);
+                             image, feat, grad_feat, grad_theta_sp, p, s);
         DSRG_CASE(4) DSRG_CASE(8) DSRG_CASE(12) DSRG_CASE(16) DSRG_CASE(20) DSRG_CASE(24) DSRG_CASE(28) DSRG_CASE(32)
 #undef DSRG_CASE
     }
     set_error("unsupported label count %d", e->M);
     return DSRG_E_INVALID;
+}
+
+void nan_images(Engine *e, const int *bad, float *p, int B, long long per_image, int reps, long long rep_stride,
+                cudaStream_t s) {
+    const int nblk = cdiv(per_image, kThreads);
+    const dim3 gp(nblk < 64 ? nblk : 64, B, reps);
+    DSRG_LAUNCH(e, T_FGRAD, s, k_nan_images<<<gp, kThreads, 0, s>>>(bad, p, per_image, rep_stride));
 }
 
 int meanfield_run(Engine *e, int B, const float *unary, int unary_layout, bool clamp_inplace,

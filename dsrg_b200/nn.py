@@ -479,6 +479,98 @@ class _DenseCrfTheta(torch.autograd.Function):
         return grad_u, None, gw1, gw2, gc, out[0], out[1], None
 
 
+def _potts_tensor(w1, w2, ref):
+    """The device {w1, w2} the kernels read in place of params' weights (a None one is CRF()'s), or None for both."""
+    if w1 is None and w2 is None:
+        return None
+    potts = torch.empty(2, dtype=torch.float32, device=ref.device)
+    for i, (w, d) in enumerate(zip((w1, w2), _POTTS_DEFAULT)):
+        if w is None:
+            potts[i].fill_(d)
+        else:
+            potts[i].copy_(w.detach())
+    return potts
+
+
+class _DenseCrfFeat(torch.autograd.Function):
+    """dense_crf with caller-given bilateral features: features (N, 5, H, W) float32 beside the Potts weights (w1, w2)
+    or the matrices (compat (2, M, M) {mu_bi, mu_sp}), and an optional learnable theta_sp; params carries the spatial
+    sigmas.  Nothing is read on the host."""
+
+    @staticmethod
+    @_fwd
+    def forward(ctx, unary, features, w1, w2, compat, theta_sp, params):
+        eng = _engine_for(unary)
+        maxiter = params.n_iters
+        q_hist = torch.empty((maxiter + 1,) + tuple(unary.shape), dtype=torch.float32, device=unary.device)
+        potts = _potts_tensor(w1, w2, unary) if compat is None else None
+        eng.crf_forward_train_feat_dev(unary, features, params, q_hist, potts=potts, compat=compat,
+                                       stream=_stream(unary))
+        ctx.save_for_backward(q_hist, features, potts, compat)
+        ctx.params = params
+        ctx.theta_sp = None if theta_sp is None else (theta_sp.device, theta_sp.dtype)
+        return q_hist[maxiter].clone()
+
+    @staticmethod
+    @_bwd
+    def backward(ctx, g):
+        q_hist, features, potts, compat = ctx.saved_tensors
+        B, dev = q_hist.shape[1], q_hist.device
+        need = ctx.needs_input_grad
+        grad_u = torch.empty(q_hist.shape[1:], dtype=torch.float32, device=dev)
+        grad_f = torch.empty_like(features)
+        grad_potts = grad_c = grad_tsp = None
+        if potts is not None and (need[2] or need[3]):
+            grad_potts = torch.empty((B, 2), dtype=torch.float32, device=dev)
+        if compat is not None and need[4]:
+            M = compat.shape[-1]
+            grad_c = torch.empty((B, 2, M, M), dtype=torch.float32, device=dev)
+        if ctx.theta_sp is not None and need[5]:
+            grad_tsp = torch.empty((B, 2), dtype=torch.float32, device=dev)
+        _engine_for(grad_u).crf_backward_feat_dev(q_hist, features, ctx.params, g.contiguous(), grad_u, grad_f,
+                                                  potts=potts, compat=compat, grad_potts=grad_potts,
+                                                  grad_compat=grad_c, grad_theta_sp=grad_tsp, stream=_stream(grad_u))
+        gw1 = grad_potts[:, 0].sum() if grad_potts is not None and need[2] else None
+        gw2 = grad_potts[:, 1].sum() if grad_potts is not None and need[3] else None
+        gc = None if grad_c is None else grad_c.sum(0)
+        gt = None if grad_tsp is None else grad_tsp.sum(0).to(ctx.theta_sp[0], ctx.theta_sp[1])
+        return grad_u, grad_f if need[1] else None, gw1, gw2, gc, gt, None
+
+
+def _features(t, ref):
+    """The bilateral features (N, 5, H, W) float32 on ref's device, made contiguous."""
+    N, _, H, W = ref.shape
+    if (not isinstance(t, torch.Tensor) or t.dtype != torch.float32 or tuple(t.shape) != (N, 5, H, W)
+            or t.device != ref.device):
+        raise ValueError("features_bi must be a (%d, 5, %d, %d) float32 tensor on %s (got %r)"
+                         % (N, H, W, ref.device,
+                            t if not isinstance(t, torch.Tensor) else (t.dtype, tuple(t.shape), t.device)))
+    return t.contiguous()
+
+
+def _dense_crf_feat(u, image, features_bi, scale_factor, color_factor, maxiter, w1, w2, compat_bi, compat_sp,
+                    theta_bi, theta_sp):
+    """dense_crf's path with caller-given bilateral features; every check before the first launch."""
+    if image is not None:
+        raise ValueError("image is not used when features_bi is given: pass None")
+    if theta_bi is not None:
+        raise ValueError("theta_bi and features_bi are two forms of the bilateral features: give one of them")
+    f = _features(features_bi, u)
+    th_sp = _theta_values(theta_sp, "theta_sp", 2, u)
+    _cuda(u, "unary")
+    w1, w2 = _potts_weight(w1, "w1", u), _potts_weight(w2, "w2", u)
+    if int(maxiter) < 0:
+        raise ValueError("maxiter must be >= 0 (got %d)" % maxiter)
+    params = api.crf_params(float(scale_factor), float(color_factor), int(maxiter))
+    if th_sp is not None:
+        params.theta_gamma_x, params.theta_gamma_y = th_sp
+    compat = None
+    if compat_bi is not None or compat_sp is not None:
+        compat = _compat_stack(u, u.shape[1], w1, w2, compat_bi, compat_sp)
+        w1 = w2 = None
+    return _DenseCrfFeat.apply(u, f, w1, w2, compat, theta_sp, params)
+
+
 def _theta_values(theta, name, n, ref):
     """A learnable bandwidth vector's values as floats (one synchronising copy for a CUDA tensor)."""
     if theta is None:
@@ -509,7 +601,7 @@ def _compat_matrix(mu, name, ref, M):
 
 
 def dense_crf(unary, image, scale_factor=1.0, color_factor=13, maxiter=10, w1=None, w2=None, compat_bi=None,
-              compat_sp=None, theta_bi=None, theta_sp=None):
+              compat_sp=None, theta_bi=None, theta_sp=None, features_bi=None):
     """The dense CRF of CRF() (CRF/krahenbuhl2013/CRF.py:4-37) as a differentiable layer: unary (N, M, H, W) float32,
     M <= 32, the values CRF(image, unary) takes (energy = -unary); image (N, H, W, 3) uint8 at the map size ->
     marginals (N, M, H, W) after `maxiter` mean-field iterations.  The backward is the exact gradient of the
@@ -530,13 +622,27 @@ def dense_crf(unary, image, scale_factor=1.0, color_factor=13, maxiter=10, w1=No
     exact derivative of the function the device computes with every pixel's simplex held, summed over the batch and
     returned on the tensor's own device and dtype; it works with the Potts weights and with the matrices.  The
     lattice build takes the sigmas as host values, so the forward reads a given theta on the host: one synchronising
-    copy for a CUDA tensor, which is why a given theta is refused inside CUDA-graph capture."""
+    copy for a CUDA tensor, which is why a given theta is refused inside CUDA-graph capture.
+
+    features_bi (N, 5, H, W) float32 on unary's device: the bilateral kernel's features, in place of
+    (x/theta_alpha_x, y/theta_alpha_y, r/theta_beta_r, g/theta_beta_g, b/theta_beta_b) of an image, which must then be
+    None (theta_bi too).  The lattice is built on the given values as they are; the spatial kernel keeps the sigmas of
+    scale_factor (or theta_sp).  The gradient to features_bi is dL/df per pixel, exact with every pixel's simplex held,
+    so a learned transform of any guidance (the reference's FULL_KERNEL is f = P @ raw) trains through autograd.  The
+    features are never read on the host: without theta_sp a step can be captured in a CUDA graph.  Keep every feature
+    within +-150 (the CRF does not change when a channel is shifted, so centre them): an image whose lattice keys leave
+    the packed range gets NaN marginals and gradients (Engine.feature_range_flags names it)."""
     if torch.is_autocast_enabled("cuda"):   # what custom_fwd(cast_inputs=float32) does, before the checks
         unary = unary.float() if isinstance(unary, torch.Tensor) and unary.is_floating_point() else unary
+        if isinstance(features_bi, torch.Tensor) and features_bi.is_floating_point():
+            features_bi = features_bi.float()
     u = _maps(unary, "unary")
     N, M, H, W = u.shape
     if M > FUSED_LABELS:
         raise ValueError("dense_crf supports at most %d labels (got %d)" % (FUSED_LABELS, M))
+    if features_bi is not None:
+        return _dense_crf_feat(u, image, features_bi, scale_factor, color_factor, maxiter, w1, w2, compat_bi,
+                               compat_sp, theta_bi, theta_sp)
     if (not isinstance(image, torch.Tensor) or image.dtype != torch.uint8 or tuple(image.shape) != (N, H, W, 3)
             or image.device != u.device):
         raise ValueError("image must be a (%d, %d, %d, 3) uint8 tensor on %s" % (N, H, W, u.device))

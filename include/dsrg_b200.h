@@ -197,6 +197,37 @@ int dsrg_crf_backward_compat_theta_dev(dsrg_engine *e, const float *q_hist_dev, 
                                        const dsrg_crf_params *params, const float *compat_dev,
                                        const float *grad_q_dev, float *grad_unary_dev, float *grad_compat_dev,
                                        float *grad_theta_dev, void *stream);
+/*
+ * The training forward and its backward with caller-given bilateral features (the reference's
+ * addPairwiseEnergy(features, PottsCompatibility(w1) or MatrixCompatibility, DIAG_KERNEL, NORMALIZE_SYMMETRIC) at
+ * p = 1): features_dev [B][5][H][W] float32 replaces (x/theta_alpha_x, y/theta_alpha_y, r/theta_beta_r, g/theta_beta_g,
+ * b/theta_beta_b) for the bilateral kernel, taken as the given float values (no division, no shift).  The spatial
+ * kernel is unchanged (params' theta_gamma); params' bilateral sigmas are not used.  Either potts_dev ({w1, w2}, or
+ * NULL for params' w1 / w2) or compat_dev ({mu_bi, mu_sp} [2][M][M]), not both.  At most 32 labels.
+ *
+ * The backward writes grad_unary [B][M][H][W] and grad_features [B][5][H][W] = dL/df per pixel, and if given
+ * grad_potts [B][2] (Potts only), grad_compat [B][2][M][M] (matrices only) and grad_theta_sp [B][2] =
+ * dL/d{theta_gamma_x, theta_gamma_y}.  dL/df is exact for the function the device computes with every pixel's simplex
+ * held (as grad_theta), in the exact K convention (DESIGN.md section 1), and sum_i f_i dL/df_i over the pixels is
+ * the reference's DIAG dL/dp of the kernel.  The backward rebuilds the lattices, so other passes may run in between;
+ * it needs the kernel-bandwidth backward's buffers plus nothing per pixel beyond its outputs.
+ *
+ * Feature range: the lattice packs 12 bits per coordinate.  A pixel's keys stay in range while every feature lies
+ * within +-150 (the image path's host bound: sum_i |f_i| scale_i + max_i (i+1) |f_i| scale_i + 20 < 2047, with the
+ * elevation scales 3.46, 2.00, 1.41, 1.10, 0.89); the CRF is
+ * invariant to a common shift of a feature channel, so centre the features first.  Nothing is checked on the host: an
+ * image with a key outside the range is flagged on the device, the forward writes NaN to every kept iterate of that
+ * image and the backward NaN to its gradients.  dsrg_engine_feature_range_flags reads the flags of the engine's last
+ * feature pass (flags_out [B]: 1 = out of range); it synchronises the device and is the only host read.
+ */
+int dsrg_crf_forward_train_feat_dev(dsrg_engine *e, const float *unary_dev, int B, const float *features_dev,
+                                    const dsrg_crf_params *params, const float *potts_dev, const float *compat_dev,
+                                    float *q_hist_dev, void *stream);
+int dsrg_crf_backward_feat_dev(dsrg_engine *e, const float *q_hist_dev, int B, const float *features_dev,
+                               const dsrg_crf_params *params, const float *potts_dev, const float *compat_dev,
+                               const float *grad_q_dev, float *grad_unary_dev, float *grad_features_dev,
+                               float *grad_potts_dev, float *grad_compat_dev, float *grad_theta_sp_dev, void *stream);
+int dsrg_engine_feature_range_flags(dsrg_engine *e, int B, int32_t *flags_out);
 /* arg-max labelling after inference: DenseCRFWrapper::map, densecrf_wrapper.cpp:39-43 */
 int dsrg_crf_map_batch_dev(dsrg_engine *e, int B, const float *unary_dev, int unary_layout,
                            const uint8_t *image_dev, const dsrg_crf_params *params,

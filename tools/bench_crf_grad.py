@@ -9,6 +9,10 @@
             (--kernel) the train (and with --compat the compat) step with the backward that also gives the gradient
             to the seven kernel bandwidths (dsrg_crf_backward_theta_dev, dsrg_crf_backward_compat_theta_dev); the
             line also reports the device memory the first such backward allocates (kgrad_bytes)
+  train_feat
+            (--features) the Potts step on caller-given bilateral features (dsrg_crf_forward_train_feat_dev +
+            dsrg_crf_backward_feat_dev with grad_theta_sp): the image's own float32(x)/theta_alpha, ..., so the
+            lattice is the image path's; timed beside train_theta (implied) and train
 
 on three workloads: train-s's shape (batch 20, 41 x 41 maps, 21 labels, scale_factor 12, smooth images) and batch 64
 at 321 x 321 with scale_factor 1 on smooth and on photo-like images; 10 mean-field iterations.  The legs run on a side
@@ -17,7 +21,7 @@ window is timed with CUDA events.  Prints one JSON line per workload with the me
 card's name, power limit and SM clocks read in the same run.
 
 usage: python tools/bench_crf_grad.py [--steps 20] [--warmup 3] [--rounds 5] [--workloads train_s,b64_smooth,b64_photo]
-                                     [--compat] [--kernel]
+                                     [--compat] [--kernel] [--features]
 """
 import argparse
 import json
@@ -40,7 +44,7 @@ WORKLOADS = {   # name -> (B, H, W, M, scale factor, image)
 T = 10
 
 
-def run(name, steps, warmup, rounds, compat=False, kernel=False):
+def run(name, steps, warmup, rounds, compat=False, kernel=False, features=False):
     import torch
     from dsrg_b200 import api, synth
     B, H, W, M, sf, img = WORKLOADS[name]
@@ -84,6 +88,18 @@ def run(name, steps, warmup, rounds, compat=False, kernel=False):
             legs["train_theta"]()
         torch.cuda.synchronize()
         extra["kgrad_bytes"] = int(_lib.lib().dsrg_engine_device_bytes(eng.h) - before)
+    if features:
+        sig = torch.tensor([p.theta_alpha_x, p.theta_alpha_y, p.theta_beta_r, p.theta_beta_g, p.theta_beta_b],
+                           device="cuda").view(1, 5, 1, 1)
+        yy, xx = torch.meshgrid(torch.arange(H, device="cuda"), torch.arange(W, device="cuda"), indexing="ij")
+        raw = torch.cat([xx.expand(B, 1, H, W).float(), yy.expand(B, 1, H, W).float(),
+                         image.permute(0, 3, 1, 2).float()], 1)
+        feat = (raw / sig).contiguous()
+        gf, gsp = torch.empty_like(feat), torch.empty((B, 2), device="cuda")
+        legs["train_feat"] = lambda: (
+            eng.crf_forward_train_feat_dev(unary, feat, p, q_hist, stream=s.cuda_stream),
+            eng.crf_backward_feat_dev(q_hist, feat, p, G, gu, gf, grad_potts=gw, grad_theta_sp=gsp,
+                                      stream=s.cuda_stream))
     times = {k: [] for k in legs}
     with torch.cuda.stream(s):
         for fn in legs.values():
@@ -103,6 +119,8 @@ def run(name, steps, warmup, rounds, compat=False, kernel=False):
     med = {k: float(np.median(v)) for k, v in times.items()}
     if compat:
         extra["compat_over_train"] = round(med["compat"] / med["train"], 2)
+    if features:
+        extra["train_feat_over_train"] = round(med["train_feat"] / med["train"], 2)
     if kernel:
         extra["train_theta_over_train"] = round(med["train_theta"] / med["train"], 2)
         if compat:
@@ -122,13 +140,16 @@ def main():
     ap.add_argument("--workloads", default=",".join(WORKLOADS))
     ap.add_argument("--compat", action="store_true", help="also time the compatibility-matrix step")
     ap.add_argument("--kernel", action="store_true", help="also time the steps with the kernel-bandwidth gradient")
+    ap.add_argument("--features", action="store_true",
+                    help="also time the step with caller-given bilateral features (implies --kernel)")
     a = ap.parse_args()
+    a.kernel = a.kernel or a.features
     import torch
     if not torch.cuda.is_available():
         sys.exit("bench_crf_grad.py needs a CUDA device")
     info = card()
     for name in a.workloads.split(","):
-        r = run(name, a.steps, a.warmup, a.rounds, a.compat, a.kernel)
+        r = run(name, a.steps, a.warmup, a.rounds, a.compat, a.kernel, a.features)
         r.update(info)
         print(json.dumps(r), flush=True)
 
