@@ -219,6 +219,24 @@ class Engine(object):
                                                  _dptr(grad_theta_sp), _stream(stream)))
         return grad_unary
 
+    def crf_forward_train_wide_dev(self, unary, image, params, q_hist, potts=None, compat=None, stream=None):
+        """crf_forward_train_dev / crf_forward_train_compat_dev above 32 labels (33 to 255): potts {w1, w2} or compat
+        (2, M, M) {mu_bi, mu_sp}, not both; neither: params.w1 / w2.  An engine of 32 labels or fewer refuses."""
+        B = unary.shape[0]
+        check(self._L.dsrg_crf_forward_train_wide_dev(self.h, _dptr(unary), B, _dptr(image), C.byref(params),
+                                                      _dptr(potts), _dptr(compat), _dptr(q_hist), _stream(stream)))
+        return q_hist
+
+    def crf_backward_wide_dev(self, q_hist, image, params, grad_q, grad_unary, potts=None, compat=None,
+                              grad_potts=None, grad_compat=None, stream=None):
+        """The backward of crf_forward_train_wide_dev: grad_unary (B, M, H, W) and, if given, grad_potts (B, 2)
+        (Potts) or grad_compat (B, 2, M, M) (matrices) per image."""
+        B = grad_q.shape[0]
+        check(self._L.dsrg_crf_backward_wide_dev(self.h, _dptr(q_hist), B, _dptr(image), C.byref(params),
+                                                 _dptr(potts), _dptr(compat), _dptr(grad_q), _dptr(grad_unary),
+                                                 _dptr(grad_potts), _dptr(grad_compat), _stream(stream)))
+        return grad_unary
+
     def feature_range_flags(self, B):
         """(B,) bool: which images of the engine's last feature pass (a batch of B) had lattice keys outside the packed
         range, and so NaN results.  Synchronises the device."""

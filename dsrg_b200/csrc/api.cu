@@ -342,7 +342,7 @@ using namespace dsrg;
 
 extern "C" {
 
-int dsrg_version(void) { return 114; }
+int dsrg_version(void) { return 115; }
 
 const char *dsrg_last_error(void) { return g_err; }
 
@@ -515,7 +515,7 @@ void dsrg_engine_destroy(dsrg_engine *h) {
     void *ptrs[] = {e->U, e->Q0, e->spA, e->spB, e->spC, e->biA, e->biB, e->biC, e->nvA, e->nvB, e->lmap,
                     e->lflag, e->parent, e->hc, e->loss_acc, e->sec_rec, e->sec_img, e->sec_part, e->sec_w, e->dev_err,
                     e->hy_list, e->hy_count, e->potts_part, e->compat_part, e->kg_g, e->kg_csum, e->kg_part, e->kg_sp[0],
-                    e->kg_sp[1], e->kg_bi[0], e->kg_bi[1], e->feat_bad, e->st_unary, e->st_out, e->st_cues, e->st_labels, e->st_image, e->st_lmap, e->st_raw, e->st_idx,
+                    e->kg_sp[1], e->kg_bi[0], e->kg_bi[1], e->feat_bad, e->wide_ppart, e->wide_g, e->wide_cpart, e->st_unary, e->st_out, e->st_cues, e->st_labels, e->st_image, e->st_lmap, e->st_raw, e->st_idx,
                     e->st_prep, e->st_sel};
     for (void *p : ptrs) cudaFree(p);
     if (e->own_stream) cudaStreamDestroy(e->own_stream);
@@ -582,7 +582,7 @@ static const char *kTagNames[T_COUNT] = {
     "lattice_insert", "lattice_misc", "lattice_norm", "mf_init", "mf_zero", "mf_blur_spatial",
     "mf_blur_bilateral", "mf_tile", "mf_export", "srg_label", "srg_merge", "srg_flag", "srg_emit",
     "seedloss", "wire_bits", "prepare_image", "postprocess", "annotation", "mf_tile_hybrid",
-    "kernel_grad", "feature_grad"};
+    "kernel_grad", "feature_grad", "wide_grad"};
 
 int dsrg_profile_tag_count(void) { return T_COUNT; }
 
@@ -661,11 +661,20 @@ int dsrg_crf_batch_dev(dsrg_engine *h, int B, const float *unary, int unary_layo
     });
 }
 
-// the CRF gradient runs on the fused kernels only
+// one training path per label count: these entry points run the fused kernels, the *_wide_dev pair the label-chunked
+// ones above them
 static int grad_labels_ok(const Engine *e) {
     if (e->MP <= DSRG_MAX_LABELS) return DSRG_OK;
-    set_error("the CRF gradient supports at most %d labels (got %d); the label-chunked path above that has no backward",
+    set_error("this CRF gradient supports at most %d labels (got %d); above 32 labels use "
+              "dsrg_crf_forward_train_wide_dev / dsrg_crf_backward_wide_dev (Potts weights or matrices only)",
               DSRG_MAX_LABELS, e->M);
+    return DSRG_E_INVALID;
+}
+
+static int wide_labels_ok(const Engine *e) {
+    if (e->M > DSRG_MAX_LABELS) return DSRG_OK;
+    set_error("the label-chunked CRF gradient takes more than %d labels (got %d); use the fused pair "
+              "dsrg_crf_forward_train_dev / dsrg_crf_backward_dev (or its _compat twin)", DSRG_MAX_LABELS, e->M);
     return DSRG_E_INVALID;
 }
 
@@ -897,6 +906,63 @@ int dsrg_engine_feature_range_flags(dsrg_engine *h, int B, int32_t *flags_out) {
     DSRG_CUDA_TRY(cudaDeviceSynchronize());
     DSRG_CUDA_TRY(cudaMemcpy(flags_out, e->feat_bad, sizeof(int32_t) * B, cudaMemcpyDeviceToHost));
     return DSRG_OK;
+}
+
+int dsrg_crf_forward_train_wide_dev(dsrg_engine *h, const float *unary, int B, const uint8_t *image,
+                                    const dsrg_crf_params *params, const float *potts, const float *compat,
+                                    float *q_hist, void *stream) {
+    const cudaStream_t s = (cudaStream_t)stream;
+    return dev_call(h, B, s, unary && image && params && q_hist && !(potts && compat), [&](Engine *e) {
+        if (int rc = wide_labels_ok(e)) return rc;
+        GraphKey args;
+        args.add(unary).add(image).add(potts).add(compat).add(q_hist);
+        const int rc = crf_pass(e, s, PassKind::crf_train_wide, B, params, args, [&]() {
+            int r = prepare_lattices(e, B, image, *params, s);
+            if (r) return r;
+            return meanfield_run_train_wide(e, B, unary, q_hist, potts, compat, *params, s);
+        });
+        e->last_crf_B = 0;   // the marginals are q_hist[T]; e->U and e->Q0 were scratch
+        return rc;
+    });
+}
+
+// The label-chunked backward's buffers on its first call (as ensure_compat_part): the Potts partials, and for the
+// matrices G and the outer-product partials, sized for the engine's capacity
+static int ensure_wide(Engine *e, bool compat) {
+    if (e->wide_ppart && (!compat || e->wide_g)) return DSRG_OK;
+    cudaStreamCaptureMode mode = cudaStreamCaptureModeRelaxed;
+    DSRG_CUDA_TRY(cudaThreadExchangeStreamCaptureMode(&mode));
+    int rc = 0;
+    if (!e->wide_ppart) rc |= dalloc(e, &e->wide_ppart, (size_t)e->maxB * (e->MP / 4) * ((e->Ncap + kThreads - 1) / kThreads));
+    if (compat && !e->wide_g) {
+        rc |= dalloc(e, &e->wide_g, (size_t)e->maxB * e->M * e->Ncap);
+        rc |= dalloc(e, &e->wide_cpart, (size_t)e->maxB * kWideChunks * 2 * e->M * e->M);
+    }
+    DSRG_CUDA_TRY(cudaThreadExchangeStreamCaptureMode(&mode));
+    return rc ? DSRG_E_NOMEM : DSRG_OK;
+}
+
+int dsrg_crf_backward_wide_dev(dsrg_engine *h, const float *q_hist, int B, const uint8_t *image,
+                               const dsrg_crf_params *params, const float *potts, const float *compat,
+                               const float *grad_q, float *grad_unary, float *grad_potts, float *grad_compat,
+                               void *stream) {
+    const cudaStream_t s = (cudaStream_t)stream;
+    const bool ok = q_hist && image && params && grad_q && grad_unary && !(potts && compat) &&
+                    !(grad_potts && compat) && !(grad_compat && !compat);
+    return dev_call(h, B, s, ok, [&](Engine *e) {
+        if (int rc = wide_labels_ok(e)) return rc;
+        if (int rc = ensure_wide(e, compat != nullptr)) return rc;
+        GraphKey args;
+        args.add(q_hist).add(image).add(potts).add(compat).add(grad_q).add(grad_unary).add(grad_potts).add(grad_compat);
+        const int rc = crf_pass(e, s, PassKind::crf_backward_wide, B, params, args, [&]() {
+            int r = prepare_lattices(e, B, image, *params, s);   // as in dsrg_crf_backward_dev
+            if (r) return r;
+            return meanfield_backward_wide(e, B, q_hist, potts, compat, grad_q, grad_unary, grad_potts, grad_compat,
+                                           *params, s);
+        });
+        e->last_crf_B = 0;
+        return rc;
+    });
 }
 
 int dsrg_crf_map_batch_dev(dsrg_engine *h, int B, const float *unary, int unary_layout,

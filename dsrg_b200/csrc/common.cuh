@@ -83,7 +83,7 @@ struct Engine;
 enum KTag {
     T_LAT_INSERT = 0, T_LAT_MISC, T_LAT_NORM, T_MF_INIT, T_MF_ZERO, T_MF_BLUR_SP,
     T_MF_BLUR_BI, T_MF_TILE, T_MF_EXPORT, T_SRG_LABEL, T_SRG_MERGE, T_SRG_FLAG, T_SRG_EMIT,
-    T_LOSS, T_WIRE, T_PREP, T_POST, T_ANNOT, T_MF_TILE_HY, T_KGRAD, T_FGRAD, T_COUNT
+    T_LOSS, T_WIRE, T_PREP, T_POST, T_ANNOT, T_MF_TILE_HY, T_KGRAD, T_FGRAD, T_WIDE_GRAD, T_COUNT
 };
 
 // ---- lattice.cu ----
@@ -174,10 +174,23 @@ int meanfield_backward(Engine *e, int B, const float *q_hist, const float *potts
 // NaN into every image b of p (reps slabs rep_stride apart, per_image floats per image) with bad[b] set
 void nan_images(Engine *e, const int *bad, float *p, int B, long long per_image, int reps, long long rep_stride,
                 cudaStream_t s);
+// the backward's per-image parameter sums, in a fixed order: part [B][nparts] {spatial, bilateral} -> out [B][2]
+// {dL/dw1, dL/dw2}; part [B][nparts][mm2] -> out [B][mm2] = -sum over the parts
+void potts_reduce(Engine *e, const float2 *part, float *out, int nparts, int B, int tag, cudaStream_t s);
+void compat_reduce(Engine *e, const float *part, float *out, int nparts, int mm2, int B, int tag, cudaStream_t s);
 // ---- meanfield_wide.cu: label counts above DSRG_MAX_LABELS ----
 int meanfield_run_wide(Engine *e, int B, const float *unary, int unary_layout, bool clamp_inplace,
                        float *unary_rw, const dsrg_crf_params &p, cudaStream_t s);
 int wide_weights(Engine *e, Lattice &L, int nb, cudaStream_t s);
+// the training forward and its backward above DSRG_MAX_LABELS labels, as meanfield_run_train / meanfield_backward
+// (potts or compat, not both); the backward needs e->wide_ppart, and with compat e->wide_g and e->wide_cpart
+// (ensure_wide).  The matrices' outer products are summed per image over kWideChunks fixed pixel chunks.
+constexpr int kWideChunks = 16;
+int meanfield_run_train_wide(Engine *e, int B, const float *unary, float *q_hist, const float *potts,
+                             const float *compat, const dsrg_crf_params &p, cudaStream_t s);
+int meanfield_backward_wide(Engine *e, int B, const float *q_hist, const float *potts, const float *compat,
+                            const float *grad_q, float *grad_unary, float *grad_potts, float *grad_compat,
+                            const dsrg_crf_params &p, cudaStream_t s);
 int meanfield_export(Engine *e, int B, float *out, int layout, cudaStream_t s);
 int meanfield_export_map(Engine *e, int B, int32_t *labels, cudaStream_t s);
 int meanfield_export_renorm(Engine *e, int B, float *result_out, float *log_out, cudaStream_t s);
@@ -225,6 +238,11 @@ struct Engine {
     // the feature passes' per-image key-range flags [maxB] (allocated by the first one) and that pass's batch
     int *feat_bad = nullptr;
     int feat_B = 0;
+    // the label-chunked backward's buffers, allocated by its first call (ensure_wide): the Potts partials
+    // [maxB][MP/4][blocks] float2, and for matrices G [maxB][M][N] and the outer-product partials
+    // [maxB][kWideChunks][2][M][M]
+    float2 *wide_ppart = nullptr;
+    float *wide_g = nullptr, *wide_cpart = nullptr;
     int *hy_count = nullptr;   // their number (device-resident)
     // 1-channel buffers for the normalisation pass
     float *nvA = nullptr, *nvB = nullptr;
@@ -435,7 +453,7 @@ cudaError_t numa_host_alloc(void **p, size_t bytes, int device);
 // or if capture fails.  `body` issues the launches on `s` and returns a DSRG_* code.
 enum class PassKind : int { crf, crf_map, forward, crflayer, densecrf, post, crf_train, crf_backward, crf_train_compat,
                             crf_backward_compat, crf_backward_theta, crf_backward_compat_theta, crf_train_feat,
-                            crf_backward_feat };
+                            crf_backward_feat, crf_train_wide, crf_backward_wide };
 struct GraphKey {
     std::string bytes;
     GraphKey() = default;

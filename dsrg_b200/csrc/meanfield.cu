@@ -1951,14 +1951,8 @@ static int bwd_impl(Engine *e, int B, const float *q_hist, const float *potts, c
 #undef DSRG_BWD_LAUNCH_COMPAT
 #undef DSRG_BWD_LAUNCH
 #undef DSRG_BWD_LAUNCH_AT
-    if (g_compat) {
-        const int mm2 = 2 * M * M;
-        DSRG_LAUNCH(e, T_MF_EXPORT, s,
-                    k_mf_compat_reduce<<<dim3(cdiv(mm2, kThreads), B), kThreads, 0, s>>>(e->compat_part, g_compat,
-                                                                                         e->ntiles, mm2));
-    }
-    if (g_potts)
-        DSRG_LAUNCH(e, T_MF_EXPORT, s, k_mf_potts_reduce<<<B, kThreads, 0, s>>>(e->potts_part, g_potts, e->ntiles));
+    if (g_compat) compat_reduce(e, e->compat_part, g_compat, e->ntiles, 2 * M * M, B, T_MF_EXPORT, s);
+    if (g_potts) potts_reduce(e, e->potts_part, g_potts, e->ntiles, B, T_MF_EXPORT, s);
     if (kg) kg_finish(e, ka, B, g_theta, bgrid, s, feat, g_feat, kg_tag);
     DSRG_CUDA_TRY(cudaGetLastError());
     return DSRG_OK;
@@ -1997,6 +1991,15 @@ void nan_images(Engine *e, const int *bad, float *p, int B, long long per_image,
     const int nblk = cdiv(per_image, kThreads);
     const dim3 gp(nblk < 64 ? nblk : 64, B, reps);
     DSRG_LAUNCH(e, T_FGRAD, s, k_nan_images<<<gp, kThreads, 0, s>>>(bad, p, per_image, rep_stride));
+}
+
+void potts_reduce(Engine *e, const float2 *part, float *out, int nparts, int B, int tag, cudaStream_t s) {
+    DSRG_LAUNCH(e, tag, s, k_mf_potts_reduce<<<B, kThreads, 0, s>>>(part, out, nparts));
+}
+
+void compat_reduce(Engine *e, const float *part, float *out, int nparts, int mm2, int B, int tag, cudaStream_t s) {
+    DSRG_LAUNCH(e, tag, s,
+                k_mf_compat_reduce<<<dim3(cdiv(mm2, kThreads), B), kThreads, 0, s>>>(part, out, nparts, mm2));
 }
 
 int meanfield_run(Engine *e, int B, const float *unary, int unary_layout, bool clamp_inplace,

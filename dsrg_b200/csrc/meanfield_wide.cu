@@ -203,4 +203,333 @@ int meanfield_run_wide(Engine *e, int B, const float *unary, int layout, bool cl
     return DSRG_OK;
 }
 
+// ---------------------------------------------------------------------------------------------
+// Training above 32 labels: the forward keeping Q_0..Q_T, and the backward of the mean field (DenseCRF::gradient,
+// densecrf.cpp:238-297) on the label-chunked kernels.  With F(X) = alpha n K(n X) (wn = bary * norm, alpha on the
+// slice):
+//   Potts forward : t = U + w2 F_sp(Q) + w1 F_bi(Q)
+//   matrix forward: t = U - mu_sp F_sp(Q) - mu_bi F_bi(Q)      (compat = {mu_bi, mu_sp} [2][M][M])
+//   backward, t = T..0: g_t = Q_t (G_t - <G_t, Q_t>), grad_U += g_t, G_T = dL/dQ_T; for t > 0 splat wn g_t, blur
+//   the axes d..0 (K^T: every single-axis blur is symmetric), slice S_k = F_k^T(g_t) and form
+//     Potts : G_{t-1} = w2 S_sp + w1 S_bi,            dL/dw_k  += <S_k, Q_{t-1}>
+//     matrix: G_{t-1} = -(mu_sp^T S_sp + mu_bi^T S_bi), dL/dmu_k += -sum_i S_k,i (x) Q_{t-1},i
+// The parameter sums are kept per block (Potts) or per (image, pixel chunk) (matrices) and reduced in a fixed order:
+// no float atomics outside the splat.  The slices and mat-vecs run in meanfield.cu's operation order (fma chains
+// from zero with weights alpha wn, the spatial lattice first, labels ascending).
+// ---------------------------------------------------------------------------------------------
+
+// the quad c of pixel i: t += coef * wn_r * row_r over the d+1 vertices of L
+__device__ __forceinline__ void wide_slice_quad(const WideLat &L, float coef, int b, int i, int c, int N, int CH,
+                                                float t[4]) {
+    const size_t px = (size_t)(L.shared ? 0 : b) * L.dp1 * N + i;
+    const int base = L.rowbase[b];
+    const float4 *val = reinterpret_cast<const float4 *>(L.val);
+    for (int r = 0; r < L.dp1; r++) {
+        const float wr = coef * L.wn[px + (size_t)r * N];
+        const float4 v = val[(size_t)(base + L.off[px + (size_t)r * N]) * CH + c];
+        t[0] = fmaf(wr, v.x, t[0]);
+        t[1] = fmaf(wr, v.y, t[1]);
+        t[2] = fmaf(wr, v.z, t[2]);
+        t[3] = fmaf(wr, v.w, t[3]);
+    }
+}
+
+// k_wide_slice with the Potts weights read on the device (potts = {w1, w2})
+__global__ void __launch_bounds__(kThreads)
+k_wide_slice_dev(const float *U, float *T, WideLat sp, WideLat bi, const float *potts, float a_sp, float a_bi, int M,
+                 int N, int CH) {
+    const int b = blockIdx.z, c = blockIdx.y;
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= N) return;
+    const float c_sp = __ldg(potts + 1) * a_sp, c_bi = __ldg(potts) * a_bi;
+    float t[4];
+#pragma unroll
+    for (int k = 0; k < 4; k++) t[k] = (4 * c + k < M) ? U[((size_t)b * M + 4 * c + k) * N + i] : 0.0f;
+    wide_slice_quad(sp, c_sp, b, i, c, N, CH, t);
+    wide_slice_quad(bi, c_bi, b, i, c, N, CH, t);
+#pragma unroll
+    for (int k = 0; k < 4; k++)
+        if (4 * c + k < M) T[((size_t)b * M + 4 * c + k) * N + i] = t[k];
+}
+
+// S_sp = F_sp(.), S_bi = F_bi(.) of the blurred values, each sliced from zero, planar [B][M][N]
+__global__ void __launch_bounds__(kThreads)
+k_wide_slice_planar(float *S_sp, float *S_bi, WideLat sp, WideLat bi, float a_sp, float a_bi, int M, int N, int CH) {
+    const int b = blockIdx.z, c = blockIdx.y;
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= N) return;
+    float t[4] = {0.0f, 0.0f, 0.0f, 0.0f}, u[4] = {0.0f, 0.0f, 0.0f, 0.0f};
+    wide_slice_quad(sp, a_sp, b, i, c, N, CH, t);
+    wide_slice_quad(bi, a_bi, b, i, c, N, CH, u);
+#pragma unroll
+    for (int k = 0; k < 4; k++) {
+        if (4 * c + k < M) {
+            S_sp[((size_t)b * M + 4 * c + k) * N + i] = t[k];
+            S_bi[((size_t)b * M + 4 * c + k) * N + i] = u[k];
+        }
+    }
+}
+
+// out[l] = U[l] - sum_l' mu_sp[l, l'] S_sp[l'] - sum_l' mu_bi[l, l'] S_bi[l']  (U == nullptr: from zero), or with
+// mu^T (TRANSPOSE: the backward's G).  One thread per (pixel, label quad); the block's quad needs four rows (columns)
+// of each matrix, 8 M floats in shared memory (both whole matrices would not fit above 80 labels).
+template <bool TRANSPOSE>
+__global__ void __launch_bounds__(kThreads)
+k_wide_compat_msg(const float *U, const float *S_sp, const float *S_bi, const float *compat, float *out, int M, int N) {
+    extern __shared__ float mus[];   // [2 = sp, bi][4][M]
+    const int b = blockIdx.z, c = blockIdx.y;
+    for (int e = threadIdx.x; e < 8 * M; e += blockDim.x) {
+        const int m = e / (4 * M), k = (e / M) & 3, l2 = e % M, l = 4 * c + k;
+        const float *mu = compat + (m ? 0 : (size_t)M * M);   // compat = {mu_bi, mu_sp}
+        mus[e] = l < M ? (TRANSPOSE ? mu[(size_t)l2 * M + l] : mu[(size_t)l * M + l2]) : 0.0f;
+    }
+    __syncthreads();
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= N) return;
+    float t[4];
+#pragma unroll
+    for (int k = 0; k < 4; k++) t[k] = (U && 4 * c + k < M) ? U[((size_t)b * M + 4 * c + k) * N + i] : 0.0f;
+#pragma unroll
+    for (int m = 0; m < 2; m++) {
+        const float *S = (m ? S_bi : S_sp) + (size_t)b * M * N + i;
+        const float *mu = mus + m * 4 * M;
+        for (int l2 = 0; l2 < M; l2++) {
+            const float s = S[(size_t)l2 * N];
+#pragma unroll
+            for (int k = 0; k < 4; k++) t[k] = fmaf(-mu[k * M + l2], s, t[k]);
+        }
+    }
+#pragma unroll
+    for (int k = 0; k < 4; k++)
+        if (4 * c + k < M) out[((size_t)b * M + 4 * c + k) * N + i] = t[k];
+}
+
+// g = Q (G - <G, Q>) per pixel over all labels; gU = g (first) or gU += g; g also to gout when given (gout may be G)
+__global__ void __launch_bounds__(kThreads)
+k_wide_vjp(const float *G, const float *Q, float *gU, float *gout, int first, int M, int N) {
+    const int b = blockIdx.y;
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= N) return;
+    const size_t at = (size_t)b * M * N + i;
+    float dot = 0.0f;
+    for (int k = 0; k < M; k++) dot = fmaf(G[at + (size_t)k * N], Q[at + (size_t)k * N], dot);
+    for (int k = 0; k < M; k++) {
+        const size_t a = at + (size_t)k * N;
+        const float g = Q[a] * (G[a] - dot);
+        gU[a] = first ? g : gU[a] + g;
+        if (gout) gout[a] = g;
+    }
+}
+
+// Potts: G = w2 S_sp + w1 S_bi per (pixel, label quad) with the block's {<S_sp, Q>, <S_bi, Q>} to
+// part[b][c][block] (first: written, else added)
+__global__ void __launch_bounds__(kThreads)
+k_wide_potts_bwd(const float *Qt, float *G, WideLat sp, WideLat bi, const float *potts, float w1, float w2,
+                 float a_sp, float a_bi, float2 *part, int first, int M, int N, int CH) {
+    __shared__ float2 red[kThreads / 32];
+    const int b = blockIdx.z, c = blockIdx.y;
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (potts) {
+        w1 = __ldg(potts);
+        w2 = __ldg(potts + 1);
+    }
+    float p_sp = 0.0f, p_bi = 0.0f;
+    if (i < N) {
+        float q[4], s[4] = {0.0f, 0.0f, 0.0f, 0.0f}, g[4];
+#pragma unroll
+        for (int k = 0; k < 4; k++) q[k] = (4 * c + k < M) ? Qt[((size_t)b * M + 4 * c + k) * N + i] : 0.0f;
+        wide_slice_quad(sp, a_sp, b, i, c, N, CH, s);
+#pragma unroll
+        for (int k = 0; k < 4; k++) {
+            p_sp = fmaf(s[k], q[k], p_sp);
+            g[k] = w2 * s[k];
+            s[k] = 0.0f;
+        }
+        wide_slice_quad(bi, a_bi, b, i, c, N, CH, s);
+#pragma unroll
+        for (int k = 0; k < 4; k++) {
+            p_bi = fmaf(s[k], q[k], p_bi);
+            g[k] = fmaf(w1, s[k], g[k]);
+            if (4 * c + k < M) G[((size_t)b * M + 4 * c + k) * N + i] = g[k];
+        }
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+        p_sp += __shfl_down_sync(0xffffffffu, p_sp, o);
+        p_bi += __shfl_down_sync(0xffffffffu, p_bi, o);
+    }
+    if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = make_float2(p_sp, p_bi);
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        float2 a = make_float2(0.0f, 0.0f);
+#pragma unroll
+        for (int w = 0; w < kThreads / 32; w++) {
+            a.x += red[w].x;
+            a.y += red[w].y;
+        }
+        float2 *pp = part + ((size_t)b * CH + c) * gridDim.x + blockIdx.x;
+        if (!first) {
+            a.x += pp->x;
+            a.y += pp->y;
+        }
+        *pp = a;
+    }
+}
+
+// The matrices' outer products, an FP32 tiled GEMM per image: part[b][chunk][k][l][l'] (+)= sum over the chunk's
+// pixels of S_k[l] Q[l'] (k = 0: bilateral, 1: spatial).  A CTA owns a 32 x 32 block of (l, l') over one pixel chunk
+// and stages 32-pixel slabs of S and Q; each thread owns 2 x 2 entries and sums a slab, then adds the slab to its
+// total, so a sum's depth stays near 32 + N / (32 kWideChunks) rather than N / kWideChunks.
+constexpr int kWideOuterTile = 32;
+__global__ void __launch_bounds__(kThreads)
+k_wide_outer(const float *S_sp, const float *S_bi, const float *Qt, float *part, int first, int M, int N,
+             int chunk_px) {
+    constexpr int TL = kWideOuterTile;
+    __shared__ float ss[TL][TL + 1], qs[TL][TL + 1];   // [pixel][label]
+    const int tl = (M + TL - 1) / TL;
+    const int l0 = (blockIdx.x / tl) * TL, m0 = (blockIdx.x % tl) * TL;
+    const int k = blockIdx.y / kWideChunks, chunk = blockIdx.y % kWideChunks, b = blockIdx.z;
+    const float *S = (k ? S_sp : S_bi) + (size_t)b * M * N, *Q = Qt + (size_t)b * M * N;
+    const int tid = threadIdx.x, ty = tid / 16, tx = tid % 16;
+    const int p_beg = chunk * chunk_px, p_end = min(N, p_beg + chunk_px);
+    float acc[2][2] = {{0.0f, 0.0f}, {0.0f, 0.0f}};
+    for (int p0 = p_beg; p0 < p_end; p0 += TL) {
+        __syncthreads();
+        for (int e = tid; e < TL * TL; e += kThreads) {
+            const int r = e / TL, px = e % TL, p = p0 + px;
+            const bool pin = p < p_end;
+            ss[px][r] = (pin && l0 + r < M) ? S[(size_t)(l0 + r) * N + p] : 0.0f;
+            qs[px][r] = (pin && m0 + r < M) ? Q[(size_t)(m0 + r) * N + p] : 0.0f;
+        }
+        __syncthreads();
+        float sl[2][2] = {{0.0f, 0.0f}, {0.0f, 0.0f}};
+#pragma unroll 8
+        for (int px = 0; px < TL; px++) {
+            const float a0 = ss[px][2 * ty], a1 = ss[px][2 * ty + 1], q0 = qs[px][2 * tx], q1 = qs[px][2 * tx + 1];
+            sl[0][0] = fmaf(a0, q0, sl[0][0]);
+            sl[0][1] = fmaf(a0, q1, sl[0][1]);
+            sl[1][0] = fmaf(a1, q0, sl[1][0]);
+            sl[1][1] = fmaf(a1, q1, sl[1][1]);
+        }
+#pragma unroll
+        for (int u = 0; u < 2; u++)
+#pragma unroll
+            for (int v = 0; v < 2; v++) acc[u][v] += sl[u][v];
+    }
+    float *pp = part + (((size_t)b * kWideChunks + chunk) * 2 + k) * M * M;
+#pragma unroll
+    for (int u = 0; u < 2; u++)
+#pragma unroll
+        for (int v = 0; v < 2; v++) {
+            const int l = l0 + 2 * ty + u, l2 = m0 + 2 * tx + v;
+            if (l < M && l2 < M) {
+                float *o = pp + (size_t)l * M + l2;
+                *o = first ? acc[u][v] : *o + acc[u][v];
+            }
+        }
+}
+
+static WideLat wide_lat(const Lattice &L, float *val) { return WideLat{L.off, L.wn, L.rowbase, val, L.shared, L.d + 1}; }
+
+// zero Y, splat X planar into it, blur every axis (d..0 when `reverse`, K^T); returns the blurred buffers
+static void wide_filter(Engine *e, int B, const float *X, bool reverse, int tag, cudaStream_t s, float **sp_out,
+                        float **bi_out) {
+    const int M = e->M, N = e->N, CH = e->MP / 4, grid = 8 * e->sm_count;
+    const dim3 gq(cdiv(N, kThreads), CH, B);
+    float *spY = e->spA, *spZ = e->spB, *biY = e->biA, *biZ = e->biB;
+    DSRG_LAUNCH(e, tag, s, k_wide_zero<<<grid, kThreads, 0, s>>>((float4 *)spY, e->sp.rowbase, (float4 *)biY, e->bi.rowbase, B, CH));
+    DSRG_LAUNCH(e, tag, s, k_wide_splat<<<gq, kThreads, 0, s>>>(X, wide_lat(e->sp, spY), wide_lat(e->bi, biY), M, N, CH));
+    for (int l = 0; l < 2; l++) {
+        Lattice &L = l ? e->bi : e->sp;
+        float *&src = l ? biY : spY, *&dst = l ? biZ : spZ;
+        for (int p = 0; p <= L.d; p++) {
+            const int j = reverse ? L.d - p : p;
+            DSRG_LAUNCH(e, tag, s,
+                        k_wide_blur<<<grid, kThreads, 0, s>>>((const float4 *)src, (float4 *)dst, L.nbr + (size_t)j * L.nbr_stride,
+                                                              L.rowbase, B, L.shared, CH));
+            float *t = src; src = dst; dst = t;
+        }
+    }
+    *sp_out = spY;
+    *bi_out = biY;
+}
+
+static float wide_alpha(const Lattice &L) { return 1.0f / (1 + powf(2, -L.d)); }   // permutohedral.cpp:571
+
+int meanfield_run_train_wide(Engine *e, int B, const float *unary, float *q_hist, const float *potts,
+                             const float *compat, const dsrg_crf_params &p, cudaStream_t s) {
+    const int M = e->M, N = e->N, CH = e->MP / 4, T = p.n_iters;
+    const size_t slab = (size_t)B * M * N;
+    const dim3 gp(cdiv(N, kThreads), B), gq(cdiv(N, kThreads), CH, B);
+    const float a_sp = wide_alpha(e->sp), a_bi = wide_alpha(e->bi);
+    DSRG_LAUNCH(e, T_WIDE_GRAD, s, k_wide_init<<<gp, kThreads, 0, s>>>(unary, nullptr, DSRG_LAYOUT_NCHW, 0, e->U, q_hist, M, N));
+    for (int it = 1; it <= T; it++) {
+        float *spV, *biV, *qt = q_hist + (size_t)it * slab;
+        wide_filter(e, B, q_hist + (size_t)(it - 1) * slab, false, T_WIDE_GRAD, s, &spV, &biV);
+        const WideLat sp = wide_lat(e->sp, spV), bi = wide_lat(e->bi, biV);
+        if (compat) {   // e->U and e->Q0 hold S_sp and S_bi
+            DSRG_LAUNCH(e, T_WIDE_GRAD, s, k_wide_slice_planar<<<gq, kThreads, 0, s>>>(e->U, e->Q0, sp, bi, a_sp, a_bi, M, N, CH));
+            DSRG_LAUNCH(e, T_WIDE_GRAD, s,
+                        k_wide_compat_msg<false><<<gq, kThreads, 8 * M * sizeof(float), s>>>(unary, e->U, e->Q0, compat, qt, M, N));
+        } else if (potts) {
+            DSRG_LAUNCH(e, T_WIDE_GRAD, s, k_wide_slice_dev<<<gq, kThreads, 0, s>>>(unary, qt, sp, bi, potts, a_sp, a_bi, M, N, CH));
+        } else {
+            DSRG_LAUNCH(e, T_WIDE_GRAD, s,
+                        k_wide_slice<<<gq, kThreads, 0, s>>>(unary, qt, sp, bi, p.w2 * a_sp, p.w1 * a_bi, M, N, CH));
+        }
+        DSRG_LAUNCH(e, T_WIDE_GRAD, s, k_wide_softmax<<<gp, kThreads, 0, s>>>(qt, M, N));
+    }
+    DSRG_CUDA_TRY(cudaGetLastError());
+    return DSRG_OK;
+}
+
+int meanfield_backward_wide(Engine *e, int B, const float *q_hist, const float *potts, const float *compat,
+                            const float *grad_q, float *grad_unary, float *grad_potts, float *grad_compat,
+                            const dsrg_crf_params &p, cudaStream_t s) {
+    const int M = e->M, N = e->N, CH = e->MP / 4, T = p.n_iters;
+    const size_t slab = (size_t)B * M * N;
+    const int nblk = cdiv(N, kThreads);
+    const dim3 gp(nblk, B), gq(nblk, CH, B);
+    const float a_sp = wide_alpha(e->sp), a_bi = wide_alpha(e->bi);
+    // e->Q0: g_t, then S_sp (matrices) or G_{t-1} (Potts); e->U: S_bi; e->wide_g: the matrices' G_{t-1}
+    float *X = e->Q0;
+    const float *G = grad_q;
+    const int tl = (M + kWideOuterTile - 1) / kWideOuterTile;
+    const int chunk_px = cdiv(cdiv(N, kWideChunks), kWideOuterTile) * kWideOuterTile;
+    for (int it = T; it > 0; it--) {
+        const float *qt = q_hist + (size_t)it * slab, *qp = q_hist + (size_t)(it - 1) * slab;
+        const int first = it == T;
+        DSRG_LAUNCH(e, T_WIDE_GRAD, s, k_wide_vjp<<<gp, kThreads, 0, s>>>(G, qt, grad_unary, X, first, M, N));
+        float *spV, *biV;
+        wide_filter(e, B, X, true, T_WIDE_GRAD, s, &spV, &biV);
+        const WideLat sp = wide_lat(e->sp, spV), bi = wide_lat(e->bi, biV);
+        if (compat) {
+            DSRG_LAUNCH(e, T_WIDE_GRAD, s, k_wide_slice_planar<<<gq, kThreads, 0, s>>>(X, e->U, sp, bi, a_sp, a_bi, M, N, CH));
+            DSRG_LAUNCH(e, T_WIDE_GRAD, s,
+                        k_wide_compat_msg<true><<<gq, kThreads, 8 * M * sizeof(float), s>>>(nullptr, X, e->U, compat, e->wide_g, M, N));
+            if (grad_compat)
+                DSRG_LAUNCH(e, T_WIDE_GRAD, s,
+                            k_wide_outer<<<dim3(tl * tl, 2 * kWideChunks, B), kThreads, 0, s>>>(X, e->U, qp, e->wide_cpart,
+                                                                                               first, M, N, chunk_px));
+            G = e->wide_g;
+        } else {
+            DSRG_LAUNCH(e, T_WIDE_GRAD, s,
+                        k_wide_potts_bwd<<<gq, kThreads, 0, s>>>(qp, X, sp, bi, potts, p.w1, p.w2, a_sp, a_bi, e->wide_ppart,
+                                                                 first, M, N, CH));
+            G = X;
+        }
+    }
+    DSRG_LAUNCH(e, T_WIDE_GRAD, s, k_wide_vjp<<<gp, kThreads, 0, s>>>(G, q_hist, grad_unary, nullptr, T == 0, M, N));
+    if (T == 0) {
+        if (grad_potts) DSRG_CUDA_TRY(cudaMemsetAsync(grad_potts, 0, sizeof(float) * 2 * B, s));
+        if (grad_compat) DSRG_CUDA_TRY(cudaMemsetAsync(grad_compat, 0, sizeof(float) * 2 * M * M * B, s));
+    } else if (grad_potts) {
+        potts_reduce(e, e->wide_ppart, grad_potts, CH * nblk, B, T_WIDE_GRAD, s);
+    } else if (grad_compat) {
+        compat_reduce(e, e->wide_cpart, grad_compat, kWideChunks, 2 * M * M, B, T_WIDE_GRAD, s);
+    }
+    DSRG_CUDA_TRY(cudaGetLastError());
+    return DSRG_OK;
+}
+
 }  // namespace dsrg

@@ -639,7 +639,8 @@ def dense_crf(unary, image, scale_factor=1.0, color_factor=13, maxiter=10, w1=No
     u = _maps(unary, "unary")
     N, M, H, W = u.shape
     if M > FUSED_LABELS:
-        raise ValueError("dense_crf supports at most %d labels (got %d)" % (FUSED_LABELS, M))
+        raise ValueError("dense_crf supports at most %d labels (got %d); dense_crf_wide takes up to %d"
+                         % (FUSED_LABELS, M, MAX_LABELS))
     if features_bi is not None:
         return _dense_crf_feat(u, image, features_bi, scale_factor, color_factor, maxiter, w1, w2, compat_bi,
                                compat_sp, theta_bi, theta_sp)
@@ -682,6 +683,72 @@ def _compat_stack(u, M, w1, w2, compat_bi, compat_sp):
         else:
             mats.append(_compat_matrix(mu, name, u, M))
     return torch.stack(mats)
+
+
+class _DenseCrfWide(torch.autograd.Function):
+    """dense_crf_wide above 32 labels: Potts weights (w1, w2) or the matrices (compat (2, M, M) {mu_bi, mu_sp}) on the
+    label-chunked kernels."""
+
+    @staticmethod
+    @_fwd
+    def forward(ctx, unary, image, w1, w2, compat, params):
+        eng = _engine_for(unary)
+        maxiter = params.n_iters
+        q_hist = torch.empty((maxiter + 1,) + tuple(unary.shape), dtype=torch.float32, device=unary.device)
+        potts = _potts_tensor(w1, w2, unary) if compat is None else None
+        eng.crf_forward_train_wide_dev(unary, image, params, q_hist, potts=potts, compat=compat, stream=_stream(unary))
+        ctx.save_for_backward(q_hist, image, potts, compat)
+        ctx.params = params
+        return q_hist[maxiter].clone()
+
+    @staticmethod
+    @_bwd
+    def backward(ctx, g):
+        q_hist, image, potts, compat = ctx.saved_tensors
+        B, dev = q_hist.shape[1], q_hist.device
+        need = ctx.needs_input_grad
+        grad_u = torch.empty(q_hist.shape[1:], dtype=torch.float32, device=dev)
+        grad_potts = grad_c = None
+        if potts is not None and (need[2] or need[3]):
+            grad_potts = torch.empty((B, 2), dtype=torch.float32, device=dev)
+        if compat is not None and need[4]:
+            M = compat.shape[-1]
+            grad_c = torch.empty((B, 2, M, M), dtype=torch.float32, device=dev)
+        _engine_for(grad_u).crf_backward_wide_dev(q_hist, image, ctx.params, g.contiguous(), grad_u, potts=potts,
+                                                  compat=compat, grad_potts=grad_potts, grad_compat=grad_c,
+                                                  stream=_stream(grad_u))
+        gw1 = grad_potts[:, 0].sum() if grad_potts is not None and need[2] else None
+        gw2 = grad_potts[:, 1].sum() if grad_potts is not None and need[3] else None
+        return grad_u, None, gw1, gw2, None if grad_c is None else grad_c.sum(0), None
+
+
+def dense_crf_wide(unary, image, scale_factor=1.0, color_factor=13, maxiter=10, w1=None, w2=None, compat_bi=None,
+                   compat_sp=None):
+    """dense_crf for any label count from 1 to 255 (COCO's 81 classes), with the Potts weights or the
+    label-compatibility matrices learnable as there; the kernel bandwidths and caller-given features stay with
+    dense_crf (at most 32 labels).  At 32 labels or fewer it is dense_crf itself; above that the mean field and its
+    exact backward run on the label-chunked kernels, whose per-label cost is several times the fused path's.
+    Nothing is read on the host, so a step can be captured in a CUDA graph.  The forward keeps every iteration's
+    marginals: (maxiter + 1) * N * M * H * W * 4 bytes, 120 MB at batch 20 @ 41x41 with 81 labels."""
+    if torch.is_autocast_enabled("cuda"):
+        unary = unary.float() if isinstance(unary, torch.Tensor) and unary.is_floating_point() else unary
+    u = _maps(unary, "unary")
+    N, M, H, W = u.shape
+    if M <= FUSED_LABELS:
+        return dense_crf(u, image, scale_factor, color_factor, maxiter, w1, w2, compat_bi, compat_sp)
+    if (not isinstance(image, torch.Tensor) or image.dtype != torch.uint8 or tuple(image.shape) != (N, H, W, 3)
+            or image.device != u.device):
+        raise ValueError("image must be a (%d, %d, %d, 3) uint8 tensor on %s" % (N, H, W, u.device))
+    _cuda(u, "unary")
+    w1, w2 = _potts_weight(w1, "w1", u), _potts_weight(w2, "w2", u)
+    if int(maxiter) < 0:
+        raise ValueError("maxiter must be >= 0 (got %d)" % maxiter)
+    params = api.crf_params(float(scale_factor), float(color_factor), int(maxiter))
+    compat = None
+    if compat_bi is not None or compat_sp is not None:
+        compat = _compat_stack(u, M, w1, w2, compat_bi, compat_sp)
+        w1 = w2 = None
+    return _DenseCrfWide.apply(u, image.contiguous(), w1, w2, compat, params)
 
 
 def softmax(fc8):

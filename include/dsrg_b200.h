@@ -139,7 +139,7 @@ int dsrg_crf_batch_host(dsrg_engine *e, int B, const float *unary_host, int unar
 /*
  * The CRF as a differentiable layer: the forward keeps every iteration's marginals and the backward runs the mean
  * field backwards through them (DenseCRF::gradient, densecrf.cpp:238-297, with the objective's gradient given).
- * Label counts up to DSRG_MAX_LABELS; more return DSRG_E_INVALID.
+ * Label counts up to DSRG_MAX_LABELS; more return DSRG_E_INVALID (dsrg_crf_forward_train_wide_dev below serves them).
  *   unary  : [B][M][H][W] (NCHW) values as passed to CRF(image, unary), energy = -unary; not clamped
  *   potts  : optional device float[2] {w1, w2} read by the kernels in place of params->w1 / w2, so that a caller can
  *            learn the Potts weights without a host synchronisation.  Its address is part of a cached graph's key,
@@ -228,6 +228,25 @@ int dsrg_crf_backward_feat_dev(dsrg_engine *e, const float *q_hist_dev, int B, c
                                const float *grad_q_dev, float *grad_unary_dev, float *grad_features_dev,
                                float *grad_potts_dev, float *grad_compat_dev, float *grad_theta_sp_dev, void *stream);
 int dsrg_engine_feature_range_flags(dsrg_engine *e, int B, int32_t *flags_out);
+/*
+ * The training forward and its backward above DSRG_MAX_LABELS labels (DSRG_MAX_LABELS < M <= DSRG_MAX_LABELS_WIDE,
+ * e.g. COCO's 81), on the label-chunked kernels of dsrg_crf_batch_dev at those counts.  The arguments mean what they
+ * mean in dsrg_crf_forward_train_dev / dsrg_crf_backward_dev and their _compat twins: potts_dev ({w1, w2}) or
+ * compat_dev ({mu_bi, mu_sp} [2][M][M]), at most one of them; with neither, params->w1 / w2 apply.  grad_potts
+ * (Potts only) and grad_compat (matrices only) are optional.  An engine of 32 labels or fewer is refused with
+ * DSRG_E_INVALID: the fused pairs serve it, so each label count has one path.
+ * q_hist takes (T+1)*B*M*H*W*4 bytes: 120 MB at batch 20 @ 41x41 with 81 labels and T = 10.  The first backward
+ * allocates the Potts partials, maxB * ceil(M/4) * ceil(H*W/256) * 8 bytes, and with matrices G (maxB * M * H*W * 4
+ * bytes) and the outer-product partials (maxB * 16 * 2 * M^2 * 4 bytes): 23.5 KB and 27.7 MB for an engine of batch
+ * 20 @ 41x41 with 81 labels (dsrg_engine_device_bytes before and after).
+ */
+int dsrg_crf_forward_train_wide_dev(dsrg_engine *e, const float *unary_dev, int B, const uint8_t *image_dev,
+                                    const dsrg_crf_params *params, const float *potts_dev, const float *compat_dev,
+                                    float *q_hist_dev, void *stream);
+int dsrg_crf_backward_wide_dev(dsrg_engine *e, const float *q_hist_dev, int B, const uint8_t *image_dev,
+                               const dsrg_crf_params *params, const float *potts_dev, const float *compat_dev,
+                               const float *grad_q_dev, float *grad_unary_dev, float *grad_potts_dev,
+                               float *grad_compat_dev, void *stream);
 /* arg-max labelling after inference: DenseCRFWrapper::map, densecrf_wrapper.cpp:39-43 */
 int dsrg_crf_map_batch_dev(dsrg_engine *e, int B, const float *unary_dev, int unary_layout,
                            const uint8_t *image_dev, const dsrg_crf_params *params,

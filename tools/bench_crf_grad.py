@@ -14,6 +14,12 @@
             dsrg_crf_backward_feat_dev with grad_theta_sp): the image's own float32(x)/theta_alpha, ..., so the
             lattice is the image path's; timed beside train_theta (implied) and train
 
+  wide_potts, wide_compat
+            (--wide, on its own workloads at COCO's 81 labels) dsrg_crf_forward_train_wide_dev +
+            dsrg_crf_backward_wide_dev, the label-chunked step with device Potts weights and with a matrix per kernel,
+            timed beside the label-chunked inference forward; the line also reports the device memory the first
+            backwards allocate (wide_bytes) and the FLOPs of the matrices' outer products (outer_flops)
+
 on three workloads: train-s's shape (batch 20, 41 x 41 maps, 21 labels, scale_factor 12, smooth images) and batch 64
 at 321 x 321 with scale_factor 1 on smooth and on photo-like images; 10 mean-field iterations.  The legs run on a side
 stream (the engine's CUDA graphs need one), are warmed up, and are alternated in rounds within one session; each
@@ -21,7 +27,7 @@ window is timed with CUDA events.  Prints one JSON line per workload with the me
 card's name, power limit and SM clocks read in the same run.
 
 usage: python tools/bench_crf_grad.py [--steps 20] [--warmup 3] [--rounds 5] [--workloads train_s,b64_smooth,b64_photo]
-                                     [--compat] [--kernel] [--features]
+                                     [--compat] [--kernel] [--features] [--wide]
 """
 import argparse
 import json
@@ -41,13 +47,17 @@ WORKLOADS = {   # name -> (B, H, W, M, scale factor, image)
     "b64_smooth": (64, 321, 321, 21, 1.0, "smooth"),
     "b64_photo": (64, 321, 321, 21, 1.0, "photo"),
 }
+WIDE_WORKLOADS = {   # --wide: COCO's training shape, and large photo-like images
+    "coco_train": (20, 41, 41, 81, 12.0, "photo"),
+    "b8_photo": (8, 321, 321, 81, 1.0, "photo"),
+}
 T = 10
 
 
-def run(name, steps, warmup, rounds, compat=False, kernel=False, features=False):
+def run(name, steps, warmup, rounds, compat=False, kernel=False, features=False, wide=False):
     import torch
     from dsrg_b200 import api, synth
-    B, H, W, M, sf, img = WORKLOADS[name]
+    B, H, W, M, sf, img = (WIDE_WORKLOADS if wide else WORKLOADS)[name]
     batch = synth.make_batch(B, H, W, C=M, image=img, start=3, unique=8)
     unary = torch.from_numpy(np.log(np.maximum(batch["probs"], 1e-5)).astype(np.float32)).cuda()
     image = torch.from_numpy(batch["image"]).cuda()
@@ -67,11 +77,31 @@ def run(name, steps, warmup, rounds, compat=False, kernel=False, features=False)
         "train": lambda: (eng.crf_forward_train_dev(unary, image, p, q_hist, stream=s.cuda_stream),
                           eng.crf_backward_dev(q_hist, image, p, G, gu, grad_potts=gw, stream=s.cuda_stream)),
     }
+    extra = {}
+    if wide:
+        from dsrg_b200 import _lib
+        del legs["train"]
+        potts = torch.tensor([10.0, 3.0], device="cuda")
+        mu = (torch.randn((2, M, M), generator=torch.Generator().manual_seed(5)) - 2 * torch.eye(M)).cuda()
+        gmu = torch.empty((B, 2, M, M), device="cuda")
+        legs["wide_potts"] = lambda: (
+            eng.crf_forward_train_wide_dev(unary, image, p, q_hist, potts=potts, stream=s.cuda_stream),
+            eng.crf_backward_wide_dev(q_hist, image, p, G, gu, potts=potts, grad_potts=gw, stream=s.cuda_stream))
+        legs["wide_compat"] = lambda: (
+            eng.crf_forward_train_wide_dev(unary, image, p, q_hist, compat=mu, stream=s.cuda_stream),
+            eng.crf_backward_wide_dev(q_hist, image, p, G, gu, compat=mu, grad_compat=gmu, stream=s.cuda_stream))
+        before = _lib.lib().dsrg_engine_device_bytes(eng.h)
+        with torch.cuda.stream(s):
+            legs["wide_potts"]()
+            extra["wide_bytes_potts"] = int(_lib.lib().dsrg_engine_device_bytes(eng.h) - before)
+            legs["wide_compat"]()
+        torch.cuda.synchronize()
+        extra["wide_bytes"] = int(_lib.lib().dsrg_engine_device_bytes(eng.h) - before)
+        extra["outer_flops"] = 2 * 2 * M * M * H * W * B * T   # two lattices, a multiply-add per (l, l', pixel, t)
     if compat:
         legs["compat"] = lambda: (eng.crf_forward_train_compat_dev(unary, image, p, mu, q_hist, stream=s.cuda_stream),
                                   eng.crf_backward_compat_dev(q_hist, image, p, mu, G, gu, grad_compat=gmu,
                                                               stream=s.cuda_stream))
-    extra = {}
     if kernel:
         from dsrg_b200 import _lib
         gt = torch.empty((B, 7), device="cuda")
@@ -121,6 +151,9 @@ def run(name, steps, warmup, rounds, compat=False, kernel=False, features=False)
         extra["compat_over_train"] = round(med["compat"] / med["train"], 2)
     if features:
         extra["train_feat_over_train"] = round(med["train_feat"] / med["train"], 2)
+    if wide:
+        extra["wide_potts_over_forward"] = round(med["wide_potts"] / med["forward"], 2)
+        extra["wide_compat_over_forward"] = round(med["wide_compat"] / med["forward"], 2)
     if kernel:
         extra["train_theta_over_train"] = round(med["train_theta"] / med["train"], 2)
         if compat:
@@ -128,7 +161,7 @@ def run(name, steps, warmup, rounds, compat=False, kernel=False, features=False)
     return dict(**extra, workload=name, B=B, H=H, W=W, M=M, scale_factor=sf, image=img, n_iters=T,
                 ms_per_step={k: round(v, 3) for k, v in med.items()},
                 spread_ms={k: [round(min(v), 3), round(max(v), 3)] for k, v in times.items()},
-                train_over_forward=round(med["train"] / med["forward"], 2),
+                **({} if wide else dict(train_over_forward=round(med["train"] / med["forward"], 2))),
                 q_hist_bytes=(T + 1) * B * M * H * W * 4)
 
 
@@ -142,14 +175,19 @@ def main():
     ap.add_argument("--kernel", action="store_true", help="also time the steps with the kernel-bandwidth gradient")
     ap.add_argument("--features", action="store_true",
                     help="also time the step with caller-given bilateral features (implies --kernel)")
+    ap.add_argument("--wide", action="store_true",
+                    help="time the label-chunked steps at 81 labels instead, on their own workloads")
     a = ap.parse_args()
     a.kernel = a.kernel or a.features
+    if a.wide and a.workloads == ",".join(WORKLOADS):
+        a.workloads = ",".join(WIDE_WORKLOADS)
     import torch
     if not torch.cuda.is_available():
         sys.exit("bench_crf_grad.py needs a CUDA device")
     info = card()
     for name in a.workloads.split(","):
-        r = run(name, a.steps, a.warmup, a.rounds, a.compat, a.kernel, a.features)
+        fused = not a.wide   # --compat, --kernel and --features time fused-path legs
+        r = run(name, a.steps, a.warmup, a.rounds, a.compat and fused, a.kernel and fused, a.features and fused, a.wide)
         r.update(info)
         print(json.dumps(r), flush=True)
 
