@@ -66,6 +66,9 @@ SIGNATURES = {
     "dsrg_crf_backward_feat_dev": (_i, [_vp, _vp, _i, _vp, _pp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "dsrg_crf_forward_train_wide_dev": (_i, [_vp, _vp, _i, _vp, _pp, _vp, _vp, _vp, _vp]),
     "dsrg_crf_backward_wide_dev": (_i, [_vp, _vp, _i, _vp, _pp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "dsrg_crf_backward_wide_theta_dev": (_i, [_vp, _vp, _i, _vp, _pp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "dsrg_crf_forward_train_wide_feat_dev": (_i, [_vp, _vp, _i, _vp, _pp, _vp, _vp, _vp, _vp]),
+    "dsrg_crf_backward_wide_feat_dev": (_i, [_vp, _vp, _i, _vp, _pp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "dsrg_engine_feature_range_flags": (_i, [_vp, _i, _vp]),
     "dsrg_srg_batch_dev": (_i, [_vp, _i, _vp, _vp, _vp, _d, _d, _i, _vp, _vp, _vp]),
     "dsrg_srg_batch_host": (_i, [_vp, _i, _vp, _vp, _vp, _d, _d, _i, _vp, _vp]),

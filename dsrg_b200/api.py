@@ -237,6 +237,35 @@ class Engine(object):
                                                  _dptr(grad_potts), _dptr(grad_compat), _stream(stream)))
         return grad_unary
 
+    def crf_backward_wide_theta_dev(self, q_hist, image, params, grad_q, grad_unary, grad_theta, potts=None,
+                                    compat=None, grad_potts=None, grad_compat=None, stream=None):
+        """crf_backward_wide_dev that also writes grad_theta (B, 7) as crf_backward_theta_dev does; its forward is
+        crf_forward_train_wide_dev with the same params."""
+        B = grad_q.shape[0]
+        check(self._L.dsrg_crf_backward_wide_theta_dev(self.h, _dptr(q_hist), B, _dptr(image), C.byref(params),
+                                                       _dptr(potts), _dptr(compat), _dptr(grad_q), _dptr(grad_unary),
+                                                       _dptr(grad_potts), _dptr(grad_compat), _dptr(grad_theta),
+                                                       _stream(stream)))
+        return grad_unary
+
+    def crf_forward_train_wide_feat_dev(self, unary, features, params, q_hist, potts=None, compat=None, stream=None):
+        """crf_forward_train_feat_dev above 32 labels (33 to 255), on the label-chunked kernels."""
+        B = unary.shape[0]
+        check(self._L.dsrg_crf_forward_train_wide_feat_dev(self.h, _dptr(unary), B, _dptr(features), C.byref(params),
+                                                           _dptr(potts), _dptr(compat), _dptr(q_hist),
+                                                           _stream(stream)))
+        return q_hist
+
+    def crf_backward_wide_feat_dev(self, q_hist, features, params, grad_q, grad_unary, grad_features, potts=None,
+                                   compat=None, grad_potts=None, grad_compat=None, grad_theta_sp=None, stream=None):
+        """The backward of crf_forward_train_wide_feat_dev, with crf_backward_feat_dev's outputs."""
+        B = grad_q.shape[0]
+        check(self._L.dsrg_crf_backward_wide_feat_dev(self.h, _dptr(q_hist), B, _dptr(features), C.byref(params),
+                                                      _dptr(potts), _dptr(compat), _dptr(grad_q), _dptr(grad_unary),
+                                                      _dptr(grad_features), _dptr(grad_potts), _dptr(grad_compat),
+                                                      _dptr(grad_theta_sp), _stream(stream)))
+        return grad_unary
+
     def feature_range_flags(self, B):
         """(B,) bool: which images of the engine's last feature pass (a batch of B) had lattice keys outside the packed
         range, and so NaN results.  Synchronises the device."""

@@ -342,7 +342,7 @@ using namespace dsrg;
 
 extern "C" {
 
-int dsrg_version(void) { return 115; }
+int dsrg_version(void) { return 116; }
 
 const char *dsrg_last_error(void) { return g_err; }
 
@@ -666,7 +666,7 @@ int dsrg_crf_batch_dev(dsrg_engine *h, int B, const float *unary, int unary_layo
 static int grad_labels_ok(const Engine *e) {
     if (e->MP <= DSRG_MAX_LABELS) return DSRG_OK;
     set_error("this CRF gradient supports at most %d labels (got %d); above 32 labels use "
-              "dsrg_crf_forward_train_wide_dev / dsrg_crf_backward_wide_dev (Potts weights or matrices only)",
+              "dsrg_crf_forward_train_wide_dev / dsrg_crf_backward_wide_dev (or _wide_theta / _wide_feat)",
               DSRG_MAX_LABELS, e->M);
     return DSRG_E_INVALID;
 }
@@ -961,6 +961,110 @@ int dsrg_crf_backward_wide_dev(dsrg_engine *h, const float *q_hist, int B, const
                                            *params, s);
         });
         e->last_crf_B = 0;
+        return rc;
+    });
+}
+
+// The label-chunked kernel-bandwidth and feature backward's buffers on its first call (as ensure_compat_part): c per
+// pixel [2][maxB][N] and the per-block sums, as ensure_kgrad, and the normalisation term's two value buffers per
+// lattice at 4 floats per row.  g_t stays in e->Q0 and Vy in the mean-field buffers, so nothing here grows with the
+// label count.
+static int ensure_kgrad_wide(Engine *e) {
+    if (e->kg_csum) return DSRG_OK;
+    cudaStreamCaptureMode mode = cudaStreamCaptureModeRelaxed;
+    DSRG_CUDA_TRY(cudaThreadExchangeStreamCaptureMode(&mode));
+    int rc = 0;
+    rc |= dalloc(e, &e->kg_csum, (size_t)2 * e->maxB * e->Ncap);
+    rc |= dalloc(e, &e->kg_part, (size_t)e->maxB * ((e->Ncap + kThreads - 1) / kThreads) * 8);
+    for (int i = 0; i < 2; i++) {
+        rc |= dalloc(e, &e->kg_sp[i], (size_t)e->sp.rows_cap * 4);
+        rc |= dalloc(e, &e->kg_bi[i], (size_t)e->bi.rows_cap * 4);
+    }
+    DSRG_CUDA_TRY(cudaThreadExchangeStreamCaptureMode(&mode));
+    return rc ? DSRG_E_NOMEM : DSRG_OK;
+}
+
+int dsrg_crf_backward_wide_theta_dev(dsrg_engine *h, const float *q_hist, int B, const uint8_t *image,
+                                     const dsrg_crf_params *params, const float *potts, const float *compat,
+                                     const float *grad_q, float *grad_unary, float *grad_potts, float *grad_compat,
+                                     float *grad_theta, void *stream) {
+    const cudaStream_t s = (cudaStream_t)stream;
+    const bool ok = q_hist && image && params && grad_q && grad_unary && grad_theta && !(potts && compat) &&
+                    !(grad_potts && compat) && !(grad_compat && !compat);
+    return dev_call(h, B, s, ok, [&](Engine *e) {
+        if (int rc = wide_labels_ok(e)) return rc;
+        if (int rc = ensure_wide(e, compat != nullptr)) return rc;
+        if (int rc = ensure_kgrad_wide(e)) return rc;
+        GraphKey args;
+        args.add(q_hist).add(image).add(potts).add(compat).add(grad_q).add(grad_unary).add(grad_potts).add(grad_compat)
+            .add(grad_theta);
+        const int rc = crf_pass(e, s, PassKind::crf_backward_wide_theta, B, params, args, [&]() {
+            int r = prepare_lattices(e, B, image, *params, s);   // as in dsrg_crf_backward_dev
+            if (r) return r;
+            return meanfield_backward_wide(e, B, q_hist, potts, compat, grad_q, grad_unary, grad_potts, grad_compat,
+                                           *params, s, grad_theta, image);
+        });
+        e->last_crf_B = 0;
+        return rc;
+    });
+}
+
+int dsrg_crf_forward_train_wide_feat_dev(dsrg_engine *h, const float *unary, int B, const float *features,
+                                         const dsrg_crf_params *params, const float *potts, const float *compat,
+                                         float *q_hist, void *stream) {
+    const cudaStream_t s = (cudaStream_t)stream;
+    return dev_call(h, B, s, unary && features && params && q_hist && !(potts && compat), [&](Engine *e) {
+        if (int rc = wide_labels_ok(e)) return rc;
+        if (int rc = ensure_feat(e)) return rc;
+        GraphKey args;
+        args.add(unary).add(features).add(potts).add(compat).add(q_hist);
+        const int rc = crf_pass(e, s, PassKind::crf_train_wide_feat, B, params, args, [&]() {
+            int r = prepare_lattices_feat(e, B, features, *params, s);
+            if (!r) r = meanfield_run_train_wide(e, B, unary, q_hist, potts, compat, *params, s);
+            if (r) return r;
+            const long long mn = (long long)e->M * e->N;
+            nan_images(e, e->feat_bad, q_hist, B, mn, params->n_iters + 1, B * mn, s);   // every kept iterate
+            DSRG_CUDA_TRY(cudaGetLastError());
+            return DSRG_OK;
+        });
+        e->last_crf_B = 0;
+        e->feat_B = rc == DSRG_OK ? B : 0;
+        return rc;
+    });
+}
+
+int dsrg_crf_backward_wide_feat_dev(dsrg_engine *h, const float *q_hist, int B, const float *features,
+                                    const dsrg_crf_params *params, const float *potts, const float *compat,
+                                    const float *grad_q, float *grad_unary, float *grad_features, float *grad_potts,
+                                    float *grad_compat, float *grad_theta_sp, void *stream) {
+    const cudaStream_t s = (cudaStream_t)stream;
+    const bool ok = q_hist && features && params && grad_q && grad_unary && grad_features && !(potts && compat) &&
+                    !(grad_potts && compat) && !(grad_compat && !compat);
+    return dev_call(h, B, s, ok, [&](Engine *e) {
+        if (int rc = wide_labels_ok(e)) return rc;
+        if (int rc = ensure_wide(e, compat != nullptr)) return rc;
+        if (int rc = ensure_kgrad_wide(e)) return rc;
+        if (int rc = ensure_feat(e)) return rc;
+        GraphKey args;
+        args.add(q_hist).add(features).add(potts).add(compat).add(grad_q).add(grad_unary).add(grad_features)
+            .add(grad_potts).add(grad_compat).add(grad_theta_sp);
+        const int rc = crf_pass(e, s, PassKind::crf_backward_wide_feat, B, params, args, [&]() {
+            int r = prepare_lattices_feat(e, B, features, *params, s);   // as in dsrg_crf_backward_dev
+            if (!r)
+                r = meanfield_backward_wide(e, B, q_hist, potts, compat, grad_q, grad_unary, grad_potts, grad_compat,
+                                            *params, s, nullptr, nullptr, features, grad_features, grad_theta_sp);
+            if (r) return r;
+            const long long M = e->M, N = e->N;
+            const std::pair<float *, long long> outs[] = {{grad_unary, M * N}, {grad_features, 5 * N},
+                                                          {grad_potts, 2}, {grad_compat, 2 * M * M},
+                                                          {grad_theta_sp, 2}};
+            for (const auto &o : outs)
+                if (o.first) nan_images(e, e->feat_bad, o.first, B, o.second, 1, 0, s);
+            DSRG_CUDA_TRY(cudaGetLastError());
+            return DSRG_OK;
+        });
+        e->last_crf_B = 0;
+        e->feat_B = rc == DSRG_OK ? B : 0;
         return rc;
     });
 }

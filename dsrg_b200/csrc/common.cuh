@@ -184,13 +184,17 @@ int meanfield_run_wide(Engine *e, int B, const float *unary, int unary_layout, b
 int wide_weights(Engine *e, Lattice &L, int nb, cudaStream_t s);
 // the training forward and its backward above DSRG_MAX_LABELS labels, as meanfield_run_train / meanfield_backward
 // (potts or compat, not both); the backward needs e->wide_ppart, and with compat e->wide_g and e->wide_cpart
-// (ensure_wide).  The matrices' outer products are summed per image over kWideChunks fixed pixel chunks.
+// (ensure_wide).  The matrices' outer products are summed per image over kWideChunks fixed pixel chunks.  grad_theta,
+// or feat / grad_feat / grad_theta_sp, mean what they mean in meanfield_backward and need e->kg_csum, e->kg_part and
+// the 4-wide e->kg_sp / e->kg_bi (ensure_kgrad_wide)
 constexpr int kWideChunks = 16;
 int meanfield_run_train_wide(Engine *e, int B, const float *unary, float *q_hist, const float *potts,
                              const float *compat, const dsrg_crf_params &p, cudaStream_t s);
 int meanfield_backward_wide(Engine *e, int B, const float *q_hist, const float *potts, const float *compat,
                             const float *grad_q, float *grad_unary, float *grad_potts, float *grad_compat,
-                            const dsrg_crf_params &p, cudaStream_t s);
+                            const dsrg_crf_params &p, cudaStream_t s, float *grad_theta = nullptr,
+                            const uint8_t *image = nullptr, const float *feat = nullptr, float *grad_feat = nullptr,
+                            float *grad_theta_sp = nullptr);
 int meanfield_export(Engine *e, int B, float *out, int layout, cudaStream_t s);
 int meanfield_export_map(Engine *e, int B, int32_t *labels, cudaStream_t s);
 int meanfield_export_renorm(Engine *e, int B, float *result_out, float *log_out, cudaStream_t s);
@@ -232,7 +236,9 @@ struct Engine {
     // first call (ensure_compat_part)
     float *compat_part = nullptr;
     // the kernel-bandwidth backward's buffers, allocated by its first call (ensure_kgrad): g_t [maxB][M][N], c per
-    // pixel [2][maxB][N], per-block sums [maxB][blocks][8], and two value buffers per lattice [rows][MP]
+    // pixel [2][maxB][N], per-block sums [maxB][blocks][8], and two value buffers per lattice [rows][MP].  Above
+    // DSRG_MAX_LABELS (ensure_kgrad_wide) there is no kg_g, and the value buffers are [rows][4]: the label-chunked
+    // backward uses them only for the normalisation term
     float *kg_g = nullptr, *kg_csum = nullptr, *kg_part = nullptr;
     float *kg_sp[2] = {nullptr, nullptr}, *kg_bi[2] = {nullptr, nullptr};
     // the feature passes' per-image key-range flags [maxB] (allocated by the first one) and that pass's batch
@@ -453,7 +459,8 @@ cudaError_t numa_host_alloc(void **p, size_t bytes, int device);
 // or if capture fails.  `body` issues the launches on `s` and returns a DSRG_* code.
 enum class PassKind : int { crf, crf_map, forward, crflayer, densecrf, post, crf_train, crf_backward, crf_train_compat,
                             crf_backward_compat, crf_backward_theta, crf_backward_compat_theta, crf_train_feat,
-                            crf_backward_feat, crf_train_wide, crf_backward_wide };
+                            crf_backward_feat, crf_train_wide, crf_backward_wide, crf_backward_wide_theta,
+                            crf_train_wide_feat, crf_backward_wide_feat };
 struct GraphKey {
     std::string bytes;
     GraphKey() = default;

@@ -10,6 +10,7 @@
 // (the reference pads 21 -> 24 the same way, permutohedral.cpp:531).
 #include "common.cuh"
 #include "simplex.cuh"
+#include "kgrad.cuh"
 
 namespace dsrg {
 
@@ -1077,67 +1078,6 @@ k_mf_compat_reduce(const float *part, float *out, int ntiles, int mm2) {
 // elevation matrix, and to the DIAG parameters as dL/dp_i = sum f_i (dL/df)_i.  Each 256-pixel block keeps its seven
 // sums in part[b][block] (the first pass writes them), and k_kg_reduce adds the blocks in order: no float atomics.
 // ---------------------------------------------------------------------------------------------
-struct KgLat {
-    const int32_t *off;      // [nimg][d+1][N]
-    const float *bary, *wn;  // [nimg][d+1][N]
-    const float *norm;       // [nimg][N]
-    const int32_t *rowbase;
-    int shared;
-    float alpha;
-    float sigma[5], scale[5];
-};
-struct KgArgs {
-    KgLat sp, bi;
-    const uint8_t *image;  // [B][N][3]
-    const float *potts;    // {w1, w2} on the device, or nullptr: w1, w2
-    float w1, w2;
-    float *part;           // [B][nblk][8] per-block sums of dL/dp in theta order
-    float *csum;           // [2][B][N] c per pixel: spatial, bilateral
-    int M, N, W, nblk;
-};
-
-// per-incidence s_r of one lattice -> the pixel's dL/dp over that lattice's features (added to dp), scaled by sign.
-// FEAT: the features are the caller's (feat [B][D][N]), and the pixel's dL/df also goes to gfeat [B][D][N] (written
-// when `first`, else added).
-template <int D, bool FEAT = false>
-__device__ __forceinline__ void kg_features(const KgLat &L, int x, int y, const uint8_t *image, int b, int N,
-                                            int i, const float *s, float sign, float *dp, const float *feat = nullptr,
-                                            float *gfeat = nullptr, bool first = false) {
-    float f[D], el[D + 1], rem0[D + 1];
-    int rank[D + 1];
-    if constexpr (FEAT) {
-#pragma unroll
-        for (int j = 0; j < D; j++) f[j] = __ldg(feat + ((size_t)b * D + j) * N + i);
-    } else {
-        lattice_features<D>(x, y, image, b, N, i, L.sigma, f);
-    }
-    lattice_simplex<D>(f, L.scale, el, rem0, rank);
-    const float c = sign * L.alpha / (float)(D + 1);
-    float gel[D + 1];
-#pragma unroll
-    for (int j = 0; j <= D; j++) {
-        const int r0 = D - rank[j], r1 = r0 == D ? 0 : r0 + 1;
-        float a = 0.0f, b = 0.0f;
-#pragma unroll
-        for (int r = 0; r <= D; r++) {
-            if (r == r0) a = s[r];
-            if (r == r1) b = s[r];
-        }
-        gel[j] = c * (a - b);
-    }
-    float sm = gel[0];
-#pragma unroll
-    for (int j = 1; j <= D; j++) {
-        const float df = L.scale[j - 1] * (sm - (float)j * gel[j]);   // dL/df_{j-1}
-        dp[j - 1] = fmaf(f[j - 1], df, dp[j - 1]);
-        if constexpr (FEAT) {
-            float *o = gfeat + ((size_t)b * D + j - 1) * N + i;
-            *o = first ? df : *o + df;
-        }
-        sm += gel[j];
-    }
-}
-
 // s_r = n * w * (x . Vy[r] + u . Vg[r]) at every incidence of one lattice; c = 1/2 n^2 alpha sum_r bary_r s_r
 template <int MP, int D>
 __device__ __forceinline__ float kg_incidences(const KgLat &L, int b, int i, int N, const float *x, const float *u,
@@ -1167,29 +1107,6 @@ __device__ __forceinline__ float kg_incidences(const KgLat &L, int b, int i, int
         cs = fmaf(__ldg(L.bary + at + (size_t)r * N), s[r], cs);
     }
     return 0.5f * n * n * L.alpha * cs;
-}
-
-// the block's seven sums into part[b][block] (written when `first`, else added), in a fixed order
-__device__ __forceinline__ void kg_block_sum(const KgArgs &a, int b, const float *dp, bool first) {
-    __shared__ float red[kThreads / 32][7];
-    float v[7];
-#pragma unroll
-    for (int k = 0; k < 7; k++) {
-        v[k] = dp[k];
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) v[k] += __shfl_down_sync(0xffffffffu, v[k], o);
-    }
-    if ((threadIdx.x & 31) == 0) {
-#pragma unroll
-        for (int k = 0; k < 7; k++) red[threadIdx.x >> 5][k] = v[k];
-    }
-    __syncthreads();
-    if (threadIdx.x < 7) {
-        float acc = 0.0f;
-        for (int w = 0; w < kThreads / 32; w++) acc += red[w][threadIdx.x];
-        float *pp = a.part + ((size_t)b * a.nblk + blockIdx.x) * 8 + threadIdx.x;
-        *pp = first ? acc : *pp + acc;
-    }
 }
 
 // splat wn Q_t into both lattices' zeroed targets (the forward's splat, straight to global rows)
@@ -1750,7 +1667,7 @@ static int run_impl(Engine *e, int B, const float *unary, int layout, bool clamp
 // The backward of a training forward (DenseCRF::gradient, densecrf.cpp:238-297) on the lattices the pass just built:
 // k_mf_tile_bwd from T down to 0 with the transposed blur in between, then the per-image Potts sums -- or, with
 // `compat` ({mu_bi, mu_sp}), the MODE_COMPAT kernels and the per-image compatibility sums to g_compat ([B][2][M][M]).
-static KgLat kg_lat(const Lattice &L) {
+KgLat kg_lat(const Lattice &L) {
     KgLat k;
     k.off = L.off;
     k.bary = L.bary;
@@ -1811,8 +1728,8 @@ static void kg_iter(Engine *e, const KgArgs &ka, bool compat, int B, const float
 // by now: spA / biA take the reverse-blurred splat of c, the kernel-gradient buffers the forward-blurred one of ones.
 // With `feat`: k_kgf_norm adds the term's dL/df to gfeat, and only the spatial sums are reduced (to g_theta [B][2],
 // when given).
-static void kg_finish(Engine *e, const KgArgs &ka, int B, float *g_theta, int bgrid, cudaStream_t s,
-                      const float *feat, float *gfeat, int tag) {
+void kg_finish(Engine *e, const KgArgs &ka, int B, float *g_theta, int bgrid, cudaStream_t s, const float *feat,
+               float *gfeat, int tag) {
     const dim3 gp(ka.nblk, B);
     DSRG_LAUNCH(e, tag, s,
                 k_mf_zero<4><<<bgrid, kThreads, 0, s>>>((float4 *)e->kg_sp[0], e->sp.rowbase, (float4 *)e->kg_bi[0],

@@ -8,6 +8,7 @@
 // labels (densecrf.cpp:98-106).  It moves every value through L2 and is several times slower per label than the
 // fused path -- it exists so that the boundary has no hole, not for the 21-class hot path.
 #include "common.cuh"
+#include "kgrad.cuh"
 
 namespace dsrg {
 
@@ -429,14 +430,139 @@ k_wide_outer(const float *S_sp, const float *S_bi, const float *Qt, float *part,
         }
 }
 
+// ---------------------------------------------------------------------------------------------
+// The kernel-bandwidth and feature gradient above 32 labels: the math of the fused path (kgrad.cuh, the comment above
+// KgLat in meanfield.cu) with the label dimension chunked into quads.  Iteration it (T down to 1) pairs g_it with
+// Q_{it-1}, as kg_iter pairs g_{t+1} with Q_t: Vg = B^T S(n g_it) is the reverse-blurred buffer the backward slices,
+// Vy = B S(n Q_{it-1}) a forward splat and blur into the buffers Vg leaves free, and per lattice
+//   Potts : x = g_it, u = Q_{it-1}, and the lattice's weight w
+//   matrix: x = -mu^T g_it, u = -mu Q_{it-1} (k_wide_compat_xu), w = 1
+// k_wide_kg_pass forms s_r at every incidence and the pixel's c, then kg_features rotates s into dL/dp (and for
+// caller-given features dL/df).  The normalisation term and the per-image sums after the loop are kg_finish's.
+// ---------------------------------------------------------------------------------------------
+
+// x = -mu^T g and u = -mu Q for one matrix mu ([M][M]), planar [B][M][N], one thread per (pixel, label quad); the
+// block's quad needs four columns and four rows of mu, 8 M floats in shared memory (as k_wide_compat_msg)
+__global__ void __launch_bounds__(kThreads)
+k_wide_compat_xu(const float *g, const float *Q, const float *mu, float *x, float *u, int M, int N) {
+    extern __shared__ float mus[];   // [2 = mu^T, mu][4][M]
+    const int b = blockIdx.z, c = blockIdx.y;
+    for (int e = threadIdx.x; e < 8 * M; e += blockDim.x) {
+        const int m = e / (4 * M), k = (e / M) & 3, l2 = e % M, l = 4 * c + k;
+        mus[e] = l < M ? (m ? mu[(size_t)l * M + l2] : mu[(size_t)l2 * M + l]) : 0.0f;
+    }
+    __syncthreads();
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= N) return;
+    const float *gp = g + (size_t)b * M * N + i, *qp = Q + (size_t)b * M * N + i;
+    float xa[4] = {0.0f, 0.0f, 0.0f, 0.0f}, ua[4] = {0.0f, 0.0f, 0.0f, 0.0f};
+    for (int l2 = 0; l2 < M; l2++) {
+        const float gv = gp[(size_t)l2 * N], qv = qp[(size_t)l2 * N];
+#pragma unroll
+        for (int k = 0; k < 4; k++) {
+            xa[k] = fmaf(-mus[k * M + l2], gv, xa[k]);
+            ua[k] = fmaf(-mus[(4 + k) * M + l2], qv, ua[k]);
+        }
+    }
+#pragma unroll
+    for (int k = 0; k < 4; k++) {
+        if (4 * c + k < M) {
+            x[((size_t)b * M + 4 * c + k) * N + i] = xa[k];
+            u[((size_t)b * M + 4 * c + k) * N + i] = ua[k];
+        }
+    }
+}
+
+// s_r = n w sum over the label quads, ascending, of x . Vy[r] + u . Vg[r] at the D + 1 incidences of one lattice;
+// returns c = 1/2 n^2 alpha sum_r bary_r s_r (kg_incidences with the labels chunked)
+template <int D>
+__device__ __forceinline__ float wide_kg_incidences(const KgLat &L, int b, int i, int M, int N, int CH, const float *x,
+                                                    const float *u, float w, const float4 *vy, const float4 *vg,
+                                                    float *s) {
+    const size_t at = (size_t)(L.shared ? 0 : b) * (D + 1) * N + i;
+    const int base = L.rowbase[b];
+    const float n = __ldg(L.norm + (size_t)(L.shared ? 0 : b) * N + i);
+    size_t row[D + 1];
+    float acc[D + 1];
+#pragma unroll
+    for (int r = 0; r <= D; r++) {
+        row[r] = (size_t)(base + __ldg(L.off + at + (size_t)r * N)) * CH;
+        acc[r] = 0.0f;
+    }
+    const float *xp = x + (size_t)b * M * N + i, *up = u + (size_t)b * M * N + i;
+    for (int c = 0; c < CH; c++) {
+        float xv[4], uv[4];
+#pragma unroll
+        for (int k = 0; k < 4; k++) {
+            const int l = 4 * c + k;
+            xv[k] = l < M ? __ldg(xp + (size_t)l * N) : 0.0f;
+            uv[k] = l < M ? __ldg(up + (size_t)l * N) : 0.0f;
+        }
+#pragma unroll
+        for (int r = 0; r <= D; r++) {
+            const float4 a = vy[row[r] + c], g = vg[row[r] + c];
+            float t = acc[r];
+            t = fmaf(xv[0], a.x, t);
+            t = fmaf(xv[1], a.y, t);
+            t = fmaf(xv[2], a.z, t);
+            t = fmaf(xv[3], a.w, t);
+            t = fmaf(uv[0], g.x, t);
+            t = fmaf(uv[1], g.y, t);
+            t = fmaf(uv[2], g.z, t);
+            t = fmaf(uv[3], g.w, t);
+            acc[r] = t;
+        }
+    }
+    float cs = 0.0f;
+#pragma unroll
+    for (int r = 0; r <= D; r++) {
+        s[r] = n * w * acc[r];
+        cs = fmaf(__ldg(L.bary + at + (size_t)r * N), s[r], cs);
+    }
+    return 0.5f * n * n * L.alpha * cs;
+}
+
+// One thread per pixel, for each lattice whose x is given (the Potts pass runs both, the matrices one per launch):
+// s_r and c (added to csum), the rotation to dL/dp (FEAT: the bilateral features are feat's and the pixel's dL/df goes
+// to gfeat), then the block's sums to part.  `first`: csum and gfeat of the given lattices are written, not added;
+// `part_first`: the same for part.  The weights are a.potts ({w1, w2}, device) or a.w1 / a.w2 (1 for the matrices).
+template <bool FEAT>
+__global__ void __launch_bounds__(kThreads)
+k_wide_kg_pass(KgArgs a, const float *x_sp, const float *u_sp, const float *x_bi, const float *u_bi,
+               const float4 *vy_sp, const float4 *vg_sp, const float4 *vy_bi, const float4 *vg_bi, int CH, int first,
+               int part_first, const float *feat, float *gfeat) {
+    const int b = blockIdx.y, i = blockIdx.x * kThreads + threadIdx.x;
+    float dp[7];
+#pragma unroll
+    for (int k = 0; k < 7; k++) dp[k] = 0.0f;
+    if (i < a.N) {
+        const int x = i % a.W, y = i / a.W;
+        float s[6];
+        float *csum_sp = a.csum + (size_t)b * a.N + i, *csum_bi = csum_sp + (size_t)gridDim.y * a.N;
+        if (x_sp) {
+            const float w = a.potts ? __ldg(a.potts + 1) : a.w2;
+            const float c = wide_kg_incidences<2>(a.sp, b, i, a.M, a.N, CH, x_sp, u_sp, w, vy_sp, vg_sp, s);
+            kg_features<2>(a.sp, x, y, a.image, b, a.N, i, s, 1.0f, dp + 5);
+            *csum_sp = first ? c : *csum_sp + c;
+        }
+        if (x_bi) {
+            const float w = a.potts ? __ldg(a.potts) : a.w1;
+            const float c = wide_kg_incidences<5>(a.bi, b, i, a.M, a.N, CH, x_bi, u_bi, w, vy_bi, vg_bi, s);
+            kg_features<5, FEAT>(a.bi, x, y, a.image, b, a.N, i, s, 1.0f, dp, feat, gfeat, first != 0);
+            *csum_bi = first ? c : *csum_bi + c;
+        }
+    }
+    kg_block_sum(a, b, dp, part_first != 0);
+}
+
 static WideLat wide_lat(const Lattice &L, float *val) { return WideLat{L.off, L.wn, L.rowbase, val, L.shared, L.d + 1}; }
 
-// zero Y, splat X planar into it, blur every axis (d..0 when `reverse`, K^T); returns the blurred buffers
-static void wide_filter(Engine *e, int B, const float *X, bool reverse, int tag, cudaStream_t s, float **sp_out,
-                        float **bi_out) {
+// zero Y, splat X planar into it, blur every axis (d..0 when `reverse`, K^T) ping-ponging with Z; returns the
+// blurred buffers
+static void wide_filter_to(Engine *e, int B, const float *X, bool reverse, int tag, cudaStream_t s, float *spY,
+                           float *spZ, float *biY, float *biZ, float **sp_out, float **bi_out) {
     const int M = e->M, N = e->N, CH = e->MP / 4, grid = 8 * e->sm_count;
     const dim3 gq(cdiv(N, kThreads), CH, B);
-    float *spY = e->spA, *spZ = e->spB, *biY = e->biA, *biZ = e->biB;
     DSRG_LAUNCH(e, tag, s, k_wide_zero<<<grid, kThreads, 0, s>>>((float4 *)spY, e->sp.rowbase, (float4 *)biY, e->bi.rowbase, B, CH));
     DSRG_LAUNCH(e, tag, s, k_wide_splat<<<gq, kThreads, 0, s>>>(X, wide_lat(e->sp, spY), wide_lat(e->bi, biY), M, N, CH));
     for (int l = 0; l < 2; l++) {
@@ -452,6 +578,12 @@ static void wide_filter(Engine *e, int B, const float *X, bool reverse, int tag,
     }
     *sp_out = spY;
     *bi_out = biY;
+}
+
+// wide_filter_to on the mean-field buffers spA / spB and biA / biB
+static void wide_filter(Engine *e, int B, const float *X, bool reverse, int tag, cudaStream_t s, float **sp_out,
+                        float **bi_out) {
+    wide_filter_to(e, B, X, reverse, tag, s, e->spA, e->spB, e->biA, e->biB, sp_out, bi_out);
 }
 
 static float wide_alpha(const Lattice &L) { return 1.0f / (1 + powf(2, -L.d)); }   // permutohedral.cpp:571
@@ -485,13 +617,35 @@ int meanfield_run_train_wide(Engine *e, int B, const float *unary, float *q_hist
 
 int meanfield_backward_wide(Engine *e, int B, const float *q_hist, const float *potts, const float *compat,
                             const float *grad_q, float *grad_unary, float *grad_potts, float *grad_compat,
-                            const dsrg_crf_params &p, cudaStream_t s) {
+                            const dsrg_crf_params &p, cudaStream_t s, float *grad_theta, const uint8_t *image,
+                            const float *feat, float *grad_feat, float *grad_theta_sp) {
     const int M = e->M, N = e->N, CH = e->MP / 4, T = p.n_iters;
     const size_t slab = (size_t)B * M * N;
     const int nblk = cdiv(N, kThreads);
     const dim3 gp(nblk, B), gq(nblk, CH, B);
     const float a_sp = wide_alpha(e->sp), a_bi = wide_alpha(e->bi);
-    // e->Q0: g_t, then S_sp (matrices) or G_{t-1} (Potts); e->U: S_bi; e->wide_g: the matrices' G_{t-1}
+    // the kernel-bandwidth gradient (grad_theta), or the feature gradient (grad_feat) with the spatial sums to
+    // grad_theta_sp: per iteration Vy into the buffers Vg leaves free and k_wide_kg_pass, kg_finish after the loop
+    if (grad_feat) grad_theta = grad_theta_sp;
+    const bool kg = grad_theta || grad_feat;
+    const int kg_tag = grad_feat ? T_FGRAD : T_KGRAD;
+    KgArgs ka{};
+    if (kg) {
+        ka.sp = kg_lat(e->sp);
+        ka.bi = kg_lat(e->bi);
+        ka.image = image;
+        ka.potts = compat ? nullptr : potts;
+        ka.w1 = compat ? 1.0f : p.w1;   // the matrices' x and u carry mu
+        ka.w2 = compat ? 1.0f : p.w2;
+        ka.part = e->kg_part;
+        ka.csum = e->kg_csum;
+        ka.M = M;
+        ka.N = N;
+        ka.W = e->W;
+        ka.nblk = nblk;
+    }
+    // e->Q0: g_t, then S_sp (matrices) or G_{t-1} (Potts); e->U: S_bi; e->wide_g: the matrices' G_{t-1}.  With kg and
+    // matrices, e->U and e->wide_g hold x and u of one lattice before the slice (G_t was read by the VJP by then).
     float *X = e->Q0;
     const float *G = grad_q;
     const int tl = (M + kWideOuterTile - 1) / kWideOuterTile;
@@ -502,6 +656,36 @@ int meanfield_backward_wide(Engine *e, int B, const float *q_hist, const float *
         DSRG_LAUNCH(e, T_WIDE_GRAD, s, k_wide_vjp<<<gp, kThreads, 0, s>>>(G, qt, grad_unary, X, first, M, N));
         float *spV, *biV;
         wide_filter(e, B, X, true, T_WIDE_GRAD, s, &spV, &biV);
+        if (kg) {
+            // Vy = B S(n Q_{it-1}) in the mean-field buffer Vg does not hold and spC / biC
+            float *vy_sp, *vy_bi;
+            wide_filter_to(e, B, qp, false, kg_tag, s, spV == e->spA ? e->spB : e->spA, e->spC,
+                           biV == e->biA ? e->biB : e->biA, e->biC, &vy_sp, &vy_bi);
+            const float4 *ysp = (const float4 *)vy_sp, *ybi = (const float4 *)vy_bi;
+            const float4 *gsp = (const float4 *)spV, *gbi = (const float4 *)biV;
+#define DSRG_KG_PASS(XS, US, XB, UB, PF)                                                                              \
+    do {                                                                                                              \
+        if (feat)                                                                                                     \
+            DSRG_LAUNCH(e, kg_tag, s,                                                                                 \
+                        k_wide_kg_pass<true><<<gp, kThreads, 0, s>>>(ka, XS, US, XB, UB, ysp, gsp, ybi, gbi, CH,      \
+                                                                     first, PF, feat, grad_feat));                    \
+        else                                                                                                          \
+            DSRG_LAUNCH(e, kg_tag, s,                                                                                 \
+                        k_wide_kg_pass<false><<<gp, kThreads, 0, s>>>(ka, XS, US, XB, UB, ysp, gsp, ybi, gbi, CH,     \
+                                                                      first, PF, nullptr, nullptr));                  \
+    } while (0)
+            if (compat) {   // one lattice per launch: x, u of the spatial matrix, then of the bilateral one
+                const size_t smem = 8 * M * sizeof(float);
+                DSRG_LAUNCH(e, kg_tag, s,
+                            k_wide_compat_xu<<<gq, kThreads, smem, s>>>(X, qp, compat + (size_t)M * M, e->U, e->wide_g, M, N));
+                DSRG_KG_PASS(e->U, e->wide_g, nullptr, nullptr, first);
+                DSRG_LAUNCH(e, kg_tag, s, k_wide_compat_xu<<<gq, kThreads, smem, s>>>(X, qp, compat, e->U, e->wide_g, M, N));
+                DSRG_KG_PASS(nullptr, nullptr, e->U, e->wide_g, 0);
+            } else {
+                DSRG_KG_PASS(X, qp, X, qp, first);
+            }
+#undef DSRG_KG_PASS
+        }
         const WideLat sp = wide_lat(e->sp, spV), bi = wide_lat(e->bi, biV);
         if (compat) {
             DSRG_LAUNCH(e, T_WIDE_GRAD, s, k_wide_slice_planar<<<gq, kThreads, 0, s>>>(X, e->U, sp, bi, a_sp, a_bi, M, N, CH));
@@ -523,10 +707,15 @@ int meanfield_backward_wide(Engine *e, int B, const float *q_hist, const float *
     if (T == 0) {
         if (grad_potts) DSRG_CUDA_TRY(cudaMemsetAsync(grad_potts, 0, sizeof(float) * 2 * B, s));
         if (grad_compat) DSRG_CUDA_TRY(cudaMemsetAsync(grad_compat, 0, sizeof(float) * 2 * M * M * B, s));
-    } else if (grad_potts) {
-        potts_reduce(e, e->wide_ppart, grad_potts, CH * nblk, B, T_WIDE_GRAD, s);
-    } else if (grad_compat) {
-        compat_reduce(e, e->wide_cpart, grad_compat, kWideChunks, 2 * M * M, B, T_WIDE_GRAD, s);
+        if (grad_feat) DSRG_CUDA_TRY(cudaMemsetAsync(grad_feat, 0, sizeof(float) * 5 * N * B, s));
+        if (grad_theta) DSRG_CUDA_TRY(cudaMemsetAsync(grad_theta, 0, sizeof(float) * (grad_feat ? 2 : 7) * B, s));
+    } else {
+        if (grad_potts) {
+            potts_reduce(e, e->wide_ppart, grad_potts, CH * nblk, B, T_WIDE_GRAD, s);
+        } else if (grad_compat) {
+            compat_reduce(e, e->wide_cpart, grad_compat, kWideChunks, 2 * M * M, B, T_WIDE_GRAD, s);
+        }
+        if (kg) kg_finish(e, ka, B, grad_theta, 8 * e->sm_count, s, feat, grad_feat, kg_tag);
     }
     DSRG_CUDA_TRY(cudaGetLastError());
     return DSRG_OK;

@@ -420,29 +420,26 @@ class _DenseCrfCompat(torch.autograd.Function):
 
 class _DenseCrfTheta(torch.autograd.Function):
     """dense_crf with learnable kernel bandwidths: theta_bi (5,), theta_sp (2,) (None: params' own values) beside
-    the Potts weights (w1, w2) or the matrices (compat (2, M, M) {mu_bi, mu_sp}); params carries the sigmas."""
+    the Potts weights (w1, w2) or the matrices (compat (2, M, M) {mu_bi, mu_sp}); params carries the sigmas.  wide: the
+    label-chunked entry points (dense_crf_wide above 32 labels) in place of the fused ones."""
 
     @staticmethod
     @_fwd
-    def forward(ctx, unary, image, w1, w2, compat, theta_bi, theta_sp, params):
+    def forward(ctx, unary, image, w1, w2, compat, theta_bi, theta_sp, params, wide):
         eng = _engine_for(unary)
         s = _stream(unary)
         maxiter = params.n_iters
         q_hist = torch.empty((maxiter + 1,) + tuple(unary.shape), dtype=torch.float32, device=unary.device)
-        potts = None
-        if compat is not None:
+        potts = _potts_tensor(w1, w2, unary) if compat is None else None
+        if wide:
+            eng.crf_forward_train_wide_dev(unary, image, params, q_hist, potts=potts, compat=compat, stream=s)
+        elif compat is not None:
             eng.crf_forward_train_compat_dev(unary, image, params, compat, q_hist, stream=s)
         else:
-            if w1 is not None or w2 is not None:
-                potts = torch.empty(2, dtype=torch.float32, device=unary.device)
-                for i, (w, d) in enumerate(zip((w1, w2), _POTTS_DEFAULT)):
-                    if w is None:
-                        potts[i].fill_(d)
-                    else:
-                        potts[i].copy_(w.detach())
             eng.crf_forward_train_dev(unary, image, params, q_hist, potts=potts, stream=s)
         ctx.save_for_backward(q_hist, image, potts, compat)
         ctx.params = params
+        ctx.wide = wide
         ctx.theta = [(t.device, t.dtype) if t is not None else None for t in (theta_bi, theta_sp)]
         return q_hist[maxiter].clone()
 
@@ -450,33 +447,34 @@ class _DenseCrfTheta(torch.autograd.Function):
     @_bwd
     def backward(ctx, g):
         q_hist, image, potts, compat = ctx.saved_tensors
-        B = q_hist.shape[1]
-        grad_u = torch.empty(q_hist.shape[1:], dtype=torch.float32, device=q_hist.device)
-        grad_t = torch.empty((B, 7), dtype=torch.float32, device=q_hist.device)
+        B, dev = q_hist.shape[1], q_hist.device
+        need = ctx.needs_input_grad
+        grad_u = torch.empty(q_hist.shape[1:], dtype=torch.float32, device=dev)
+        grad_t = torch.empty((B, 7), dtype=torch.float32, device=dev)
         eng, s = _engine_for(grad_u), _stream(grad_u)
-        gw1 = gw2 = gc = None
-        if compat is not None:
-            grad_c = None
-            if ctx.needs_input_grad[4]:
-                M = compat.shape[-1]
-                grad_c = torch.empty((B, 2, M, M), dtype=torch.float32, device=q_hist.device)
+        grad_potts = grad_c = None
+        if potts is not None and (need[2] or need[3]):
+            grad_potts = torch.empty((B, 2), dtype=torch.float32, device=dev)
+        if compat is not None and need[4]:
+            M = compat.shape[-1]
+            grad_c = torch.empty((B, 2, M, M), dtype=torch.float32, device=dev)
+        if ctx.wide:
+            eng.crf_backward_wide_theta_dev(q_hist, image, ctx.params, g.contiguous(), grad_u, grad_t, potts=potts,
+                                            compat=compat, grad_potts=grad_potts, grad_compat=grad_c, stream=s)
+        elif compat is not None:
             eng.crf_backward_compat_theta_dev(q_hist, image, ctx.params, compat, g.contiguous(), grad_u, grad_t,
                                               grad_compat=grad_c, stream=s)
-            gc = None if grad_c is None else grad_c.sum(0)
         else:
-            grad_potts = None
-            if potts is not None and (ctx.needs_input_grad[2] or ctx.needs_input_grad[3]):
-                grad_potts = torch.empty((B, 2), dtype=torch.float32, device=q_hist.device)
             eng.crf_backward_theta_dev(q_hist, image, ctx.params, g.contiguous(), grad_u, grad_t,
                                        grad_potts=grad_potts, potts=potts, stream=s)
-            gw1 = grad_potts[:, 0].sum() if grad_potts is not None and ctx.needs_input_grad[2] else None
-            gw2 = grad_potts[:, 1].sum() if grad_potts is not None and ctx.needs_input_grad[3] else None
+        gw1 = grad_potts[:, 0].sum() if grad_potts is not None and need[2] else None
+        gw2 = grad_potts[:, 1].sum() if grad_potts is not None and need[3] else None
+        gc = None if grad_c is None else grad_c.sum(0)
         gt = grad_t.sum(0)
         out = []
-        for part, spec, need in ((gt[0:5], ctx.theta[0], ctx.needs_input_grad[5]),
-                                 (gt[5:7], ctx.theta[1], ctx.needs_input_grad[6])):
-            out.append(part.to(spec[0], spec[1]) if spec is not None and need else None)
-        return grad_u, None, gw1, gw2, gc, out[0], out[1], None
+        for part, spec, n in ((gt[0:5], ctx.theta[0], need[5]), (gt[5:7], ctx.theta[1], need[6])):
+            out.append(part.to(spec[0], spec[1]) if spec is not None and n else None)
+        return grad_u, None, gw1, gw2, gc, out[0], out[1], None, None
 
 
 def _potts_tensor(w1, w2, ref):
@@ -495,19 +493,20 @@ def _potts_tensor(w1, w2, ref):
 class _DenseCrfFeat(torch.autograd.Function):
     """dense_crf with caller-given bilateral features: features (N, 5, H, W) float32 beside the Potts weights (w1, w2)
     or the matrices (compat (2, M, M) {mu_bi, mu_sp}), and an optional learnable theta_sp; params carries the spatial
-    sigmas.  Nothing is read on the host."""
+    sigmas.  Nothing is read on the host.  wide: the label-chunked entry points (dense_crf_wide above 32 labels)."""
 
     @staticmethod
     @_fwd
-    def forward(ctx, unary, features, w1, w2, compat, theta_sp, params):
+    def forward(ctx, unary, features, w1, w2, compat, theta_sp, params, wide):
         eng = _engine_for(unary)
         maxiter = params.n_iters
         q_hist = torch.empty((maxiter + 1,) + tuple(unary.shape), dtype=torch.float32, device=unary.device)
         potts = _potts_tensor(w1, w2, unary) if compat is None else None
-        eng.crf_forward_train_feat_dev(unary, features, params, q_hist, potts=potts, compat=compat,
-                                       stream=_stream(unary))
+        fwd = eng.crf_forward_train_wide_feat_dev if wide else eng.crf_forward_train_feat_dev
+        fwd(unary, features, params, q_hist, potts=potts, compat=compat, stream=_stream(unary))
         ctx.save_for_backward(q_hist, features, potts, compat)
         ctx.params = params
+        ctx.wide = wide
         ctx.theta_sp = None if theta_sp is None else (theta_sp.device, theta_sp.dtype)
         return q_hist[maxiter].clone()
 
@@ -527,14 +526,15 @@ class _DenseCrfFeat(torch.autograd.Function):
             grad_c = torch.empty((B, 2, M, M), dtype=torch.float32, device=dev)
         if ctx.theta_sp is not None and need[5]:
             grad_tsp = torch.empty((B, 2), dtype=torch.float32, device=dev)
-        _engine_for(grad_u).crf_backward_feat_dev(q_hist, features, ctx.params, g.contiguous(), grad_u, grad_f,
-                                                  potts=potts, compat=compat, grad_potts=grad_potts,
-                                                  grad_compat=grad_c, grad_theta_sp=grad_tsp, stream=_stream(grad_u))
+        eng = _engine_for(grad_u)
+        bwd = eng.crf_backward_wide_feat_dev if ctx.wide else eng.crf_backward_feat_dev
+        bwd(q_hist, features, ctx.params, g.contiguous(), grad_u, grad_f, potts=potts, compat=compat,
+            grad_potts=grad_potts, grad_compat=grad_c, grad_theta_sp=grad_tsp, stream=_stream(grad_u))
         gw1 = grad_potts[:, 0].sum() if grad_potts is not None and need[2] else None
         gw2 = grad_potts[:, 1].sum() if grad_potts is not None and need[3] else None
         gc = None if grad_c is None else grad_c.sum(0)
         gt = None if grad_tsp is None else grad_tsp.sum(0).to(ctx.theta_sp[0], ctx.theta_sp[1])
-        return grad_u, grad_f if need[1] else None, gw1, gw2, gc, gt, None
+        return grad_u, grad_f if need[1] else None, gw1, gw2, gc, gt, None, None
 
 
 def _features(t, ref):
@@ -549,8 +549,9 @@ def _features(t, ref):
 
 
 def _dense_crf_feat(u, image, features_bi, scale_factor, color_factor, maxiter, w1, w2, compat_bi, compat_sp,
-                    theta_bi, theta_sp):
-    """dense_crf's path with caller-given bilateral features; every check before the first launch."""
+                    theta_bi, theta_sp, wide=False):
+    """dense_crf's path with caller-given bilateral features; every check before the first launch.  wide: the
+    label-chunked entry points (dense_crf_wide above 32 labels)."""
     if image is not None:
         raise ValueError("image is not used when features_bi is given: pass None")
     if theta_bi is not None:
@@ -568,7 +569,7 @@ def _dense_crf_feat(u, image, features_bi, scale_factor, color_factor, maxiter, 
     if compat_bi is not None or compat_sp is not None:
         compat = _compat_stack(u, u.shape[1], w1, w2, compat_bi, compat_sp)
         w1 = w2 = None
-    return _DenseCrfFeat.apply(u, f, w1, w2, compat, theta_sp, params)
+    return _DenseCrfFeat.apply(u, f, w1, w2, compat, theta_sp, params, wide)
 
 
 def _theta_values(theta, name, n, ref):
@@ -663,7 +664,7 @@ def dense_crf(unary, image, scale_factor=1.0, color_factor=13, maxiter=10, w1=No
         if compat_bi is not None or compat_sp is not None:
             compat = _compat_stack(u, M, w1, w2, compat_bi, compat_sp)
             w1 = w2 = None
-        return _DenseCrfTheta.apply(u, image.contiguous(), w1, w2, compat, theta_bi, theta_sp, params)
+        return _DenseCrfTheta.apply(u, image.contiguous(), w1, w2, compat, theta_bi, theta_sp, params, False)
     if compat_bi is None and compat_sp is None:
         return _DenseCrf.apply(u, image.contiguous(), w1, w2, float(scale_factor), float(color_factor), int(maxiter))
     return _DenseCrfCompat.apply(u, image.contiguous(), _compat_stack(u, M, w1, w2, compat_bi, compat_sp),
@@ -723,31 +724,46 @@ class _DenseCrfWide(torch.autograd.Function):
 
 
 def dense_crf_wide(unary, image, scale_factor=1.0, color_factor=13, maxiter=10, w1=None, w2=None, compat_bi=None,
-                   compat_sp=None):
-    """dense_crf for any label count from 1 to 255 (COCO's 81 classes), with the Potts weights or the
-    label-compatibility matrices learnable as there; the kernel bandwidths and caller-given features stay with
-    dense_crf (at most 32 labels).  At 32 labels or fewer it is dense_crf itself; above that the mean field and its
-    exact backward run on the label-chunked kernels, whose per-label cost is several times the fused path's.
-    Nothing is read on the host, so a step can be captured in a CUDA graph.  The forward keeps every iteration's
+                   compat_sp=None, theta_bi=None, theta_sp=None, features_bi=None):
+    """dense_crf for any label count from 1 to 255 (COCO's 81 classes), with every parameter dense_crf learns learnable
+    as there: the Potts weights or the label-compatibility matrices, the kernel bandwidths theta_bi / theta_sp and the
+    caller-given bilateral features features_bi (same arguments, same checks, same gradients).  At 32 labels or fewer
+    it is dense_crf itself; above that the mean field and its exact backward run on the label-chunked kernels, whose
+    per-label cost is several times the fused path's.  Nothing is read on the host unless a theta is given (its values
+    build the lattices), so without one a step can be captured in a CUDA graph.  The forward keeps every iteration's
     marginals: (maxiter + 1) * N * M * H * W * 4 bytes, 120 MB at batch 20 @ 41x41 with 81 labels."""
     if torch.is_autocast_enabled("cuda"):
         unary = unary.float() if isinstance(unary, torch.Tensor) and unary.is_floating_point() else unary
+        if isinstance(features_bi, torch.Tensor) and features_bi.is_floating_point():
+            features_bi = features_bi.float()
     u = _maps(unary, "unary")
     N, M, H, W = u.shape
     if M <= FUSED_LABELS:
-        return dense_crf(u, image, scale_factor, color_factor, maxiter, w1, w2, compat_bi, compat_sp)
+        return dense_crf(u, image, scale_factor, color_factor, maxiter, w1, w2, compat_bi, compat_sp, theta_bi,
+                         theta_sp, features_bi)
+    if features_bi is not None:
+        return _dense_crf_feat(u, image, features_bi, scale_factor, color_factor, maxiter, w1, w2, compat_bi,
+                               compat_sp, theta_bi, theta_sp, wide=True)
     if (not isinstance(image, torch.Tensor) or image.dtype != torch.uint8 or tuple(image.shape) != (N, H, W, 3)
             or image.device != u.device):
         raise ValueError("image must be a (%d, %d, %d, 3) uint8 tensor on %s" % (N, H, W, u.device))
+    th_bi, th_sp = _theta_values(theta_bi, "theta_bi", 5, u), _theta_values(theta_sp, "theta_sp", 2, u)
     _cuda(u, "unary")
     w1, w2 = _potts_weight(w1, "w1", u), _potts_weight(w2, "w2", u)
     if int(maxiter) < 0:
         raise ValueError("maxiter must be >= 0 (got %d)" % maxiter)
     params = api.crf_params(float(scale_factor), float(color_factor), int(maxiter))
+    if th_bi is not None:
+        (params.theta_alpha_x, params.theta_alpha_y, params.theta_beta_r, params.theta_beta_g,
+         params.theta_beta_b) = th_bi
+    if th_sp is not None:
+        params.theta_gamma_x, params.theta_gamma_y = th_sp
     compat = None
     if compat_bi is not None or compat_sp is not None:
         compat = _compat_stack(u, M, w1, w2, compat_bi, compat_sp)
         w1 = w2 = None
+    if th_bi is not None or th_sp is not None:
+        return _DenseCrfTheta.apply(u, image.contiguous(), w1, w2, compat, theta_bi, theta_sp, params, True)
     return _DenseCrfWide.apply(u, image.contiguous(), w1, w2, compat, params)
 
 

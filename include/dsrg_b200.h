@@ -247,6 +247,33 @@ int dsrg_crf_backward_wide_dev(dsrg_engine *e, const float *q_hist_dev, int B, c
                                const dsrg_crf_params *params, const float *potts_dev, const float *compat_dev,
                                const float *grad_q_dev, float *grad_unary_dev, float *grad_potts_dev,
                                float *grad_compat_dev, void *stream);
+/*
+ * The kernel bandwidths and caller-given bilateral features above DSRG_MAX_LABELS labels: the label-chunked twins of
+ * dsrg_crf_backward_theta_dev and of the dsrg_crf_forward_train_feat_dev / dsrg_crf_backward_feat_dev pair, with the
+ * same arguments, outputs and conventions (grad_theta [B][7] in the struct's order; the feature range, its per-image
+ * NaN policy and dsrg_engine_feature_range_flags), and potts_dev or compat_dev as in dsrg_crf_backward_wide_dev.
+ * dsrg_crf_backward_wide_theta_dev is the backward of dsrg_crf_forward_train_wide_dev with the sigmas in params.
+ * An engine of 32 labels or fewer is refused with DSRG_E_INVALID.  The parameter and per-pixel reductions contain no
+ * float atomics and run in a fixed order, but the splats into the lattices (of g_t, of Q_{t-1} and of the
+ * normalisation term) add with float atomics, as in dsrg_crf_backward_wide_dev: two calls on the same inputs agree to
+ * the rounding of those additions' order, not bit for bit.  The first call allocates, beyond
+ * dsrg_crf_backward_wide_dev's buffers, the c term per pixel, the per-block sums and two 4-float value buffers per
+ * lattice: 10.0 MB for an engine of batch 20 @ 41x41 and 244 MB for one of batch 8 @ 321x321, both with 81 labels
+ * (measured with dsrg_engine_device_bytes before and after).  g_t and the per-iteration splat of Q_{t-1} use the
+ * engine's own buffers.
+ */
+int dsrg_crf_backward_wide_theta_dev(dsrg_engine *e, const float *q_hist_dev, int B, const uint8_t *image_dev,
+                                     const dsrg_crf_params *params, const float *potts_dev, const float *compat_dev,
+                                     const float *grad_q_dev, float *grad_unary_dev, float *grad_potts_dev,
+                                     float *grad_compat_dev, float *grad_theta_dev, void *stream);
+int dsrg_crf_forward_train_wide_feat_dev(dsrg_engine *e, const float *unary_dev, int B, const float *features_dev,
+                                         const dsrg_crf_params *params, const float *potts_dev,
+                                         const float *compat_dev, float *q_hist_dev, void *stream);
+int dsrg_crf_backward_wide_feat_dev(dsrg_engine *e, const float *q_hist_dev, int B, const float *features_dev,
+                                    const dsrg_crf_params *params, const float *potts_dev, const float *compat_dev,
+                                    const float *grad_q_dev, float *grad_unary_dev, float *grad_features_dev,
+                                    float *grad_potts_dev, float *grad_compat_dev, float *grad_theta_sp_dev,
+                                    void *stream);
 /* arg-max labelling after inference: DenseCRFWrapper::map, densecrf_wrapper.cpp:39-43 */
 int dsrg_crf_map_batch_dev(dsrg_engine *e, int B, const float *unary_dev, int unary_layout,
                            const uint8_t *image_dev, const dsrg_crf_params *params,

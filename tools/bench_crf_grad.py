@@ -19,6 +19,11 @@
             dsrg_crf_backward_wide_dev, the label-chunked step with device Potts weights and with a matrix per kernel,
             timed beside the label-chunked inference forward; the line also reports the device memory the first
             backwards allocate (wide_bytes) and the FLOPs of the matrices' outer products (outer_flops)
+  wide_theta, wide_feat
+            (--wide --kernel, --wide --features) the label-chunked Potts step whose backward also gives the seven
+            kernel bandwidths' gradient (dsrg_crf_backward_wide_theta_dev), and the one on the image's own features
+            (dsrg_crf_forward_train_wide_feat_dev + dsrg_crf_backward_wide_feat_dev with grad_theta_sp), timed beside
+            wide_potts; the line also reports what the first of them allocates (wide_kgrad_bytes)
 
 on three workloads: train-s's shape (batch 20, 41 x 41 maps, 21 labels, scale_factor 12, smooth images) and batch 64
 at 321 x 321 with scale_factor 1 on smooth and on photo-like images; 10 mean-field iterations.  The legs run on a side
@@ -52,6 +57,17 @@ WIDE_WORKLOADS = {   # --wide: COCO's training shape, and large photo-like image
     "b8_photo": (8, 321, 321, 81, 1.0, "photo"),
 }
 T = 10
+
+
+def _image_features(torch, image, p):
+    """The image's own bilateral features float32(x)/theta_alpha, ... (B, 5, H, W): the lattice is the image path's."""
+    B, H, W = image.shape[:3]
+    sig = torch.tensor([p.theta_alpha_x, p.theta_alpha_y, p.theta_beta_r, p.theta_beta_g, p.theta_beta_b],
+                       device="cuda").view(1, 5, 1, 1)
+    yy, xx = torch.meshgrid(torch.arange(H, device="cuda"), torch.arange(W, device="cuda"), indexing="ij")
+    raw = torch.cat([xx.expand(B, 1, H, W).float(), yy.expand(B, 1, H, W).float(),
+                     image.permute(0, 3, 1, 2).float()], 1)
+    return (raw / sig).contiguous()
 
 
 def run(name, steps, warmup, rounds, compat=False, kernel=False, features=False, wide=False):
@@ -98,11 +114,31 @@ def run(name, steps, warmup, rounds, compat=False, kernel=False, features=False,
         torch.cuda.synchronize()
         extra["wide_bytes"] = int(_lib.lib().dsrg_engine_device_bytes(eng.h) - before)
         extra["outer_flops"] = 2 * 2 * M * M * H * W * B * T   # two lattices, a multiply-add per (l, l', pixel, t)
-    if compat:
+        if kernel or features:
+            gt = torch.empty((B, 7), device="cuda")
+            before = _lib.lib().dsrg_engine_device_bytes(eng.h)
+            legs["wide_theta"] = lambda: (
+                eng.crf_forward_train_wide_dev(unary, image, p, q_hist, potts=potts, stream=s.cuda_stream),
+                eng.crf_backward_wide_theta_dev(q_hist, image, p, G, gu, gt, potts=potts, grad_potts=gw,
+                                                stream=s.cuda_stream))
+            with torch.cuda.stream(s):
+                legs["wide_theta"]()
+            torch.cuda.synchronize()
+            extra["wide_kgrad_bytes"] = int(_lib.lib().dsrg_engine_device_bytes(eng.h) - before)
+            if not kernel:
+                del legs["wide_theta"]
+        if features:
+            feat = _image_features(torch, image, p)
+            gf, gsp = torch.empty_like(feat), torch.empty((B, 2), device="cuda")
+            legs["wide_feat"] = lambda: (
+                eng.crf_forward_train_wide_feat_dev(unary, feat, p, q_hist, potts=potts, stream=s.cuda_stream),
+                eng.crf_backward_wide_feat_dev(q_hist, feat, p, G, gu, gf, potts=potts, grad_potts=gw,
+                                               grad_theta_sp=gsp, stream=s.cuda_stream))
+    if compat and not wide:
         legs["compat"] = lambda: (eng.crf_forward_train_compat_dev(unary, image, p, mu, q_hist, stream=s.cuda_stream),
                                   eng.crf_backward_compat_dev(q_hist, image, p, mu, G, gu, grad_compat=gmu,
                                                               stream=s.cuda_stream))
-    if kernel:
+    if kernel and not wide:
         from dsrg_b200 import _lib
         gt = torch.empty((B, 7), device="cuda")
         before = _lib.lib().dsrg_engine_device_bytes(eng.h)
@@ -118,13 +154,8 @@ def run(name, steps, warmup, rounds, compat=False, kernel=False, features=False,
             legs["train_theta"]()
         torch.cuda.synchronize()
         extra["kgrad_bytes"] = int(_lib.lib().dsrg_engine_device_bytes(eng.h) - before)
-    if features:
-        sig = torch.tensor([p.theta_alpha_x, p.theta_alpha_y, p.theta_beta_r, p.theta_beta_g, p.theta_beta_b],
-                           device="cuda").view(1, 5, 1, 1)
-        yy, xx = torch.meshgrid(torch.arange(H, device="cuda"), torch.arange(W, device="cuda"), indexing="ij")
-        raw = torch.cat([xx.expand(B, 1, H, W).float(), yy.expand(B, 1, H, W).float(),
-                         image.permute(0, 3, 1, 2).float()], 1)
-        feat = (raw / sig).contiguous()
+    if features and not wide:
+        feat = _image_features(torch, image, p)
         gf, gsp = torch.empty_like(feat), torch.empty((B, 2), device="cuda")
         legs["train_feat"] = lambda: (
             eng.crf_forward_train_feat_dev(unary, feat, p, q_hist, stream=s.cuda_stream),
@@ -149,12 +180,15 @@ def run(name, steps, warmup, rounds, compat=False, kernel=False, features=False,
     med = {k: float(np.median(v)) for k, v in times.items()}
     if compat:
         extra["compat_over_train"] = round(med["compat"] / med["train"], 2)
-    if features:
+    if features and not wide:
         extra["train_feat_over_train"] = round(med["train_feat"] / med["train"], 2)
     if wide:
         extra["wide_potts_over_forward"] = round(med["wide_potts"] / med["forward"], 2)
         extra["wide_compat_over_forward"] = round(med["wide_compat"] / med["forward"], 2)
-    if kernel:
+        for k in ("wide_theta", "wide_feat"):
+            if k in med:
+                extra[k + "_over_wide_potts"] = round(med[k] / med["wide_potts"], 2)
+    elif kernel:
         extra["train_theta_over_train"] = round(med["train_theta"] / med["train"], 2)
         if compat:
             extra["compat_theta_over_compat"] = round(med["compat_theta"] / med["compat"], 2)
@@ -174,11 +208,11 @@ def main():
     ap.add_argument("--compat", action="store_true", help="also time the compatibility-matrix step")
     ap.add_argument("--kernel", action="store_true", help="also time the steps with the kernel-bandwidth gradient")
     ap.add_argument("--features", action="store_true",
-                    help="also time the step with caller-given bilateral features (implies --kernel)")
+                    help="also time the step with caller-given bilateral features (implies --kernel without --wide)")
     ap.add_argument("--wide", action="store_true",
                     help="time the label-chunked steps at 81 labels instead, on their own workloads")
     a = ap.parse_args()
-    a.kernel = a.kernel or a.features
+    a.kernel = a.kernel or (a.features and not a.wide)
     if a.wide and a.workloads == ",".join(WORKLOADS):
         a.workloads = ",".join(WIDE_WORKLOADS)
     import torch
@@ -186,8 +220,8 @@ def main():
         sys.exit("bench_crf_grad.py needs a CUDA device")
     info = card()
     for name in a.workloads.split(","):
-        fused = not a.wide   # --compat, --kernel and --features time fused-path legs
-        r = run(name, a.steps, a.warmup, a.rounds, a.compat and fused, a.kernel and fused, a.features and fused, a.wide)
+        # --compat times a fused-path leg; --kernel and --features the fused or the label-chunked ones (--wide)
+        r = run(name, a.steps, a.warmup, a.rounds, a.compat and not a.wide, a.kernel, a.features, a.wide)
         r.update(info)
         print(json.dumps(r), flush=True)
 
