@@ -55,6 +55,7 @@ SIGNATURES = {
     "dsrg_engine_hybrid_tiles": (_ll, [_vp]),
     "dsrg_crf_batch_dev": (_i, [_vp, _i, _vp, _i, _vp, _pp, _vp, _i, _vp]),
     "dsrg_crf_batch_host": (_i, [_vp, _i, _vp, _i, _vp, _pp, _vp, _i]),
+    "dsrg_crf_batch_learned_dev": (_i, [_vp, _vp, _i, _i, _vp, _vp, _pp, _vp, _vp, _i, _vp]),
     "dsrg_crf_map_batch_dev": (_i, [_vp, _i, _vp, _i, _vp, _pp, _vp, _vp]),
     "dsrg_crf_forward_train_dev": (_i, [_vp, _vp, _i, _vp, _pp, _vp, _vp, _vp]),
     "dsrg_crf_backward_dev": (_i, [_vp, _vp, _i, _vp, _pp, _vp, _vp, _vp, _vp, _vp]),
@@ -95,6 +96,8 @@ SIGNATURES = {
     "dsrg_predict_mask_host": (_i, [_vp, _i, _i, _vp, _vp, _vp, _vp, _f, _i, _pp, _vp, _i, _vp, _vp]),
     "dsrg_predict_mask_batch_dev": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _vp, _f, _i, _pp, _vp, _vp, _vp, _vp]),
     "dsrg_predict_mask_batch_host": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _vp, _f, _i, _pp, _vp, _vp, _vp]),
+    "dsrg_predict_mask_batch_learned_dev": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _vp, _vp, _f, _pp, _vp, _vp, _vp,
+                                                 _vp, _vp]),
     "dsrg_annotation_forward_dev": (_i, [_vp, _i, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _vp, _vp, _vp, _vp]),
     "dsrg_annotation_forward_host": (_i, [_vp, _i, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _vp, _vp, _vp]),
     "dsrg_annotation_coco_forward_dev": (_i, [_vp, _vp, _vp, _vp, _i, _vp, _vp, _i, _i, _vp, _i, _vp, _vp, _vp, _vp,

@@ -273,6 +273,17 @@ class Engine(object):
         check(self._L.dsrg_engine_feature_range_flags(self.h, B, _hptr(out, np.int32)))
         return out.astype(bool)
 
+    def crf_learned_dev(self, unary, image, params, out, features=None, compat=None, unary_layout=LAYOUT_NHWC,
+                        out_layout=LAYOUT_NHWC, stream=None):
+        """crf_dev with the learned CRF: compat an optional device float32 (2, M, M) {mu_bi, mu_sp} in place of params.w1
+        / w2, features optional (B, 5, H, W) float32 bilateral features in place of the image (then None).  Only the
+        marginals are kept; a feature image whose lattice keys leave the packed range gets NaN (feature_range_flags)."""
+        B = unary.shape[0]
+        check(self._L.dsrg_crf_batch_learned_dev(self.h, _dptr(unary), B, unary_layout, _dptr(image), _dptr(features),
+                                                 C.byref(params), _dptr(compat), _dptr(out), out_layout,
+                                                 _stream(stream)))
+        return out
+
     def crf_map_dev(self, unary, image, params, labels_out, unary_layout=LAYOUT_NHWC, stream=None):
         B = image.shape[0]
         check(self._L.dsrg_crf_map_batch_dev(self.h, B, _dptr(unary), unary_layout, _dptr(image), C.byref(params),
@@ -673,6 +684,19 @@ class Engine(object):
         check(self._L.dsrg_predict_mask_batch_dev(self.h, ptrs, hs, ws, n, B, int(mode), _dptr(images), float(eps),
                                                   int(bool(smooth)), C.byref(params), _dptr(sel), _dptr(result_out),
                                                   _dptr(probs_out), _stream(stream)))
+        return result_out
+
+    def predict_mask_batch_learned_dev(self, scores, images, result_out, params, mode=POST_SUM_SCORES, eps=0.00001,
+                                       features=None, compat=None, sel=None, probs_out=None, stream=None):
+        """predict_mask_batch_dev (smooth) with the learned CRF of crf_learned_dev: images (B,H,W,3) uint8 or
+        features (B,5,H,W) float32 (exactly one), compat optional (2, M, M).  A feature image whose lattice keys leave
+        the packed range gets -1 in every pixel of its result and NaN in probs_out."""
+        n, B, hs, ws = self._post_batch_args(scores)
+        ptrs = (C.c_void_p * n)(*[_dptr(a).value for a in scores])
+        check(self._L.dsrg_predict_mask_batch_learned_dev(self.h, ptrs, hs, ws, n, B, int(mode), _dptr(images),
+                                                          _dptr(features), float(eps), C.byref(params), _dptr(compat),
+                                                          _dptr(sel), _dptr(result_out), _dptr(probs_out),
+                                                          _stream(stream)))
         return result_out
 
     # ---- AnnotationLayer.forward (pylayers.py:369-387) ----

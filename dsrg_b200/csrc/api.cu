@@ -206,6 +206,16 @@ static int prepare_lattices(Engine *e, int B, const uint8_t *image, const dsrg_c
     return lattice_build(e, e->bi, B, image, s);
 }
 
+// The feature passes' per-image key-range flags on their first call (as ensure_compat_part)
+int ensure_feat(Engine *e) {
+    if (e->feat_bad) return DSRG_OK;
+    cudaStreamCaptureMode mode = cudaStreamCaptureModeRelaxed;
+    DSRG_CUDA_TRY(cudaThreadExchangeStreamCaptureMode(&mode));
+    const int rc = dalloc(e, &e->feat_bad, (size_t)e->maxB);
+    DSRG_CUDA_TRY(cudaThreadExchangeStreamCaptureMode(&mode));
+    return rc;
+}
+
 // prepare_lattices with caller-given bilateral features ([B][5][N]): the bilateral sigmas of `p` are not used, and the
 // key range is checked per image on the device (e->feat_bad, which ensure_feat allocates)
 static int prepare_lattices_feat(Engine *e, int B, const float *feat, const dsrg_crf_params &p, cudaStream_t s) {
@@ -250,14 +260,20 @@ void crf_pass_end(Engine *e, const dsrg_crf_params &p, int B, int rc) {
 }
 
 int crf_core(Engine *e, int B, const float *unary, int layout, bool clamp, float *unary_rw, const uint8_t *image,
-             const dsrg_crf_params *p, cudaStream_t s) {
+             const dsrg_crf_params *p, cudaStream_t s, const LearnedCrf *lc) {
     if (layout != DSRG_LAYOUT_NHWC && layout != DSRG_LAYOUT_NCHW) {
         set_error("bad layout %d", layout);
         return DSRG_E_INVALID;
     }
-    int rc = prepare_lattices(e, B, image, *p, s);
+    const float *feat = lc ? lc->features : nullptr;
+    int rc = feat ? prepare_lattices_feat(e, B, feat, *p, s) : prepare_lattices(e, B, image, *p, s);
     if (rc) return rc;
-    return meanfield_run(e, B, unary, layout, clamp, unary_rw, *p, s);
+    if (!lc) return meanfield_run(e, B, unary, layout, clamp, unary_rw, *p, s);
+    rc = meanfield_run(e, B, unary, layout, clamp, unary_rw, *p, s, lc->compat);
+    if (rc || !feat) return rc;
+    nan_images(e, e->feat_bad, e->Q0, B, (long long)e->M * e->N, 1, 0, s);   // the training forward's policy
+    DSRG_CUDA_TRY(cudaGetLastError());
+    return DSRG_OK;
 }
 
 static int crf_batch_pass(Engine *e, int B, const float *unary, int unary_layout, const uint8_t *image,
@@ -342,7 +358,7 @@ using namespace dsrg;
 
 extern "C" {
 
-int dsrg_version(void) { return 116; }
+int dsrg_version(void) { return 117; }
 
 const char *dsrg_last_error(void) { return g_err; }
 
@@ -823,16 +839,6 @@ int dsrg_crf_backward_compat_theta_dev(dsrg_engine *h, const float *q_hist, int 
     });
 }
 
-// The feature passes' per-image key-range flags on their first call (as ensure_compat_part)
-static int ensure_feat(Engine *e) {
-    if (e->feat_bad) return DSRG_OK;
-    cudaStreamCaptureMode mode = cudaStreamCaptureModeRelaxed;
-    DSRG_CUDA_TRY(cudaThreadExchangeStreamCaptureMode(&mode));
-    const int rc = dalloc(e, &e->feat_bad, (size_t)e->maxB);
-    DSRG_CUDA_TRY(cudaThreadExchangeStreamCaptureMode(&mode));
-    return rc;
-}
-
 int dsrg_crf_forward_train_feat_dev(dsrg_engine *h, const float *unary, int B, const float *features,
                                     const dsrg_crf_params *params, const float *potts, const float *compat,
                                     float *q_hist, void *stream) {
@@ -1065,6 +1071,28 @@ int dsrg_crf_backward_wide_feat_dev(dsrg_engine *h, const float *q_hist, int B, 
         });
         e->last_crf_B = 0;
         e->feat_B = rc == DSRG_OK ? B : 0;
+        return rc;
+    });
+}
+
+int dsrg_crf_batch_learned_dev(dsrg_engine *h, const float *unary, int B, int unary_layout, const uint8_t *image,
+                               const float *features, const dsrg_crf_params *params, const float *compat, float *out,
+                               int out_layout, void *stream) {
+    const cudaStream_t s = (cudaStream_t)stream;
+    const bool ok = unary && params && out && layout_ok(unary_layout) && layout_ok(out_layout) &&
+                    (image != nullptr) != (features != nullptr);
+    return dev_call(h, B, s, ok, [&](Engine *e) {
+        if (features)
+            if (int rc = ensure_feat(e)) return rc;
+        const LearnedCrf lc{features, compat};
+        GraphKey args;
+        args.add(unary).add(unary_layout).add(image).add(features).add(compat).add(out).add(out_layout);
+        const int rc = crf_pass(e, s, PassKind::crf_learned, B, params, args, [&]() {
+            int r = crf_core(e, B, unary, unary_layout, false, nullptr, image, params, s, &lc);
+            if (r) return r;
+            return meanfield_export(e, B, out, out_layout, s);
+        });
+        if (features) e->feat_B = rc == DSRG_OK ? B : 0;
         return rc;
     });
 }

@@ -155,8 +155,9 @@ int tiles_build(Engine *e, Lattice &L, int nb, cudaStream_t s);
 // outweigh what it saves -- and every overflow tile stays on k_mf_tile's direct path
 inline bool hybrid_tiles_on(const Engine *e, int B);
 // ---- meanfield.cu ----
+// The inference: Q_T to e->Q0.  `compat` ({mu_bi, mu_sp} [2][M][M], device) replaces the Potts weights of p.
 int meanfield_run(Engine *e, int B, const float *unary, int unary_layout, bool clamp_inplace,
-                  float *unary_rw, const dsrg_crf_params &p, cudaStream_t s);
+                  float *unary_rw, const dsrg_crf_params &p, cudaStream_t s, const float *compat = nullptr);
 // the training forward (NCHW unary, Q_0..Q_T to q_hist) and its backward; at most DSRG_MAX_LABELS labels
 // (with `compat` = {mu_bi, mu_sp} [2][M][M] in place of the Potts weights: the compatibility-matrix variant, whose
 // backward needs e->compat_part, ensure_compat_part)
@@ -180,7 +181,7 @@ void potts_reduce(Engine *e, const float2 *part, float *out, int nparts, int B, 
 void compat_reduce(Engine *e, const float *part, float *out, int nparts, int mm2, int B, int tag, cudaStream_t s);
 // ---- meanfield_wide.cu: label counts above DSRG_MAX_LABELS ----
 int meanfield_run_wide(Engine *e, int B, const float *unary, int unary_layout, bool clamp_inplace,
-                       float *unary_rw, const dsrg_crf_params &p, cudaStream_t s);
+                       float *unary_rw, const dsrg_crf_params &p, cudaStream_t s, const float *compat);
 int wide_weights(Engine *e, Lattice &L, int nb, cudaStream_t s);
 // the training forward and its backward above DSRG_MAX_LABELS labels, as meanfield_run_train / meanfield_backward
 // (potts or compat, not both); the backward needs e->wide_ppart, and with compat e->wide_g and e->wide_cpart
@@ -206,8 +207,15 @@ int srg_run(Engine *e, int B, const float *labels, const float *probs, const flo
 int dsrg_forward_core(Engine *e, int B, const float *labels, float *probs, const float *cues, const uint32_t *cue_bits,
                       const uint8_t *image, const dsrg_crf_params *params, double th1, double th2, float *seeds_out,
                       uint32_t *seed_bits, float *crf_out, cudaStream_t s);
+// The learned CRF at inference (dsrg_crf_batch_learned_dev, dsrg_predict_mask_batch_learned_dev): caller-given
+// bilateral features ([B][5][N], in place of the image; they need e->feat_bad, ensure_feat) and / or the matrices
+// ({mu_bi, mu_sp} [2][M][M]).  An image whose feature lattice leaves the packed key range gets NaN marginals in e->Q0.
+struct LearnedCrf {
+    const float *features, *compat;
+};
 int crf_core(Engine *e, int B, const float *unary, int layout, bool clamp, float *unary_rw, const uint8_t *image,
-             const dsrg_crf_params *p, cudaStream_t s);
+             const dsrg_crf_params *p, cudaStream_t s, const LearnedCrf *lc = nullptr);
+int ensure_feat(Engine *e);
 // ---- sec_loss.cu ----
 constexpr int kSecPlainChunks = 16;  // CTAs per image of SeedLossLayer's sums (fixed, so is their order)
 
@@ -460,7 +468,7 @@ cudaError_t numa_host_alloc(void **p, size_t bytes, int device);
 enum class PassKind : int { crf, crf_map, forward, crflayer, densecrf, post, crf_train, crf_backward, crf_train_compat,
                             crf_backward_compat, crf_backward_theta, crf_backward_compat_theta, crf_train_feat,
                             crf_backward_feat, crf_train_wide, crf_backward_wide, crf_backward_wide_theta,
-                            crf_train_wide_feat, crf_backward_wide_feat };
+                            crf_train_wide_feat, crf_backward_wide_feat, crf_learned, post_learned };
 struct GraphKey {
     std::string bytes;
     GraphKey() = default;

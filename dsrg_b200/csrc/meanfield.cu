@@ -95,9 +95,12 @@ struct TileLat {
 // stores every iteration's Q_t to the caller's history for the backward, never clamps the unary, and reads the Potts
 // weights from device memory when the U_rw argument (unused without the clamp) carries them: {w1, w2}, with c_sp /
 // c_bi then passed as alpha alone.  Without MODE_HIST the instantiations are the inference kernels, unchanged.
-// MODE_COMPAT (with MODE_HIST: dsrg_crf_forward_train_compat_dev; in k_mf_tile_bwd: dsrg_crf_backward_compat_dev)
-// replaces the Potts messages by label-compatibility matrices, t = U - mu_sp F_sp(Q) - mu_bi F_bi(Q): U_rw (potts in
-// the backward) then carries {mu_bi, mu_sp} ([2][M][M], row l = the message to label l), c_sp / c_bi are alpha alone.
+// MODE_COMPAT (with MODE_HIST: dsrg_crf_forward_train_compat_dev; without it: the learned inference,
+// dsrg_crf_batch_learned_dev, storing Q_T alone; in k_mf_tile_bwd: dsrg_crf_backward_compat_dev) replaces the Potts
+// messages by label-compatibility matrices, t = U - mu_sp F_sp(Q) - mu_bi F_bi(Q): U_rw (potts in the backward) then
+// carries {mu_bi, mu_sp} ([2][M][M], row l = the message to label l), c_sp / c_bi are alpha alone.  The tile kernels
+// write U_rw only in the clamp of a MODE_FIRST inference instantiation, and MODE_COMPAT has no MODE_FIRST there (the
+// first iteration slices nothing and runs the Potts kernel), so the matrices are never written.
 enum { MODE_FIRST = 0, MODE_MID = 1, MODE_LAST = 2, MODE_HIST = 4, MODE_COMPAT = 8, MODE_GSTORE = 16 };
 
 // exp(x) for x <= 0 via ex2.approx with the rounding error of x*log2(e) folded back in
@@ -514,6 +517,7 @@ template <int MP, int MODE>
 __global__ void __launch_bounds__(kTileThreads, (MODE & MODE_COMPAT) ? (MP > 12 ? 1 : 2) : DSRG_TILE_CTAS)
 k_mf_tile(const float *U, float *U_rw, int clamp, float *__restrict__ Qout, TileLat sp, TileLat bi, float c_sp,
           float c_bi, int M, int N, int W, int H, int tiles_x, int ntiles, int tile_w) {
+    static_assert(!(MODE & MODE_COMPAT) || (MODE & 3) != MODE_FIRST, "U_rw carries the matrices: nothing may clamp");
     constexpr int kRowBytes = MP * 4;
     using SM = TileSmem<MP>;
     using ST = TileStage<MP>;
@@ -638,6 +642,7 @@ __global__ void __launch_bounds__(kTileThreads, (MODE & MODE_COMPAT) ? (MP > 12 
 k_mf_tile_hy(const float *U, float *U_rw, int clamp, float *__restrict__ Qout, TileLat sp, TileLat bi, float c_sp,
              float c_bi, int M, int N, int W, int H, int tiles_x, int ntiles, int tile_w, const int2 *hy_list,
              const int *hy_count) {
+    static_assert(!(MODE & MODE_COMPAT) || (MODE & 3) != MODE_FIRST, "U_rw carries the matrices: nothing may clamp");
     constexpr int kRowBytes = MP * 4;
     using ST = TileStage<MP, kMaxLocHy>;
     constexpr int CHP = ST::CHP;
@@ -1535,7 +1540,8 @@ static float *blur_all(Engine *e, const Lattice &L, float *buf, float *tmp, floa
 
 // q_hist != nullptr: the training forward (MODE_HIST), Q_t of every iteration to q_hist[t] ([T+1][B][M][N]), with
 // the Potts weights read from `potts` ({w1, w2}, device) when it is given, or the compatibility matrices `compat`
-// ({mu_bi, mu_sp}, device) in their place (MODE_COMPAT)
+// ({mu_bi, mu_sp}, device) in their place (MODE_COMPAT).  `compat` without q_hist: the inference with matrices, Q_T
+// alone to e->Q0 as the Potts inference leaves it
 template <int MP>
 static int run_impl(Engine *e, int B, const float *unary, int layout, bool clamp, float *unary_rw,
                     const dsrg_crf_params &p, cudaStream_t s, float *q_hist = nullptr, const float *potts = nullptr,
@@ -1583,6 +1589,10 @@ static int run_impl(Engine *e, int B, const float *unary, int layout, bool clamp
         DSRG_CUDA_TRY(cudaFuncSetAttribute(k_mf_tile<MP, MODE_LAST | MODE_HIST | MODE_COMPAT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_c));
         DSRG_CUDA_TRY(cudaFuncSetAttribute(k_mf_tile_hy<MP, MODE_MID | MODE_HIST | MODE_COMPAT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_hy_c));
         DSRG_CUDA_TRY(cudaFuncSetAttribute(k_mf_tile_hy<MP, MODE_LAST | MODE_HIST | MODE_COMPAT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_hy_c));
+        DSRG_CUDA_TRY(cudaFuncSetAttribute(k_mf_tile<MP, MODE_MID | MODE_COMPAT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_c));
+        DSRG_CUDA_TRY(cudaFuncSetAttribute(k_mf_tile<MP, MODE_LAST | MODE_COMPAT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_c));
+        DSRG_CUDA_TRY(cudaFuncSetAttribute(k_mf_tile_hy<MP, MODE_MID | MODE_COMPAT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_hy_c));
+        DSRG_CUDA_TRY(cudaFuncSetAttribute(k_mf_tile_hy<MP, MODE_LAST | MODE_COMPAT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_hy_c));
         attr_done[dv] = true;
     }
 #ifndef DSRG_BLUR_GRID
@@ -1618,7 +1628,17 @@ static int run_impl(Engine *e, int B, const float *unary, int layout, bool clamp
     DSRG_TILE_LAUNCH_AT(MODEV | MODE_HIST | MODE_COMPAT, QOUT, const_cast<float *>(compat), smem_c, smem_hy_c)
     for (int it = 0; it <= T; it++) {
         TileLat vsp = make_tile_view(e->sp, spX, spY), vbi = make_tile_view(e->bi, biX, biY);
-        if (compat) {
+        if (compat && !hist) {
+            // the matrices passed as the matrices, never as the clamp's U_rw; the first iteration is the Potts one
+            if (it == T) {
+                DSRG_TILE_LAUNCH_AT(MODE_LAST | MODE_COMPAT, e->Q0, const_cast<float *>(compat), smem_c, smem_hy_c);
+                break;
+            }
+            if (it == 0)
+                DSRG_TILE_LAUNCH_AT(MODE_FIRST, nullptr, nullptr, smem, smem_hy);
+            else
+                DSRG_TILE_LAUNCH_AT(MODE_MID | MODE_COMPAT, nullptr, const_cast<float *>(compat), smem_c, smem_hy_c);
+        } else if (compat) {
             // the first iteration slices nothing: the plain training kernel, without weights
             float *qt = q_hist + (size_t)it * slab;
             if (it == T) {
@@ -1920,17 +1940,14 @@ void compat_reduce(Engine *e, const float *part, float *out, int nparts, int mm2
 }
 
 int meanfield_run(Engine *e, int B, const float *unary, int unary_layout, bool clamp_inplace,
-                  float *unary_rw, const dsrg_crf_params &p, cudaStream_t s) {
-    if (e->MP > DSRG_MAX_LABELS) return meanfield_run_wide(e, B, unary, unary_layout, clamp_inplace, unary_rw, p, s);
+                  float *unary_rw, const dsrg_crf_params &p, cudaStream_t s, const float *compat) {
+    if (e->MP > DSRG_MAX_LABELS)
+        return meanfield_run_wide(e, B, unary, unary_layout, clamp_inplace, unary_rw, p, s, compat);
     switch (e->MP) {
-        case 4: return run_impl<4>(e, B, unary, unary_layout, clamp_inplace, unary_rw, p, s);
-        case 8: return run_impl<8>(e, B, unary, unary_layout, clamp_inplace, unary_rw, p, s);
-        case 12: return run_impl<12>(e, B, unary, unary_layout, clamp_inplace, unary_rw, p, s);
-        case 16: return run_impl<16>(e, B, unary, unary_layout, clamp_inplace, unary_rw, p, s);
-        case 20: return run_impl<20>(e, B, unary, unary_layout, clamp_inplace, unary_rw, p, s);
-        case 24: return run_impl<24>(e, B, unary, unary_layout, clamp_inplace, unary_rw, p, s);
-        case 28: return run_impl<28>(e, B, unary, unary_layout, clamp_inplace, unary_rw, p, s);
-        case 32: return run_impl<32>(e, B, unary, unary_layout, clamp_inplace, unary_rw, p, s);
+#define DSRG_CASE(MPV) \
+    case MPV: return run_impl<MPV>(e, B, unary, unary_layout, clamp_inplace, unary_rw, p, s, nullptr, nullptr, compat);
+        DSRG_CASE(4) DSRG_CASE(8) DSRG_CASE(12) DSRG_CASE(16) DSRG_CASE(20) DSRG_CASE(24) DSRG_CASE(28) DSRG_CASE(32)
+#undef DSRG_CASE
     }
     set_error("unsupported label count %d", e->M);
     return DSRG_E_INVALID;

@@ -170,40 +170,6 @@ k_wide_softmax(float *T, int M, int N) {
     for (int k = 0; k < M; k++) p[(size_t)k * N] /= sum;
 }
 
-int meanfield_run_wide(Engine *e, int B, const float *unary, int layout, bool clamp, float *unary_rw,
-                       const dsrg_crf_params &p, cudaStream_t s) {
-    const int M = e->M, N = e->N, CH = e->MP / 4, T = p.n_iters;
-    dim3 gp(cdiv(N, kThreads), B), gq(cdiv(N, kThreads), CH, B);
-    DSRG_LAUNCH(e, T_MF_INIT, s, k_wide_init<<<gp, kThreads, 0, s>>>(unary, unary_rw, layout, clamp ? 1 : 0, e->U, e->Q0, M, N));
-    if (T == 0) return DSRG_OK;
-    const float alpha_sp = 1.0f / (1 + powf(2, -e->sp.d)), alpha_bi = 1.0f / (1 + powf(2, -e->bi.d));  // permutohedral.cpp:571
-    const float c_sp = p.w2 * alpha_sp, c_bi = p.w1 * alpha_bi;
-    const int grid = 8 * e->sm_count;
-    float *spY = e->spA, *spZ = e->spB, *biY = e->biA, *biZ = e->biB;
-    for (int it = 0; it < T; it++) {
-        DSRG_LAUNCH(e, T_MF_ZERO, s, k_wide_zero<<<grid, kThreads, 0, s>>>((float4 *)spY, e->sp.rowbase, (float4 *)biY, e->bi.rowbase, B, CH));
-        WideLat sp{e->sp.off, e->sp.wn, e->sp.rowbase, spY, e->sp.shared, e->sp.d + 1};
-        WideLat bi{e->bi.off, e->bi.wn, e->bi.rowbase, biY, e->bi.shared, e->bi.d + 1};
-        DSRG_LAUNCH(e, T_MF_TILE, s, k_wide_splat<<<gq, kThreads, 0, s>>>(e->Q0, sp, bi, M, N, CH));
-        for (int l = 0; l < 2; l++) {
-            Lattice &L = l ? e->bi : e->sp;
-            float *&src = l ? biY : spY, *&dst = l ? biZ : spZ;
-            for (int j = 0; j <= L.d; j++) {
-                DSRG_LAUNCH(e, T_MF_BLUR_BI, s,
-                            k_wide_blur<<<grid, kThreads, 0, s>>>((const float4 *)src, (float4 *)dst, L.nbr + (size_t)j * L.nbr_stride,
-                                                                  L.rowbase, B, L.shared, CH));
-                float *t = src; src = dst; dst = t;
-            }
-        }
-        sp.val = spY;
-        bi.val = biY;
-        DSRG_LAUNCH(e, T_MF_TILE, s, k_wide_slice<<<gq, kThreads, 0, s>>>(e->U, e->Q0, sp, bi, c_sp, c_bi, M, N, CH));
-        DSRG_LAUNCH(e, T_MF_TILE, s, k_wide_softmax<<<gp, kThreads, 0, s>>>(e->Q0, M, N));
-    }
-    DSRG_CUDA_TRY(cudaGetLastError());
-    return DSRG_OK;
-}
-
 // ---------------------------------------------------------------------------------------------
 // Training above 32 labels: the forward keeping Q_0..Q_T, and the backward of the mean field (DenseCRF::gradient,
 // densecrf.cpp:238-297) on the label-chunked kernels.  With F(X) = alpha n K(n X) (wn = bary * norm, alpha on the
@@ -553,6 +519,53 @@ k_wide_kg_pass(KgArgs a, const float *x_sp, const float *u_sp, const float *x_bi
         }
     }
     kg_block_sum(a, b, dp, part_first != 0);
+}
+
+// With `compat` the messages are the matrices' (the training forward's slice_planar + compat_msg, below): S_sp, S_bi
+// to two [B][M][N] planes, then t = U - mu_sp S_sp - mu_bi S_bi over Q, whose values the splat has consumed by then.
+// The planes live in e->biC, which this loop never touches (it ping-pongs spA / spB and biA / biB) and which holds
+// maxB * (6 (Ncap + P) + 1) * MP >= 2 * B * M * N floats: the matrices cost no memory beyond the Potts inference.
+int meanfield_run_wide(Engine *e, int B, const float *unary, int layout, bool clamp, float *unary_rw,
+                       const dsrg_crf_params &p, cudaStream_t s, const float *compat) {
+    const int M = e->M, N = e->N, CH = e->MP / 4, T = p.n_iters;
+    float *s_sp = e->biC, *s_bi = e->biC + (size_t)B * M * N;
+    dim3 gp(cdiv(N, kThreads), B), gq(cdiv(N, kThreads), CH, B);
+    DSRG_LAUNCH(e, T_MF_INIT, s, k_wide_init<<<gp, kThreads, 0, s>>>(unary, unary_rw, layout, clamp ? 1 : 0, e->U, e->Q0, M, N));
+    if (T == 0) return DSRG_OK;
+    const float alpha_sp = 1.0f / (1 + powf(2, -e->sp.d)), alpha_bi = 1.0f / (1 + powf(2, -e->bi.d));  // permutohedral.cpp:571
+    const float c_sp = p.w2 * alpha_sp, c_bi = p.w1 * alpha_bi;
+    const int grid = 8 * e->sm_count;
+    float *spY = e->spA, *spZ = e->spB, *biY = e->biA, *biZ = e->biB;
+    for (int it = 0; it < T; it++) {
+        DSRG_LAUNCH(e, T_MF_ZERO, s, k_wide_zero<<<grid, kThreads, 0, s>>>((float4 *)spY, e->sp.rowbase, (float4 *)biY, e->bi.rowbase, B, CH));
+        WideLat sp{e->sp.off, e->sp.wn, e->sp.rowbase, spY, e->sp.shared, e->sp.d + 1};
+        WideLat bi{e->bi.off, e->bi.wn, e->bi.rowbase, biY, e->bi.shared, e->bi.d + 1};
+        DSRG_LAUNCH(e, T_MF_TILE, s, k_wide_splat<<<gq, kThreads, 0, s>>>(e->Q0, sp, bi, M, N, CH));
+        for (int l = 0; l < 2; l++) {
+            Lattice &L = l ? e->bi : e->sp;
+            float *&src = l ? biY : spY, *&dst = l ? biZ : spZ;
+            for (int j = 0; j <= L.d; j++) {
+                DSRG_LAUNCH(e, T_MF_BLUR_BI, s,
+                            k_wide_blur<<<grid, kThreads, 0, s>>>((const float4 *)src, (float4 *)dst, L.nbr + (size_t)j * L.nbr_stride,
+                                                                  L.rowbase, B, L.shared, CH));
+                float *t = src; src = dst; dst = t;
+            }
+        }
+        sp.val = spY;
+        bi.val = biY;
+        if (compat) {
+            DSRG_LAUNCH(e, T_MF_TILE, s,
+                        k_wide_slice_planar<<<gq, kThreads, 0, s>>>(s_sp, s_bi, sp, bi, alpha_sp, alpha_bi, M, N, CH));
+            DSRG_LAUNCH(e, T_MF_TILE, s,
+                        k_wide_compat_msg<false><<<gq, kThreads, 8 * M * sizeof(float), s>>>(e->U, s_sp, s_bi, compat,
+                                                                                            e->Q0, M, N));
+        } else {
+            DSRG_LAUNCH(e, T_MF_TILE, s, k_wide_slice<<<gq, kThreads, 0, s>>>(e->U, e->Q0, sp, bi, c_sp, c_bi, M, N, CH));
+        }
+        DSRG_LAUNCH(e, T_MF_TILE, s, k_wide_softmax<<<gp, kThreads, 0, s>>>(e->Q0, M, N));
+    }
+    DSRG_CUDA_TRY(cudaGetLastError());
+    return DSRG_OK;
 }
 
 static WideLat wide_lat(const Lattice &L, float *val) { return WideLat{L.off, L.wn, L.rowbase, val, L.shared, L.d + 1}; }

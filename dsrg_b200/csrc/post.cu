@@ -212,10 +212,19 @@ k_post_argmax_batch(const float *q, int32_t *out, int N, int M, long long ls, lo
     out[(size_t)b * N + i] = arg;
 }
 
-// sel: device rows as k_post_argmax_batch reads them, or NULL; row (B = 1): a selection written to st_sel by the pass
+// -1 over every pixel of the images whose feature lattice left the packed key range (bad[b] set), which
+// dsrg_confusion_add_dev counts as invalid
+__global__ void __launch_bounds__(kThreads) k_post_bad_images(const int *bad, int32_t *out, int N) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < N && bad[blockIdx.y]) out[(size_t)blockIdx.y * N + i] = -1;
+}
+
+// sel: device rows as k_post_argmax_batch reads them, or NULL; row (B = 1): a selection written to st_sel by the pass.
+// features / compat (smooth only): the learned CRF (LearnedCrf), images then NULL when features are given
 static int predict_mask_batch_body(Engine *e, int B, int mode, const ZoomScales &sc, const uint8_t *images, float eps,
                                    int smooth, const dsrg_crf_params *p, const int32_t *sel, const LabelRow *row,
-                                   int32_t *result, float *probs_out, cudaStream_t s) {
+                                   int32_t *result, float *probs_out, cudaStream_t s, const float *features,
+                                   const float *compat) {
     const int N = e->N, M = e->M;
     const long long n = (long long)B * N * M;
     float *unary = e->st_unary;                       // [B][H][W][M]
@@ -239,10 +248,14 @@ static int predict_mask_batch_body(Engine *e, int B, int mode, const ZoomScales 
     DSRG_CUDA_TRY(cudaGetLastError());
     const dim3 ga(cdiv(N, kThreads), B);
     if (smooth) {
-        if (int rc = crf_core(e, B, unary, DSRG_LAYOUT_NHWC, false, nullptr, images, p, s)) return rc;
+        const LearnedCrf lc{features, compat};
+        const bool learned = features || compat;
+        if (int rc = crf_core(e, B, unary, DSRG_LAYOUT_NHWC, false, nullptr, images, p, s, learned ? &lc : nullptr))
+            return rc;
         if (probs_out)
             if (int rc = meanfield_export(e, B, probs_out, DSRG_LAYOUT_NHWC, s)) return rc;
         DSRG_LAUNCH(e, T_POST, s, k_post_argmax_batch<<<ga, kThreads, 0, s>>>(e->Q0, result, N, M, N, 1, sel));
+        if (features) DSRG_LAUNCH(e, T_POST, s, k_post_bad_images<<<ga, kThreads, 0, s>>>(e->feat_bad, result, N));
     } else {
         DSRG_LAUNCH(e, T_POST, s, k_post_argmax_batch<<<ga, kThreads, 0, s>>>(clamped, result, N, M, 1, M, sel));
     }
@@ -272,9 +285,9 @@ static int post_batch_check(const Engine *e, int mode, int n_scales, const float
 static int predict_mask_batch(Engine *e, int B, int mode, int n_scales, const float *const *scores, const int *hs,
                               const int *ws, const uint8_t *images, float eps, int smooth, const dsrg_crf_params *p,
                               const int32_t *sel, const LabelRow *row, int32_t *result, float *probs_out,
-                              cudaStream_t s) {
+                              cudaStream_t s, const float *features = nullptr, const float *compat = nullptr) {
     int rc = post_batch_check(e, mode, n_scales, scores, hs, ws);
-    if (rc || (rc = ensure_staging(e))) return rc;
+    if (rc || (rc = ensure_staging(e)) || (features && (rc = ensure_feat(e)))) return rc;
     ZoomScales sc = {};
     sc.n = n_scales;
     for (int k = 0; k < n_scales; k++) {
@@ -290,10 +303,17 @@ static int predict_mask_batch(Engine *e, int B, int mode, int n_scales, const fl
         .add(row != nullptr);
     for (int k = 0; k < n_scales; k++) args.add(scores[k]).add(hs[k]).add(ws[k]);
     if (row) args.add(*row);
+    const bool learned = features || compat;
+    if (learned) args.add(features).add(compat);
     auto body = [&]() {
-        return predict_mask_batch_body(e, B, mode, sc, images, eps, smooth, p, sel, row, result, probs_out, s);
+        return predict_mask_batch_body(e, B, mode, sc, images, eps, smooth, p, sel, row, result, probs_out, s,
+                                       features, compat);
     };
-    if (smooth) return crf_pass(e, s, PassKind::post, B, p, args, body);
+    if (smooth) {
+        rc = crf_pass(e, s, learned ? PassKind::post_learned : PassKind::post, B, p, args, body);
+        if (features) e->feat_B = rc == DSRG_OK ? B : 0;
+        return rc;
+    }
     return run_pass(e, s, GraphKey(PassKind::post, B, e, args), true, body);
 }
 
@@ -438,6 +458,21 @@ extern "C" int dsrg_predict_mask_batch_dev(dsrg_engine *h, const float *const *s
     return dev_call(h, B, s, ok, [&](Engine *e) {
         return predict_mask_batch(e, B, mode, n_scales, scores_dev, hs, ws, images_dev, eps, smooth, params, sel_dev,
                                   nullptr, result_out_dev, probs_out_dev, s);
+    });
+}
+
+extern "C" int dsrg_predict_mask_batch_learned_dev(dsrg_engine *h, const float *const *scores_dev, const int *hs,
+                                                   const int *ws, int n_scales, int B, int mode,
+                                                   const uint8_t *images_dev, const float *features_dev, float eps,
+                                                   const dsrg_crf_params *params, const float *compat_dev,
+                                                   const int32_t *sel_dev, int32_t *result_out_dev, float *probs_out_dev,
+                                                   void *stream) {
+    const cudaStream_t s = (cudaStream_t)stream;
+    const bool ok = post_args_ok(n_scales, scores_dev, hs, ws, nullptr, 0, nullptr, nullptr, 0, result_out_dev) &&
+                    params && (images_dev != nullptr) != (features_dev != nullptr);
+    return dev_call(h, B, s, ok, [&](Engine *e) {
+        return predict_mask_batch(e, B, mode, n_scales, scores_dev, hs, ws, images_dev, eps, 1, params, sel_dev,
+                                  nullptr, result_out_dev, probs_out_dev, s, features_dev, compat_dev);
     });
 }
 

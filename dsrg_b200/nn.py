@@ -767,6 +767,82 @@ def dense_crf_wide(unary, image, scale_factor=1.0, color_factor=13, maxiter=10, 
     return _DenseCrfWide.apply(u, image.contiguous(), w1, w2, compat, params)
 
 
+def _learned_crf(ref, N, M, H, W, params, w1=None, w2=None, compat_bi=None, compat_sp=None, theta_bi=None,
+                 theta_sp=None, features_bi=None):
+    """The learned CRF's inference arguments, checked as dense_crf checks them: params takes the sigmas and, on the
+    Potts path, the weights (read on the host, so refused inside CUDA-graph capture); returns (features, compat) for
+    the device, either of them None.  ref: any tensor on the CRF's device."""
+    f = None
+    if features_bi is not None:
+        if theta_bi is not None:
+            raise ValueError("theta_bi and features_bi are two forms of the bilateral features: give one of them")
+        if (not isinstance(features_bi, torch.Tensor) or features_bi.dtype != torch.float32
+                or tuple(features_bi.shape) != (N, 5, H, W) or features_bi.device != ref.device):
+            raise ValueError("features_bi must be a (%d, 5, %d, %d) float32 tensor on %s (got %r)"
+                             % (N, H, W, ref.device, features_bi if not isinstance(features_bi, torch.Tensor) else
+                                (features_bi.dtype, tuple(features_bi.shape), features_bi.device)))
+        f = features_bi.contiguous()
+    th_bi, th_sp = _theta_values(theta_bi, "theta_bi", 5, ref), _theta_values(theta_sp, "theta_sp", 2, ref)
+    w1, w2 = _potts_weight(w1, "w1", ref), _potts_weight(w2, "w2", ref)
+    if th_bi is not None:
+        (params.theta_alpha_x, params.theta_alpha_y, params.theta_beta_r, params.theta_beta_g,
+         params.theta_beta_b) = th_bi
+    if th_sp is not None:
+        params.theta_gamma_x, params.theta_gamma_y = th_sp
+    if compat_bi is not None or compat_sp is not None:
+        with torch.no_grad():   # a missing matrix is -w I of its weight, formed on the device
+            return f, _compat_stack(ref, M, w1, w2, compat_bi, compat_sp).contiguous()
+    given = [(i, w) for i, w in enumerate((w1, w2)) if w is not None]
+    if given:
+        if torch.cuda.is_current_stream_capturing():
+            raise ValueError("w1 / w2 are read on the host at inference: they cannot be given inside CUDA-graph "
+                             "capture (pass compat_bi / compat_sp = -w I to keep them on the device)")
+        vals = torch.stack([w.detach().to(torch.float64) for _, w in given]).cpu().tolist()   # one synchronising copy
+        for (i, _), v in zip(given, vals):
+            setattr(params, "w1" if i == 0 else "w2", v)
+    return f, None
+
+
+def dense_crf_inference(unary, image, scale_factor=1.0, color_factor=13, maxiter=10, w1=None, w2=None,
+                        compat_bi=None, compat_sp=None, theta_bi=None, theta_sp=None, features_bi=None):
+    """dense_crf's forward at inference cost: the same arguments, semantics and checks as dense_crf / dense_crf_wide,
+    for 1 to 255 labels, returning the (N, M, H, W) marginals after `maxiter` iterations without autograd and without
+    keeping the iterates (the output is the only allocation).  So a CRF trained with dense_crf evaluates and
+    pseudo-labels with the same parameters.
+      w1 / w2, theta_bi / theta_sp : read on the host (one synchronising copy each), so refused inside CUDA-graph
+                                     capture; on the matrix path a weight only forms -w I of a missing matrix, on the
+                                     device
+      compat_bi / compat_sp        : read on the device (a matrix left None is -w I of its weight)
+      features_bi                  : read on the device, in place of image (which must then be None); an image whose
+                                     lattice keys leave the packed range gets NaN marginals (Engine.feature_range_flags)
+    A call with only matrices and features can be captured.  With no learned argument it is Engine.crf_dev's Potts
+    inference itself."""
+    if torch.is_autocast_enabled("cuda"):
+        unary = unary.float() if isinstance(unary, torch.Tensor) and unary.is_floating_point() else unary
+        if isinstance(features_bi, torch.Tensor) and features_bi.is_floating_point():
+            features_bi = features_bi.float()
+    u = _maps(unary, "unary")
+    N, M, H, W = u.shape
+    if features_bi is not None:
+        if image is not None:
+            raise ValueError("image is not used when features_bi is given: pass None")
+    elif (not isinstance(image, torch.Tensor) or image.dtype != torch.uint8 or tuple(image.shape) != (N, H, W, 3)
+          or image.device != u.device):
+        raise ValueError("image must be a (%d, %d, %d, 3) uint8 tensor on %s" % (N, H, W, u.device))
+    if int(maxiter) < 0:
+        raise ValueError("maxiter must be >= 0 (got %d)" % maxiter)
+    _cuda(u, "unary")
+    params = api.crf_params(float(scale_factor), float(color_factor), int(maxiter))
+    f, compat = _learned_crf(u, N, M, H, W, params, w1, w2, compat_bi, compat_sp, theta_bi, theta_sp, features_bi)
+    eng = _engine_for(u)
+    out = torch.empty(u.shape, dtype=torch.float32, device=u.device)
+    s = _stream(u)
+    if f is None and compat is None:
+        return eng.crf_dev(u, image.contiguous(), params, out, api.LAYOUT_NCHW, api.LAYOUT_NCHW, stream=s)
+    return eng.crf_learned_dev(u, None if f is not None else image.contiguous(), params, out, features=f,
+                               compat=compat, unary_layout=api.LAYOUT_NCHW, out_layout=api.LAYOUT_NCHW, stream=s)
+
+
 def softmax(fc8):
     """SoftmaxLayer (pylayers.py:23-51): probs = (softmax(fc8) + 1e-4) / sum over labels.  fc8 (N, M, H, W),
     M <= 32 (more labels raise the library's DsrgError)."""

@@ -269,7 +269,26 @@ def predict_masks_gt(ims, scores, labels_per_image, smooth=True, batch=16):
 _MODES = {"ms": _api.POST_SUM_SCORES, "gt": _api.POST_ZOOM_PROBS}
 
 
-def predict_mask_batch_dev(images, scores, labels=None, mode="ms", smooth=True, out=None):
+def _learned(ref, B, M, H, W, kw):
+    """(params, features, compat) of the learned-CRF keywords in kw that are given, checked as nn.dense_crf_inference
+    checks them, with the weights and sigmas read on the host once; None when none is given (CRF()'s own pass)."""
+    kw = {k: v for k, v in kw.items() if v is not None}
+    if not kw:
+        return None
+    from . import nn as _nn
+    params = _api.crf_params(1.0)
+    feats, compat = _nn._learned_crf(ref, B, M, H, W, params, **kw)
+    return params, feats, compat
+
+
+def _smooth_for(smooth, kw):
+    given = sorted(k for k, v in kw.items() if v is not None)
+    if given and not smooth:
+        raise ValueError("%s configure the CRF: they need smooth=True" % ", ".join(given))
+
+
+def predict_mask_batch_dev(images, scores, labels=None, mode="ms", smooth=True, out=None, *, w1=None, w2=None,
+                           compat_bi=None, compat_sp=None, theta_bi=None, theta_sp=None, features_bi=None):
     """The post-processing of a batch that never leaves the device, queued on the current CUDA stream (so it can be
     captured in a CUDA graph).
       images : (B,H,W,3) uint8 CUDA tensor
@@ -280,7 +299,24 @@ def predict_mask_batch_dev(images, scores, labels=None, mode="ms", smooth=True, 
                synchronisation, and read when the pass runs
       out    : optional (B,H,W) int32 CUDA tensor to write into (a fixed output lets the engine replay its own graph)
     Returns the (B,H,W) int32 label maps, which api.Confusion.add_dev counts directly.  Every argument is checked
-    (ValueError) before anything is queued."""
+    (ValueError) before anything is queued.
+
+    The keyword-only arguments run the learned CRF of nn.dense_crf_inference in place of CRF()'s, with the meanings
+    they have there (smooth only): the Potts weights w1 / w2 or the matrices compat_bi / compat_sp, the bandwidths
+    theta_bi / theta_sp and the bilateral features features_bi ((B, 5, H, W) float32; the images then give only the
+    shape).  The sigmas are absolute, at the image's resolution: a CRF learned on 41x41 maps with scale factor 12
+    passes theta * 12.  An image whose feature lattice leaves the packed key range gets -1 in every pixel.  With all
+    of them None the pass is CRF()'s, as before."""
+    kw = dict(w1=w1, w2=w2, compat_bi=compat_bi, compat_sp=compat_sp, theta_bi=theta_bi, theta_sp=theta_sp,
+              features_bi=features_bi)
+    _smooth_for(smooth, kw)
+    return _predict_mask_batch(images, scores, labels, mode, smooth, out,
+                               lambda B, M, H, W: _learned(images, B, M, H, W, kw))
+
+
+def _predict_mask_batch(images, scores, labels, mode, smooth, out, learned):
+    """predict_mask_batch_dev's pass; learned(B, M, H, W) checks and resolves the learned CRF (see _learned) once the
+    shapes are known, before anything is queued."""
     import torch
     if mode not in _MODES:
         raise ValueError("mode must be 'ms' or 'gt', not %r" % (mode,))
@@ -307,6 +343,7 @@ def predict_mask_batch_dev(images, scores, labels=None, mode="ms", smooth=True, 
     if out is not None and not (isinstance(out, torch.Tensor) and out.device == dev and out.dtype == torch.int32
                                 and tuple(out.shape) == (B, H, W) and out.is_contiguous()):
         raise ValueError("out must be a contiguous (B, H, W) int32 tensor on %s" % dev)
+    resolved = learned(B, M, H, W)
     eng = _batch_engine_for(B, H, W, M, dev.index)
     hc, wc = eng.capacity
     for s in scores:
@@ -323,11 +360,17 @@ def predict_mask_batch_dev(images, scores, labels=None, mode="ms", smooth=True, 
     if out is None:
         out = torch.empty((B, H, W), dtype=torch.int32, device=dev)
     with torch.cuda.device(dev):
-        eng.predict_mask_batch_dev(scores, images, out, _api.crf_params(1.0), _MODES[mode], EPS, smooth, sel)
+        if resolved is not None:
+            params, feats, compat = resolved
+            eng.predict_mask_batch_learned_dev(scores, None if feats is not None else images, out, params,
+                                               _MODES[mode], EPS, features=feats, compat=compat, sel=sel)
+        else:
+            eng.predict_mask_batch_dev(scores, images, out, _api.crf_params(1.0), _MODES[mode], EPS, smooth, sel)
     return out
 
 
-def predict_masks_dev(images, scores, labels=None, mode="ms", smooth=True):
+def predict_masks_dev(images, scores, labels=None, mode="ms", smooth=True, *, w1=None, w2=None, compat_bi=None,
+                      compat_sp=None, theta_bi=None, theta_sp=None, features_bi=None):
     """predict_mask_batch_dev over a batch of images of mixed sizes, the device analogue of predict_masks_ms /
     predict_masks_gt after one batched forward per scale (preprocess_batch_dev gives every image the same network
     input shape):
@@ -339,8 +382,13 @@ def predict_masks_dev(images, scores, labels=None, mode="ms", smooth=True):
     (H_i, W_i) int32 label maps in input order, queued on the current stream.  Every argument is checked (ValueError)
     before anything is queued.  The batch engine's capacity is ensured once for the largest group and image (outside
     a capture: run the largest batch and image once first); each group then selects its size without waiting for
-    the device (dsrg_engine_set_size_ordered), so nothing synchronises the host and a call can be captured."""
+    the device (dsrg_engine_set_size_ordered), so nothing synchronises the host and a call can be captured.
+    The keyword-only arguments are predict_mask_batch_dev's learned CRF; features_bi is then a list of (5, H_i, W_i)
+    float32 tensors aligned with images, grouped with them.  They are checked, and a weight or sigma tensor read on the
+    host, once per call."""
     import torch
+    kw = dict(w1=w1, w2=w2, compat_bi=compat_bi, compat_sp=compat_sp, theta_bi=theta_bi, theta_sp=theta_sp)
+    _smooth_for(smooth, dict(kw, features_bi=features_bi))
     if mode not in _MODES:
         raise ValueError("mode must be 'ms' or 'gt', not %r" % (mode,))
     images = list(images)
@@ -368,6 +416,16 @@ def predict_masks_dev(images, scores, labels=None, mode="ms", smooth=True):
                                    tuple(labels.shape) in ((B, M), (B, 1, 1, M))):
         raise ValueError("labels must be a (B, M) or (B, 1, 1, M) tensor on %s" % dev)
     sizes = [tuple(int(v) for v in im.shape[:2]) for im in images]
+    if features_bi is not None:
+        features_bi = list(features_bi)
+        if len(features_bi) != B or any(
+                not (isinstance(f, torch.Tensor) and f.device == dev and f.dtype == torch.float32
+                     and tuple(f.shape) == (5,) + hw) for f, hw in zip(features_bi, sizes)):
+            raise ValueError("features_bi must be a list of %d float32 tensors on %s, of shapes %s"
+                             % (B, dev, [(5,) + hw for hw in sizes]))
+    resolved = _learned(images[0], B, M, 1, 1, kw)   # the features go with their group below
+    if resolved is None and features_bi is not None:
+        resolved = (_api.crf_params(1.0), None, None)
     groups = _chunks(sizes, B)
     need = (max(len(g) for g in groups), max(h for h, _ in sizes), max(w for _, w in sizes))
     _, hc, wc = _batch_capacity(*need, M, dev.index)
@@ -386,7 +444,11 @@ def predict_masks_dev(images, scores, labels=None, mode="ms", smooth=True):
             g_images = torch.stack([images[i] for i in idx])
             g_scores = [torch.stack([s[i] for i in idx]) for s in scores]
             g_labels = None if labels is None else torch.stack([labels[i] for i in idx])
-        res = predict_mask_batch_dev(g_images, g_scores, g_labels, mode, smooth)
+        g_learned = None
+        if resolved is not None:
+            g_features = None if features_bi is None else torch.stack([features_bi[i] for i in idx])
+            g_learned = (resolved[0], g_features, resolved[2])
+        res = _predict_mask_batch(g_images, g_scores, g_labels, mode, smooth, None, lambda *_: g_learned)
         for r, i in enumerate(idx):
             out[i] = res[r]
     return out

@@ -274,6 +274,23 @@ int dsrg_crf_backward_wide_feat_dev(dsrg_engine *e, const float *q_hist_dev, int
                                     const float *grad_q_dev, float *grad_unary_dev, float *grad_features_dev,
                                     float *grad_potts_dev, float *grad_compat_dev, float *grad_theta_sp_dev,
                                     void *stream);
+/*
+ * The learned CRF at inference: DenseCRF::inference with MatrixCompatibility terms and / or
+ * addPairwiseEnergy(features, ...), for 1 to 255 labels.  It is the mean field of the training forwards above with the
+ * same parameters and conventions, keeping only Q_T (no history, no MODE_HIST kernels):
+ *   unary, image, params, out, layouts : as dsrg_crf_batch_dev (energy = -unary; no clamp)
+ *   compat_dev   : optional [2][M][M] {mu_bi, mu_sp}, as dsrg_crf_forward_train_compat_dev (params->w1 / w2 ignored)
+ *   features_dev : optional [B][5][H][W] bilateral features, as dsrg_crf_forward_train_feat_dev; image_dev then NULL
+ * Exactly one of image_dev / features_dev, else DSRG_E_INVALID before anything is queued.  Addresses are part of a
+ * cached graph's key, values not.  A feature image whose lattice keys leave the packed range gets NaN marginals, the
+ * other images are unaffected (dsrg_engine_feature_range_flags names it).  The marginals stay in the engine for the
+ * *_last_* entry points, as after dsrg_crf_batch_dev.  Nothing is allocated beyond the feature passes' per-image flags:
+ * above 32 labels the matrix messages use a lattice value buffer the label-chunked mean field leaves idle.  The batch
+ * size follows the array it describes, as in the training entry points.
+ */
+int dsrg_crf_batch_learned_dev(dsrg_engine *e, const float *unary_dev, int B, int unary_layout,
+                               const uint8_t *image_dev, const float *features_dev, const dsrg_crf_params *params,
+                               const float *compat_dev, float *out_dev, int out_layout, void *stream);
 /* arg-max labelling after inference: DenseCRFWrapper::map, densecrf_wrapper.cpp:39-43 */
 int dsrg_crf_map_batch_dev(dsrg_engine *e, int B, const float *unary_dev, int unary_layout,
                            const uint8_t *image_dev, const dsrg_crf_params *params,
@@ -455,6 +472,17 @@ int dsrg_predict_mask_batch_host(dsrg_engine *e, const float *const *scores_host
                                  int n_scales, int B, int mode, const uint8_t *images_host, float eps, int smooth,
                                  const dsrg_crf_params *params, const int32_t *sel_host, int32_t *result_out_host,
                                  float *probs_out_host);
+/*
+ * dsrg_predict_mask_batch_dev with dsrg_crf_batch_learned_dev's CRF step (smooth == 1 only): images_dev or
+ * features_dev (exactly one), compat_dev optional, the sigmas of params absolute at the image's resolution.  An image
+ * whose feature lattice leaves the packed key range gets NaN in probs_out and -1 in every pixel of its result.  The
+ * matrix messages above 32 labels use no extra memory, as in dsrg_crf_batch_learned_dev.
+ */
+int dsrg_predict_mask_batch_learned_dev(dsrg_engine *e, const float *const *scores_dev, const int *hs, const int *ws,
+                                        int n_scales, int B, int mode, const uint8_t *images_dev,
+                                        const float *features_dev, float eps, const dsrg_crf_params *params,
+                                        const float *compat_dev, const int32_t *sel_dev, int32_t *result_out_dev,
+                                        float *probs_out_dev, void *stream);
 
 /*
  * AnnotationLayer.forward (pylayers/pylayers/pylayers.py:369-387): image tags + sparse localisation cues
