@@ -143,6 +143,7 @@ SIGNATURES = {
     "dsrg_engine_lattice_bary": (_i, [_vp, _i, _i, _vp]),
     "dsrg_engine_lattice_idle": (_i, [_vp, _i, _vp]),
     "dsrg_engine_tile_views": (_i, [_vp, _i, _i, _vp, _vp, _vp, _vp, _vp]),
+    "dsrg_engine_tile_blocks": (_i, [_vp, _i, _i, _vp, _vp]),
     "dsrg_densecrf_create": (_vp, [_i, _i, _i]),
     "dsrg_densecrf_destroy": (None, [_vp]),
     "dsrg_densecrf_npixels": (_i, [_vp]),

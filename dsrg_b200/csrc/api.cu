@@ -126,6 +126,8 @@ static int lattice_alloc(Engine *e, Lattice &L, int d, int shared) {
     rc |= dalloc(e, &L.tl_pack, nt * L.entcap);
     rc |= dalloc(e, &L.tl_loc, n * (d + 1) * L.N);
     rc |= dalloc(e, &L.wn, n * (d + 1) * L.N);
+    rc |= dalloc(e, &L.tl_w, nt * (d + 1) * kTileThreads);
+    rc |= dalloc(e, &L.tl_li, nt * (d + 1) * kTileThreads);
     if (rc) return DSRG_E_NOMEM;
     if (cudaMemset(L.hkeys, 0xFF, sizeof(uint64_t) * n * L.cap) != cudaSuccess) return DSRG_E_CUDA;
     if (cudaMemset(L.tl_hy, 0, nt) != cudaSuccess) return DSRG_E_CUDA;
@@ -154,6 +156,8 @@ static void lattice_free(Lattice &L) {
     cudaFree(L.tl_pack);
     cudaFree(L.tl_loc);
     cudaFree(L.wn);
+    cudaFree(L.tl_w);
+    cudaFree(L.tl_li);
 }
 
 int check_device_flag(Engine *e, cudaStream_t s) {
@@ -1296,6 +1300,23 @@ int dsrg_engine_tile_views(dsrg_engine *h, int which, int b, int *nloc_out, uint
         DSRG_CUDA_TRY(cudaMemcpy(hdr_out, L.tl_hdr + sb * nt * L.maxloc, sizeof(int2) * nt * L.maxloc,
                                  cudaMemcpyDeviceToHost));
     if (loc_out) DSRG_CUDA_TRY(cudaMemcpy(loc_out, L.tl_loc + sb * n, sizeof(uint16_t) * n, cudaMemcpyDeviceToHost));
+    return DSRG_OK;
+}
+
+int dsrg_engine_tile_blocks(dsrg_engine *h, int which, int b, float *w_out, uint16_t *loc_out) {
+    Engine *e = (Engine *)h;
+    DeviceScope dev_scope(e);
+    int rc = check_entry(e, 1, e && (which == 0 || which == 1) && b >= 0 && b < e->maxB);
+    if (rc) return rc;
+    if (e->MP > DSRG_MAX_LABELS) {
+        set_error("the tile-local views are not built for %d labels (more than %d)", e->M, DSRG_MAX_LABELS);
+        return DSRG_E_STATE;
+    }
+    const Lattice &L = which == 0 ? e->sp : e->bi;
+    const size_t n = (size_t)e->ntiles * (L.d + 1) * kTileThreads, at = (L.shared ? 0 : b) * n;
+    DSRG_CUDA_TRY(cudaDeviceSynchronize());
+    if (w_out) DSRG_CUDA_TRY(cudaMemcpy(w_out, L.tl_w + at, sizeof(float) * n, cudaMemcpyDeviceToHost));
+    if (loc_out) DSRG_CUDA_TRY(cudaMemcpy(loc_out, L.tl_li + at, sizeof(uint16_t) * n, cudaMemcpyDeviceToHost));
     return DSRG_OK;
 }
 

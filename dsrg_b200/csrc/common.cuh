@@ -73,6 +73,10 @@ struct Lattice {
     int entcap = 0;                // 256*(d+1) + maxloc, a multiple of 8 (16-byte blocks for the bulk copy)
     uint16_t *tl_loc = nullptr;    // [nimg][d+1][N] local vertex index of (pixel, r), kLocRemote if not in the tile's list
     float *wn = nullptr;           // [nimg][d+1][N] barycentric weight * norm
+    // the same two per tile, in the order the forward tile kernels keep them in shared memory (one bulk copy each):
+    // [nimg][ntiles][d+1][kTileThreads], slot t = the tile's pixel t; outside the image weight 0 and kLocRemote
+    float *tl_w = nullptr;
+    uint16_t *tl_li = nullptr;
     float scale[5] = {0, 0, 0, 0, 0};  // elevation scale factors (permutohedral.cpp:179-182)
     float sigma[5] = {0, 0, 0, 0, 0};  // feature sigmas: x, y[, c0, c1, c2]
 };

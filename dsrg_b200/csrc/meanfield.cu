@@ -83,8 +83,10 @@ struct TileLat {
     const uint8_t *tl_hy;    // [nimg][ntiles] 1: hybrid tile (bilateral view only)
     const int2 *tl_hdr;
     const uint16_t *tl_pack;
+    // per (pixel, r): the local vertex index and the weight wn.  k_mf_tile_bwd reads them planar ([nimg][dp1][N], tl_loc
+    // and wn), the forward kernels as the tile-major blocks tl_li / tl_w ([nimg][ntiles][dp1][kTileThreads])
     const uint16_t *tl_loc;
-    const float *wn;         // [nimg][dp1][N]
+    const float *wn;
     const float *val_in;     // blurred values of the previous splat (slice source)
     float *val_out;          // zeroed values (splat target)
     int entcap;
@@ -176,12 +178,22 @@ struct TileSmem {
     float wtab[kEntZero + 4];  // [r][thread] weights of the tile being splatted, then the zero slot
 };
 
+// The forward kernels' shared memory: the weight blocks of the tile (tiles.cu) are bulk-copied into wtab, its local-index
+// blocks into loc, both [r][thread]; a thread reads its own slot of each row, so the slice is free of bank conflicts
+template <int MP, int MAXBI = kMaxLocBi>
+struct TileSmemFwd {
+    static_assert(sizeof(TileStage<MP, MAXBI>) % 16 == 0, "wtab's rows are bulk-copy destinations");
+    TileSmem<MP, MAXBI> t;
+    alignas(16) uint16_t loc[kEntRows * kTileThreads];
+};
+
 // the size of a lattice's CSR entry block as bulk-copied, from the header of its last segment
 __device__ __forceinline__ uint32_t ent_block_bytes(int2 last) {
     return ((uint32_t)((last.x & 0xffff) + (((last.x >> 16) + 1) & ~1)) * 2u + 15u) & ~15u;
 }
 
-// the current tile's weights into the table its CSR entries index; the CTA's thread t is the tile's pixel t
+// the current tile's weights into the table its CSR entries index (k_mf_tile_bwd; the forward kernels bulk-copy the
+// tile's tl_w blocks there); the CTA's thread t is the tile's pixel t
 __device__ __forceinline__ void tile_put_weights(float *wtab, const float *w_sp, const float *w_bi) {
 #pragma unroll
     for (int r = 0; r < 3; r++) wtab[(ent_r0(3) + r) * kTileThreads + threadIdx.x] = w_sp[r];
@@ -189,17 +201,27 @@ __device__ __forceinline__ void tile_put_weights(float *wtab, const float *w_sp,
     for (int r = 0; r < 6; r++) wtab[(ent_r0(6) + r) * kTileThreads + threadIdx.x] = w_bi[r];
 }
 
+// A pixel's weight and local vertex index at incidence r.  k_mf_tile_bwd holds the weights in registers and reads the
+// indices from the planar tl_loc, `stride` apart; the forward kernels (SW) read both from their shared tables, rows
+// kTileThreads apart, w and loc pointing at the thread's own slot of row 0.
+template <bool SW>
+__device__ __forceinline__ float w_at(const float *w, int r) { return w[SW ? r * kTileThreads : r]; }
+template <bool SW>
+__device__ __forceinline__ int loc_at(const uint16_t *loc, size_t stride, int r) {
+    return SW ? (int)loc[r * kTileThreads] : (int)__ldg(loc + r * stride);
+}
+
 // slice one lattice from the staged rows (shared memory): t += coef * sum_r wn_r * row_r
 // tail1: M = MP - 3 (e.g. 21 labels in 24 lanes): the last chunk holds ONE real channel, so a 32-bit load
 // (one shared-memory wavefront per warp) replaces the 128-bit one (four)
-template <int MP, int DP1>
+template <int MP, int DP1, bool SW = false>
 __device__ __forceinline__ void tile_slice_smem(const float4 *vs, const uint16_t *loc, size_t stride,
                                                 const float *w, float coef, float *t, bool tail1) {
     constexpr int CH = MP / 4, CHP = TileRow<MP>::CHP;
 #pragma unroll
     for (int r = 0; r < DP1; r++) {
-        const float4 *row = vs + (int)__ldg(loc + r * stride) * CHP;
-        const float wr = coef * w[r];
+        const float4 *row = vs + loc_at<SW>(loc, stride, r) * CHP;
+        const float wr = coef * w_at<SW>(w, r);
 #pragma unroll
         for (int c = 0; c < CH - 1; c++) {
             const float4 v = row[c];
@@ -223,14 +245,14 @@ __device__ __forceinline__ void tile_slice_smem(const float4 *vs, const uint16_t
 }
 
 // fallback: slice straight from the global value rows
-template <int MP, int DP1>
+template <int MP, int DP1, bool SW = false>
 __device__ __forceinline__ void tile_slice_global(const float4 *vin, const int32_t *off, size_t stride,
                                                   int base, const float *w, float coef, float *t) {
     constexpr int CH = MP / 4;
 #pragma unroll
     for (int r = 0; r < DP1; r++) {
         const float4 *row = vin + (size_t)(base + off[r * stride]) * CH;
-        const float wr = coef * w[r];
+        const float wr = coef * w_at<SW>(w, r);
 #pragma unroll
         for (int c = 0; c < CH; c++) {
             const float4 v = row[c];
@@ -244,7 +266,7 @@ __device__ __forceinline__ void tile_slice_global(const float4 *vin, const int32
 
 // hybrid tiles (tiles.cu): an incidence whose vertex is in the tile-local list is sliced from the staged rows, the
 // others (tl_loc == kLocRemote) straight from the global value rows; returns the mask of the remote ones
-template <int MP, int DP1>
+template <int MP, int DP1, bool SW = false>
 __device__ __forceinline__ unsigned tile_slice_mixed(const float4 *vs, const uint16_t *loc, const float4 *vin,
                                                      const int32_t *off, size_t stride, int base, const float *w,
                                                      float coef, float *t) {
@@ -252,8 +274,8 @@ __device__ __forceinline__ unsigned tile_slice_mixed(const float4 *vs, const uin
     unsigned remote = 0;  // bit r: incidence r of this pixel goes direct
 #pragma unroll
     for (int r = 0; r < DP1; r++) {
-        const int l = (int)__ldg(loc + r * stride);
-        const float wr = coef * w[r];
+        const int l = loc_at<SW>(loc, stride, r);
+        const float wr = coef * w_at<SW>(w, r);
         if (l != kLocRemote) {
             const float4 *row = vs + l * CHP;
 #pragma unroll
@@ -281,12 +303,12 @@ __device__ __forceinline__ unsigned tile_slice_mixed(const float4 *vs, const uin
 }
 
 // which incidences of this pixel are remote (first iteration: nothing is sliced)
-template <int DP1>
+template <int DP1, bool SW = false>
 __device__ __forceinline__ unsigned tile_remote_mask(const uint16_t *loc, size_t stride) {
     unsigned remote = 0;
 #pragma unroll
     for (int r = 0; r < DP1; r++)
-        if ((int)__ldg(loc + r * stride) == kLocRemote) remote |= 1u << r;
+        if (loc_at<SW>(loc, stride, r) == kLocRemote) remote |= 1u << r;
     return remote;
 }
 
@@ -345,22 +367,22 @@ __device__ __forceinline__ void tile_splat_csr(float4 *vout_sp, float4 *vout_bi,
 }
 
 // direct splat of one pixel (fallback tiles): d+1 rows x MP/4 vector reductions
-template <int MP, int DP1>
+template <int MP, int DP1, bool SW = false>
 __device__ __forceinline__ void tile_splat_direct(float4 *vout, const int32_t *off, size_t stride,
                                                   int base, const float *w, const float *q) {
     constexpr int CH = MP / 4;
 #pragma unroll
     for (int r = 0; r < DP1; r++) {
         float4 *row = vout + (size_t)(base + off[r * stride]) * CH;
+        const float wr = w_at<SW>(w, r);
 #pragma unroll
         for (int c = 0; c < CH; c++)
-            atomicAdd(row + c, make_float4(w[r] * q[4 * c], w[r] * q[4 * c + 1], w[r] * q[4 * c + 2],
-                                           w[r] * q[4 * c + 3]));
+            atomicAdd(row + c, make_float4(wr * q[4 * c], wr * q[4 * c + 1], wr * q[4 * c + 2], wr * q[4 * c + 3]));
     }
 }
 
 // direct splat of one pixel's remote incidences (hybrid tiles): MP/4 vector reductions per such row
-template <int MP, int DP1>
+template <int MP, int DP1, bool SW = false>
 __device__ __forceinline__ void tile_splat_remote(float4 *vout, unsigned remote, const int32_t *off, size_t stride,
                                                   int base, const float *w, const float *q) {
     constexpr int CH = MP / 4;
@@ -368,10 +390,10 @@ __device__ __forceinline__ void tile_splat_remote(float4 *vout, unsigned remote,
     for (int r = 0; r < DP1; r++) {
         if (!(remote >> r & 1u)) continue;
         float4 *row = vout + (size_t)(base + __ldg(off + r * stride)) * CH;
+        const float wr = w_at<SW>(w, r);
 #pragma unroll
         for (int c = 0; c < CH; c++)
-            atomicAdd(row + c, make_float4(w[r] * q[4 * c], w[r] * q[4 * c + 1], w[r] * q[4 * c + 2],
-                                           w[r] * q[4 * c + 3]));
+            atomicAdd(row + c, make_float4(wr * q[4 * c], wr * q[4 * c + 1], wr * q[4 * c + 2], wr * q[4 * c + 3]));
     }
 }
 
@@ -413,7 +435,7 @@ __device__ __forceinline__ void compat_apply(const float *mu, const float *sl, f
 }
 
 // tile_slice_smem / tile_slice_global one row at a time (the same fma chain): at 32 labels ptxas otherwise issued a
-// whole lattice's row loads ahead of the previous lattice's message and spilled
+// whole lattice's row loads ahead of the previous lattice's message and spilled.  w and loc are the shared tables (SW).
 template <int MP, int DP1>
 __device__ __forceinline__ void compat_slice(bool direct, const float4 *vs, const uint16_t *loc, const float4 *vin,
                                              const int32_t *off, size_t stride, int base, const float *w, float coef,
@@ -421,9 +443,9 @@ __device__ __forceinline__ void compat_slice(bool direct, const float4 *vs, cons
 #pragma unroll
     for (int r = 0; r < DP1; r++) {
         if (!direct)
-            tile_slice_smem<MP, 1>(vs, loc + r * stride, stride, w + r, coef, sl, tail1);
+            tile_slice_smem<MP, 1, true>(vs, loc + r * kTileThreads, stride, w + r * kTileThreads, coef, sl, tail1);
         else
-            tile_slice_global<MP, 1>(vin, off + r * stride, stride, base, w + r, coef, sl);
+            tile_slice_global<MP, 1, true>(vin, off + r * stride, stride, base, w + r * kTileThreads, coef, sl);
         asm volatile("" ::: "memory");
     }
 }
@@ -432,9 +454,9 @@ __device__ __forceinline__ void compat_slice(bool direct, const float4 *vs, cons
 // The tile coordinates and the bulk-copy staging are still written out in each kernel: moved into a shared helper,
 // either one changed the SASS of some k_mf_tile / k_mf_tile_hy instantiations (register choice, loop offsets).
 //
-// Park the pixel's Q row in the staging buffer (once every thread is done reading the staged rows) and its weights
-// in wtab, for the CSR splat; returns the Q rows
-template <int MP, int MAXBI>
+// Park the pixel's Q row in the staging buffer (once every thread is done reading the staged rows) and, with PUT_W
+// (k_mf_tile_bwd: the forward kernels bulk-copy theirs), its weights in wtab, for the CSR splat; returns the Q rows
+template <int MP, int MAXBI, bool PUT_W = true>
 __device__ __forceinline__ const float4 *tile_park(TileSmem<MP, MAXBI> &smt, const float *t, const float *w_sp,
                                                    const float *w_bi) {
     constexpr int CH = MP / 4, CHP = TileStage<MP, MAXBI>::CHP;
@@ -443,9 +465,23 @@ __device__ __forceinline__ const float4 *tile_park(TileSmem<MP, MAXBI> &smt, con
     float4 *qs = smt.st.buf;
 #pragma unroll
     for (int c = 0; c < CH; c++) qs[tid * CHP + c] = make_float4(t[4 * c], t[4 * c + 1], t[4 * c + 2], t[4 * c + 3]);
-    tile_put_weights(smt.wtab, w_sp, w_bi);
+    if (PUT_W) tile_put_weights(smt.wtab, w_sp, w_bi);
     __syncthreads();
     return qs;
+}
+
+// The forward kernels' per-tile blocks (tiles.cu), as ONE arrival on the tile's barrier: both weight blocks (the slice
+// and every splat read them) into wtab and, where the slice reads them (li_*), the local-index blocks into loc
+template <int MP, int MAXBI>
+__device__ __forceinline__ void tile_fetch_blocks(TileSmemFwd<MP, MAXBI> &smf, const TileLat &sp, const TileLat &bi,
+                                                  size_t ti_sp, size_t ti_bi, bool li_sp, bool li_bi) {
+    constexpr uint32_t kSp = 3 * kTileThreads, kBi = 6 * kTileThreads;  // slots per block
+    uint64_t *bar = &smf.t.st.bar;
+    mbar_arrive_expect_tx(bar, (kSp + kBi) * 4u + (li_sp ? kSp * 2u : 0u) + (li_bi ? kBi * 2u : 0u));
+    bulk_g2s(smf.t.wtab + ent_r0(3) * kTileThreads, sp.wn + ti_sp * kSp, kSp * 4u, bar);
+    bulk_g2s(smf.t.wtab + ent_r0(6) * kTileThreads, bi.wn + ti_bi * kBi, kBi * 4u, bar);
+    if (li_sp) bulk_g2s(smf.loc + ent_r0(3) * kTileThreads, sp.tl_loc + ti_sp * kSp, kSp * 2u, bar);
+    if (li_bi) bulk_g2s(smf.loc + ent_r0(6) * kTileThreads, bi.tl_loc + ti_bi * kBi, kBi * 2u, bar);
 }
 
 // Q = softmax(t) in place (expAndNormalize, densecrf.cpp:98-106); the last iteration (every one with MODE_HIST) stores
@@ -477,13 +513,12 @@ __device__ __forceinline__ void tile_update(float *t, int M, int N, float *__res
     }
 }
 
-// The pixel's unaries into t and its folded weights into w_sp / w_bi (zeros outside the image).  U is either the
-// engine's planar copy or, for NCHW callers, the caller's buffer itself; the reference's in-place clamp
-// (pylayers.py:312) is then applied on the fly and written back once, by the first iteration.
+// The pixel's unaries into t (zeros outside the image).  U is either the engine's planar copy or, for NCHW callers,
+// the caller's buffer itself; the reference's in-place clamp (pylayers.py:312) is then applied on the fly and written
+// back once, by the first iteration.
 template <int MP, int MODE>
 __device__ __forceinline__ void tile_load_pixel(const float *U, float *U_rw, int clamp, int M, int N, int b, int pix,
-                                                bool in, const float *wn_sp, const float *wn_bi, float *t,
-                                                float *w_sp, float *w_bi) {
+                                                bool in, float *t) {
     {
         const size_t ub = (size_t)b * M * N + pix;
         const float *Ub = U + ub;
@@ -501,14 +536,6 @@ __device__ __forceinline__ void tile_load_pixel(const float *U, float *U_rw, int
             Ub += N;
         }
     }
-    {
-        const float *p = wn_sp;
-#pragma unroll
-        for (int r = 0; r < 3; r++, p += N) w_sp[r] = in ? __ldg(p) : 0.0f;
-        p = wn_bi;
-#pragma unroll
-        for (int r = 0; r < 6; r++, p += N) w_bi[r] = in ? __ldg(p) : 0.0f;
-    }
 }
 
 // MODE_COMPAT holds a slice beside t (2 MP floats): like k_mf_tile_bwd it runs one CTA per SM above 12 labels rather
@@ -519,10 +546,11 @@ k_mf_tile(const float *U, float *U_rw, int clamp, float *__restrict__ Qout, Tile
           float c_bi, int M, int N, int W, int H, int tiles_x, int ntiles, int tile_w) {
     static_assert(!(MODE & MODE_COMPAT) || (MODE & 3) != MODE_FIRST, "U_rw carries the matrices: nothing may clamp");
     constexpr int kRowBytes = MP * 4;
-    using SM = TileSmem<MP>;
+    using SF = TileSmemFwd<MP>;
     using ST = TileStage<MP>;
     extern __shared__ __align__(128) unsigned char smem_raw[];
-    SM &smt = *reinterpret_cast<SM *>(smem_raw);
+    SF &smf = *reinterpret_cast<SF *>(smem_raw);
+    TileSmem<MP> &smt = smf.t;
     ST &sm = smt.st;
     // A hybrid tile is k_mf_tile_hy's.  The test reads a byte map of its own and stands before anything else: the
     // same test on the tile's vertex count, wherever it was placed, made ptxas allocate this kernel's 64 registers
@@ -530,7 +558,7 @@ k_mf_tile(const float *U, float *U_rw, int clamp, float *__restrict__ Qout, Tile
     if (bi.tl_hy[(size_t)blockIdx.y * ntiles + blockIdx.x]) return;
     const float *mu = nullptr;
     if constexpr ((MODE & MODE_COMPAT) != 0) {
-        mu = compat_stage<MP>(smem_raw + sizeof(SM), U_rw, M);
+        mu = compat_stage<MP>(smem_raw + sizeof(SF), U_rw, M);
     } else if ((MODE & MODE_HIST) && U_rw) {
         c_sp *= __ldg(U_rw + 1);
         c_bi *= __ldg(U_rw);
@@ -553,15 +581,17 @@ k_mf_tile(const float *U, float *U_rw, int clamp, float *__restrict__ Qout, Tile
     const size_t strideN = (size_t)N;
     const size_t px_sp = (size_t)sb_sp * 3 * N + pix, px_bi = (size_t)sb_bi * 6 * N + pix;
 
-    // ---- asynchronous staging: every local vertex's value row (96 B) and the two CSR entry blocks
-    // are pulled into shared memory by the bulk-copy engine while the threads load their per-pixel data
+    // ---- asynchronous staging: every local vertex's value row (96 B), the two CSR entry blocks and the tile's weight
+    // and local-index blocks are pulled into shared memory by the bulk-copy engine while the threads load their unaries
     const int n_copies = ((MODE & 3) != MODE_FIRST ? n_sp + n_bi : 0) + ((MODE & 3) != MODE_LAST ? (n_sp > 0) + (n_bi > 0) : 0);
     if (tid == 0) {
-        mbar_init(&sm.bar, n_copies > 0 ? n_copies : 1);
+        mbar_init(&sm.bar, n_copies + 1);
         smt.wtab[kEntZero] = 0.0f;
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
     __syncthreads();
+    if (tid == kTileThreads - 1)  // the last thread stages a vertex only when the tile has more than 256
+        tile_fetch_blocks(smf, sp, bi, ti_sp, ti_bi, (MODE & 3) != MODE_FIRST && !fb_sp, (MODE & 3) != MODE_FIRST && !fb_bi);
     for (int i = tid; i < n_sp + n_bi; i += kTileThreads) {  // up to kMaxLocSp + kMaxLocBi local vertices
         const bool is_sp = i < n_sp;
         const int lv = is_sp ? i : i - n_sp;
@@ -579,11 +609,12 @@ k_mf_tile(const float *U, float *U_rw, int clamp, float *__restrict__ Qout, Tile
                      is_sp ? sp.tl_pack + ti_sp * sp.entcap : bi.tl_pack + ti_bi * bi.entcap, bytes, &sm.bar);
         }
     }
-    if (n_copies == 0 && tid == 0) mbar_arrive_expect_tx(&sm.bar, 0);
 
-    // ---- per-pixel data (thread = pixel) ----
-    float t[MP], w_sp[3], w_bi[6];
-    tile_load_pixel<MP, MODE>(U, U_rw, clamp, M, N, b, pix, in, sp.wn + px_sp, bi.wn + px_bi, t, w_sp, w_bi);
+    // ---- per-pixel data (thread = pixel); its weights and local indices are its slots of the shared tables ----
+    float t[MP];
+    tile_load_pixel<MP, MODE>(U, U_rw, clamp, M, N, b, pix, in, t);
+    const float *w_sp = smt.wtab + ent_r0(3) * kTileThreads + tid, *w_bi = smt.wtab + ent_r0(6) * kTileThreads + tid;
+    const uint16_t *loc_sp = smf.loc + ent_r0(3) * kTileThreads + tid, *loc_bi = smf.loc + ent_r0(6) * kTileThreads + tid;
     mbar_wait(&sm.bar, 0);
 
     // ---- slice + update ----
@@ -598,36 +629,36 @@ k_mf_tile(const float *U, float *U_rw, int clamp, float *__restrict__ Qout, Tile
             float sl[MP];
 #pragma unroll
             for (int k = 0; k < MP; k++) sl[k] = 0.0f;
-            compat_slice<MP, 3>(fb_sp, vs_sp, sp.tl_loc + px_sp, reinterpret_cast<const float4 *>(sp.val_in),
-                                sp.off + px_sp, strideN, base_sp, w_sp, c_sp, sl, tail1);
+            compat_slice<MP, 3>(fb_sp, vs_sp, loc_sp, reinterpret_cast<const float4 *>(sp.val_in), sp.off + px_sp,
+                                strideN, base_sp, w_sp, c_sp, sl, tail1);
             compat_clear_phantoms<MP>(sl, M);
             compat_apply<MP, false>(mu + MP * MP, sl, t);
 #pragma unroll
             for (int k = 0; k < MP; k++) sl[k] = 0.0f;
-            compat_slice<MP, 6>(fb_bi, vs_bi, bi.tl_loc + px_bi, reinterpret_cast<const float4 *>(bi.val_in),
-                                bi.off + px_bi, strideN, base_bi, w_bi, c_bi, sl, tail1);
+            compat_slice<MP, 6>(fb_bi, vs_bi, loc_bi, reinterpret_cast<const float4 *>(bi.val_in), bi.off + px_bi,
+                                strideN, base_bi, w_bi, c_bi, sl, tail1);
             compat_clear_phantoms<MP>(sl, M);
             compat_apply<MP, false>(mu, sl, t);
         } else {
             if (!fb_sp)
-                tile_slice_smem<MP, 3>(vs_sp, sp.tl_loc + px_sp, strideN, w_sp, c_sp, t, tail1);
+                tile_slice_smem<MP, 3, true>(vs_sp, loc_sp, strideN, w_sp, c_sp, t, tail1);
             else
-                tile_slice_global<MP, 3>(reinterpret_cast<const float4 *>(sp.val_in), sp.off + px_sp, strideN,
-                                         base_sp, w_sp, c_sp, t);
+                tile_slice_global<MP, 3, true>(reinterpret_cast<const float4 *>(sp.val_in), sp.off + px_sp, strideN,
+                                               base_sp, w_sp, c_sp, t);
             if (!fb_bi)
-                tile_slice_smem<MP, 6>(vs_bi, bi.tl_loc + px_bi, strideN, w_bi, c_bi, t, tail1);
+                tile_slice_smem<MP, 6, true>(vs_bi, loc_bi, strideN, w_bi, c_bi, t, tail1);
             else
-                tile_slice_global<MP, 6>(reinterpret_cast<const float4 *>(bi.val_in), bi.off + px_bi, strideN,
-                                         base_bi, w_bi, c_bi, t);
+                tile_slice_global<MP, 6, true>(reinterpret_cast<const float4 *>(bi.val_in), bi.off + px_bi, strideN,
+                                               base_bi, w_bi, c_bi, t);
         }
     }
     tile_update<MP, MODE>(t, M, N, Qout, b, pix, in);
     if ((MODE & 3) == MODE_LAST) return;
-    const float4 *qs = tile_park(smt, t, w_sp, w_bi);
+    const float4 *qs = tile_park<MP, kMaxLocBi, false>(smt, t, nullptr, nullptr);
     // ---- splat ----
     float4 *vout_sp = reinterpret_cast<float4 *>(sp.val_out), *vout_bi = reinterpret_cast<float4 *>(bi.val_out);
-    if (fb_sp && in) tile_splat_direct<MP, 3>(vout_sp, sp.off + px_sp, strideN, base_sp, w_sp, t);
-    if (fb_bi && in) tile_splat_direct<MP, 6>(vout_bi, bi.off + px_bi, strideN, base_bi, w_bi, t);
+    if (fb_sp && in) tile_splat_direct<MP, 3, true>(vout_sp, sp.off + px_sp, strideN, base_sp, w_sp, t);
+    if (fb_bi && in) tile_splat_direct<MP, 6, true>(vout_bi, bi.off + px_bi, strideN, base_bi, w_bi, t);
     tile_splat_csr<MP>(vout_sp, vout_bi, n_sp, n_bi, hdr_sp, hdr_bi, base_sp, base_bi, ent_sp, ent_bi, qs, smt.wtab);
 }
 
@@ -645,15 +676,17 @@ k_mf_tile_hy(const float *U, float *U_rw, int clamp, float *__restrict__ Qout, T
     static_assert(!(MODE & MODE_COMPAT) || (MODE & 3) != MODE_FIRST, "U_rw carries the matrices: nothing may clamp");
     constexpr int kRowBytes = MP * 4;
     using ST = TileStage<MP, kMaxLocHy>;
+    using SF = TileSmemFwd<MP, kMaxLocHy>;
     constexpr int CHP = ST::CHP;
     extern __shared__ __align__(128) unsigned char smem_raw[];
-    TileSmem<MP, kMaxLocHy> &smt = *reinterpret_cast<TileSmem<MP, kMaxLocHy> *>(smem_raw);
+    SF &smf = *reinterpret_cast<SF *>(smem_raw);
+    TileSmem<MP, kMaxLocHy> &smt = smf.t;
     ST &sm = smt.st;
     const int tid = threadIdx.x;
     const int nhy = *hy_count;
     const float *mu = nullptr;   // visible after the first tile's barriers
     if constexpr ((MODE & MODE_COMPAT) != 0) {
-        mu = compat_stage<MP>(smem_raw + sizeof(TileSmem<MP, kMaxLocHy>), U_rw, M);
+        mu = compat_stage<MP>(smem_raw + sizeof(SF), U_rw, M);
     } else if ((MODE & MODE_HIST) && U_rw) {
         c_sp *= __ldg(U_rw + 1);
         c_bi *= __ldg(U_rw);
@@ -662,6 +695,8 @@ k_mf_tile_hy(const float *U, float *U_rw, int clamp, float *__restrict__ Qout, T
     float4 *vs_sp = sm.buf, *vs_bi = sm.buf + kMaxLocSp * CHP;
     uint16_t *ent_sp = sm.ent, *ent_bi = sm.ent + ST::kEntSp;
     if (tid == 0) smt.wtab[kEntZero] = 0.0f;  // visible after the first tile's barriers
+    const float *w_sp = smt.wtab + ent_r0(3) * kTileThreads + tid, *w_bi = smt.wtab + ent_r0(6) * kTileThreads + tid;
+    const uint16_t *loc_sp = smf.loc + ent_r0(3) * kTileThreads + tid, *loc_bi = smf.loc + ent_r0(6) * kTileThreads + tid;
     float4 *vout_sp = reinterpret_cast<float4 *>(sp.val_out), *vout_bi = reinterpret_cast<float4 *>(bi.val_out);
     for (int item = blockIdx.x; item < nhy; item += gridDim.x) {
         const int2 bt = hy_list[item];
@@ -680,16 +715,19 @@ k_mf_tile_hy(const float *U, float *U_rw, int clamp, float *__restrict__ Qout, T
         const int2 *hdr_sp = sp.tl_hdr + ti_sp * kMaxLocSp, *hdr_bi = bi.tl_hdr + ti_bi * kMaxLocHy;
         const size_t px_sp = (size_t)sb_sp * 3 * N + pix, px_bi = (size_t)sb_bi * 6 * N + pix;
 
-        // ---- asynchronous staging of the local vertices' rows and the CSR entry blocks (as in k_mf_tile) ----
+        // ---- asynchronous staging of the local vertices' rows, the CSR entry blocks and the tile's weight and
+        // local-index blocks (as in k_mf_tile; every incidence of the bilateral lattice may be remote) ----
         const int n_copies = ((MODE & 3) != MODE_FIRST ? n_sp + n_bi : 0) + ((MODE & 3) != MODE_LAST ? (n_sp > 0) + (n_bi > 0) : 0);
         if (tid == 0) {
-            mbar_init(&sm.bar, n_copies > 0 ? n_copies : 1);
+            mbar_init(&sm.bar, n_copies + 1);
             asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
         }
         __syncthreads();
         // the previous tile of this CTA wrote its Q rows into the same shared memory through the generic proxy: order
         // those writes before the bulk copies (async proxy) of this tile
         asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+        if (tid == kTileThreads - 1)
+            tile_fetch_blocks(smf, sp, bi, ti_sp, ti_bi, (MODE & 3) != MODE_FIRST || hy_sp, true);
         for (int i = tid; i < n_sp + n_bi; i += kTileThreads) {
             const bool is_sp = i < n_sp;
             const int lv = is_sp ? i : i - n_sp;
@@ -707,11 +745,10 @@ k_mf_tile_hy(const float *U, float *U_rw, int clamp, float *__restrict__ Qout, T
                          is_sp ? sp.tl_pack + ti_sp * sp.entcap : bi.tl_pack + ti_bi * bi.entcap, bytes, &sm.bar);
             }
         }
-        if (n_copies == 0 && tid == 0) mbar_arrive_expect_tx(&sm.bar, 0);
 
         // ---- per-pixel data ----
-        float t[MP], w_sp[3], w_bi[6];
-        tile_load_pixel<MP, MODE>(U, U_rw, clamp, M, N, b, pix, in, sp.wn + px_sp, bi.wn + px_bi, t, w_sp, w_bi);
+        float t[MP];
+        tile_load_pixel<MP, MODE>(U, U_rw, clamp, M, N, b, pix, in, t);
         mbar_wait(&sm.bar, 0);
 
         // ---- slice + update ----
@@ -721,32 +758,32 @@ k_mf_tile_hy(const float *U, float *U_rw, int clamp, float *__restrict__ Qout, T
                 float sl[MP];
 #pragma unroll
                 for (int k = 0; k < MP; k++) sl[k] = 0.0f;
-                rm_sp = tile_slice_mixed<MP, 3>(vs_sp, sp.tl_loc + px_sp, reinterpret_cast<const float4 *>(sp.val_in),
-                                                sp.off + px_sp, strideN, base_sp, w_sp, c_sp, sl);
+                rm_sp = tile_slice_mixed<MP, 3, true>(vs_sp, loc_sp, reinterpret_cast<const float4 *>(sp.val_in),
+                                                      sp.off + px_sp, strideN, base_sp, w_sp, c_sp, sl);
                 compat_clear_phantoms<MP>(sl, M);
                 compat_apply<MP, false>(mu + MP * MP, sl, t);
 #pragma unroll
                 for (int k = 0; k < MP; k++) sl[k] = 0.0f;
-                rm_bi = tile_slice_mixed<MP, 6>(vs_bi, bi.tl_loc + px_bi, reinterpret_cast<const float4 *>(bi.val_in),
-                                                bi.off + px_bi, strideN, base_bi, w_bi, c_bi, sl);
+                rm_bi = tile_slice_mixed<MP, 6, true>(vs_bi, loc_bi, reinterpret_cast<const float4 *>(bi.val_in),
+                                                      bi.off + px_bi, strideN, base_bi, w_bi, c_bi, sl);
                 compat_clear_phantoms<MP>(sl, M);
                 compat_apply<MP, false>(mu, sl, t);
             } else if ((MODE & 3) != MODE_FIRST) {
-                rm_sp = tile_slice_mixed<MP, 3>(vs_sp, sp.tl_loc + px_sp, reinterpret_cast<const float4 *>(sp.val_in),
-                                                sp.off + px_sp, strideN, base_sp, w_sp, c_sp, t);
-                rm_bi = tile_slice_mixed<MP, 6>(vs_bi, bi.tl_loc + px_bi, reinterpret_cast<const float4 *>(bi.val_in),
-                                                bi.off + px_bi, strideN, base_bi, w_bi, c_bi, t);
+                rm_sp = tile_slice_mixed<MP, 3, true>(vs_sp, loc_sp, reinterpret_cast<const float4 *>(sp.val_in),
+                                                      sp.off + px_sp, strideN, base_sp, w_sp, c_sp, t);
+                rm_bi = tile_slice_mixed<MP, 6, true>(vs_bi, loc_bi, reinterpret_cast<const float4 *>(bi.val_in),
+                                                      bi.off + px_bi, strideN, base_bi, w_bi, c_bi, t);
             } else {
-                if (hy_sp) rm_sp = tile_remote_mask<3>(sp.tl_loc + px_sp, strideN);
-                if (hy_bi) rm_bi = tile_remote_mask<6>(bi.tl_loc + px_bi, strideN);
+                if (hy_sp) rm_sp = tile_remote_mask<3, true>(loc_sp, strideN);
+                if (hy_bi) rm_bi = tile_remote_mask<6, true>(loc_bi, strideN);
             }
         }
         tile_update<MP, MODE>(t, M, N, Qout, b, pix, in);
         if ((MODE & 3) != MODE_LAST) {
             // ---- splat: remote incidences straight from the registers, the local vertices through the CSR ----
-            if (rm_sp) tile_splat_remote<MP, 3>(vout_sp, rm_sp, sp.off + px_sp, strideN, base_sp, w_sp, t);
-            if (rm_bi) tile_splat_remote<MP, 6>(vout_bi, rm_bi, bi.off + px_bi, strideN, base_bi, w_bi, t);
-            const float4 *qs = tile_park(smt, t, w_sp, w_bi);
+            if (rm_sp) tile_splat_remote<MP, 3, true>(vout_sp, rm_sp, sp.off + px_sp, strideN, base_sp, w_sp, t);
+            if (rm_bi) tile_splat_remote<MP, 6, true>(vout_bi, rm_bi, bi.off + px_bi, strideN, base_bi, w_bi, t);
+            const float4 *qs = tile_park<MP, kMaxLocHy, false>(smt, t, nullptr, nullptr);
             tile_splat_csr<MP>(vout_sp, vout_bi, n_sp, n_bi, hdr_sp, hdr_bi, base_sp, base_bi, ent_sp, ent_bi, qs,
                                smt.wtab);
         }
@@ -1474,7 +1511,8 @@ k_mf_export_renorm(const float *Q, float *result_out, float *log_out, int M, int
     }
 }
 
-static TileLat make_tile_view(const Lattice &L, const float *val_in, float *val_out) {
+// tile_major: the forward kernels' view, whose wn / tl_loc are the per-tile blocks (TileLat)
+static TileLat make_tile_view(const Lattice &L, const float *val_in, float *val_out, bool tile_major = false) {
     TileLat v;
     v.off = L.off;
     v.rowbase = L.rowbase;
@@ -1483,8 +1521,8 @@ static TileLat make_tile_view(const Lattice &L, const float *val_in, float *val_
     v.tl_hdr = L.tl_hdr;
     v.tl_pack = L.tl_pack;
     v.entcap = L.entcap;
-    v.tl_loc = L.tl_loc;
-    v.wn = L.wn;
+    v.tl_loc = tile_major ? L.tl_li : L.tl_loc;
+    v.wn = tile_major ? L.tl_w : L.wn;
     v.val_in = val_in;
     v.val_out = val_out;
     v.shared = L.shared;
@@ -1567,8 +1605,8 @@ static int run_impl(Engine *e, int B, const float *unary, int layout, bool clamp
     // device-resident weights: the kernels multiply alpha by them (MODE_HIST)
     const float c_sp = (potts || compat) ? alpha_sp : p.w2 * alpha_sp, c_bi = (potts || compat) ? alpha_bi : p.w1 * alpha_bi;
     float *urw = hist ? const_cast<float *>(potts) : Urw;
-    const size_t smem = sizeof(TileSmem<MP>);
-    const size_t smem_hy = sizeof(TileSmem<MP, kMaxLocHy>);
+    const size_t smem = sizeof(TileSmemFwd<MP>);
+    const size_t smem_hy = sizeof(TileSmemFwd<MP, kMaxLocHy>);
     const size_t smem_c = smem + kCompatSmem<MP>, smem_hy_c = smem_hy + kCompatSmem<MP>;
     static bool attr_done[64] = {false};   // function attributes are per device
     const int dv = e->device & 63;
@@ -1627,7 +1665,7 @@ static int run_impl(Engine *e, int B, const float *unary, int layout, bool clamp
 #define DSRG_TILE_LAUNCH_COMPAT(MODEV, QOUT)                                                                          \
     DSRG_TILE_LAUNCH_AT(MODEV | MODE_HIST | MODE_COMPAT, QOUT, const_cast<float *>(compat), smem_c, smem_hy_c)
     for (int it = 0; it <= T; it++) {
-        TileLat vsp = make_tile_view(e->sp, spX, spY), vbi = make_tile_view(e->bi, biX, biY);
+        TileLat vsp = make_tile_view(e->sp, spX, spY, true), vbi = make_tile_view(e->bi, biX, biY, true);
         if (compat && !hist) {
             // the matrices passed as the matrices, never as the clamp's U_rw; the first iteration is the Potts one
             if (it == T) {

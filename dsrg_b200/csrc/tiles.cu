@@ -11,6 +11,8 @@
 // one 16-byte-aligned block for a bulk copy.  Local vertices are numbered
 // by decreasing segment length.  Tiles with too many distinct rows keep their most-shared ones (hybrid tiles).
 // The symmetric normalisation is folded into the weights: wn = bary * norm (pairwise.cpp:66,79).
+// wn and tl_loc are written twice: planar per pixel (tl_loc, wn: the backward, the gradient passes) and per tile in
+// [r][thread] blocks (tl_li, tl_w), which the forward tile kernels bulk-copy into their shared tables as they are.
 #include "common.cuh"
 
 namespace dsrg {
@@ -18,8 +20,8 @@ namespace dsrg {
 template <int DP1, int MAXA, int MAXLOC>
 __global__ void __launch_bounds__(kTileThreads)
 k_tile_build(const int32_t *off, const float *bary, const float *norm, int32_t *tl_nloc, uint8_t *tl_hy, int2 *tl_hdr,
-             uint16_t *tl_pack, uint16_t *tl_loc, float *wn, int N, int W, int H, int tiles_x, int ntiles,
-             int entcap, int tile_w, int2 *hy_list, int *hy_count) {
+             uint16_t *tl_pack, uint16_t *tl_loc, float *wn, float *tl_w, uint16_t *tl_li, int N, int W, int H,
+             int tiles_x, int ntiles, int entcap, int tile_w, int2 *hy_list, int *hy_count) {
     constexpr int HS = kTileThreads * 8;  // >= kTileThreads*DP1 distinct rows in the worst case, power of two
     constexpr int HBITS = (HS == 1024) ? 10 : (HS == 2048) ? 11 : (HS == 4096) ? 12 : -1;
     static_assert(HBITS > 0, "hash size");
@@ -76,6 +78,10 @@ k_tile_build(const int32_t *off, const float *bary, const float *norm, int32_t *
             slot[r] = (int)s;
         }
     }
+    // this tile's blocks: slot tid of row r
+    const size_t blk = ((size_t)b * ntiles + tile) * DP1 * kTileThreads + tid;
+#pragma unroll
+    for (int r = 0; r < DP1; r++) tl_w[blk + r * kTileThreads] = in ? w[r] : 0.0f;
     __syncthreads();
     tl_nloc += (size_t)b * ntiles;
     tl_hy += (size_t)b * ntiles;
@@ -156,6 +162,8 @@ k_tile_build(const int32_t *off, const float *bary, const float *norm, int32_t *
 #pragma unroll
                 for (int r = 0; r < DP1; r++) tl_loc[((size_t)b * DP1 + r) * N + pix] = (uint16_t)kLocRemote;
             }
+#pragma unroll
+            for (int r = 0; r < DP1; r++) tl_li[blk + r * kTileThreads] = (uint16_t)kLocRemote;
             if (tid == 0) {
                 tl_nloc[tile] = -1;
                 tl_hy[tile] = 0;
@@ -218,18 +226,23 @@ k_tile_build(const int32_t *off, const float *bary, const float *norm, int32_t *
     }
     __syncthreads();
     uint16_t *pack = tl_pack + ((size_t)b * ntiles + tile) * entcap;
-    if (in) {
+    if (!in) {
+#pragma unroll
+        for (int r = 0; r < DP1; r++) tl_li[blk + r * kTileThreads] = (uint16_t)kLocRemote;
+    } else {
 #pragma unroll
         for (int r = 0; r < DP1; r++) {
             uint16_t *loc = tl_loc + ((size_t)b * DP1 + r) * N + pix;
             if (lv[r] < 0) {
                 *loc = (uint16_t)kLocRemote;
+                tl_li[blk + r * kTileThreads] = (uint16_t)kLocRemote;
                 continue;
             }
             const int nv = perm[lv[r]];
             *loc = (uint16_t)nv;
+            tl_li[blk + r * kTileThreads] = (uint16_t)nv;
             const int pos = ptr[nv] + atomicAdd(&cnt[nv], 1);
-            pack[pos] = (uint16_t)((ent_r0(DP1) + r) << 8 | tid);  // the weight is w[r] = wn, which the consumer holds
+            pack[pos] = (uint16_t)((ent_r0(DP1) + r) << 8 | tid);  // its weight: slot tid of row r of the tile's tl_w block
         }
     }
     if (tid < nloc) {
@@ -267,8 +280,9 @@ int tiles_build(Engine *e, Lattice &L, int nb, cudaStream_t s) {
 #define DSRG_TILE_BUILD(DP1, MAXA, MAXLOC)                                                                   \
     DSRG_LAUNCH(e, T_LAT_MISC, s,                                                                            \
                 (k_tile_build<DP1, MAXA, MAXLOC><<<g, kTileThreads, 0, s>>>(L.off, L.bary, L.norm, L.tl_nloc, L.tl_hy, L.tl_hdr, \
-                                                                  L.tl_pack, L.tl_loc, L.wn, L.N, e->W, e->H,  \
-                                                                  e->tiles_x, e->ntiles, L.entcap, e->tile_w,  \
+                                                                  L.tl_pack, L.tl_loc, L.wn, L.tl_w, L.tl_li,  \
+                                                                  L.N, e->W, e->H, e->tiles_x, e->ntiles,      \
+                                                                  L.entcap, e->tile_w,                         \
                                                                   hy_on ? e->hy_list : nullptr, e->hy_count)))
     if (L.d == 2) DSRG_TILE_BUILD(3, kMaxLocSp, kMaxLocSp);
     else DSRG_TILE_BUILD(6, kMaxLocBi, kMaxLocHy);

@@ -737,6 +737,11 @@ int dsrg_engine_lattice_idle(dsrg_engine *e, int which, long long *counts_out);
  * labels, where the views are not built.  For tests. */
 int dsrg_engine_tile_views(dsrg_engine *e, int which, int b, int *nloc_out, uint8_t *hy_out, int *hdr_out,
                            uint16_t *loc_out, float *wn_out);
+/* The same weights and local vertices per tile, as the forward mean-field kernels copy them into shared memory:
+ * w_out [ntiles][d+1][256] floats and loc_out [ntiles][d+1][256], slot t of a row being the tile's pixel t (column
+ * t % 32, row t / 32 of the tile); a slot outside the image holds weight 0 and 0xFFFF.  Either may be NULL.  Refused
+ * (DSRG_E_STATE) above DSRG_MAX_LABELS labels, where the views are not built.  For tests. */
+int dsrg_engine_tile_blocks(dsrg_engine *e, int which, int b, float *w_out, uint16_t *loc_out);
 
 /* ------------------------------------------------------------------------------------------
  * Per-object API with the exact surface of the reference's C++ class DenseCRFWrapper
