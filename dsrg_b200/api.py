@@ -219,6 +219,26 @@ class Engine(object):
                                                  _dptr(grad_theta_sp), _stream(stream)))
         return grad_unary
 
+    def crf_energy_dev(self, q, unary, image, params, terms, features=None, potts=None, compat=None, stream=None):
+        """The CRF's energy of q (B, M, H, W) (DenseCRF::klDivergence), per term: terms (B, 4) = {entropy, unary,
+        spatial pairwise, bilateral pairwise}, whose sum is the reference's value.  unary (B, M, H, W) or None, image
+        (B, H, W, 3) uint8 or None with features (B, 5, H, W); potts {w1, w2} or compat (2, M, M) {mu_bi, mu_sp}, not
+        both (neither: params.w1 / w2).  At most 32 labels."""
+        B = q.shape[0]
+        check(self._L.dsrg_crf_energy_dev(self.h, _dptr(q), B, _dptr(unary), _dptr(image), _dptr(features),
+                                          C.byref(params), _dptr(potts), _dptr(compat), _dptr(terms), _stream(stream)))
+        return terms
+
+    def crf_energy_backward_dev(self, q, unary, image, params, grad_terms, grad_q, grad_unary=None, features=None,
+                                potts=None, compat=None, stream=None):
+        """The gradient of crf_energy_dev's terms for grad_terms (B, 4): grad_q (B, M, H, W) and, if given, grad_unary
+        (B, M, H, W).  The other arguments as crf_energy_dev's."""
+        B = q.shape[0]
+        check(self._L.dsrg_crf_energy_backward_dev(self.h, _dptr(q), B, _dptr(unary), _dptr(image), _dptr(features),
+                                                   C.byref(params), _dptr(potts), _dptr(compat), _dptr(grad_terms),
+                                                   _dptr(grad_q), _dptr(grad_unary), _stream(stream)))
+        return grad_q
+
     def crf_forward_train_wide_dev(self, unary, image, params, q_hist, potts=None, compat=None, stream=None):
         """crf_forward_train_dev / crf_forward_train_compat_dev above 32 labels (33 to 255): potts {w1, w2} or compat
         (2, M, M) {mu_bi, mu_sp}, not both; neither: params.w1 / w2.  An engine of 32 labels or fewer refuses."""

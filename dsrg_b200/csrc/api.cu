@@ -362,7 +362,7 @@ using namespace dsrg;
 
 extern "C" {
 
-int dsrg_version(void) { return 117; }
+int dsrg_version(void) { return 118; }
 
 const char *dsrg_last_error(void) { return g_err; }
 
@@ -535,7 +535,7 @@ void dsrg_engine_destroy(dsrg_engine *h) {
     void *ptrs[] = {e->U, e->Q0, e->spA, e->spB, e->spC, e->biA, e->biB, e->biC, e->nvA, e->nvB, e->lmap,
                     e->lflag, e->parent, e->hc, e->loss_acc, e->sec_rec, e->sec_img, e->sec_part, e->sec_w, e->dev_err,
                     e->hy_list, e->hy_count, e->potts_part, e->compat_part, e->kg_g, e->kg_csum, e->kg_part, e->kg_sp[0],
-                    e->kg_sp[1], e->kg_bi[0], e->kg_bi[1], e->feat_bad, e->wide_ppart, e->wide_g, e->wide_cpart, e->st_unary, e->st_out, e->st_cues, e->st_labels, e->st_image, e->st_lmap, e->st_raw, e->st_idx,
+                    e->kg_sp[1], e->kg_bi[0], e->kg_bi[1], e->feat_bad, e->wide_ppart, e->wide_g, e->wide_cpart, e->en_part, e->st_unary, e->st_out, e->st_cues, e->st_labels, e->st_image, e->st_lmap, e->st_raw, e->st_idx,
                     e->st_prep, e->st_sel};
     for (void *p : ptrs) cudaFree(p);
     if (e->own_stream) cudaStreamDestroy(e->own_stream);
@@ -602,7 +602,7 @@ static const char *kTagNames[T_COUNT] = {
     "lattice_insert", "lattice_misc", "lattice_norm", "mf_init", "mf_zero", "mf_blur_spatial",
     "mf_blur_bilateral", "mf_tile", "mf_export", "srg_label", "srg_merge", "srg_flag", "srg_emit",
     "seedloss", "wire_bits", "prepare_image", "postprocess", "annotation", "mf_tile_hybrid",
-    "kernel_grad", "feature_grad", "wide_grad"};
+    "kernel_grad", "feature_grad", "wide_grad", "crf_energy"};
 
 int dsrg_profile_tag_count(void) { return T_COUNT; }
 
@@ -1075,6 +1075,83 @@ int dsrg_crf_backward_wide_feat_dev(dsrg_engine *h, const float *q_hist, int B, 
         });
         e->last_crf_B = 0;
         e->feat_B = rc == DSRG_OK ? B : 0;
+        return rc;
+    });
+}
+
+// The energy's per-block sums on its first call (as ensure_compat_part), and with features the per-image flags
+static int ensure_energy(Engine *e, bool feat) {
+    if (feat)
+        if (int rc = ensure_feat(e)) return rc;
+    if (e->en_part) return DSRG_OK;
+    cudaStreamCaptureMode mode = cudaStreamCaptureModeRelaxed;
+    DSRG_CUDA_TRY(cudaThreadExchangeStreamCaptureMode(&mode));
+    const int rc = dalloc(e, &e->en_part, (size_t)e->maxB * ((e->Ncap + kThreads - 1) / kThreads) * 4);
+    DSRG_CUDA_TRY(cudaThreadExchangeStreamCaptureMode(&mode));
+    return rc;
+}
+
+// The body of both energy entry points: the lattices of the image or of the features, the energy (terms) or its
+// gradient (grad_terms given), and the feature passes' NaN policy for the outputs
+static int energy_pass(Engine *e, int B, const float *q, const float *unary, const uint8_t *image, const float *features,
+                       const dsrg_crf_params &p, const float *potts, const float *compat, float *terms,
+                       const float *grad_terms, float *grad_q, float *grad_unary, cudaStream_t s) {
+    int r = features ? prepare_lattices_feat(e, B, features, p, s) : prepare_lattices(e, B, image, p, s);
+    if (!r) r = meanfield_energy(e, B, q, unary, potts, compat, p, terms, grad_terms, grad_q, grad_unary, s);
+    if (r || !features) return r;
+    const long long MN = (long long)e->M * e->N;
+    const std::pair<float *, long long> outs[] = {{terms, 4}, {grad_q, MN}, {grad_unary, MN}};
+    for (const auto &o : outs)
+        if (o.first) nan_images(e, e->feat_bad, o.first, B, o.second, 1, 0, s, T_CRF_ENERGY);
+    DSRG_CUDA_TRY(cudaGetLastError());
+    return DSRG_OK;
+}
+
+static int energy_labels_ok(const Engine *e) {
+    if (e->MP <= DSRG_MAX_LABELS) return DSRG_OK;
+    set_error("the CRF energy supports at most %d labels (got %d)", DSRG_MAX_LABELS, e->M);
+    return DSRG_E_INVALID;
+}
+
+int dsrg_crf_energy_dev(dsrg_engine *h, const float *q, int B, const float *unary, const uint8_t *image,
+                        const float *features, const dsrg_crf_params *params, const float *potts, const float *compat,
+                        float *terms, void *stream) {
+    const cudaStream_t s = (cudaStream_t)stream;
+    const bool ok = q && params && terms && (image != nullptr) != (features != nullptr) && !(potts && compat);
+    return dev_call(h, B, s, ok, [&](Engine *e) {
+        if (int rc = energy_labels_ok(e)) return rc;
+        if (int rc = ensure_energy(e, features != nullptr)) return rc;
+        GraphKey args;
+        args.add(q).add(unary).add(image).add(features).add(potts).add(compat).add(terms);
+        const int rc = crf_pass(e, s, PassKind::crf_energy, B, params, args, [&]() {
+            return energy_pass(e, B, q, unary, image, features, *params, potts, compat, terms, nullptr, nullptr,
+                               nullptr, s);
+        });
+        e->last_crf_B = 0;   // no marginals in the engine: the *_last_* entry points refuse
+        if (features) e->feat_B = rc == DSRG_OK ? B : 0;
+        return rc;
+    });
+}
+
+int dsrg_crf_energy_backward_dev(dsrg_engine *h, const float *q, int B, const float *unary, const uint8_t *image,
+                                 const float *features, const dsrg_crf_params *params, const float *potts,
+                                 const float *compat, const float *grad_terms, float *grad_q, float *grad_unary,
+                                 void *stream) {
+    const cudaStream_t s = (cudaStream_t)stream;
+    const bool ok = q && params && grad_terms && grad_q && (image != nullptr) != (features != nullptr) &&
+                    !(potts && compat);
+    return dev_call(h, B, s, ok, [&](Engine *e) {
+        if (int rc = energy_labels_ok(e)) return rc;
+        if (int rc = ensure_energy(e, features != nullptr)) return rc;
+        GraphKey args;
+        args.add(q).add(unary).add(image).add(features).add(potts).add(compat).add(grad_terms).add(grad_q)
+            .add(grad_unary);
+        const int rc = crf_pass(e, s, PassKind::crf_energy_backward, B, params, args, [&]() {
+            return energy_pass(e, B, q, unary, image, features, *params, potts, compat, nullptr, grad_terms, grad_q,
+                               grad_unary, s);
+        });
+        e->last_crf_B = 0;
+        if (features) e->feat_B = rc == DSRG_OK ? B : 0;
         return rc;
     });
 }

@@ -87,7 +87,7 @@ struct Engine;
 enum KTag {
     T_LAT_INSERT = 0, T_LAT_MISC, T_LAT_NORM, T_MF_INIT, T_MF_ZERO, T_MF_BLUR_SP,
     T_MF_BLUR_BI, T_MF_TILE, T_MF_EXPORT, T_SRG_LABEL, T_SRG_MERGE, T_SRG_FLAG, T_SRG_EMIT,
-    T_LOSS, T_WIRE, T_PREP, T_POST, T_ANNOT, T_MF_TILE_HY, T_KGRAD, T_FGRAD, T_WIDE_GRAD, T_COUNT
+    T_LOSS, T_WIRE, T_PREP, T_POST, T_ANNOT, T_MF_TILE_HY, T_KGRAD, T_FGRAD, T_WIDE_GRAD, T_CRF_ENERGY, T_COUNT
 };
 
 // ---- lattice.cu ----
@@ -176,9 +176,16 @@ int meanfield_backward(Engine *e, int B, const float *q_hist, const float *potts
                        const dsrg_crf_params &p, cudaStream_t s, float *grad_theta = nullptr,
                        const uint8_t *image = nullptr, const float *feat = nullptr, float *grad_feat = nullptr,
                        float *grad_theta_sp = nullptr);
-// NaN into every image b of p (reps slabs rep_stride apart, per_image floats per image) with bad[b] set
+// NaN into every image b of p (reps slabs rep_stride apart, per_image floats per image) with bad[b] set; timed under tag
 void nan_images(Engine *e, const int *bad, float *p, int B, long long per_image, int reps, long long rep_stride,
-                cudaStream_t s);
+                cudaStream_t s, int tag = T_FGRAD);
+// The energy of given marginals q [B][M][N] (DenseCRF::klDivergence) on the lattices the pass just built, at most
+// DSRG_MAX_LABELS labels: terms [B][4] {entropy, unary, spatial, bilateral} or, with grad_terms [B][4], its gradient
+// grad_q [B][M][N] and, if given, grad_unary.  unary may be nullptr; potts {w1, w2} or compat {mu_bi, mu_sp} [2][M][M]
+// (neither: p's w1 / w2).  Needs e->en_part (ensure_energy); uses the mean-field value buffers.
+int meanfield_energy(Engine *e, int B, const float *q, const float *unary, const float *potts, const float *compat,
+                     const dsrg_crf_params &p, float *terms, const float *grad_terms, float *grad_q, float *grad_unary,
+                     cudaStream_t s);
 // the backward's per-image parameter sums, in a fixed order: part [B][nparts] {spatial, bilateral} -> out [B][2]
 // {dL/dw1, dL/dw2}; part [B][nparts][mm2] -> out [B][mm2] = -sum over the parts
 void potts_reduce(Engine *e, const float2 *part, float *out, int nparts, int B, int tag, cudaStream_t s);
@@ -262,6 +269,8 @@ struct Engine {
     float2 *wide_ppart = nullptr;
     float *wide_g = nullptr, *wide_cpart = nullptr;
     int *hy_count = nullptr;   // their number (device-resident)
+    // the energy's per-block sums [maxB][blocks][4], allocated by its first call (ensure_energy)
+    double *en_part = nullptr;
     // 1-channel buffers for the normalisation pass
     float *nvA = nullptr, *nvB = nullptr;
     // SRG state
@@ -472,7 +481,8 @@ cudaError_t numa_host_alloc(void **p, size_t bytes, int device);
 enum class PassKind : int { crf, crf_map, forward, crflayer, densecrf, post, crf_train, crf_backward, crf_train_compat,
                             crf_backward_compat, crf_backward_theta, crf_backward_compat_theta, crf_train_feat,
                             crf_backward_feat, crf_train_wide, crf_backward_wide, crf_backward_wide_theta,
-                            crf_train_wide_feat, crf_backward_wide_feat, crf_learned, post_learned };
+                            crf_train_wide_feat, crf_backward_wide_feat, crf_learned, post_learned, crf_energy,
+                            crf_energy_backward };
 struct GraphKey {
     std::string bytes;
     GraphKey() = default;

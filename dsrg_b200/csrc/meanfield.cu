@@ -1962,10 +1962,10 @@ int meanfield_backward(Engine *e, int B, const float *q_hist, const float *potts
 }
 
 void nan_images(Engine *e, const int *bad, float *p, int B, long long per_image, int reps, long long rep_stride,
-                cudaStream_t s) {
+                cudaStream_t s, int tag) {
     const int nblk = cdiv(per_image, kThreads);
     const dim3 gp(nblk < 64 ? nblk : 64, B, reps);
-    DSRG_LAUNCH(e, T_FGRAD, s, k_nan_images<<<gp, kThreads, 0, s>>>(bad, p, per_image, rep_stride));
+    DSRG_LAUNCH(e, tag, s, k_nan_images<<<gp, kThreads, 0, s>>>(bad, p, per_image, rep_stride));
 }
 
 void potts_reduce(Engine *e, const float2 *part, float *out, int nparts, int B, int tag, cudaStream_t s) {
@@ -2010,6 +2010,260 @@ int meanfield_export_renorm(Engine *e, int B, float *result_out, float *log_out,
     DSRG_LAUNCH(e, T_MF_EXPORT, s, k_mf_export_renorm<<<gp, kThreads, 0, s>>>(e->Q0, result_out, log_out, e->M, e->N));
     DSRG_CUDA_TRY(cudaGetLastError());
     return DSRG_OK;
+}
+
+// ---------------------------------------------------------------------------------------------
+// The energy of given marginals (DenseCRF::klDivergence, densecrf.cpp:213-235) and its gradient to them.  Per lattice
+// F(Q) = n K(n Q), the message the mean field subtracts (t = unary - mu_sp F_sp(Q) - mu_bi F_bi(Q), Potts mu = -w I):
+//   terms[b] = {sum Q log max(Q, 1e-20), -sum unary Q, sum Q . mu_sp F_sp(Q), sum Q . mu_bi F_bi(Q)}
+// k_kg_splatq splats wn Q (wn = bary n) into each lattice and blur_all blurs it in K's order; the gradient blurs a
+// copy of the splat in K^T's order too, since the device's K is not symmetric (DESIGN.md section 1):
+//   grad_q = g0 (Q > 1e-20 ? log Q + 1 : log 1e-20) - g1 unary + sum_k g_k (mu_k F_k(Q) + mu_k^T F_k^T(Q))
+// k_crf_energy slices both per pixel as the tile kernels do (weights alpha wn, an fma chain from zero).  The forward's
+// per-pixel terms go to per-block double sums part [B][nblk][4], which k_crf_energy_reduce adds in block order: no
+// float atomics in the sums, only in the splats.
+// ---------------------------------------------------------------------------------------------
+struct EnergyArgs {
+    KgLat sp, bi;
+    const float *q, *unary;     // [B][M][N]; unary may be nullptr (no unary term)
+    const float *potts;         // {w1, w2} on the device, or nullptr: w1, w2
+    const float *compat;        // {mu_bi, mu_sp} [2][M][M], or nullptr: Potts
+    float w1, w2;
+    const float *grad_terms;    // [B][4] (the backward)
+    float *grad_q, *grad_unary; // [B][M][N]; grad_unary may be nullptr
+    double *part;               // [B][nblk][4] (the forward)
+    int M, N, nblk;
+};
+
+// F(Q) of one lattice at pixel i from its blurred values v: alpha sum_r wn_r v[row_r]
+template <int MP, int D>
+__device__ __forceinline__ void energy_slice(const KgLat &L, int b, int i, int N, const float4 *v, float *f) {
+    constexpr int CH = MP / 4;
+    const size_t at = (size_t)(L.shared ? 0 : b) * (D + 1) * N + i;
+    const int base = L.rowbase[b];
+#pragma unroll
+    for (int k = 0; k < MP; k++) f[k] = 0.0f;
+#pragma unroll
+    for (int r = 0; r <= D; r++) {
+        const float w = L.alpha * __ldg(L.wn + at + (size_t)r * N);
+        const size_t row = (size_t)(base + __ldg(L.off + at + (size_t)r * N)) * CH;
+#pragma unroll
+        for (int c = 0; c < CH; c++) {
+            const float4 a = v[row + c];
+            f[4 * c] = fmaf(w, a.x, f[4 * c]);
+            f[4 * c + 1] = fmaf(w, a.y, f[4 * c + 1]);
+            f[4 * c + 2] = fmaf(w, a.z, f[4 * c + 2]);
+            f[4 * c + 3] = fmaf(w, a.w, f[4 * c + 3]);
+        }
+    }
+}
+
+// message l of lattice kk (0 spatial, 1 bilateral): (mu f)_l, Potts -w f_l
+template <int MP, bool COMPAT>
+__device__ __forceinline__ float energy_msg(const float *mus, int kk, float w, const float *f, int l) {
+    if constexpr (COMPAT) {
+        const float *mu = mus + (kk == 0 ? MP * MP : 0);   // mus: {mu_bi, mu_sp}
+        float m = 0.0f;
+#pragma unroll
+        for (int l2 = 0; l2 < MP; l2++) m = fmaf(mu[l * MP + l2], f[l2], m);
+        return m;
+    } else {
+        return -w * f[l];
+    }
+}
+
+// one pixel per thread: vf_* = K S(wn Q), with BWD vt_* = K^T S(wn Q) too
+template <int MP, bool COMPAT, bool BWD>
+__global__ void __launch_bounds__(kThreads)
+k_crf_energy(EnergyArgs a, const float4 *vf_sp, const float4 *vf_bi, const float4 *vt_sp, const float4 *vt_bi) {
+    __shared__ float mus[COMPAT ? 2 * MP * MP : 1];
+    __shared__ double red[kThreads / 32][4];
+    const int b = blockIdx.y, i = blockIdx.x * kThreads + threadIdx.x;
+    if constexpr (COMPAT) {
+        for (int e = threadIdx.x; e < 2 * MP * MP; e += kThreads) {
+            const int k = e / (MP * MP), l = e / MP % MP, l2 = e % MP;
+            mus[e] = (l < a.M && l2 < a.M) ? __ldg(a.compat + ((size_t)k * a.M + l) * a.M + l2) : 0.0f;
+        }
+        __syncthreads();
+    }
+    float acc[4] = {0.0f, 0.0f, 0.0f, 0.0f};
+    if (i < a.N) {
+        const float w1 = a.potts ? __ldg(a.potts) : a.w1, w2 = a.potts ? __ldg(a.potts + 1) : a.w2;
+        float g0 = 0.0f, g1 = 0.0f, g2 = 0.0f, g3 = 0.0f;
+        if constexpr (BWD) {
+            g0 = __ldg(a.grad_terms + 4 * b);
+            g1 = __ldg(a.grad_terms + 4 * b + 1);
+            g2 = __ldg(a.grad_terms + 4 * b + 2);
+            g3 = __ldg(a.grad_terms + 4 * b + 3);
+        }
+        float q[MP], f[MP], g[MP];
+#pragma unroll
+        for (int k = 0; k < MP; k++) {
+            q[k] = 0.0f;
+            g[k] = 0.0f;
+            if (k < a.M) {
+                const size_t at = ((size_t)b * a.M + k) * a.N + i;
+                q[k] = __ldg(a.q + at);
+                const float u = a.unary ? __ldg(a.unary + at) : 0.0f;
+                const float lq = logf(fmaxf(q[k], 1e-20f));
+                acc[0] = fmaf(q[k], lq, acc[0]);
+                acc[1] = fmaf(-u, q[k], acc[1]);
+                if constexpr (BWD) {
+                    g[k] = fmaf(-g1, u, g0 * (q[k] > 1e-20f ? lq + 1.0f : lq));
+                    if (a.grad_unary) a.grad_unary[at] = -g1 * q[k];
+                }
+            }
+        }
+        // one lattice at a time (not unrolled: two copies of the M x M products would not fit the registers)
+#pragma unroll 1
+        for (int kk = 0; kk < 2; kk++) {
+            const float w = kk == 0 ? w2 : w1, gk = kk == 0 ? g2 : g3;
+            if (kk == 0)
+                energy_slice<MP, 2>(a.sp, b, i, a.N, vf_sp, f);
+            else
+                energy_slice<MP, 5>(a.bi, b, i, a.N, vf_bi, f);
+            float ek = 0.0f;
+#pragma unroll
+            for (int l = 0; l < MP; l++) {
+                const float m = energy_msg<MP, COMPAT>(mus, kk, w, f, l);
+                ek = fmaf(q[l], m, ek);
+                if constexpr (BWD) g[l] = fmaf(gk, m, g[l]);
+            }
+            if (kk == 0)
+                acc[2] = ek;
+            else
+                acc[3] = ek;
+            if constexpr (BWD) {
+                if (kk == 0)
+                    energy_slice<MP, 2>(a.sp, b, i, a.N, vt_sp, f);
+                else
+                    energy_slice<MP, 5>(a.bi, b, i, a.N, vt_bi, f);
+                if constexpr (COMPAT) {
+                    // g += g_k mu^T f, as mu's rows l2 scaled by g_k f[l2]
+                    const float *mu = mus + (kk == 0 ? MP * MP : 0);
+#pragma unroll
+                    for (int l2 = 0; l2 < MP; l2++) {
+                        const float c = gk * f[l2];
+#pragma unroll
+                        for (int l = 0; l < MP; l++) g[l] = fmaf(mu[l2 * MP + l], c, g[l]);
+                    }
+                } else {
+#pragma unroll
+                    for (int l = 0; l < MP; l++) g[l] = fmaf(gk, -w * f[l], g[l]);
+                }
+            }
+        }
+        if constexpr (BWD) {
+#pragma unroll
+            for (int k = 0; k < MP; k++)
+                if (k < a.M) a.grad_q[((size_t)b * a.M + k) * a.N + i] = g[k];
+        }
+    }
+    if constexpr (!BWD) {
+        double v[4];
+#pragma unroll
+        for (int k = 0; k < 4; k++) {
+            v[k] = acc[k];
+#pragma unroll
+            for (int o = 16; o > 0; o >>= 1) v[k] += __shfl_down_sync(0xffffffffu, v[k], o);
+        }
+        if ((threadIdx.x & 31) == 0) {
+#pragma unroll
+            for (int k = 0; k < 4; k++) red[threadIdx.x >> 5][k] = v[k];
+        }
+        __syncthreads();
+        if (threadIdx.x < 4) {
+            double s = 0.0;
+            for (int w = 0; w < kThreads / 32; w++) s += red[w][threadIdx.x];
+            a.part[((size_t)b * a.nblk + blockIdx.x) * 4 + threadIdx.x] = s;
+        }
+    }
+}
+
+// copy the B images' rows of both lattices' splat targets (row counts device-resident, as k_mf_zero)
+template <int MP>
+__global__ void __launch_bounds__(kThreads)
+k_crf_energy_copy(const float4 *a, float4 *a2, const int32_t *rowbase_a, const float4 *c, float4 *c2,
+                  const int32_t *rowbase_c, int B) {
+    constexpr int CH = MP / 4;
+    const long long na = (long long)rowbase_a[B] * CH, nc = (long long)rowbase_c[B] * CH;
+    for (long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x; t < na + nc;
+         t += (long long)gridDim.x * blockDim.x) {
+        if (t < na) a2[t] = a[t]; else c2[t - na] = c[t - na];
+    }
+}
+
+// per image: the blocks' sums in block order -> terms[b][4]
+__global__ void k_crf_energy_reduce(const double *part, int nblk, float *terms) {
+    const int b = blockIdx.x, k = threadIdx.x;
+    if (k >= 4) return;
+    double s = 0.0;
+    for (int i = 0; i < nblk; i++) s += part[((size_t)b * nblk + i) * 4 + k];
+    terms[(size_t)b * 4 + k] = (float)s;
+}
+
+template <int MP>
+static int energy_impl(Engine *e, int B, const float *q, const float *unary, const float *potts, const float *compat,
+                       const dsrg_crf_params &p, float *terms, const float *grad_terms, float *grad_q,
+                       float *grad_unary, cudaStream_t s) {
+    const bool bwd = grad_terms != nullptr;
+    KgArgs ka{};
+    ka.sp = kg_lat(e->sp);
+    ka.bi = kg_lat(e->bi);
+    ka.M = e->M;
+    ka.N = e->N;
+    ka.W = e->W;
+    ka.nblk = cdiv(e->N, kThreads);
+    EnergyArgs ea{ka.sp, ka.bi, q, unary, potts, compat, p.w1, p.w2, grad_terms, grad_q, grad_unary, e->en_part,
+                  e->M, e->N, ka.nblk};
+    const int bgrid = DSRG_BLUR_GRID * e->sm_count;
+    const dim3 gp(ka.nblk, B);
+    // S(wn Q) into A; the gradient copies it to C (the splat's float atomics are its costliest launch).  K S(wn Q)
+    // from A with B as scratch; K^T S(wn Q) from C with whichever of A / B the first result left free
+    DSRG_LAUNCH(e, T_CRF_ENERGY, s,
+                k_mf_zero<MP><<<bgrid, kThreads, 0, s>>>((float4 *)e->spA, e->sp.rowbase, (float4 *)e->biA,
+                                                         e->bi.rowbase, B));
+    DSRG_LAUNCH(e, T_CRF_ENERGY, s, k_kg_splatq<MP><<<gp, kThreads, 0, s>>>(ka, q, (float4 *)e->spA, (float4 *)e->biA));
+    if (bwd)
+        DSRG_LAUNCH(e, T_CRF_ENERGY, s,
+                    k_crf_energy_copy<MP><<<bgrid, kThreads, 0, s>>>((const float4 *)e->spA, (float4 *)e->spC,
+                                                                     e->sp.rowbase, (const float4 *)e->biA,
+                                                                     (float4 *)e->biC, e->bi.rowbase, B));
+    const float *vf_sp = blur_all<MP>(e, e->sp, e->spA, e->spB, nullptr, B, T_CRF_ENERGY, bgrid, s);
+    const float *vf_bi = blur_all<MP>(e, e->bi, e->biA, e->biB, nullptr, B, T_CRF_ENERGY, bgrid, s);
+    const float *vt_sp = nullptr, *vt_bi = nullptr;
+    if (bwd) {
+        vt_sp = blur_all<MP>(e, e->sp, e->spC, vf_sp == e->spA ? e->spB : e->spA, nullptr, B, T_CRF_ENERGY, bgrid, s,
+                             true);
+        vt_bi = blur_all<MP>(e, e->bi, e->biC, vf_bi == e->biA ? e->biB : e->biA, nullptr, B, T_CRF_ENERGY, bgrid, s,
+                             true);
+    }
+    const float4 *a0 = (const float4 *)vf_sp, *a1 = (const float4 *)vf_bi;
+    const float4 *a2 = (const float4 *)vt_sp, *a3 = (const float4 *)vt_bi;
+    if (bwd && compat)
+        DSRG_LAUNCH(e, T_CRF_ENERGY, s, (k_crf_energy<MP, true, true><<<gp, kThreads, 0, s>>>(ea, a0, a1, a2, a3)));
+    else if (bwd)
+        DSRG_LAUNCH(e, T_CRF_ENERGY, s, (k_crf_energy<MP, false, true><<<gp, kThreads, 0, s>>>(ea, a0, a1, a2, a3)));
+    else if (compat)
+        DSRG_LAUNCH(e, T_CRF_ENERGY, s, (k_crf_energy<MP, true, false><<<gp, kThreads, 0, s>>>(ea, a0, a1, a2, a3)));
+    else
+        DSRG_LAUNCH(e, T_CRF_ENERGY, s, (k_crf_energy<MP, false, false><<<gp, kThreads, 0, s>>>(ea, a0, a1, a2, a3)));
+    if (!bwd) DSRG_LAUNCH(e, T_CRF_ENERGY, s, k_crf_energy_reduce<<<B, 32, 0, s>>>(e->en_part, ka.nblk, terms));
+    DSRG_CUDA_TRY(cudaGetLastError());
+    return DSRG_OK;
+}
+
+int meanfield_energy(Engine *e, int B, const float *q, const float *unary, const float *potts, const float *compat,
+                     const dsrg_crf_params &p, float *terms, const float *grad_terms, float *grad_q, float *grad_unary,
+                     cudaStream_t s) {
+    switch (e->MP) {
+#define DSRG_CASE(MPV) \
+    case MPV: return energy_impl<MPV>(e, B, q, unary, potts, compat, p, terms, grad_terms, grad_q, grad_unary, s);
+        DSRG_CASE(4) DSRG_CASE(8) DSRG_CASE(12) DSRG_CASE(16) DSRG_CASE(20) DSRG_CASE(24) DSRG_CASE(28) DSRG_CASE(32)
+#undef DSRG_CASE
+    }
+    set_error("unsupported label count %d", e->M);
+    return DSRG_E_INVALID;
 }
 
 }  // namespace dsrg

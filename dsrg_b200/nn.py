@@ -843,6 +843,73 @@ def dense_crf_inference(unary, image, scale_factor=1.0, color_factor=13, maxiter
                                compat=compat, unary_layout=api.LAYOUT_NCHW, out_layout=api.LAYOUT_NCHW, stream=s)
 
 
+class _DenseCrfEnergy(torch.autograd.Function):
+    """dense_crf_energy's terms (N, 4) and their gradient to q and unary; the parameters carry none."""
+
+    @staticmethod
+    @_fwd
+    def forward(ctx, q, unary, image, features, compat, params):
+        terms = torch.empty((q.shape[0], 4), dtype=torch.float32, device=q.device)
+        _engine_for(q).crf_energy_dev(q, unary, image, params, terms, features=features, compat=compat,
+                                      stream=_stream(q))
+        ctx.save_for_backward(q, unary, image, features, compat)
+        ctx.params = params
+        return terms
+
+    @staticmethod
+    @_bwd
+    def backward(ctx, g):
+        q, unary, image, features, compat = ctx.saved_tensors
+        grad_q = torch.empty_like(q)
+        grad_u = torch.empty_like(q) if unary is not None and ctx.needs_input_grad[1] else None
+        _engine_for(q).crf_energy_backward_dev(q, unary, image, ctx.params, g.float().contiguous(), grad_q,
+                                               grad_unary=grad_u, features=features, compat=compat,
+                                               stream=_stream(q))
+        return grad_q if ctx.needs_input_grad[0] else None, grad_u, None, None, None, None
+
+
+def dense_crf_energy(q, unary, image, scale_factor=1.0, color_factor=13, w1=None, w2=None, compat_bi=None,
+                     compat_sp=None, theta_bi=None, theta_sp=None, features_bi=None):
+    """The dense CRF's energy of q (N, M, H, W), M <= 32, per term: (N, 4) = (entropy sum Q log max(Q, 1e-20), unary
+    -sum unary Q, spatial sum Q mu_sp F_sp(Q), bilateral sum Q mu_bi F_bi(Q)), so ``.sum(1)`` is the reference's
+    DenseCRF::klDivergence of each image.  q is any non-negative array: marginals, a softmax, or a one-hot label map
+    (whose result is that labelling's energy under the reference's convention).  Like the reference, the pairwise
+    terms carry no 1/2: every pair of pixels counts twice.  unary (N, M, H, W) holds the values CRF(image, unary)
+    takes (energy = -unary), or None for no unary term.
+
+    The parameters are dense_crf_inference's, with its checks and semantics (w1 / w2 and theta_bi / theta_sp read on
+    the host; compat_bi / compat_sp and features_bi on the device, features_bi in place of image).  The result is
+    differentiable to q and unary: the pairwise gradient is mu F(Q) + mu^T F^T(Q) with the device's transposed blur,
+    exact for the function the device computes.  A term's pairwise energy alone (``terms[:, 2:].sum()``) is the
+    dense-CRF regulariser of weakly-supervised segmentation.  The parameters get no gradient: a parameter tensor that
+    requires grad is refused.  A features_bi image whose lattice keys leave the packed range gets NaN terms and
+    gradients."""
+    if torch.is_autocast_enabled("cuda"):
+        q = q.float() if isinstance(q, torch.Tensor) and q.is_floating_point() else q
+        unary = unary.float() if isinstance(unary, torch.Tensor) and unary.is_floating_point() else unary
+        if isinstance(features_bi, torch.Tensor) and features_bi.is_floating_point():
+            features_bi = features_bi.float()
+    for name, t in (("w1", w1), ("w2", w2), ("compat_bi", compat_bi), ("compat_sp", compat_sp),
+                    ("theta_bi", theta_bi), ("theta_sp", theta_sp), ("features_bi", features_bi)):
+        if isinstance(t, torch.Tensor) and t.requires_grad:
+            raise ValueError("%s requires grad: dense_crf_energy differentiates q and unary only (detach it)" % name)
+    qq = _maps(q, "q")
+    N, M, H, W = qq.shape
+    if M > FUSED_LABELS:
+        raise ValueError("dense_crf_energy supports at most %d labels (got %d)" % (FUSED_LABELS, M))
+    u = None if unary is None else _like(unary, qq, "unary")
+    if features_bi is not None:
+        if image is not None:
+            raise ValueError("image is not used when features_bi is given: pass None")
+    elif (not isinstance(image, torch.Tensor) or image.dtype != torch.uint8 or tuple(image.shape) != (N, H, W, 3)
+          or image.device != qq.device):
+        raise ValueError("image must be a (%d, %d, %d, 3) uint8 tensor on %s" % (N, H, W, qq.device))
+    _cuda(qq, "q")
+    params = api.crf_params(float(scale_factor), float(color_factor), 0)
+    f, compat = _learned_crf(qq, N, M, H, W, params, w1, w2, compat_bi, compat_sp, theta_bi, theta_sp, features_bi)
+    return _DenseCrfEnergy.apply(qq, u, None if f is not None else image.contiguous(), f, compat, params)
+
+
 def softmax(fc8):
     """SoftmaxLayer (pylayers.py:23-51): probs = (softmax(fc8) + 1e-4) / sum over labels.  fc8 (N, M, H, W),
     M <= 32 (more labels raise the library's DsrgError)."""

@@ -229,6 +229,36 @@ int dsrg_crf_backward_feat_dev(dsrg_engine *e, const float *q_hist_dev, int B, c
                                float *grad_potts_dev, float *grad_compat_dev, float *grad_theta_sp_dev, void *stream);
 int dsrg_engine_feature_range_flags(dsrg_engine *e, int B, int32_t *flags_out);
 /*
+ * The CRF's energy of any marginals (the reference's DenseCRF::klDivergence, densecrf.cpp:213-235), per term, and its
+ * exact gradient.  q [B][M][H][W] is any non-negative array (marginals, a softmax, a one-hot label map); it need not be
+ * normalised.  With F_k(Q) = n_k K_k(n_k Q) the message the mean field subtracts (t = unary - mu_sp F_sp - mu_bi F_bi):
+ *   terms[b][0] = sum Q log max(Q, 1e-20)        terms[b][2] = sum Q . mu_sp F_sp(Q)
+ *   terms[b][1] = -sum unary . Q  (0 if NULL)    terms[b][3] = sum Q . mu_bi F_bi(Q)
+ * and terms[b][0..3] sum to the reference's klDivergence of image b, whose pairwise terms have no 1/2 (a pair of
+ * pixels counts twice).  unary holds the values passed to CRF(image, unary) (energy = -unary).  The arguments follow
+ * the training entry points: exactly one of image_dev / features_dev (features as dsrg_crf_forward_train_feat_dev),
+ * at most one of potts_dev ({w1, w2}) / compat_dev ({mu_bi, mu_sp} [2][M][M]; Potts is mu = -w I), with neither
+ * params->w1 / w2; the sigmas come from params.  The backward takes grad_terms [B][4] and writes
+ *   grad_q     = g0 (Q > 1e-20 ? log Q + 1 : log 1e-20) - g1 unary + sum_k g_k (mu_k F_k(Q) + mu_k^T F_k^T(Q))
+ *   grad_unary = -g1 Q  (optional)
+ * where F^T is the transposed blur: the device's K is not symmetric, and the gradient is that of the function the
+ * device computes.  At most DSRG_MAX_LABELS labels: a larger engine returns DSRG_E_INVALID before anything is queued.
+ * Nothing is read on the host, so both calls can be captured; addresses are part of a cached graph's key, values not.
+ * A feature image whose lattice keys leave the packed range gets NaN terms and gradients (the feature passes' policy,
+ * dsrg_engine_feature_range_flags).  Neither call leaves marginals for the *_last_* entry points.  The sums are per
+ * 256-pixel block in double, added in a fixed order; the splats add with float atomics, so two calls agree to the
+ * rounding of those additions' order.  The first call allocates the per-block sums, maxB * ceil(H*W/256) * 32 bytes:
+ * 825 KB for an engine of batch 64 @ 321x321, 4.5 KB at batch 20 @ 41x41 (dsrg_engine_device_bytes before and
+ * after), and with features the feature passes' flags.  The mean field's own value buffers hold the blurred values.
+ */
+int dsrg_crf_energy_dev(dsrg_engine *e, const float *q_dev, int B, const float *unary_dev, const uint8_t *image_dev,
+                        const float *features_dev, const dsrg_crf_params *params, const float *potts_dev,
+                        const float *compat_dev, float *terms_dev, void *stream);
+int dsrg_crf_energy_backward_dev(dsrg_engine *e, const float *q_dev, int B, const float *unary_dev,
+                                 const uint8_t *image_dev, const float *features_dev, const dsrg_crf_params *params,
+                                 const float *potts_dev, const float *compat_dev, const float *grad_terms_dev,
+                                 float *grad_q_dev, float *grad_unary_dev, void *stream);
+/*
  * The training forward and its backward above DSRG_MAX_LABELS labels (DSRG_MAX_LABELS < M <= DSRG_MAX_LABELS_WIDE,
  * e.g. COCO's 81), on the label-chunked kernels of dsrg_crf_batch_dev at those counts.  The arguments mean what they
  * mean in dsrg_crf_forward_train_dev / dsrg_crf_backward_dev and their _compat twins: potts_dev ({w1, w2}) or
