@@ -5,6 +5,7 @@
 #include <stdlib.h>
 #include <string.h>
 
+#include <initializer_list>
 #include <map>
 #include <mutex>
 #include <utility>
@@ -210,14 +211,73 @@ static int prepare_lattices(Engine *e, int B, const uint8_t *image, const dsrg_c
     return lattice_build(e, e->bi, B, image, s);
 }
 
-// The feature passes' per-image key-range flags on their first call (as ensure_compat_part)
-int ensure_feat(Engine *e) {
-    if (e->feat_bad) return DSRG_OK;
+// A buffer that the entry points needing it allocate on their first call, so that an engine which never runs them
+// keeps its footprint.  Sized for the engine's capacity (set_size never exceeds it).
+struct LazyBuf {
+    void **p;
+    size_t bytes;
+};
+template <typename T>
+static LazyBuf lazy(T *&p, size_t count) {
+    return {(void **)&p, count * sizeof(T)};
+}
+
+// Allocates each buffer of `bufs` that is still NULL, so a call after a failed one allocates only what is missing.  The
+// call may sit inside a caller's stream capture, where an allocation is allowed in relaxed mode only.
+static int lazy_alloc(Engine *e, std::initializer_list<LazyBuf> bufs) {
+    bool missing = false;
+    for (const LazyBuf &b : bufs) missing |= *b.p == nullptr;
+    if (!missing) return DSRG_OK;
     cudaStreamCaptureMode mode = cudaStreamCaptureModeRelaxed;
     DSRG_CUDA_TRY(cudaThreadExchangeStreamCaptureMode(&mode));
-    const int rc = dalloc(e, &e->feat_bad, (size_t)e->maxB);
+    int rc = DSRG_OK;
+    for (const LazyBuf &b : bufs)
+        if (!*b.p && device_alloc(e, b.p, b.bytes)) rc = DSRG_E_NOMEM;
     DSRG_CUDA_TRY(cudaThreadExchangeStreamCaptureMode(&mode));
     return rc;
+}
+
+// the feature passes' per-image key-range flags
+int ensure_feat(Engine *e) { return lazy_alloc(e, {lazy(e->feat_bad, e->maxB)}); }
+
+// the compatibility backward's per-tile partials, B * ntiles * 2 * M^2 floats
+static int ensure_compat_part(Engine *e) {
+    const size_t tiles = (size_t)((e->Wcap + kTileW - 1) / kTileW) * ((e->Hcap + kTileH - 1) / kTileH);
+    return lazy_alloc(e, {lazy(e->compat_part, (size_t)e->maxB * tiles * 2 * e->M * e->M)});
+}
+
+// the kernel-bandwidth backward's buffers: g_t and c per pixel, the per-block sums and two value buffers per lattice
+static int ensure_kgrad(Engine *e) {
+    const size_t sp = (size_t)e->sp.rows_cap * e->MP, bi = (size_t)e->bi.rows_cap * e->MP;
+    return lazy_alloc(e, {lazy(e->kg_g, (size_t)e->maxB * e->M * e->Ncap),
+                          lazy(e->kg_csum, (size_t)2 * e->maxB * e->Ncap),
+                          lazy(e->kg_part, (size_t)e->maxB * ((e->Ncap + kThreads - 1) / kThreads) * 8),
+                          lazy(e->kg_sp[0], sp), lazy(e->kg_bi[0], bi), lazy(e->kg_sp[1], sp), lazy(e->kg_bi[1], bi)});
+}
+
+// the label-chunked backward's buffers: the Potts partials, and for the matrices G and the outer-product partials
+static int ensure_wide(Engine *e, bool compat) {
+    const LazyBuf ppart = lazy(e->wide_ppart, (size_t)e->maxB * (e->MP / 4) * ((e->Ncap + kThreads - 1) / kThreads));
+    if (!compat) return lazy_alloc(e, {ppart});
+    return lazy_alloc(e, {ppart, lazy(e->wide_g, (size_t)e->maxB * e->M * e->Ncap),
+                          lazy(e->wide_cpart, (size_t)e->maxB * kWideChunks * 2 * e->M * e->M)});
+}
+
+// The label-chunked kernel-bandwidth and feature backward's buffers: c per pixel [2][maxB][N] and the per-block sums,
+// as ensure_kgrad, and the normalisation term's two value buffers per lattice at 4 floats per row.  g_t stays in e->Q0
+// and Vy in the mean-field buffers, so nothing here grows with the label count.
+static int ensure_kgrad_wide(Engine *e) {
+    const size_t sp = (size_t)e->sp.rows_cap * 4, bi = (size_t)e->bi.rows_cap * 4;
+    return lazy_alloc(e, {lazy(e->kg_csum, (size_t)2 * e->maxB * e->Ncap),
+                          lazy(e->kg_part, (size_t)e->maxB * ((e->Ncap + kThreads - 1) / kThreads) * 8),
+                          lazy(e->kg_sp[0], sp), lazy(e->kg_bi[0], bi), lazy(e->kg_sp[1], sp), lazy(e->kg_bi[1], bi)});
+}
+
+// the energy's per-block sums, and with features the per-image flags
+static int ensure_energy(Engine *e, bool feat) {
+    if (feat)
+        if (int rc = ensure_feat(e)) return rc;
+    return lazy_alloc(e, {lazy(e->en_part, (size_t)e->maxB * ((e->Ncap + kThreads - 1) / kThreads) * 4)});
 }
 
 // prepare_lattices with caller-given bilateral features ([B][5][N]): the bilateral sigmas of `p` are not used, and the
@@ -230,6 +290,27 @@ static int prepare_lattices_feat(Engine *e, int B, const float *feat, const dsrg
     if (int rc = prepare_spatial(e, B, p, s)) return rc;
     for (int i = 0; i < 5; i++) e->bi.sigma[i] = 1.0f;
     return lattice_build(e, e->bi, B, nullptr, s, feat, e->feat_bad);
+}
+
+// the lattices of the image, or of caller-given bilateral features
+static int prepare_lattices_for(Engine *e, int B, const uint8_t *image, const float *features,
+                                const dsrg_crf_params &p, cudaStream_t s) {
+    return features ? prepare_lattices_feat(e, B, features, p, s) : prepare_lattices(e, B, image, p, s);
+}
+
+// The feature passes' NaN policy: every value of a given output becomes NaN in the images whose feature lattice left
+// the packed key range (e->feat_bad).  An output holds per_image floats per image, `reps` times over ([reps][B]...).
+struct NanOut {
+    float *p;
+    long long per_image;
+    int reps = 1;
+};
+static int nan_flagged_outputs(Engine *e, int B, std::initializer_list<NanOut> outs, cudaStream_t s,
+                               int tag = T_FGRAD) {
+    for (const NanOut &o : outs)
+        if (o.p) nan_images(e, e->feat_bad, o.p, B, o.per_image, o.reps, s, tag);
+    DSRG_CUDA_TRY(cudaGetLastError());
+    return DSRG_OK;
 }
 
 int check_batch(Engine *e, int B) {
@@ -270,14 +351,12 @@ int crf_core(Engine *e, int B, const float *unary, int layout, bool clamp, float
         return DSRG_E_INVALID;
     }
     const float *feat = lc ? lc->features : nullptr;
-    int rc = feat ? prepare_lattices_feat(e, B, feat, *p, s) : prepare_lattices(e, B, image, *p, s);
+    int rc = prepare_lattices_for(e, B, image, feat, *p, s);
     if (rc) return rc;
     if (!lc) return meanfield_run(e, B, unary, layout, clamp, unary_rw, *p, s);
     rc = meanfield_run(e, B, unary, layout, clamp, unary_rw, *p, s, lc->compat);
     if (rc || !feat) return rc;
-    nan_images(e, e->feat_bad, e->Q0, B, (long long)e->M * e->N, 1, 0, s);   // the training forward's policy
-    DSRG_CUDA_TRY(cudaGetLastError());
-    return DSRG_OK;
+    return nan_flagged_outputs(e, B, {{e->Q0, (long long)e->M * e->N}}, s);   // the training forward's policy
 }
 
 static int crf_batch_pass(Engine *e, int B, const float *unary, int unary_layout, const uint8_t *image,
@@ -698,210 +777,131 @@ static int wide_labels_ok(const Engine *e) {
     return DSRG_E_INVALID;
 }
 
+static GraphKey train_key(const CrfTrainIo &io) {
+    GraphKey args;
+    args.add(io.unary).add(io.q_hist).add(io.grad_q).add(io.image).add(io.features).add(io.potts).add(io.compat)
+        .add(io.q_out).add(io.grad_unary).add(io.grad_potts).add(io.grad_compat).add(io.grad_theta)
+        .add(io.grad_features).add(io.grad_theta_sp);
+    return args;
+}
+
+// What a pass that leaves no marginals in the engine notes: the *_last_* entry points refuse, and a feature pass's
+// batch is the one dsrg_engine_feature_range_flags reports on
+static int learned_pass_end(Engine *e, int B, const float *features, int rc) {
+    e->last_crf_B = 0;
+    if (features) e->feat_B = rc == DSRG_OK ? B : 0;
+    return rc;
+}
+
+// The body of every training forward: Q_0..Q_T to io.q_out, on the fused kernels or (wide) the label-chunked ones
+static int train_forward(dsrg_engine *h, int B, cudaStream_t s, bool args_ok, PassKind kind, bool wide,
+                         const dsrg_crf_params *params, const CrfTrainIo &io) {
+    return dev_call(h, B, s, args_ok, [&](Engine *e) {
+        if (int rc = wide ? wide_labels_ok(e) : grad_labels_ok(e)) return rc;
+        if (io.features)
+            if (int rc = ensure_feat(e)) return rc;
+        const int rc = crf_pass(e, s, kind, B, params, train_key(io), [&]() {
+            int r = prepare_lattices_for(e, B, io.image, io.features, *params, s);
+            if (!r) r = (wide ? meanfield_run_train_wide : meanfield_run_train)(e, B, io, *params, s);
+            if (r || !io.features) return r;
+            // every kept iterate
+            return nan_flagged_outputs(e, B, {{io.q_out, (long long)e->M * e->N, params->n_iters + 1}}, s);
+        });
+        return learned_pass_end(e, B, io.features, rc);
+    });
+}
+
+// The body of every training backward: the buffers its outputs need on their first call, then the gradients
+static int train_backward(dsrg_engine *h, int B, cudaStream_t s, bool args_ok, PassKind kind, bool wide,
+                          const dsrg_crf_params *params, const CrfTrainIo &io) {
+    return dev_call(h, B, s, args_ok, [&](Engine *e) {
+        if (int rc = wide ? wide_labels_ok(e) : grad_labels_ok(e)) return rc;
+        int rc = wide ? ensure_wide(e, io.compat != nullptr) : io.compat ? ensure_compat_part(e) : DSRG_OK;
+        if (!rc && (io.grad_theta || io.features)) rc = wide ? ensure_kgrad_wide(e) : ensure_kgrad(e);
+        if (!rc && io.features) rc = ensure_feat(e);
+        if (rc) return rc;
+        rc = crf_pass(e, s, kind, B, params, train_key(io), [&]() {
+            // the lattices are rebuilt: autograd may have run other passes on this engine since the forward
+            int r = prepare_lattices_for(e, B, io.image, io.features, *params, s);
+            if (!r) r = (wide ? meanfield_backward_wide : meanfield_backward)(e, B, io, *params, s);
+            if (r || !io.features) return r;
+            const long long M = e->M, N = e->N;
+            return nan_flagged_outputs(e, B, {{io.grad_unary, M * N}, {io.grad_features, 5 * N}, {io.grad_potts, 2},
+                                              {io.grad_compat, 2 * M * M}, {io.grad_theta_sp, 2}}, s);
+        });
+        return learned_pass_end(e, B, io.features, rc);
+    });
+}
+
 int dsrg_crf_forward_train_dev(dsrg_engine *h, const float *unary, int B, const uint8_t *image,
                                const dsrg_crf_params *params, const float *potts, float *q_hist, void *stream) {
-    const cudaStream_t s = (cudaStream_t)stream;
-    return dev_call(h, B, s, unary && image && params && q_hist, [&](Engine *e) {
-        if (int rc = grad_labels_ok(e)) return rc;
-        GraphKey args;
-        args.add(unary).add(image).add(potts).add(q_hist);
-        const int rc = crf_pass(e, s, PassKind::crf_train, B, params, args, [&]() {
-            int r = prepare_lattices(e, B, image, *params, s);
-            if (r) return r;
-            return meanfield_run_train(e, B, unary, q_hist, potts, nullptr, *params, s);
-        });
-        e->last_crf_B = 0;  // the marginals are q_hist[T], not the engine's: the *_last_* entry points refuse
-        return rc;
-    });
+    return train_forward(h, B, (cudaStream_t)stream, unary && image && params && q_hist, PassKind::crf_train, false,
+                         params, {.unary = unary, .image = image, .potts = potts, .q_out = q_hist});
 }
 
 int dsrg_crf_backward_dev(dsrg_engine *h, const float *q_hist, int B, const uint8_t *image,
                           const dsrg_crf_params *params, const float *potts, const float *grad_q, float *grad_unary,
                           float *grad_potts, void *stream) {
-    const cudaStream_t s = (cudaStream_t)stream;
-    return dev_call(h, B, s, q_hist && image && params && grad_q && grad_unary, [&](Engine *e) {
-        if (int rc = grad_labels_ok(e)) return rc;
-        GraphKey args;
-        args.add(q_hist).add(image).add(potts).add(grad_q).add(grad_unary).add(grad_potts);
-        const int rc = crf_pass(e, s, PassKind::crf_backward, B, params, args, [&]() {
-            // the lattices are rebuilt: autograd may have run other passes on this engine since the forward
-            int r = prepare_lattices(e, B, image, *params, s);
-            if (r) return r;
-            return meanfield_backward(e, B, q_hist, potts, grad_q, grad_unary, grad_potts, nullptr, nullptr, *params, s);
-        });
-        e->last_crf_B = 0;
-        return rc;
-    });
+    return train_backward(h, B, (cudaStream_t)stream, q_hist && image && params && grad_q && grad_unary,
+                          PassKind::crf_backward, false, params,
+                          {.q_hist = q_hist, .grad_q = grad_q, .image = image, .potts = potts, .grad_unary = grad_unary,
+                           .grad_potts = grad_potts});
 }
 
 int dsrg_crf_forward_train_compat_dev(dsrg_engine *h, const float *unary, int B, const uint8_t *image,
                                       const dsrg_crf_params *params, const float *compat, float *q_hist, void *stream) {
-    const cudaStream_t s = (cudaStream_t)stream;
-    return dev_call(h, B, s, unary && image && params && compat && q_hist, [&](Engine *e) {
-        if (int rc = grad_labels_ok(e)) return rc;
-        GraphKey args;
-        args.add(unary).add(image).add(compat).add(q_hist);
-        const int rc = crf_pass(e, s, PassKind::crf_train_compat, B, params, args, [&]() {
-            int r = prepare_lattices(e, B, image, *params, s);
-            if (r) return r;
-            return meanfield_run_train(e, B, unary, q_hist, nullptr, compat, *params, s);
-        });
-        e->last_crf_B = 0;
-        return rc;
-    });
-}
-
-// The compatibility backward's per-tile partials, B * ntiles * 2 * M^2 floats, on its first call: an engine that never
-// learns matrices keeps its footprint.  Sized for the capacity's tile count (set_size never exceeds it).  The call may
-// sit inside a caller's stream capture, where an allocation is allowed in relaxed mode only.
-static int ensure_compat_part(Engine *e) {
-    if (e->compat_part) return DSRG_OK;
-    const size_t tiles = (size_t)((e->Wcap + kTileW - 1) / kTileW) * ((e->Hcap + kTileH - 1) / kTileH);
-    cudaStreamCaptureMode mode = cudaStreamCaptureModeRelaxed;
-    DSRG_CUDA_TRY(cudaThreadExchangeStreamCaptureMode(&mode));
-    const int rc = dalloc(e, &e->compat_part, (size_t)e->maxB * tiles * 2 * e->M * e->M);
-    DSRG_CUDA_TRY(cudaThreadExchangeStreamCaptureMode(&mode));
-    return rc;
+    return train_forward(h, B, (cudaStream_t)stream, unary && image && params && compat && q_hist,
+                         PassKind::crf_train_compat, false, params,
+                         {.unary = unary, .image = image, .compat = compat, .q_out = q_hist});
 }
 
 int dsrg_crf_backward_compat_dev(dsrg_engine *h, const float *q_hist, int B, const uint8_t *image,
                                  const dsrg_crf_params *params, const float *compat, const float *grad_q,
                                  float *grad_unary, float *grad_compat, void *stream) {
-    const cudaStream_t s = (cudaStream_t)stream;
-    return dev_call(h, B, s, q_hist && image && params && compat && grad_q && grad_unary, [&](Engine *e) {
-        if (int rc = grad_labels_ok(e)) return rc;
-        if (int rc = ensure_compat_part(e)) return rc;
-        GraphKey args;
-        args.add(q_hist).add(image).add(compat).add(grad_q).add(grad_unary).add(grad_compat);
-        const int rc = crf_pass(e, s, PassKind::crf_backward_compat, B, params, args, [&]() {
-            int r = prepare_lattices(e, B, image, *params, s);   // as in dsrg_crf_backward_dev
-            if (r) return r;
-            return meanfield_backward(e, B, q_hist, nullptr, grad_q, grad_unary, nullptr, compat, grad_compat, *params,
-                                      s);
-        });
-        e->last_crf_B = 0;
-        return rc;
-    });
-}
-
-// The kernel-bandwidth backward's buffers on its first call (as ensure_compat_part): g_t and c per pixel, the per-block
-// sums and two value buffers per lattice, sized for the engine's capacity.
-static int ensure_kgrad(Engine *e) {
-    if (e->kg_g) return DSRG_OK;
-    cudaStreamCaptureMode mode = cudaStreamCaptureModeRelaxed;
-    DSRG_CUDA_TRY(cudaThreadExchangeStreamCaptureMode(&mode));
-    int rc = 0;
-    rc |= dalloc(e, &e->kg_g, (size_t)e->maxB * e->M * e->Ncap);
-    rc |= dalloc(e, &e->kg_csum, (size_t)2 * e->maxB * e->Ncap);
-    rc |= dalloc(e, &e->kg_part, (size_t)e->maxB * ((e->Ncap + kThreads - 1) / kThreads) * 8);
-    for (int i = 0; i < 2; i++) {
-        rc |= dalloc(e, &e->kg_sp[i], (size_t)e->sp.rows_cap * e->MP);
-        rc |= dalloc(e, &e->kg_bi[i], (size_t)e->bi.rows_cap * e->MP);
-    }
-    DSRG_CUDA_TRY(cudaThreadExchangeStreamCaptureMode(&mode));
-    return rc ? DSRG_E_NOMEM : DSRG_OK;
+    return train_backward(h, B, (cudaStream_t)stream, q_hist && image && params && compat && grad_q && grad_unary,
+                          PassKind::crf_backward_compat, false, params,
+                          {.q_hist = q_hist, .grad_q = grad_q, .image = image, .compat = compat,
+                           .grad_unary = grad_unary, .grad_compat = grad_compat});
 }
 
 int dsrg_crf_backward_theta_dev(dsrg_engine *h, const float *q_hist, int B, const uint8_t *image,
                                 const dsrg_crf_params *params, const float *potts, const float *grad_q,
                                 float *grad_unary, float *grad_potts, float *grad_theta, void *stream) {
-    const cudaStream_t s = (cudaStream_t)stream;
-    return dev_call(h, B, s, q_hist && image && params && grad_q && grad_unary && grad_theta, [&](Engine *e) {
-        if (int rc = grad_labels_ok(e)) return rc;
-        if (int rc = ensure_kgrad(e)) return rc;
-        GraphKey args;
-        args.add(q_hist).add(image).add(potts).add(grad_q).add(grad_unary).add(grad_potts).add(grad_theta);
-        const int rc = crf_pass(e, s, PassKind::crf_backward_theta, B, params, args, [&]() {
-            int r = prepare_lattices(e, B, image, *params, s);   // as in dsrg_crf_backward_dev
-            if (r) return r;
-            return meanfield_backward(e, B, q_hist, potts, grad_q, grad_unary, grad_potts, nullptr, nullptr, *params, s,
-                                      grad_theta, image);
-        });
-        e->last_crf_B = 0;
-        return rc;
-    });
+    return train_backward(h, B, (cudaStream_t)stream,
+                          q_hist && image && params && grad_q && grad_unary && grad_theta,
+                          PassKind::crf_backward_theta, false, params,
+                          {.q_hist = q_hist, .grad_q = grad_q, .image = image, .potts = potts,
+                           .grad_unary = grad_unary, .grad_potts = grad_potts, .grad_theta = grad_theta});
 }
 
 int dsrg_crf_backward_compat_theta_dev(dsrg_engine *h, const float *q_hist, int B, const uint8_t *image,
                                        const dsrg_crf_params *params, const float *compat, const float *grad_q,
                                        float *grad_unary, float *grad_compat, float *grad_theta, void *stream) {
-    const cudaStream_t s = (cudaStream_t)stream;
-    return dev_call(h, B, s, q_hist && image && params && compat && grad_q && grad_unary && grad_theta, [&](Engine *e) {
-        if (int rc = grad_labels_ok(e)) return rc;
-        if (int rc = ensure_compat_part(e)) return rc;
-        if (int rc = ensure_kgrad(e)) return rc;
-        GraphKey args;
-        args.add(q_hist).add(image).add(compat).add(grad_q).add(grad_unary).add(grad_compat).add(grad_theta);
-        const int rc = crf_pass(e, s, PassKind::crf_backward_compat_theta, B, params, args, [&]() {
-            int r = prepare_lattices(e, B, image, *params, s);
-            if (r) return r;
-            return meanfield_backward(e, B, q_hist, nullptr, grad_q, grad_unary, nullptr, compat, grad_compat, *params,
-                                      s, grad_theta, image);
-        });
-        e->last_crf_B = 0;
-        return rc;
-    });
+    return train_backward(h, B, (cudaStream_t)stream,
+                          q_hist && image && params && compat && grad_q && grad_unary && grad_theta,
+                          PassKind::crf_backward_compat_theta, false, params,
+                          {.q_hist = q_hist, .grad_q = grad_q, .image = image, .compat = compat,
+                           .grad_unary = grad_unary, .grad_compat = grad_compat, .grad_theta = grad_theta});
 }
 
 int dsrg_crf_forward_train_feat_dev(dsrg_engine *h, const float *unary, int B, const float *features,
                                     const dsrg_crf_params *params, const float *potts, const float *compat,
                                     float *q_hist, void *stream) {
-    const cudaStream_t s = (cudaStream_t)stream;
-    return dev_call(h, B, s, unary && features && params && q_hist && !(potts && compat), [&](Engine *e) {
-        if (int rc = grad_labels_ok(e)) return rc;
-        if (int rc = ensure_feat(e)) return rc;
-        GraphKey args;
-        args.add(unary).add(features).add(potts).add(compat).add(q_hist);
-        const int rc = crf_pass(e, s, PassKind::crf_train_feat, B, params, args, [&]() {
-            int r = prepare_lattices_feat(e, B, features, *params, s);
-            if (!r) r = meanfield_run_train(e, B, unary, q_hist, potts, compat, *params, s);
-            if (r) return r;
-            const long long mn = (long long)e->M * e->N;
-            nan_images(e, e->feat_bad, q_hist, B, mn, params->n_iters + 1, B * mn, s);   // every kept iterate
-            DSRG_CUDA_TRY(cudaGetLastError());
-            return DSRG_OK;
-        });
-        e->last_crf_B = 0;
-        e->feat_B = rc == DSRG_OK ? B : 0;
-        return rc;
-    });
+    return train_forward(h, B, (cudaStream_t)stream, unary && features && params && q_hist && !(potts && compat),
+                         PassKind::crf_train_feat, false, params,
+                         {.unary = unary, .features = features, .potts = potts, .compat = compat, .q_out = q_hist});
 }
 
 int dsrg_crf_backward_feat_dev(dsrg_engine *h, const float *q_hist, int B, const float *features,
                                const dsrg_crf_params *params, const float *potts, const float *compat,
                                const float *grad_q, float *grad_unary, float *grad_features, float *grad_potts,
                                float *grad_compat, float *grad_theta_sp, void *stream) {
-    const cudaStream_t s = (cudaStream_t)stream;
     const bool ok = q_hist && features && params && grad_q && grad_unary && grad_features && !(potts && compat) &&
                     !(grad_potts && compat) && !(grad_compat && !compat);
-    return dev_call(h, B, s, ok, [&](Engine *e) {
-        if (int rc = grad_labels_ok(e)) return rc;
-        if (compat)
-            if (int rc = ensure_compat_part(e)) return rc;
-        if (int rc = ensure_kgrad(e)) return rc;
-        if (int rc = ensure_feat(e)) return rc;
-        GraphKey args;
-        args.add(q_hist).add(features).add(potts).add(compat).add(grad_q).add(grad_unary).add(grad_features)
-            .add(grad_potts).add(grad_compat).add(grad_theta_sp);
-        const int rc = crf_pass(e, s, PassKind::crf_backward_feat, B, params, args, [&]() {
-            int r = prepare_lattices_feat(e, B, features, *params, s);   // as in dsrg_crf_backward_dev
-            if (!r)
-                r = meanfield_backward(e, B, q_hist, potts, grad_q, grad_unary, grad_potts, compat, grad_compat,
-                                       *params, s, nullptr, nullptr, features, grad_features, grad_theta_sp);
-            if (r) return r;
-            const long long M = e->M, N = e->N;
-            const std::pair<float *, long long> outs[] = {{grad_unary, M * N}, {grad_features, 5 * N},
-                                                          {grad_potts, 2}, {grad_compat, 2 * M * M},
-                                                          {grad_theta_sp, 2}};
-            for (const auto &o : outs)
-                if (o.first) nan_images(e, e->feat_bad, o.first, B, o.second, 1, 0, s);
-            DSRG_CUDA_TRY(cudaGetLastError());
-            return DSRG_OK;
-        });
-        e->last_crf_B = 0;
-        e->feat_B = rc == DSRG_OK ? B : 0;
-        return rc;
-    });
+    return train_backward(h, B, (cudaStream_t)stream, ok, PassKind::crf_backward_feat, false, params,
+                          {.q_hist = q_hist, .grad_q = grad_q, .features = features, .potts = potts, .compat = compat,
+                           .grad_unary = grad_unary, .grad_potts = grad_potts, .grad_compat = grad_compat,
+                           .grad_features = grad_features, .grad_theta_sp = grad_theta_sp});
 }
 
 int dsrg_engine_feature_range_flags(dsrg_engine *h, int B, int32_t *flags_out) {
@@ -921,174 +921,52 @@ int dsrg_engine_feature_range_flags(dsrg_engine *h, int B, int32_t *flags_out) {
 int dsrg_crf_forward_train_wide_dev(dsrg_engine *h, const float *unary, int B, const uint8_t *image,
                                     const dsrg_crf_params *params, const float *potts, const float *compat,
                                     float *q_hist, void *stream) {
-    const cudaStream_t s = (cudaStream_t)stream;
-    return dev_call(h, B, s, unary && image && params && q_hist && !(potts && compat), [&](Engine *e) {
-        if (int rc = wide_labels_ok(e)) return rc;
-        GraphKey args;
-        args.add(unary).add(image).add(potts).add(compat).add(q_hist);
-        const int rc = crf_pass(e, s, PassKind::crf_train_wide, B, params, args, [&]() {
-            int r = prepare_lattices(e, B, image, *params, s);
-            if (r) return r;
-            return meanfield_run_train_wide(e, B, unary, q_hist, potts, compat, *params, s);
-        });
-        e->last_crf_B = 0;   // the marginals are q_hist[T]; e->U and e->Q0 were scratch
-        return rc;
-    });
-}
-
-// The label-chunked backward's buffers on its first call (as ensure_compat_part): the Potts partials, and for the
-// matrices G and the outer-product partials, sized for the engine's capacity
-static int ensure_wide(Engine *e, bool compat) {
-    if (e->wide_ppart && (!compat || e->wide_g)) return DSRG_OK;
-    cudaStreamCaptureMode mode = cudaStreamCaptureModeRelaxed;
-    DSRG_CUDA_TRY(cudaThreadExchangeStreamCaptureMode(&mode));
-    int rc = 0;
-    if (!e->wide_ppart) rc |= dalloc(e, &e->wide_ppart, (size_t)e->maxB * (e->MP / 4) * ((e->Ncap + kThreads - 1) / kThreads));
-    if (compat && !e->wide_g) {
-        rc |= dalloc(e, &e->wide_g, (size_t)e->maxB * e->M * e->Ncap);
-        rc |= dalloc(e, &e->wide_cpart, (size_t)e->maxB * kWideChunks * 2 * e->M * e->M);
-    }
-    DSRG_CUDA_TRY(cudaThreadExchangeStreamCaptureMode(&mode));
-    return rc ? DSRG_E_NOMEM : DSRG_OK;
+    return train_forward(h, B, (cudaStream_t)stream, unary && image && params && q_hist && !(potts && compat),
+                         PassKind::crf_train_wide, true, params,
+                         {.unary = unary, .image = image, .potts = potts, .compat = compat, .q_out = q_hist});
 }
 
 int dsrg_crf_backward_wide_dev(dsrg_engine *h, const float *q_hist, int B, const uint8_t *image,
                                const dsrg_crf_params *params, const float *potts, const float *compat,
                                const float *grad_q, float *grad_unary, float *grad_potts, float *grad_compat,
                                void *stream) {
-    const cudaStream_t s = (cudaStream_t)stream;
     const bool ok = q_hist && image && params && grad_q && grad_unary && !(potts && compat) &&
                     !(grad_potts && compat) && !(grad_compat && !compat);
-    return dev_call(h, B, s, ok, [&](Engine *e) {
-        if (int rc = wide_labels_ok(e)) return rc;
-        if (int rc = ensure_wide(e, compat != nullptr)) return rc;
-        GraphKey args;
-        args.add(q_hist).add(image).add(potts).add(compat).add(grad_q).add(grad_unary).add(grad_potts).add(grad_compat);
-        const int rc = crf_pass(e, s, PassKind::crf_backward_wide, B, params, args, [&]() {
-            int r = prepare_lattices(e, B, image, *params, s);   // as in dsrg_crf_backward_dev
-            if (r) return r;
-            return meanfield_backward_wide(e, B, q_hist, potts, compat, grad_q, grad_unary, grad_potts, grad_compat,
-                                           *params, s);
-        });
-        e->last_crf_B = 0;
-        return rc;
-    });
-}
-
-// The label-chunked kernel-bandwidth and feature backward's buffers on its first call (as ensure_compat_part): c per
-// pixel [2][maxB][N] and the per-block sums, as ensure_kgrad, and the normalisation term's two value buffers per
-// lattice at 4 floats per row.  g_t stays in e->Q0 and Vy in the mean-field buffers, so nothing here grows with the
-// label count.
-static int ensure_kgrad_wide(Engine *e) {
-    if (e->kg_csum) return DSRG_OK;
-    cudaStreamCaptureMode mode = cudaStreamCaptureModeRelaxed;
-    DSRG_CUDA_TRY(cudaThreadExchangeStreamCaptureMode(&mode));
-    int rc = 0;
-    rc |= dalloc(e, &e->kg_csum, (size_t)2 * e->maxB * e->Ncap);
-    rc |= dalloc(e, &e->kg_part, (size_t)e->maxB * ((e->Ncap + kThreads - 1) / kThreads) * 8);
-    for (int i = 0; i < 2; i++) {
-        rc |= dalloc(e, &e->kg_sp[i], (size_t)e->sp.rows_cap * 4);
-        rc |= dalloc(e, &e->kg_bi[i], (size_t)e->bi.rows_cap * 4);
-    }
-    DSRG_CUDA_TRY(cudaThreadExchangeStreamCaptureMode(&mode));
-    return rc ? DSRG_E_NOMEM : DSRG_OK;
+    return train_backward(h, B, (cudaStream_t)stream, ok, PassKind::crf_backward_wide, true, params,
+                          {.q_hist = q_hist, .grad_q = grad_q, .image = image, .potts = potts, .compat = compat,
+                           .grad_unary = grad_unary, .grad_potts = grad_potts, .grad_compat = grad_compat});
 }
 
 int dsrg_crf_backward_wide_theta_dev(dsrg_engine *h, const float *q_hist, int B, const uint8_t *image,
                                      const dsrg_crf_params *params, const float *potts, const float *compat,
                                      const float *grad_q, float *grad_unary, float *grad_potts, float *grad_compat,
                                      float *grad_theta, void *stream) {
-    const cudaStream_t s = (cudaStream_t)stream;
     const bool ok = q_hist && image && params && grad_q && grad_unary && grad_theta && !(potts && compat) &&
                     !(grad_potts && compat) && !(grad_compat && !compat);
-    return dev_call(h, B, s, ok, [&](Engine *e) {
-        if (int rc = wide_labels_ok(e)) return rc;
-        if (int rc = ensure_wide(e, compat != nullptr)) return rc;
-        if (int rc = ensure_kgrad_wide(e)) return rc;
-        GraphKey args;
-        args.add(q_hist).add(image).add(potts).add(compat).add(grad_q).add(grad_unary).add(grad_potts).add(grad_compat)
-            .add(grad_theta);
-        const int rc = crf_pass(e, s, PassKind::crf_backward_wide_theta, B, params, args, [&]() {
-            int r = prepare_lattices(e, B, image, *params, s);   // as in dsrg_crf_backward_dev
-            if (r) return r;
-            return meanfield_backward_wide(e, B, q_hist, potts, compat, grad_q, grad_unary, grad_potts, grad_compat,
-                                           *params, s, grad_theta, image);
-        });
-        e->last_crf_B = 0;
-        return rc;
-    });
+    return train_backward(h, B, (cudaStream_t)stream, ok, PassKind::crf_backward_wide_theta, true, params,
+                          {.q_hist = q_hist, .grad_q = grad_q, .image = image, .potts = potts, .compat = compat,
+                           .grad_unary = grad_unary, .grad_potts = grad_potts, .grad_compat = grad_compat,
+                           .grad_theta = grad_theta});
 }
 
 int dsrg_crf_forward_train_wide_feat_dev(dsrg_engine *h, const float *unary, int B, const float *features,
                                          const dsrg_crf_params *params, const float *potts, const float *compat,
                                          float *q_hist, void *stream) {
-    const cudaStream_t s = (cudaStream_t)stream;
-    return dev_call(h, B, s, unary && features && params && q_hist && !(potts && compat), [&](Engine *e) {
-        if (int rc = wide_labels_ok(e)) return rc;
-        if (int rc = ensure_feat(e)) return rc;
-        GraphKey args;
-        args.add(unary).add(features).add(potts).add(compat).add(q_hist);
-        const int rc = crf_pass(e, s, PassKind::crf_train_wide_feat, B, params, args, [&]() {
-            int r = prepare_lattices_feat(e, B, features, *params, s);
-            if (!r) r = meanfield_run_train_wide(e, B, unary, q_hist, potts, compat, *params, s);
-            if (r) return r;
-            const long long mn = (long long)e->M * e->N;
-            nan_images(e, e->feat_bad, q_hist, B, mn, params->n_iters + 1, B * mn, s);   // every kept iterate
-            DSRG_CUDA_TRY(cudaGetLastError());
-            return DSRG_OK;
-        });
-        e->last_crf_B = 0;
-        e->feat_B = rc == DSRG_OK ? B : 0;
-        return rc;
-    });
+    return train_forward(h, B, (cudaStream_t)stream, unary && features && params && q_hist && !(potts && compat),
+                         PassKind::crf_train_wide_feat, true, params,
+                         {.unary = unary, .features = features, .potts = potts, .compat = compat, .q_out = q_hist});
 }
 
 int dsrg_crf_backward_wide_feat_dev(dsrg_engine *h, const float *q_hist, int B, const float *features,
                                     const dsrg_crf_params *params, const float *potts, const float *compat,
                                     const float *grad_q, float *grad_unary, float *grad_features, float *grad_potts,
                                     float *grad_compat, float *grad_theta_sp, void *stream) {
-    const cudaStream_t s = (cudaStream_t)stream;
     const bool ok = q_hist && features && params && grad_q && grad_unary && grad_features && !(potts && compat) &&
                     !(grad_potts && compat) && !(grad_compat && !compat);
-    return dev_call(h, B, s, ok, [&](Engine *e) {
-        if (int rc = wide_labels_ok(e)) return rc;
-        if (int rc = ensure_wide(e, compat != nullptr)) return rc;
-        if (int rc = ensure_kgrad_wide(e)) return rc;
-        if (int rc = ensure_feat(e)) return rc;
-        GraphKey args;
-        args.add(q_hist).add(features).add(potts).add(compat).add(grad_q).add(grad_unary).add(grad_features)
-            .add(grad_potts).add(grad_compat).add(grad_theta_sp);
-        const int rc = crf_pass(e, s, PassKind::crf_backward_wide_feat, B, params, args, [&]() {
-            int r = prepare_lattices_feat(e, B, features, *params, s);   // as in dsrg_crf_backward_dev
-            if (!r)
-                r = meanfield_backward_wide(e, B, q_hist, potts, compat, grad_q, grad_unary, grad_potts, grad_compat,
-                                            *params, s, nullptr, nullptr, features, grad_features, grad_theta_sp);
-            if (r) return r;
-            const long long M = e->M, N = e->N;
-            const std::pair<float *, long long> outs[] = {{grad_unary, M * N}, {grad_features, 5 * N},
-                                                          {grad_potts, 2}, {grad_compat, 2 * M * M},
-                                                          {grad_theta_sp, 2}};
-            for (const auto &o : outs)
-                if (o.first) nan_images(e, e->feat_bad, o.first, B, o.second, 1, 0, s);
-            DSRG_CUDA_TRY(cudaGetLastError());
-            return DSRG_OK;
-        });
-        e->last_crf_B = 0;
-        e->feat_B = rc == DSRG_OK ? B : 0;
-        return rc;
-    });
-}
-
-// The energy's per-block sums on its first call (as ensure_compat_part), and with features the per-image flags
-static int ensure_energy(Engine *e, bool feat) {
-    if (feat)
-        if (int rc = ensure_feat(e)) return rc;
-    if (e->en_part) return DSRG_OK;
-    cudaStreamCaptureMode mode = cudaStreamCaptureModeRelaxed;
-    DSRG_CUDA_TRY(cudaThreadExchangeStreamCaptureMode(&mode));
-    const int rc = dalloc(e, &e->en_part, (size_t)e->maxB * ((e->Ncap + kThreads - 1) / kThreads) * 4);
-    DSRG_CUDA_TRY(cudaThreadExchangeStreamCaptureMode(&mode));
-    return rc;
+    return train_backward(h, B, (cudaStream_t)stream, ok, PassKind::crf_backward_wide_feat, true, params,
+                          {.q_hist = q_hist, .grad_q = grad_q, .features = features, .potts = potts, .compat = compat,
+                           .grad_unary = grad_unary, .grad_potts = grad_potts, .grad_compat = grad_compat,
+                           .grad_features = grad_features, .grad_theta_sp = grad_theta_sp});
 }
 
 // The body of both energy entry points: the lattices of the image or of the features, the energy (terms) or its
@@ -1096,15 +974,11 @@ static int ensure_energy(Engine *e, bool feat) {
 static int energy_pass(Engine *e, int B, const float *q, const float *unary, const uint8_t *image, const float *features,
                        const dsrg_crf_params &p, const float *potts, const float *compat, float *terms,
                        const float *grad_terms, float *grad_q, float *grad_unary, cudaStream_t s) {
-    int r = features ? prepare_lattices_feat(e, B, features, p, s) : prepare_lattices(e, B, image, p, s);
+    int r = prepare_lattices_for(e, B, image, features, p, s);
     if (!r) r = meanfield_energy(e, B, q, unary, potts, compat, p, terms, grad_terms, grad_q, grad_unary, s);
     if (r || !features) return r;
     const long long MN = (long long)e->M * e->N;
-    const std::pair<float *, long long> outs[] = {{terms, 4}, {grad_q, MN}, {grad_unary, MN}};
-    for (const auto &o : outs)
-        if (o.first) nan_images(e, e->feat_bad, o.first, B, o.second, 1, 0, s, T_CRF_ENERGY);
-    DSRG_CUDA_TRY(cudaGetLastError());
-    return DSRG_OK;
+    return nan_flagged_outputs(e, B, {{terms, 4}, {grad_q, MN}, {grad_unary, MN}}, s, T_CRF_ENERGY);
 }
 
 static int energy_labels_ok(const Engine *e) {
@@ -1127,9 +1001,7 @@ int dsrg_crf_energy_dev(dsrg_engine *h, const float *q, int B, const float *unar
             return energy_pass(e, B, q, unary, image, features, *params, potts, compat, terms, nullptr, nullptr,
                                nullptr, s);
         });
-        e->last_crf_B = 0;   // no marginals in the engine: the *_last_* entry points refuse
-        if (features) e->feat_B = rc == DSRG_OK ? B : 0;
-        return rc;
+        return learned_pass_end(e, B, features, rc);
     });
 }
 
@@ -1150,9 +1022,7 @@ int dsrg_crf_energy_backward_dev(dsrg_engine *h, const float *q, int B, const fl
             return energy_pass(e, B, q, unary, image, features, *params, potts, compat, nullptr, grad_terms, grad_q,
                                grad_unary, s);
         });
-        e->last_crf_B = 0;
-        if (features) e->feat_B = rc == DSRG_OK ? B : 0;
-        return rc;
+        return learned_pass_end(e, B, features, rc);
     });
 }
 

@@ -162,23 +162,31 @@ inline bool hybrid_tiles_on(const Engine *e, int B);
 // The inference: Q_T to e->Q0.  `compat` ({mu_bi, mu_sp} [2][M][M], device) replaces the Potts weights of p.
 int meanfield_run(Engine *e, int B, const float *unary, int unary_layout, bool clamp_inplace,
                   float *unary_rw, const dsrg_crf_params &p, cudaStream_t s, const float *compat = nullptr);
-// the training forward (NCHW unary, Q_0..Q_T to q_hist) and its backward; at most DSRG_MAX_LABELS labels
-// (with `compat` = {mu_bi, mu_sp} [2][M][M] in place of the Potts weights: the compatibility-matrix variant, whose
-// backward needs e->compat_part, ensure_compat_part)
-int meanfield_run_train(Engine *e, int B, const float *unary, float *q_hist, const float *potts, const float *compat,
-                        const dsrg_crf_params &p, cudaStream_t s);
-// grad_theta ([B][7], with the batch's image): the kernel-bandwidth gradient too, which needs the kg_* buffers
-// (ensure_kgrad).  With caller-given bilateral features `feat` (the lattice built on them) grad_feat [B][5][N] gets
-// the per-pixel dL/df of the bilateral lattice instead, and grad_theta_sp, if given, [B][2] dL/dtheta_gamma; this
-// needs the kg_* buffers too
-int meanfield_backward(Engine *e, int B, const float *q_hist, const float *potts, const float *grad_q,
-                       float *grad_unary, float *grad_potts, const float *compat, float *grad_compat,
-                       const dsrg_crf_params &p, cudaStream_t s, float *grad_theta = nullptr,
-                       const uint8_t *image = nullptr, const float *feat = nullptr, float *grad_feat = nullptr,
-                       float *grad_theta_sp = nullptr);
-// NaN into every image b of p (reps slabs rep_stride apart, per_image floats per image) with bad[b] set; timed under tag
-void nan_images(Engine *e, const int *bad, float *p, int B, long long per_image, int reps, long long rep_stride,
-                cudaStream_t s, int tag = T_FGRAD);
+// One call of the differentiable CRF: the training forward (unary -> q_out) or its backward (q_hist, grad_q -> the
+// grad_* outputs).  The bilateral lattice is the image's or the caller-given features'; the pairwise weights are
+// potts {w1, w2} or compat {mu_bi, mu_sp} [2][M][M] (neither: the params' w1 / w2).  A NULL output is not written.
+struct CrfTrainIo {
+    const float *unary = nullptr;     // [B][M][N] NCHW
+    const float *q_hist = nullptr;    // [T+1][B][M][N]: the forward's Q_0..Q_T
+    const float *grad_q = nullptr;    // [B][M][N] dL/dQ_T
+    const uint8_t *image = nullptr;   // [B][N][3]
+    const float *features = nullptr;  // [B][5][N]
+    const float *potts = nullptr;
+    const float *compat = nullptr;
+    float *q_out = nullptr;           // the forward's Q_0..Q_T
+    float *grad_unary = nullptr;      // [B][M][N]
+    float *grad_potts = nullptr;      // [B][2] {dL/dw1, dL/dw2}
+    float *grad_compat = nullptr;     // [B][2][M][M]
+    float *grad_theta = nullptr;      // [B][7] dL/dtheta in dsrg_crf_params' order (image lattice only)
+    float *grad_features = nullptr;   // [B][5][N] dL/df
+    float *grad_theta_sp = nullptr;   // [B][2] dL/dtheta_gamma (features only)
+};
+// the training forward and its backward; at most DSRG_MAX_LABELS labels.  The backward needs e->compat_part with
+// compat (ensure_compat_part), and the kg_* buffers (ensure_kgrad) with grad_theta or features.
+int meanfield_run_train(Engine *e, int B, const CrfTrainIo &io, const dsrg_crf_params &p, cudaStream_t s);
+int meanfield_backward(Engine *e, int B, const CrfTrainIo &io, const dsrg_crf_params &p, cudaStream_t s);
+// NaN into every image b of p ([reps][B][per_image] floats) with bad[b] set; timed under tag
+void nan_images(Engine *e, const int *bad, float *p, int B, long long per_image, int reps, cudaStream_t s, int tag);
 // The energy of given marginals q [B][M][N] (DenseCRF::klDivergence) on the lattices the pass just built, at most
 // DSRG_MAX_LABELS labels: terms [B][4] {entropy, unary, spatial, bilateral} or, with grad_terms [B][4], its gradient
 // grad_q [B][M][N] and, if given, grad_unary.  unary may be nullptr; potts {w1, w2} or compat {mu_bi, mu_sp} [2][M][M]
@@ -196,17 +204,11 @@ int meanfield_run_wide(Engine *e, int B, const float *unary, int unary_layout, b
 int wide_weights(Engine *e, Lattice &L, int nb, cudaStream_t s);
 // the training forward and its backward above DSRG_MAX_LABELS labels, as meanfield_run_train / meanfield_backward
 // (potts or compat, not both); the backward needs e->wide_ppart, and with compat e->wide_g and e->wide_cpart
-// (ensure_wide).  The matrices' outer products are summed per image over kWideChunks fixed pixel chunks.  grad_theta,
-// or feat / grad_feat / grad_theta_sp, mean what they mean in meanfield_backward and need e->kg_csum, e->kg_part and
-// the 4-wide e->kg_sp / e->kg_bi (ensure_kgrad_wide)
+// (ensure_wide).  The matrices' outer products are summed per image over kWideChunks fixed pixel chunks.  grad_theta
+// or features need e->kg_csum, e->kg_part and the 4-wide e->kg_sp / e->kg_bi (ensure_kgrad_wide)
 constexpr int kWideChunks = 16;
-int meanfield_run_train_wide(Engine *e, int B, const float *unary, float *q_hist, const float *potts,
-                             const float *compat, const dsrg_crf_params &p, cudaStream_t s);
-int meanfield_backward_wide(Engine *e, int B, const float *q_hist, const float *potts, const float *compat,
-                            const float *grad_q, float *grad_unary, float *grad_potts, float *grad_compat,
-                            const dsrg_crf_params &p, cudaStream_t s, float *grad_theta = nullptr,
-                            const uint8_t *image = nullptr, const float *feat = nullptr, float *grad_feat = nullptr,
-                            float *grad_theta_sp = nullptr);
+int meanfield_run_train_wide(Engine *e, int B, const CrfTrainIo &io, const dsrg_crf_params &p, cudaStream_t s);
+int meanfield_backward_wide(Engine *e, int B, const CrfTrainIo &io, const dsrg_crf_params &p, cudaStream_t s);
 int meanfield_export(Engine *e, int B, float *out, int layout, cudaStream_t s);
 int meanfield_export_map(Engine *e, int B, int32_t *labels, cudaStream_t s);
 int meanfield_export_renorm(Engine *e, int B, float *result_out, float *log_out, cudaStream_t s);

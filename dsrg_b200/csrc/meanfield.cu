@@ -1814,19 +1814,20 @@ void kg_finish(Engine *e, const KgArgs &ka, int B, float *g_theta, int bgrid, cu
 }
 
 template <int MP>
-static int bwd_impl(Engine *e, int B, const float *q_hist, const float *potts, const float *G, float *gU,
-                    float *g_potts, const float *compat, float *g_compat, float *g_theta, const uint8_t *image,
-                    const float *feat, float *g_feat, float *g_theta_sp, const dsrg_crf_params &p, cudaStream_t s) {
+static int bwd_impl(Engine *e, int B, const CrfTrainIo &io, const dsrg_crf_params &p, cudaStream_t s) {
     const int M = e->M, N = e->N, T = p.n_iters;
     const size_t slab = (size_t)B * M * N;
+    const float *compat = io.compat, *feat = io.features;
+    float *g_feat = io.grad_features;
     if (T == 0) {
         if (g_feat) DSRG_CUDA_TRY(cudaMemsetAsync(g_feat, 0, sizeof(float) * 5 * N * B, s));
-        if (g_theta_sp) DSRG_CUDA_TRY(cudaMemsetAsync(g_theta_sp, 0, sizeof(float) * 2 * B, s));
+        if (io.grad_theta_sp) DSRG_CUDA_TRY(cudaMemsetAsync(io.grad_theta_sp, 0, sizeof(float) * 2 * B, s));
         DSRG_LAUNCH(e, T_MF_INIT, s,
-                    k_mf_softmax_vjp<<<dim3(cdiv(N, kThreads), B), kThreads, 0, s>>>(G, q_hist, gU, M, N));
-        if (g_potts) DSRG_CUDA_TRY(cudaMemsetAsync(g_potts, 0, sizeof(float) * 2 * B, s));
-        if (g_compat) DSRG_CUDA_TRY(cudaMemsetAsync(g_compat, 0, sizeof(float) * 2 * M * M * B, s));
-        if (g_theta) DSRG_CUDA_TRY(cudaMemsetAsync(g_theta, 0, sizeof(float) * 7 * B, s));
+                    k_mf_softmax_vjp<<<dim3(cdiv(N, kThreads), B), kThreads, 0, s>>>(io.grad_q, io.q_hist,
+                                                                                      io.grad_unary, M, N));
+        if (io.grad_potts) DSRG_CUDA_TRY(cudaMemsetAsync(io.grad_potts, 0, sizeof(float) * 2 * B, s));
+        if (io.grad_compat) DSRG_CUDA_TRY(cudaMemsetAsync(io.grad_compat, 0, sizeof(float) * 2 * M * M * B, s));
+        if (io.grad_theta) DSRG_CUDA_TRY(cudaMemsetAsync(io.grad_theta, 0, sizeof(float) * 7 * B, s));
         DSRG_CUDA_TRY(cudaGetLastError());
         return DSRG_OK;
     }
@@ -1855,16 +1856,16 @@ static int bwd_impl(Engine *e, int B, const float *q_hist, const float *potts, c
     DSRG_LAUNCH(e, T_MF_ZERO, s,
                 k_mf_zero<MP><<<bgrid, kThreads, 0, s>>>((float4 *)spY, e->sp.rowbase, (float4 *)biY, e->bi.rowbase, B));
     // the kernel-bandwidth gradient (g_theta): g_t stored by the launches (MODE_GSTORE), k_kg_pass per iteration;
-    // the feature gradient (g_feat) runs the same flow on the kgf kernels and keeps g_theta_sp for the spatial sums
-    if (g_feat) g_theta = g_theta_sp;
+    // the feature gradient (g_feat) runs the same flow on the kgf kernels and keeps grad_theta_sp for the spatial sums
+    float *g_theta = g_feat ? io.grad_theta_sp : io.grad_theta;
     const bool kg = g_theta || g_feat;
     const int kg_tag = g_feat ? T_FGRAD : T_KGRAD;
     KgArgs ka{};
     if (kg) {
         ka.sp = kg_lat(e->sp);
         ka.bi = kg_lat(e->bi);
-        ka.image = image;
-        ka.potts = compat ? compat : potts;
+        ka.image = io.image;
+        ka.potts = compat ? compat : io.potts;
         ka.w1 = p.w1;
         ka.w2 = p.w2;
         ka.part = e->kg_part;
@@ -1876,16 +1877,16 @@ static int bwd_impl(Engine *e, int B, const float *q_hist, const float *potts, c
     }
 #define DSRG_BWD_LAUNCH_AT(MODEV, WP, PART, SMEM)                                                                     \
     DSRG_LAUNCH(e, T_MF_TILE, s,                                                                                      \
-                (k_mf_tile_bwd<MP, MODEV><<<gt, kTileThreads, SMEM, s>>>(G, qt, gU, vsp, vbi, a_sp, a_bi, WP, p.w1,    \
-                                                                        p.w2, PART, M, N, e->W, e->H,                 \
+                (k_mf_tile_bwd<MP, MODEV><<<gt, kTileThreads, SMEM, s>>>(io.grad_q, qt, io.grad_unary, vsp, vbi, a_sp, \
+                                                                        a_bi, WP, p.w1, p.w2, PART, M, N, e->W, e->H, \
                                                                         e->tiles_x, e->ntiles, e->tile_w,             \
                                                                         ((MODEV) & MODE_GSTORE) ? e->kg_g : nullptr)))
-#define DSRG_BWD_LAUNCH(MODEV) DSRG_BWD_LAUNCH_AT(MODEV, potts, e->potts_part, smem)
+#define DSRG_BWD_LAUNCH(MODEV) DSRG_BWD_LAUNCH_AT(MODEV, io.potts, e->potts_part, smem)
 #define DSRG_BWD_LAUNCH_COMPAT(MODEV)                                                                                 \
     DSRG_BWD_LAUNCH_AT(MODEV | MODE_COMPAT, compat, reinterpret_cast<float2 *>(e->compat_part), smem_c)
     for (int it = T; it >= 0; it--) {
         const TileLat vsp = make_tile_view(e->sp, spX, spY), vbi = make_tile_view(e->bi, biX, biY);
-        const float *qt = q_hist + (size_t)it * slab;
+        const float *qt = io.q_hist + (size_t)it * slab;
         if (kg && it < T)
             kg_iter<MP>(e, ka, compat != nullptr, B, qt, spX, biX, it == T - 1, bgrid, s, feat, g_feat, kg_tag);
         if (compat) {
@@ -1926,18 +1927,18 @@ static int bwd_impl(Engine *e, int B, const float *q_hist, const float *potts, c
 #undef DSRG_BWD_LAUNCH_COMPAT
 #undef DSRG_BWD_LAUNCH
 #undef DSRG_BWD_LAUNCH_AT
-    if (g_compat) compat_reduce(e, e->compat_part, g_compat, e->ntiles, 2 * M * M, B, T_MF_EXPORT, s);
-    if (g_potts) potts_reduce(e, e->potts_part, g_potts, e->ntiles, B, T_MF_EXPORT, s);
+    if (io.grad_compat) compat_reduce(e, e->compat_part, io.grad_compat, e->ntiles, 2 * M * M, B, T_MF_EXPORT, s);
+    if (io.grad_potts) potts_reduce(e, e->potts_part, io.grad_potts, e->ntiles, B, T_MF_EXPORT, s);
     if (kg) kg_finish(e, ka, B, g_theta, bgrid, s, feat, g_feat, kg_tag);
     DSRG_CUDA_TRY(cudaGetLastError());
     return DSRG_OK;
 }
 
-int meanfield_run_train(Engine *e, int B, const float *unary, float *q_hist, const float *potts, const float *compat,
-                        const dsrg_crf_params &p, cudaStream_t s) {
+int meanfield_run_train(Engine *e, int B, const CrfTrainIo &io, const dsrg_crf_params &p, cudaStream_t s) {
     switch (e->MP) {
 #define DSRG_CASE(MPV) \
-    case MPV: return run_impl<MPV>(e, B, unary, DSRG_LAYOUT_NCHW, false, nullptr, p, s, q_hist, potts, compat);
+    case MPV:          \
+        return run_impl<MPV>(e, B, io.unary, DSRG_LAYOUT_NCHW, false, nullptr, p, s, io.q_out, io.potts, io.compat);
         DSRG_CASE(4) DSRG_CASE(8) DSRG_CASE(12) DSRG_CASE(16) DSRG_CASE(20) DSRG_CASE(24) DSRG_CASE(28) DSRG_CASE(32)
 #undef DSRG_CASE
     }
@@ -1945,15 +1946,10 @@ int meanfield_run_train(Engine *e, int B, const float *unary, float *q_hist, con
     return DSRG_E_INVALID;
 }
 
-int meanfield_backward(Engine *e, int B, const float *q_hist, const float *potts, const float *grad_q,
-                       float *grad_unary, float *grad_potts, const float *compat, float *grad_compat,
-                       const dsrg_crf_params &p, cudaStream_t s, float *grad_theta, const uint8_t *image,
-                       const float *feat, float *grad_feat, float *grad_theta_sp) {
+int meanfield_backward(Engine *e, int B, const CrfTrainIo &io, const dsrg_crf_params &p, cudaStream_t s) {
     switch (e->MP) {
-#define DSRG_CASE(MPV)                                                                                        \
-    case MPV:                                                                                                 \
-        return bwd_impl<MPV>(e, B, q_hist, potts, grad_q, grad_unary, grad_potts, compat, grad_compat, grad_theta, \
-                             image, feat, grad_feat, grad_theta_sp, p, s);
+#define DSRG_CASE(MPV) \
+    case MPV: return bwd_impl<MPV>(e, B, io, p, s);
         DSRG_CASE(4) DSRG_CASE(8) DSRG_CASE(12) DSRG_CASE(16) DSRG_CASE(20) DSRG_CASE(24) DSRG_CASE(28) DSRG_CASE(32)
 #undef DSRG_CASE
     }
@@ -1961,11 +1957,10 @@ int meanfield_backward(Engine *e, int B, const float *q_hist, const float *potts
     return DSRG_E_INVALID;
 }
 
-void nan_images(Engine *e, const int *bad, float *p, int B, long long per_image, int reps, long long rep_stride,
-                cudaStream_t s, int tag) {
+void nan_images(Engine *e, const int *bad, float *p, int B, long long per_image, int reps, cudaStream_t s, int tag) {
     const int nblk = cdiv(per_image, kThreads);
     const dim3 gp(nblk < 64 ? nblk : 64, B, reps);
-    DSRG_LAUNCH(e, tag, s, k_nan_images<<<gp, kThreads, 0, s>>>(bad, p, per_image, rep_stride));
+    DSRG_LAUNCH(e, tag, s, k_nan_images<<<gp, kThreads, 0, s>>>(bad, p, per_image, B * per_image));
 }
 
 void potts_reduce(Engine *e, const float2 *part, float *out, int nparts, int B, int tag, cudaStream_t s) {

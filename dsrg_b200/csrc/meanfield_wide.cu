@@ -601,9 +601,10 @@ static void wide_filter(Engine *e, int B, const float *X, bool reverse, int tag,
 
 static float wide_alpha(const Lattice &L) { return 1.0f / (1 + powf(2, -L.d)); }   // permutohedral.cpp:571
 
-int meanfield_run_train_wide(Engine *e, int B, const float *unary, float *q_hist, const float *potts,
-                             const float *compat, const dsrg_crf_params &p, cudaStream_t s) {
+int meanfield_run_train_wide(Engine *e, int B, const CrfTrainIo &io, const dsrg_crf_params &p, cudaStream_t s) {
     const int M = e->M, N = e->N, CH = e->MP / 4, T = p.n_iters;
+    const float *unary = io.unary, *potts = io.potts, *compat = io.compat;
+    float *q_hist = io.q_out;
     const size_t slab = (size_t)B * M * N;
     const dim3 gp(cdiv(N, kThreads), B), gq(cdiv(N, kThreads), CH, B);
     const float a_sp = wide_alpha(e->sp), a_bi = wide_alpha(e->bi);
@@ -628,25 +629,24 @@ int meanfield_run_train_wide(Engine *e, int B, const float *unary, float *q_hist
     return DSRG_OK;
 }
 
-int meanfield_backward_wide(Engine *e, int B, const float *q_hist, const float *potts, const float *compat,
-                            const float *grad_q, float *grad_unary, float *grad_potts, float *grad_compat,
-                            const dsrg_crf_params &p, cudaStream_t s, float *grad_theta, const uint8_t *image,
-                            const float *feat, float *grad_feat, float *grad_theta_sp) {
+int meanfield_backward_wide(Engine *e, int B, const CrfTrainIo &io, const dsrg_crf_params &p, cudaStream_t s) {
     const int M = e->M, N = e->N, CH = e->MP / 4, T = p.n_iters;
+    const float *q_hist = io.q_hist, *potts = io.potts, *compat = io.compat, *feat = io.features;
+    float *grad_feat = io.grad_features;
     const size_t slab = (size_t)B * M * N;
     const int nblk = cdiv(N, kThreads);
     const dim3 gp(nblk, B), gq(nblk, CH, B);
     const float a_sp = wide_alpha(e->sp), a_bi = wide_alpha(e->bi);
     // the kernel-bandwidth gradient (grad_theta), or the feature gradient (grad_feat) with the spatial sums to
     // grad_theta_sp: per iteration Vy into the buffers Vg leaves free and k_wide_kg_pass, kg_finish after the loop
-    if (grad_feat) grad_theta = grad_theta_sp;
+    float *grad_theta = grad_feat ? io.grad_theta_sp : io.grad_theta;
     const bool kg = grad_theta || grad_feat;
     const int kg_tag = grad_feat ? T_FGRAD : T_KGRAD;
     KgArgs ka{};
     if (kg) {
         ka.sp = kg_lat(e->sp);
         ka.bi = kg_lat(e->bi);
-        ka.image = image;
+        ka.image = io.image;
         ka.potts = compat ? nullptr : potts;
         ka.w1 = compat ? 1.0f : p.w1;   // the matrices' x and u carry mu
         ka.w2 = compat ? 1.0f : p.w2;
@@ -660,13 +660,13 @@ int meanfield_backward_wide(Engine *e, int B, const float *q_hist, const float *
     // e->Q0: g_t, then S_sp (matrices) or G_{t-1} (Potts); e->U: S_bi; e->wide_g: the matrices' G_{t-1}.  With kg and
     // matrices, e->U and e->wide_g hold x and u of one lattice before the slice (G_t was read by the VJP by then).
     float *X = e->Q0;
-    const float *G = grad_q;
+    const float *G = io.grad_q;
     const int tl = (M + kWideOuterTile - 1) / kWideOuterTile;
     const int chunk_px = cdiv(cdiv(N, kWideChunks), kWideOuterTile) * kWideOuterTile;
     for (int it = T; it > 0; it--) {
         const float *qt = q_hist + (size_t)it * slab, *qp = q_hist + (size_t)(it - 1) * slab;
         const int first = it == T;
-        DSRG_LAUNCH(e, T_WIDE_GRAD, s, k_wide_vjp<<<gp, kThreads, 0, s>>>(G, qt, grad_unary, X, first, M, N));
+        DSRG_LAUNCH(e, T_WIDE_GRAD, s, k_wide_vjp<<<gp, kThreads, 0, s>>>(G, qt, io.grad_unary, X, first, M, N));
         float *spV, *biV;
         wide_filter(e, B, X, true, T_WIDE_GRAD, s, &spV, &biV);
         if (kg) {
@@ -704,7 +704,7 @@ int meanfield_backward_wide(Engine *e, int B, const float *q_hist, const float *
             DSRG_LAUNCH(e, T_WIDE_GRAD, s, k_wide_slice_planar<<<gq, kThreads, 0, s>>>(X, e->U, sp, bi, a_sp, a_bi, M, N, CH));
             DSRG_LAUNCH(e, T_WIDE_GRAD, s,
                         k_wide_compat_msg<true><<<gq, kThreads, 8 * M * sizeof(float), s>>>(nullptr, X, e->U, compat, e->wide_g, M, N));
-            if (grad_compat)
+            if (io.grad_compat)
                 DSRG_LAUNCH(e, T_WIDE_GRAD, s,
                             k_wide_outer<<<dim3(tl * tl, 2 * kWideChunks, B), kThreads, 0, s>>>(X, e->U, qp, e->wide_cpart,
                                                                                                first, M, N, chunk_px));
@@ -716,17 +716,17 @@ int meanfield_backward_wide(Engine *e, int B, const float *q_hist, const float *
             G = X;
         }
     }
-    DSRG_LAUNCH(e, T_WIDE_GRAD, s, k_wide_vjp<<<gp, kThreads, 0, s>>>(G, q_hist, grad_unary, nullptr, T == 0, M, N));
+    DSRG_LAUNCH(e, T_WIDE_GRAD, s, k_wide_vjp<<<gp, kThreads, 0, s>>>(G, q_hist, io.grad_unary, nullptr, T == 0, M, N));
     if (T == 0) {
-        if (grad_potts) DSRG_CUDA_TRY(cudaMemsetAsync(grad_potts, 0, sizeof(float) * 2 * B, s));
-        if (grad_compat) DSRG_CUDA_TRY(cudaMemsetAsync(grad_compat, 0, sizeof(float) * 2 * M * M * B, s));
+        if (io.grad_potts) DSRG_CUDA_TRY(cudaMemsetAsync(io.grad_potts, 0, sizeof(float) * 2 * B, s));
+        if (io.grad_compat) DSRG_CUDA_TRY(cudaMemsetAsync(io.grad_compat, 0, sizeof(float) * 2 * M * M * B, s));
         if (grad_feat) DSRG_CUDA_TRY(cudaMemsetAsync(grad_feat, 0, sizeof(float) * 5 * N * B, s));
         if (grad_theta) DSRG_CUDA_TRY(cudaMemsetAsync(grad_theta, 0, sizeof(float) * (grad_feat ? 2 : 7) * B, s));
     } else {
-        if (grad_potts) {
-            potts_reduce(e, e->wide_ppart, grad_potts, CH * nblk, B, T_WIDE_GRAD, s);
-        } else if (grad_compat) {
-            compat_reduce(e, e->wide_cpart, grad_compat, kWideChunks, 2 * M * M, B, T_WIDE_GRAD, s);
+        if (io.grad_potts) {
+            potts_reduce(e, e->wide_ppart, io.grad_potts, CH * nblk, B, T_WIDE_GRAD, s);
+        } else if (io.grad_compat) {
+            compat_reduce(e, e->wide_cpart, io.grad_compat, kWideChunks, 2 * M * M, B, T_WIDE_GRAD, s);
         }
         if (kg) kg_finish(e, ka, B, grad_theta, 8 * e->sm_count, s, feat, grad_feat, kg_tag);
     }

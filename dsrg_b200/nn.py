@@ -354,129 +354,6 @@ def _potts_weight(w, name, ref):
     return w
 
 
-class _DenseCrf(torch.autograd.Function):
-    @staticmethod
-    @_fwd
-    def forward(ctx, unary, image, w1, w2, scale_factor, color_factor, maxiter):
-        eng = _engine_for(unary)
-        s = _stream(unary)
-        params = api.crf_params(scale_factor, color_factor, maxiter)
-        potts = None
-        if w1 is not None or w2 is not None:   # the kernels read both weights from here (no host synchronisation)
-            potts = torch.empty(2, dtype=torch.float32, device=unary.device)
-            for i, (w, d) in enumerate(zip((w1, w2), _POTTS_DEFAULT)):
-                if w is None:
-                    potts[i].fill_(d)
-                else:
-                    potts[i].copy_(w.detach())
-        q_hist = torch.empty((maxiter + 1,) + tuple(unary.shape), dtype=torch.float32, device=unary.device)
-        eng.crf_forward_train_dev(unary, image, params, q_hist, potts=potts, stream=s)
-        ctx.save_for_backward(q_hist, image, potts)
-        ctx.params = params
-        return q_hist[maxiter].clone()
-
-    @staticmethod
-    @_bwd
-    def backward(ctx, g):
-        q_hist, image, potts = ctx.saved_tensors
-        grad_u = torch.empty(q_hist.shape[1:], dtype=torch.float32, device=q_hist.device)
-        grad_potts = None
-        if potts is not None and (ctx.needs_input_grad[2] or ctx.needs_input_grad[3]):
-            grad_potts = torch.empty((q_hist.shape[1], 2), dtype=torch.float32, device=q_hist.device)
-        _engine_for(grad_u).crf_backward_dev(q_hist, image, ctx.params, g.contiguous(), grad_u, grad_potts=grad_potts,
-                                             potts=potts, stream=_stream(grad_u))
-        gw1 = grad_potts[:, 0].sum() if grad_potts is not None and ctx.needs_input_grad[2] else None
-        gw2 = grad_potts[:, 1].sum() if grad_potts is not None and ctx.needs_input_grad[3] else None
-        return grad_u, None, gw1, gw2, None, None, None
-
-
-class _DenseCrfCompat(torch.autograd.Function):
-    """dense_crf with compatibility matrices: compat (2, M, M) float32 {mu_bi, mu_sp}."""
-
-    @staticmethod
-    @_fwd
-    def forward(ctx, unary, image, compat, scale_factor, color_factor, maxiter):
-        eng = _engine_for(unary)
-        params = api.crf_params(scale_factor, color_factor, maxiter)
-        q_hist = torch.empty((maxiter + 1,) + tuple(unary.shape), dtype=torch.float32, device=unary.device)
-        eng.crf_forward_train_compat_dev(unary, image, params, compat, q_hist, stream=_stream(unary))
-        ctx.save_for_backward(q_hist, image, compat)
-        ctx.params = params
-        return q_hist[maxiter].clone()
-
-    @staticmethod
-    @_bwd
-    def backward(ctx, g):
-        q_hist, image, compat = ctx.saved_tensors
-        grad_u = torch.empty(q_hist.shape[1:], dtype=torch.float32, device=q_hist.device)
-        grad_c = None
-        if ctx.needs_input_grad[2]:
-            M = compat.shape[-1]
-            grad_c = torch.empty((q_hist.shape[1], 2, M, M), dtype=torch.float32, device=q_hist.device)
-        _engine_for(grad_u).crf_backward_compat_dev(q_hist, image, ctx.params, compat, g.contiguous(), grad_u,
-                                                    grad_compat=grad_c, stream=_stream(grad_u))
-        return grad_u, None, None if grad_c is None else grad_c.sum(0), None, None, None
-
-
-class _DenseCrfTheta(torch.autograd.Function):
-    """dense_crf with learnable kernel bandwidths: theta_bi (5,), theta_sp (2,) (None: params' own values) beside
-    the Potts weights (w1, w2) or the matrices (compat (2, M, M) {mu_bi, mu_sp}); params carries the sigmas.  wide: the
-    label-chunked entry points (dense_crf_wide above 32 labels) in place of the fused ones."""
-
-    @staticmethod
-    @_fwd
-    def forward(ctx, unary, image, w1, w2, compat, theta_bi, theta_sp, params, wide):
-        eng = _engine_for(unary)
-        s = _stream(unary)
-        maxiter = params.n_iters
-        q_hist = torch.empty((maxiter + 1,) + tuple(unary.shape), dtype=torch.float32, device=unary.device)
-        potts = _potts_tensor(w1, w2, unary) if compat is None else None
-        if wide:
-            eng.crf_forward_train_wide_dev(unary, image, params, q_hist, potts=potts, compat=compat, stream=s)
-        elif compat is not None:
-            eng.crf_forward_train_compat_dev(unary, image, params, compat, q_hist, stream=s)
-        else:
-            eng.crf_forward_train_dev(unary, image, params, q_hist, potts=potts, stream=s)
-        ctx.save_for_backward(q_hist, image, potts, compat)
-        ctx.params = params
-        ctx.wide = wide
-        ctx.theta = [(t.device, t.dtype) if t is not None else None for t in (theta_bi, theta_sp)]
-        return q_hist[maxiter].clone()
-
-    @staticmethod
-    @_bwd
-    def backward(ctx, g):
-        q_hist, image, potts, compat = ctx.saved_tensors
-        B, dev = q_hist.shape[1], q_hist.device
-        need = ctx.needs_input_grad
-        grad_u = torch.empty(q_hist.shape[1:], dtype=torch.float32, device=dev)
-        grad_t = torch.empty((B, 7), dtype=torch.float32, device=dev)
-        eng, s = _engine_for(grad_u), _stream(grad_u)
-        grad_potts = grad_c = None
-        if potts is not None and (need[2] or need[3]):
-            grad_potts = torch.empty((B, 2), dtype=torch.float32, device=dev)
-        if compat is not None and need[4]:
-            M = compat.shape[-1]
-            grad_c = torch.empty((B, 2, M, M), dtype=torch.float32, device=dev)
-        if ctx.wide:
-            eng.crf_backward_wide_theta_dev(q_hist, image, ctx.params, g.contiguous(), grad_u, grad_t, potts=potts,
-                                            compat=compat, grad_potts=grad_potts, grad_compat=grad_c, stream=s)
-        elif compat is not None:
-            eng.crf_backward_compat_theta_dev(q_hist, image, ctx.params, compat, g.contiguous(), grad_u, grad_t,
-                                              grad_compat=grad_c, stream=s)
-        else:
-            eng.crf_backward_theta_dev(q_hist, image, ctx.params, g.contiguous(), grad_u, grad_t,
-                                       grad_potts=grad_potts, potts=potts, stream=s)
-        gw1 = grad_potts[:, 0].sum() if grad_potts is not None and need[2] else None
-        gw2 = grad_potts[:, 1].sum() if grad_potts is not None and need[3] else None
-        gc = None if grad_c is None else grad_c.sum(0)
-        gt = grad_t.sum(0)
-        out = []
-        for part, spec, n in ((gt[0:5], ctx.theta[0], need[5]), (gt[5:7], ctx.theta[1], need[6])):
-            out.append(part.to(spec[0], spec[1]) if spec is not None and n else None)
-        return grad_u, None, gw1, gw2, gc, out[0], out[1], None, None
-
-
 def _potts_tensor(w1, w2, ref):
     """The device {w1, w2} the kernels read in place of params' weights (a None one is CRF()'s), or None for both."""
     if w1 is None and w2 is None:
@@ -490,86 +367,93 @@ def _potts_tensor(w1, w2, ref):
     return potts
 
 
-class _DenseCrfFeat(torch.autograd.Function):
-    """dense_crf with caller-given bilateral features: features (N, 5, H, W) float32 beside the Potts weights (w1, w2)
-    or the matrices (compat (2, M, M) {mu_bi, mu_sp}), and an optional learnable theta_sp; params carries the spatial
-    sigmas.  Nothing is read on the host.  wide: the label-chunked entry points (dense_crf_wide above 32 labels)."""
+def _train_entry(wide, feat, compat, theta):
+    """The Engine methods (forward, backward) of one differentiable CRF call: the label-chunked path (wide) or the
+    fused one, on caller-given features (feat) or the image, with the matrices (compat) or the Potts weights, and
+    with a given theta (on the image path its backward also writes dL/dtheta; the features carry theta_sp's)."""
+    if feat:
+        return (("crf_forward_train_wide_feat_dev", "crf_backward_wide_feat_dev") if wide
+                else ("crf_forward_train_feat_dev", "crf_backward_feat_dev"))
+    if wide:
+        return "crf_forward_train_wide_dev", "crf_backward_wide_theta_dev" if theta else "crf_backward_wide_dev"
+    if compat:
+        return "crf_forward_train_compat_dev", "crf_backward_compat_theta_dev" if theta else "crf_backward_compat_dev"
+    return "crf_forward_train_dev", "crf_backward_theta_dev" if theta else "crf_backward_dev"
+
+
+class _DenseCrfTrain(torch.autograd.Function):
+    """dense_crf / dense_crf_wide on the image's lattice or on caller-given features (x, feat), with the Potts weights
+    (w1, w2) or the matrices (compat (2, M, M) {mu_bi, mu_sp}), and learnable bandwidths theta_bi (5,) / theta_sp (2,)
+    whose values params already carries.  wide: the label-chunked entry points above 32 labels."""
 
     @staticmethod
     @_fwd
-    def forward(ctx, unary, features, w1, w2, compat, theta_sp, params, wide):
-        eng = _engine_for(unary)
-        maxiter = params.n_iters
-        q_hist = torch.empty((maxiter + 1,) + tuple(unary.shape), dtype=torch.float32, device=unary.device)
-        potts = _potts_tensor(w1, w2, unary) if compat is None else None
-        fwd = eng.crf_forward_train_wide_feat_dev if wide else eng.crf_forward_train_feat_dev
-        fwd(unary, features, params, q_hist, potts=potts, compat=compat, stream=_stream(unary))
-        ctx.save_for_backward(q_hist, features, potts, compat)
-        ctx.params = params
-        ctx.wide = wide
-        ctx.theta_sp = None if theta_sp is None else (theta_sp.device, theta_sp.dtype)
-        return q_hist[maxiter].clone()
+    def forward(ctx, unary, x, w1, w2, compat, theta_bi, theta_sp, params, wide, feat):
+        fwd, ctx.bwd = _train_entry(wide, feat, compat is not None, theta_bi is not None or theta_sp is not None)
+        q_hist = torch.empty((params.n_iters + 1,) + tuple(unary.shape), dtype=torch.float32, device=unary.device)
+        potts = _potts_tensor(w1, w2, unary)
+        weights = {"potts": potts} if compat is None else {"compat": compat}
+        getattr(_engine_for(unary), fwd)(unary, x, params, q_hist=q_hist, stream=_stream(unary), **weights)
+        ctx.save_for_backward(q_hist, x, potts, compat)
+        ctx.params, ctx.feat = params, feat
+        ctx.theta = [(t.device, t.dtype) if t is not None else None for t in (theta_bi, theta_sp)]
+        return q_hist[params.n_iters].clone()
 
     @staticmethod
     @_bwd
     def backward(ctx, g):
-        q_hist, features, potts, compat = ctx.saved_tensors
-        B, dev = q_hist.shape[1], q_hist.device
+        q_hist, x, potts, compat = ctx.saved_tensors
         need = ctx.needs_input_grad
-        grad_u = torch.empty(q_hist.shape[1:], dtype=torch.float32, device=dev)
-        grad_f = torch.empty_like(features)
-        grad_potts = grad_c = grad_tsp = None
-        if potts is not None and (need[2] or need[3]):
-            grad_potts = torch.empty((B, 2), dtype=torch.float32, device=dev)
-        if compat is not None and need[4]:
-            M = compat.shape[-1]
-            grad_c = torch.empty((B, 2, M, M), dtype=torch.float32, device=dev)
-        if ctx.theta_sp is not None and need[5]:
-            grad_tsp = torch.empty((B, 2), dtype=torch.float32, device=dev)
-        eng = _engine_for(grad_u)
-        bwd = eng.crf_backward_wide_feat_dev if ctx.wide else eng.crf_backward_feat_dev
-        bwd(q_hist, features, ctx.params, g.contiguous(), grad_u, grad_f, potts=potts, compat=compat,
-            grad_potts=grad_potts, grad_compat=grad_c, grad_theta_sp=grad_tsp, stream=_stream(grad_u))
+        B, f32 = q_hist.shape[1], {"dtype": torch.float32, "device": q_hist.device}
+        grad_u = torch.empty(q_hist.shape[1:], **f32)
+        # the backward's optional arguments, by keyword
+        if compat is None:
+            kw = {"potts": potts, "grad_potts": None}
+            if potts is not None and (need[2] or need[3]):
+                kw["grad_potts"] = torch.empty((B, 2), **f32)
+        else:
+            kw = {"compat": compat, "grad_compat": torch.empty((B, 2) + compat.shape[1:], **f32) if need[4] else None}
+        if ctx.feat:
+            kw["grad_features"] = torch.empty_like(x)
+            if ctx.theta[1] is not None and need[6]:
+                kw["grad_theta_sp"] = torch.empty((B, 2), **f32)
+        elif ctx.theta != [None, None]:   # a given theta's backward writes dL/dtheta whether or not it is needed
+            kw["grad_theta"] = torch.empty((B, 7), **f32)
+        getattr(_engine_for(grad_u), ctx.bwd)(q_hist, x, ctx.params, grad_q=g.contiguous(), grad_unary=grad_u,
+                                               stream=_stream(grad_u), **kw)
+        grad_potts, grad_c = kw.get("grad_potts"), kw.get("grad_compat")
         gw1 = grad_potts[:, 0].sum() if grad_potts is not None and need[2] else None
         gw2 = grad_potts[:, 1].sum() if grad_potts is not None and need[3] else None
         gc = None if grad_c is None else grad_c.sum(0)
-        gt = None if grad_tsp is None else grad_tsp.sum(0).to(ctx.theta_sp[0], ctx.theta_sp[1])
-        return grad_u, grad_f if need[1] else None, gw1, gw2, gc, gt, None, None
+        gt = (None, None)
+        if "grad_theta" in kw:
+            gt = kw["grad_theta"].sum(0)
+            gt = (gt[0:5], gt[5:7])
+        elif "grad_theta_sp" in kw:
+            gt = (None, kw["grad_theta_sp"].sum(0))
+        gt = [t.to(spec[0], spec[1]) if t is not None and spec is not None and n else None
+              for t, spec, n in zip(gt, ctx.theta, need[5:7])]
+        gx = kw["grad_features"] if ctx.feat and need[1] else None
+        return grad_u, gx, gw1, gw2, gc, gt[0], gt[1], None, None, None
 
 
-def _features(t, ref):
-    """The bilateral features (N, 5, H, W) float32 on ref's device, made contiguous."""
-    N, _, H, W = ref.shape
+def _features(t, N, H, W, device):
+    """The bilateral features (N, 5, H, W) float32 on `device`, made contiguous."""
     if (not isinstance(t, torch.Tensor) or t.dtype != torch.float32 or tuple(t.shape) != (N, 5, H, W)
-            or t.device != ref.device):
+            or t.device != device):
         raise ValueError("features_bi must be a (%d, 5, %d, %d) float32 tensor on %s (got %r)"
-                         % (N, H, W, ref.device,
+                         % (N, H, W, device,
                             t if not isinstance(t, torch.Tensor) else (t.dtype, tuple(t.shape), t.device)))
     return t.contiguous()
 
 
-def _dense_crf_feat(u, image, features_bi, scale_factor, color_factor, maxiter, w1, w2, compat_bi, compat_sp,
-                    theta_bi, theta_sp, wide=False):
-    """dense_crf's path with caller-given bilateral features; every check before the first launch.  wide: the
-    label-chunked entry points (dense_crf_wide above 32 labels)."""
-    if image is not None:
-        raise ValueError("image is not used when features_bi is given: pass None")
-    if theta_bi is not None:
-        raise ValueError("theta_bi and features_bi are two forms of the bilateral features: give one of them")
-    f = _features(features_bi, u)
-    th_sp = _theta_values(theta_sp, "theta_sp", 2, u)
-    _cuda(u, "unary")
-    w1, w2 = _potts_weight(w1, "w1", u), _potts_weight(w2, "w2", u)
-    if int(maxiter) < 0:
-        raise ValueError("maxiter must be >= 0 (got %d)" % maxiter)
-    params = api.crf_params(float(scale_factor), float(color_factor), int(maxiter))
-    if th_sp is not None:
-        params.theta_gamma_x, params.theta_gamma_y = th_sp
-    compat = None
-    if compat_bi is not None or compat_sp is not None:
-        compat = _compat_stack(u, u.shape[1], w1, w2, compat_bi, compat_sp)
-        w1 = w2 = None
-    return _DenseCrfFeat.apply(u, f, w1, w2, compat, theta_sp, params, wide)
+def _image(t, ref):
+    """The image (N, H, W, 3) uint8 at ref's map size and on its device, made contiguous."""
+    N, _, H, W = ref.shape
+    if not isinstance(t, torch.Tensor) or t.dtype != torch.uint8 or tuple(t.shape) != (N, H, W, 3) \
+            or t.device != ref.device:
+        raise ValueError("image must be a (%d, %d, %d, 3) uint8 tensor on %s" % (N, H, W, ref.device))
+    return t.contiguous()
 
 
 def _theta_values(theta, name, n, ref):
@@ -592,6 +476,16 @@ def _theta_values(theta, name, n, ref):
     return v
 
 
+def _set_theta(params, th_bi, th_sp):
+    """params with the values of a given theta_bi / theta_sp in place of its sigmas."""
+    if th_bi is not None:
+        (params.theta_alpha_x, params.theta_alpha_y, params.theta_beta_r, params.theta_beta_g,
+         params.theta_beta_b) = th_bi
+    if th_sp is not None:
+        params.theta_gamma_x, params.theta_gamma_y = th_sp
+    return params
+
+
 def _compat_matrix(mu, name, ref, M):
     if not isinstance(mu, torch.Tensor) or tuple(mu.shape) != (M, M) or not mu.is_floating_point() \
             or mu.device != ref.device:
@@ -599,6 +493,41 @@ def _compat_matrix(mu, name, ref, M):
                          % (name, M, M, ref.device,
                             mu if not isinstance(mu, torch.Tensor) else (mu.dtype, tuple(mu.shape), mu.device)))
     return mu.float()
+
+
+def _train_args(unary, image, scale_factor, color_factor, maxiter, w1, w2, compat_bi, compat_sp, theta_bi, theta_sp,
+                features_bi, wide):
+    """dense_crf's and dense_crf_wide's arguments, every check before the first launch -> the arguments of
+    _DenseCrfTrain.  wide: dense_crf_wide, which takes any label count and runs 32 or fewer as dense_crf does."""
+    if torch.is_autocast_enabled("cuda"):   # what custom_fwd(cast_inputs=float32) does, before the checks
+        unary = unary.float() if isinstance(unary, torch.Tensor) and unary.is_floating_point() else unary
+        if isinstance(features_bi, torch.Tensor) and features_bi.is_floating_point():
+            features_bi = features_bi.float()
+    u = _maps(unary, "unary")
+    N, M, H, W = u.shape
+    if not wide and M > FUSED_LABELS:
+        raise ValueError("dense_crf supports at most %d labels (got %d); dense_crf_wide takes up to %d"
+                         % (FUSED_LABELS, M, MAX_LABELS))
+    feat = features_bi is not None
+    if feat:
+        if image is not None:
+            raise ValueError("image is not used when features_bi is given: pass None")
+        if theta_bi is not None:
+            raise ValueError("theta_bi and features_bi are two forms of the bilateral features: give one of them")
+        x = _features(features_bi, N, H, W, u.device)
+    else:
+        x = _image(image, u)
+    th_bi, th_sp = _theta_values(theta_bi, "theta_bi", 5, u), _theta_values(theta_sp, "theta_sp", 2, u)
+    _cuda(u, "unary")
+    w1, w2 = _potts_weight(w1, "w1", u), _potts_weight(w2, "w2", u)
+    if int(maxiter) < 0:
+        raise ValueError("maxiter must be >= 0 (got %d)" % maxiter)
+    params = _set_theta(api.crf_params(float(scale_factor), float(color_factor), int(maxiter)), th_bi, th_sp)
+    compat = None
+    if compat_bi is not None or compat_sp is not None:
+        compat = _compat_stack(u, M, w1, w2, compat_bi, compat_sp)
+        w1 = w2 = None
+    return u, x, w1, w2, compat, theta_bi, theta_sp, params, M > FUSED_LABELS, feat
 
 
 def dense_crf(unary, image, scale_factor=1.0, color_factor=13, maxiter=10, w1=None, w2=None, compat_bi=None,
@@ -633,42 +562,8 @@ def dense_crf(unary, image, scale_factor=1.0, color_factor=13, maxiter=10, w1=No
     features are never read on the host: without theta_sp a step can be captured in a CUDA graph.  Keep every feature
     within +-150 (the CRF does not change when a channel is shifted, so centre them): an image whose lattice keys leave
     the packed range gets NaN marginals and gradients (Engine.feature_range_flags names it)."""
-    if torch.is_autocast_enabled("cuda"):   # what custom_fwd(cast_inputs=float32) does, before the checks
-        unary = unary.float() if isinstance(unary, torch.Tensor) and unary.is_floating_point() else unary
-        if isinstance(features_bi, torch.Tensor) and features_bi.is_floating_point():
-            features_bi = features_bi.float()
-    u = _maps(unary, "unary")
-    N, M, H, W = u.shape
-    if M > FUSED_LABELS:
-        raise ValueError("dense_crf supports at most %d labels (got %d); dense_crf_wide takes up to %d"
-                         % (FUSED_LABELS, M, MAX_LABELS))
-    if features_bi is not None:
-        return _dense_crf_feat(u, image, features_bi, scale_factor, color_factor, maxiter, w1, w2, compat_bi,
-                               compat_sp, theta_bi, theta_sp)
-    if (not isinstance(image, torch.Tensor) or image.dtype != torch.uint8 or tuple(image.shape) != (N, H, W, 3)
-            or image.device != u.device):
-        raise ValueError("image must be a (%d, %d, %d, 3) uint8 tensor on %s" % (N, H, W, u.device))
-    th_bi, th_sp = _theta_values(theta_bi, "theta_bi", 5, u), _theta_values(theta_sp, "theta_sp", 2, u)
-    _cuda(u, "unary")
-    w1, w2 = _potts_weight(w1, "w1", u), _potts_weight(w2, "w2", u)
-    if int(maxiter) < 0:
-        raise ValueError("maxiter must be >= 0 (got %d)" % maxiter)
-    if th_bi is not None or th_sp is not None:
-        params = api.crf_params(float(scale_factor), float(color_factor), int(maxiter))
-        if th_bi is not None:
-            (params.theta_alpha_x, params.theta_alpha_y, params.theta_beta_r, params.theta_beta_g,
-             params.theta_beta_b) = th_bi
-        if th_sp is not None:
-            params.theta_gamma_x, params.theta_gamma_y = th_sp
-        compat = None
-        if compat_bi is not None or compat_sp is not None:
-            compat = _compat_stack(u, M, w1, w2, compat_bi, compat_sp)
-            w1 = w2 = None
-        return _DenseCrfTheta.apply(u, image.contiguous(), w1, w2, compat, theta_bi, theta_sp, params, False)
-    if compat_bi is None and compat_sp is None:
-        return _DenseCrf.apply(u, image.contiguous(), w1, w2, float(scale_factor), float(color_factor), int(maxiter))
-    return _DenseCrfCompat.apply(u, image.contiguous(), _compat_stack(u, M, w1, w2, compat_bi, compat_sp),
-                                 float(scale_factor), float(color_factor), int(maxiter))
+    return _DenseCrfTrain.apply(*_train_args(unary, image, scale_factor, color_factor, maxiter, w1, w2, compat_bi,
+                                             compat_sp, theta_bi, theta_sp, features_bi, wide=False))
 
 
 def _compat_stack(u, M, w1, w2, compat_bi, compat_sp):
@@ -686,43 +581,6 @@ def _compat_stack(u, M, w1, w2, compat_bi, compat_sp):
     return torch.stack(mats)
 
 
-class _DenseCrfWide(torch.autograd.Function):
-    """dense_crf_wide above 32 labels: Potts weights (w1, w2) or the matrices (compat (2, M, M) {mu_bi, mu_sp}) on the
-    label-chunked kernels."""
-
-    @staticmethod
-    @_fwd
-    def forward(ctx, unary, image, w1, w2, compat, params):
-        eng = _engine_for(unary)
-        maxiter = params.n_iters
-        q_hist = torch.empty((maxiter + 1,) + tuple(unary.shape), dtype=torch.float32, device=unary.device)
-        potts = _potts_tensor(w1, w2, unary) if compat is None else None
-        eng.crf_forward_train_wide_dev(unary, image, params, q_hist, potts=potts, compat=compat, stream=_stream(unary))
-        ctx.save_for_backward(q_hist, image, potts, compat)
-        ctx.params = params
-        return q_hist[maxiter].clone()
-
-    @staticmethod
-    @_bwd
-    def backward(ctx, g):
-        q_hist, image, potts, compat = ctx.saved_tensors
-        B, dev = q_hist.shape[1], q_hist.device
-        need = ctx.needs_input_grad
-        grad_u = torch.empty(q_hist.shape[1:], dtype=torch.float32, device=dev)
-        grad_potts = grad_c = None
-        if potts is not None and (need[2] or need[3]):
-            grad_potts = torch.empty((B, 2), dtype=torch.float32, device=dev)
-        if compat is not None and need[4]:
-            M = compat.shape[-1]
-            grad_c = torch.empty((B, 2, M, M), dtype=torch.float32, device=dev)
-        _engine_for(grad_u).crf_backward_wide_dev(q_hist, image, ctx.params, g.contiguous(), grad_u, potts=potts,
-                                                  compat=compat, grad_potts=grad_potts, grad_compat=grad_c,
-                                                  stream=_stream(grad_u))
-        gw1 = grad_potts[:, 0].sum() if grad_potts is not None and need[2] else None
-        gw2 = grad_potts[:, 1].sum() if grad_potts is not None and need[3] else None
-        return grad_u, None, gw1, gw2, None if grad_c is None else grad_c.sum(0), None
-
-
 def dense_crf_wide(unary, image, scale_factor=1.0, color_factor=13, maxiter=10, w1=None, w2=None, compat_bi=None,
                    compat_sp=None, theta_bi=None, theta_sp=None, features_bi=None):
     """dense_crf for any label count from 1 to 255 (COCO's 81 classes), with every parameter dense_crf learns learnable
@@ -732,39 +590,8 @@ def dense_crf_wide(unary, image, scale_factor=1.0, color_factor=13, maxiter=10, 
     per-label cost is several times the fused path's.  Nothing is read on the host unless a theta is given (its values
     build the lattices), so without one a step can be captured in a CUDA graph.  The forward keeps every iteration's
     marginals: (maxiter + 1) * N * M * H * W * 4 bytes, 120 MB at batch 20 @ 41x41 with 81 labels."""
-    if torch.is_autocast_enabled("cuda"):
-        unary = unary.float() if isinstance(unary, torch.Tensor) and unary.is_floating_point() else unary
-        if isinstance(features_bi, torch.Tensor) and features_bi.is_floating_point():
-            features_bi = features_bi.float()
-    u = _maps(unary, "unary")
-    N, M, H, W = u.shape
-    if M <= FUSED_LABELS:
-        return dense_crf(u, image, scale_factor, color_factor, maxiter, w1, w2, compat_bi, compat_sp, theta_bi,
-                         theta_sp, features_bi)
-    if features_bi is not None:
-        return _dense_crf_feat(u, image, features_bi, scale_factor, color_factor, maxiter, w1, w2, compat_bi,
-                               compat_sp, theta_bi, theta_sp, wide=True)
-    if (not isinstance(image, torch.Tensor) or image.dtype != torch.uint8 or tuple(image.shape) != (N, H, W, 3)
-            or image.device != u.device):
-        raise ValueError("image must be a (%d, %d, %d, 3) uint8 tensor on %s" % (N, H, W, u.device))
-    th_bi, th_sp = _theta_values(theta_bi, "theta_bi", 5, u), _theta_values(theta_sp, "theta_sp", 2, u)
-    _cuda(u, "unary")
-    w1, w2 = _potts_weight(w1, "w1", u), _potts_weight(w2, "w2", u)
-    if int(maxiter) < 0:
-        raise ValueError("maxiter must be >= 0 (got %d)" % maxiter)
-    params = api.crf_params(float(scale_factor), float(color_factor), int(maxiter))
-    if th_bi is not None:
-        (params.theta_alpha_x, params.theta_alpha_y, params.theta_beta_r, params.theta_beta_g,
-         params.theta_beta_b) = th_bi
-    if th_sp is not None:
-        params.theta_gamma_x, params.theta_gamma_y = th_sp
-    compat = None
-    if compat_bi is not None or compat_sp is not None:
-        compat = _compat_stack(u, M, w1, w2, compat_bi, compat_sp)
-        w1 = w2 = None
-    if th_bi is not None or th_sp is not None:
-        return _DenseCrfTheta.apply(u, image.contiguous(), w1, w2, compat, theta_bi, theta_sp, params, True)
-    return _DenseCrfWide.apply(u, image.contiguous(), w1, w2, compat, params)
+    return _DenseCrfTrain.apply(*_train_args(unary, image, scale_factor, color_factor, maxiter, w1, w2, compat_bi,
+                                             compat_sp, theta_bi, theta_sp, features_bi, wide=True))
 
 
 def _learned_crf(ref, N, M, H, W, params, w1=None, w2=None, compat_bi=None, compat_sp=None, theta_bi=None,
@@ -776,19 +603,10 @@ def _learned_crf(ref, N, M, H, W, params, w1=None, w2=None, compat_bi=None, comp
     if features_bi is not None:
         if theta_bi is not None:
             raise ValueError("theta_bi and features_bi are two forms of the bilateral features: give one of them")
-        if (not isinstance(features_bi, torch.Tensor) or features_bi.dtype != torch.float32
-                or tuple(features_bi.shape) != (N, 5, H, W) or features_bi.device != ref.device):
-            raise ValueError("features_bi must be a (%d, 5, %d, %d) float32 tensor on %s (got %r)"
-                             % (N, H, W, ref.device, features_bi if not isinstance(features_bi, torch.Tensor) else
-                                (features_bi.dtype, tuple(features_bi.shape), features_bi.device)))
-        f = features_bi.contiguous()
+        f = _features(features_bi, N, H, W, ref.device)
     th_bi, th_sp = _theta_values(theta_bi, "theta_bi", 5, ref), _theta_values(theta_sp, "theta_sp", 2, ref)
     w1, w2 = _potts_weight(w1, "w1", ref), _potts_weight(w2, "w2", ref)
-    if th_bi is not None:
-        (params.theta_alpha_x, params.theta_alpha_y, params.theta_beta_r, params.theta_beta_g,
-         params.theta_beta_b) = th_bi
-    if th_sp is not None:
-        params.theta_gamma_x, params.theta_gamma_y = th_sp
+    _set_theta(params, th_bi, th_sp)
     if compat_bi is not None or compat_sp is not None:
         with torch.no_grad():   # a missing matrix is -w I of its weight, formed on the device
             return f, _compat_stack(ref, M, w1, w2, compat_bi, compat_sp).contiguous()
@@ -822,24 +640,21 @@ def dense_crf_inference(unary, image, scale_factor=1.0, color_factor=13, maxiter
         if isinstance(features_bi, torch.Tensor) and features_bi.is_floating_point():
             features_bi = features_bi.float()
     u = _maps(unary, "unary")
-    N, M, H, W = u.shape
-    if features_bi is not None:
-        if image is not None:
-            raise ValueError("image is not used when features_bi is given: pass None")
-    elif (not isinstance(image, torch.Tensor) or image.dtype != torch.uint8 or tuple(image.shape) != (N, H, W, 3)
-          or image.device != u.device):
-        raise ValueError("image must be a (%d, %d, %d, 3) uint8 tensor on %s" % (N, H, W, u.device))
+    if features_bi is None:
+        image = _image(image, u)
+    elif image is not None:
+        raise ValueError("image is not used when features_bi is given: pass None")
     if int(maxiter) < 0:
         raise ValueError("maxiter must be >= 0 (got %d)" % maxiter)
     _cuda(u, "unary")
     params = api.crf_params(float(scale_factor), float(color_factor), int(maxiter))
-    f, compat = _learned_crf(u, N, M, H, W, params, w1, w2, compat_bi, compat_sp, theta_bi, theta_sp, features_bi)
+    f, compat = _learned_crf(u, *u.shape, params, w1, w2, compat_bi, compat_sp, theta_bi, theta_sp, features_bi)
     eng = _engine_for(u)
     out = torch.empty(u.shape, dtype=torch.float32, device=u.device)
     s = _stream(u)
     if f is None and compat is None:
-        return eng.crf_dev(u, image.contiguous(), params, out, api.LAYOUT_NCHW, api.LAYOUT_NCHW, stream=s)
-    return eng.crf_learned_dev(u, None if f is not None else image.contiguous(), params, out, features=f,
+        return eng.crf_dev(u, image, params, out, api.LAYOUT_NCHW, api.LAYOUT_NCHW, stream=s)
+    return eng.crf_learned_dev(u, image, params, out, features=f,
                                compat=compat, unary_layout=api.LAYOUT_NCHW, out_layout=api.LAYOUT_NCHW, stream=s)
 
 
@@ -894,20 +709,18 @@ def dense_crf_energy(q, unary, image, scale_factor=1.0, color_factor=13, w1=None
         if isinstance(t, torch.Tensor) and t.requires_grad:
             raise ValueError("%s requires grad: dense_crf_energy differentiates q and unary only (detach it)" % name)
     qq = _maps(q, "q")
-    N, M, H, W = qq.shape
+    M = qq.shape[1]
     if M > FUSED_LABELS:
         raise ValueError("dense_crf_energy supports at most %d labels (got %d)" % (FUSED_LABELS, M))
     u = None if unary is None else _like(unary, qq, "unary")
-    if features_bi is not None:
-        if image is not None:
-            raise ValueError("image is not used when features_bi is given: pass None")
-    elif (not isinstance(image, torch.Tensor) or image.dtype != torch.uint8 or tuple(image.shape) != (N, H, W, 3)
-          or image.device != qq.device):
-        raise ValueError("image must be a (%d, %d, %d, 3) uint8 tensor on %s" % (N, H, W, qq.device))
+    if features_bi is None:
+        image = _image(image, qq)
+    elif image is not None:
+        raise ValueError("image is not used when features_bi is given: pass None")
     _cuda(qq, "q")
     params = api.crf_params(float(scale_factor), float(color_factor), 0)
-    f, compat = _learned_crf(qq, N, M, H, W, params, w1, w2, compat_bi, compat_sp, theta_bi, theta_sp, features_bi)
-    return _DenseCrfEnergy.apply(qq, u, None if f is not None else image.contiguous(), f, compat, params)
+    f, compat = _learned_crf(qq, *qq.shape, params, w1, w2, compat_bi, compat_sp, theta_bi, theta_sp, features_bi)
+    return _DenseCrfEnergy.apply(qq, u, image, f, compat, params)
 
 
 def softmax(fc8):
