@@ -67,6 +67,8 @@ SIGNATURES = {
     "dsrg_crf_backward_feat_dev": (_i, [_vp, _vp, _i, _vp, _pp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "dsrg_crf_energy_dev": (_i, [_vp, _vp, _i, _vp, _vp, _vp, _pp, _vp, _vp, _vp, _vp]),
     "dsrg_crf_energy_backward_dev": (_i, [_vp, _vp, _i, _vp, _vp, _vp, _pp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "dsrg_crf_energy_wide_dev": (_i, [_vp, _vp, _i, _vp, _vp, _vp, _pp, _vp, _vp, _vp, _vp]),
+    "dsrg_crf_energy_backward_wide_dev": (_i, [_vp, _vp, _i, _vp, _vp, _vp, _pp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "dsrg_crf_forward_train_wide_dev": (_i, [_vp, _vp, _i, _vp, _pp, _vp, _vp, _vp, _vp]),
     "dsrg_crf_backward_wide_dev": (_i, [_vp, _vp, _i, _vp, _pp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "dsrg_crf_backward_wide_theta_dev": (_i, [_vp, _vp, _i, _vp, _pp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),

@@ -239,6 +239,26 @@ class Engine(object):
                                                    _dptr(grad_q), _dptr(grad_unary), _stream(stream)))
         return grad_q
 
+    def crf_energy_wide_dev(self, q, unary, image, params, terms, features=None, potts=None, compat=None,
+                            stream=None):
+        """crf_energy_dev above 32 labels (33 to 255), on the label-chunked kernels: the same arguments and terms.  An
+        engine of 32 labels or fewer refuses."""
+        B = q.shape[0]
+        check(self._L.dsrg_crf_energy_wide_dev(self.h, _dptr(q), B, _dptr(unary), _dptr(image), _dptr(features),
+                                               C.byref(params), _dptr(potts), _dptr(compat), _dptr(terms),
+                                               _stream(stream)))
+        return terms
+
+    def crf_energy_backward_wide_dev(self, q, unary, image, params, grad_terms, grad_q, grad_unary=None,
+                                     features=None, potts=None, compat=None, stream=None):
+        """crf_energy_backward_dev above 32 labels (33 to 255): the gradient of crf_energy_wide_dev's terms."""
+        B = q.shape[0]
+        check(self._L.dsrg_crf_energy_backward_wide_dev(self.h, _dptr(q), B, _dptr(unary), _dptr(image),
+                                                        _dptr(features), C.byref(params), _dptr(potts),
+                                                        _dptr(compat), _dptr(grad_terms), _dptr(grad_q),
+                                                        _dptr(grad_unary), _stream(stream)))
+        return grad_q
+
     def crf_forward_train_wide_dev(self, unary, image, params, q_hist, potts=None, compat=None, stream=None):
         """crf_forward_train_dev / crf_forward_train_compat_dev above 32 labels (33 to 255): potts {w1, w2} or compat
         (2, M, M) {mu_bi, mu_sp}, not both; neither: params.w1 / w2.  An engine of 32 labels or fewer refuses."""

@@ -441,7 +441,7 @@ using namespace dsrg;
 
 extern "C" {
 
-int dsrg_version(void) { return 118; }
+int dsrg_version(void) { return 119; }
 
 const char *dsrg_last_error(void) { return g_err; }
 
@@ -969,61 +969,100 @@ int dsrg_crf_backward_wide_feat_dev(dsrg_engine *h, const float *q_hist, int B, 
                            .grad_features = grad_features, .grad_theta_sp = grad_theta_sp});
 }
 
-// The body of both energy entry points: the lattices of the image or of the features, the energy (terms) or its
-// gradient (grad_terms given), and the feature passes' NaN policy for the outputs
+// The body of the energy entry points: the lattices of the image or of the features, the energy (terms) or its
+// gradient (grad_terms given) on the fused kernels or (wide) the label-chunked ones, and the feature passes' NaN policy
+// for the outputs
 static int energy_pass(Engine *e, int B, const float *q, const float *unary, const uint8_t *image, const float *features,
                        const dsrg_crf_params &p, const float *potts, const float *compat, float *terms,
-                       const float *grad_terms, float *grad_q, float *grad_unary, cudaStream_t s) {
+                       const float *grad_terms, float *grad_q, float *grad_unary, bool wide, cudaStream_t s) {
     int r = prepare_lattices_for(e, B, image, features, p, s);
-    if (!r) r = meanfield_energy(e, B, q, unary, potts, compat, p, terms, grad_terms, grad_q, grad_unary, s);
+    if (!r)
+        r = (wide ? meanfield_energy_wide : meanfield_energy)(e, B, q, unary, potts, compat, p, terms, grad_terms,
+                                                                grad_q, grad_unary, s);
     if (r || !features) return r;
     const long long MN = (long long)e->M * e->N;
     return nan_flagged_outputs(e, B, {{terms, 4}, {grad_q, MN}, {grad_unary, MN}}, s, T_CRF_ENERGY);
 }
 
-static int energy_labels_ok(const Engine *e) {
+// one energy path per label count, as for the training entry points
+static int energy_labels_ok(const Engine *e, bool wide) {
+    if (wide) {
+        if (e->M > DSRG_MAX_LABELS) return DSRG_OK;
+        set_error("the label-chunked CRF energy takes more than %d labels (got %d); use dsrg_crf_energy_dev / "
+                  "dsrg_crf_energy_backward_dev", DSRG_MAX_LABELS, e->M);
+        return DSRG_E_INVALID;
+    }
     if (e->MP <= DSRG_MAX_LABELS) return DSRG_OK;
     set_error("the CRF energy supports at most %d labels (got %d)", DSRG_MAX_LABELS, e->M);
     return DSRG_E_INVALID;
 }
 
-int dsrg_crf_energy_dev(dsrg_engine *h, const float *q, int B, const float *unary, const uint8_t *image,
-                        const float *features, const dsrg_crf_params *params, const float *potts, const float *compat,
-                        float *terms, void *stream) {
+static int energy_forward(dsrg_engine *h, const float *q, int B, const float *unary, const uint8_t *image,
+                          const float *features, const dsrg_crf_params *params, const float *potts,
+                          const float *compat, float *terms, void *stream, bool wide) {
     const cudaStream_t s = (cudaStream_t)stream;
     const bool ok = q && params && terms && (image != nullptr) != (features != nullptr) && !(potts && compat);
     return dev_call(h, B, s, ok, [&](Engine *e) {
-        if (int rc = energy_labels_ok(e)) return rc;
+        if (int rc = energy_labels_ok(e, wide)) return rc;
         if (int rc = ensure_energy(e, features != nullptr)) return rc;
         GraphKey args;
         args.add(q).add(unary).add(image).add(features).add(potts).add(compat).add(terms);
-        const int rc = crf_pass(e, s, PassKind::crf_energy, B, params, args, [&]() {
+        const int rc = crf_pass(e, s, wide ? PassKind::crf_energy_wide : PassKind::crf_energy, B, params, args, [&]() {
             return energy_pass(e, B, q, unary, image, features, *params, potts, compat, terms, nullptr, nullptr,
-                               nullptr, s);
+                               nullptr, wide, s);
         });
         return learned_pass_end(e, B, features, rc);
     });
+}
+
+static int energy_backward(dsrg_engine *h, const float *q, int B, const float *unary, const uint8_t *image,
+                           const float *features, const dsrg_crf_params *params, const float *potts,
+                           const float *compat, const float *grad_terms, float *grad_q, float *grad_unary,
+                           void *stream, bool wide) {
+    const cudaStream_t s = (cudaStream_t)stream;
+    const bool ok = q && params && grad_terms && grad_q && (image != nullptr) != (features != nullptr) &&
+                    !(potts && compat);
+    return dev_call(h, B, s, ok, [&](Engine *e) {
+        if (int rc = energy_labels_ok(e, wide)) return rc;
+        if (int rc = ensure_energy(e, features != nullptr)) return rc;
+        GraphKey args;
+        args.add(q).add(unary).add(image).add(features).add(potts).add(compat).add(grad_terms).add(grad_q)
+            .add(grad_unary);
+        const PassKind kind = wide ? PassKind::crf_energy_backward_wide : PassKind::crf_energy_backward;
+        const int rc = crf_pass(e, s, kind, B, params, args, [&]() {
+            return energy_pass(e, B, q, unary, image, features, *params, potts, compat, nullptr, grad_terms, grad_q,
+                               grad_unary, wide, s);
+        });
+        return learned_pass_end(e, B, features, rc);
+    });
+}
+
+int dsrg_crf_energy_dev(dsrg_engine *h, const float *q, int B, const float *unary, const uint8_t *image,
+                        const float *features, const dsrg_crf_params *params, const float *potts, const float *compat,
+                        float *terms, void *stream) {
+    return energy_forward(h, q, B, unary, image, features, params, potts, compat, terms, stream, false);
 }
 
 int dsrg_crf_energy_backward_dev(dsrg_engine *h, const float *q, int B, const float *unary, const uint8_t *image,
                                  const float *features, const dsrg_crf_params *params, const float *potts,
                                  const float *compat, const float *grad_terms, float *grad_q, float *grad_unary,
                                  void *stream) {
-    const cudaStream_t s = (cudaStream_t)stream;
-    const bool ok = q && params && grad_terms && grad_q && (image != nullptr) != (features != nullptr) &&
-                    !(potts && compat);
-    return dev_call(h, B, s, ok, [&](Engine *e) {
-        if (int rc = energy_labels_ok(e)) return rc;
-        if (int rc = ensure_energy(e, features != nullptr)) return rc;
-        GraphKey args;
-        args.add(q).add(unary).add(image).add(features).add(potts).add(compat).add(grad_terms).add(grad_q)
-            .add(grad_unary);
-        const int rc = crf_pass(e, s, PassKind::crf_energy_backward, B, params, args, [&]() {
-            return energy_pass(e, B, q, unary, image, features, *params, potts, compat, nullptr, grad_terms, grad_q,
-                               grad_unary, s);
-        });
-        return learned_pass_end(e, B, features, rc);
-    });
+    return energy_backward(h, q, B, unary, image, features, params, potts, compat, grad_terms, grad_q, grad_unary,
+                           stream, false);
+}
+
+int dsrg_crf_energy_wide_dev(dsrg_engine *h, const float *q, int B, const float *unary, const uint8_t *image,
+                             const float *features, const dsrg_crf_params *params, const float *potts,
+                             const float *compat, float *terms, void *stream) {
+    return energy_forward(h, q, B, unary, image, features, params, potts, compat, terms, stream, true);
+}
+
+int dsrg_crf_energy_backward_wide_dev(dsrg_engine *h, const float *q, int B, const float *unary, const uint8_t *image,
+                                      const float *features, const dsrg_crf_params *params, const float *potts,
+                                      const float *compat, const float *grad_terms, float *grad_q, float *grad_unary,
+                                      void *stream) {
+    return energy_backward(h, q, B, unary, image, features, params, potts, compat, grad_terms, grad_q, grad_unary,
+                           stream, true);
 }
 
 int dsrg_crf_batch_learned_dev(dsrg_engine *h, const float *unary, int B, int unary_layout, const uint8_t *image,

@@ -209,6 +209,13 @@ int wide_weights(Engine *e, Lattice &L, int nb, cudaStream_t s);
 constexpr int kWideChunks = 16;
 int meanfield_run_train_wide(Engine *e, int B, const CrfTrainIo &io, const dsrg_crf_params &p, cudaStream_t s);
 int meanfield_backward_wide(Engine *e, int B, const CrfTrainIo &io, const dsrg_crf_params &p, cudaStream_t s);
+// meanfield_energy above DSRG_MAX_LABELS labels, with the same arguments and buffers (e->en_part); it also overwrites
+// e->U and e->Q0 (the matrices' planes)
+int meanfield_energy_wide(Engine *e, int B, const float *q, const float *unary, const float *potts, const float *compat,
+                          const dsrg_crf_params &p, float *terms, const float *grad_terms, float *grad_q,
+                          float *grad_unary, cudaStream_t s);
+// (meanfield.cu) per image: the energy's block sums part [B][nblk][4] in block order -> terms [B][4]; <<<B, 32>>>
+__global__ void k_crf_energy_reduce(const double *part, int nblk, float *terms);
 int meanfield_export(Engine *e, int B, float *out, int layout, cudaStream_t s);
 int meanfield_export_map(Engine *e, int B, int32_t *labels, cudaStream_t s);
 int meanfield_export_renorm(Engine *e, int B, float *result_out, float *log_out, cudaStream_t s);
@@ -484,7 +491,7 @@ enum class PassKind : int { crf, crf_map, forward, crflayer, densecrf, post, crf
                             crf_backward_compat, crf_backward_theta, crf_backward_compat_theta, crf_train_feat,
                             crf_backward_feat, crf_train_wide, crf_backward_wide, crf_backward_wide_theta,
                             crf_train_wide_feat, crf_backward_wide_feat, crf_learned, post_learned, crf_energy,
-                            crf_energy_backward };
+                            crf_energy_backward, crf_energy_wide, crf_energy_backward_wide };
 struct GraphKey {
     std::string bytes;
     GraphKey() = default;

@@ -570,6 +570,20 @@ int meanfield_run_wide(Engine *e, int B, const float *unary, int layout, bool cl
 
 static WideLat wide_lat(const Lattice &L, float *val) { return WideLat{L.off, L.wn, L.rowbase, val, L.shared, L.d + 1}; }
 
+// blur every axis of L (d..0 when `reverse`, K^T) ping-ponging between *src and *dst; afterwards *src holds the
+// result and *dst is free
+static void wide_blur_axes(Engine *e, const Lattice &L, int B, bool reverse, int tag, cudaStream_t s, float **src,
+                           float **dst) {
+    const int CH = e->MP / 4, grid = 8 * e->sm_count;
+    for (int p = 0; p <= L.d; p++) {
+        const int j = reverse ? L.d - p : p;
+        DSRG_LAUNCH(e, tag, s,
+                    k_wide_blur<<<grid, kThreads, 0, s>>>((const float4 *)*src, (float4 *)*dst, L.nbr + (size_t)j * L.nbr_stride,
+                                                          L.rowbase, B, L.shared, CH));
+        float *t = *src; *src = *dst; *dst = t;
+    }
+}
+
 // zero Y, splat X planar into it, blur every axis (d..0 when `reverse`, K^T) ping-ponging with Z; returns the
 // blurred buffers
 static void wide_filter_to(Engine *e, int B, const float *X, bool reverse, int tag, cudaStream_t s, float *spY,
@@ -578,17 +592,8 @@ static void wide_filter_to(Engine *e, int B, const float *X, bool reverse, int t
     const dim3 gq(cdiv(N, kThreads), CH, B);
     DSRG_LAUNCH(e, tag, s, k_wide_zero<<<grid, kThreads, 0, s>>>((float4 *)spY, e->sp.rowbase, (float4 *)biY, e->bi.rowbase, B, CH));
     DSRG_LAUNCH(e, tag, s, k_wide_splat<<<gq, kThreads, 0, s>>>(X, wide_lat(e->sp, spY), wide_lat(e->bi, biY), M, N, CH));
-    for (int l = 0; l < 2; l++) {
-        Lattice &L = l ? e->bi : e->sp;
-        float *&src = l ? biY : spY, *&dst = l ? biZ : spZ;
-        for (int p = 0; p <= L.d; p++) {
-            const int j = reverse ? L.d - p : p;
-            DSRG_LAUNCH(e, tag, s,
-                        k_wide_blur<<<grid, kThreads, 0, s>>>((const float4 *)src, (float4 *)dst, L.nbr + (size_t)j * L.nbr_stride,
-                                                              L.rowbase, B, L.shared, CH));
-            float *t = src; src = dst; dst = t;
-        }
-    }
+    wide_blur_axes(e, e->sp, B, reverse, tag, s, &spY, &spZ);
+    wide_blur_axes(e, e->bi, B, reverse, tag, s, &biY, &biZ);
     *sp_out = spY;
     *bi_out = biY;
 }
@@ -730,6 +735,285 @@ int meanfield_backward_wide(Engine *e, int B, const CrfTrainIo &io, const dsrg_c
         }
         if (kg) kg_finish(e, ka, B, grad_theta, 8 * e->sm_count, s, feat, grad_feat, kg_tag);
     }
+    DSRG_CUDA_TRY(cudaGetLastError());
+    return DSRG_OK;
+}
+
+// ---------------------------------------------------------------------------------------------
+// The energy above 32 labels: the fused energy's definition and operation order (the comment above EnergyArgs in
+// meanfield.cu) with the labels chunked into quads.  wn q is splatted once into spA / biA (the backward copies the
+// splat to spC / biC) and blurred in K's order, the copy in K^T's.  Then
+//   Potts   : one per-pixel pass slices each quad of each lattice and forms the terms or grad_q, with no planes;
+//   matrices: the forward slices F_sp / F_bi into e->U / e->Q0 and mixes them with mu per pixel; the backward slices
+//             F_k and F_k^T of one lattice at a time into those planes and forms g_k (mu_k F_k + mu_k^T F_k^T), the
+//             spatial launch writing grad_q and the bilateral one adding to it.
+// The forward's per-pixel terms go to per-block double sums e->en_part [B][nblk][4], which k_crf_energy_reduce adds in
+// block order: no float atomics outside the splat, and no device memory beyond the fused energy's.
+// ---------------------------------------------------------------------------------------------
+struct WideEnergyArgs {
+    WideLat sp, bi;             // values K S(wn q)
+    WideLat spt, bit;           // values K^T S(wn q) (the backward)
+    const float *q, *unary;     // [B][M][N]; unary may be nullptr
+    const float *potts;         // {w1, w2} on the device, or nullptr: w1, w2
+    float w1, w2, a_sp, a_bi;
+    const float *grad_terms;    // [B][4] (the backward)
+    float *grad_q, *grad_unary; // [B][M][N]; grad_unary may be nullptr
+    double *part;               // [B][nblk][4] (the forward)
+    int M, N, CH;
+};
+
+// the entropy and unary terms of one label (q at `at`) into acc[0..1]; BWD: returns the start of its grad_q and
+// writes its grad_unary
+template <bool BWD>
+__device__ __forceinline__ float wide_energy_local(const WideEnergyArgs &a, size_t at, float q, float g0, float g1,
+                                                   float acc[4]) {
+    const float u = a.unary ? __ldg(a.unary + at) : 0.0f;
+    const float lq = logf(fmaxf(q, 1e-20f));
+    acc[0] = fmaf(q, lq, acc[0]);
+    acc[1] = fmaf(-u, q, acc[1]);
+    if constexpr (BWD) {
+        if (a.grad_unary) a.grad_unary[at] = -g1 * q;
+        return fmaf(-g1, u, g0 * (q > 1e-20f ? lq + 1.0f : lq));
+    }
+    return 0.0f;
+}
+
+// the block's per-pixel terms summed in double to part[b][block][4] (k_crf_energy's reduction)
+__device__ __forceinline__ void wide_energy_block_sum(const float acc[4], double *part, int b) {
+    __shared__ double red[kThreads / 32][4];
+    double v[4];
+#pragma unroll
+    for (int k = 0; k < 4; k++) {
+        v[k] = acc[k];
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) v[k] += __shfl_down_sync(0xffffffffu, v[k], o);
+    }
+    if ((threadIdx.x & 31) == 0) {
+#pragma unroll
+        for (int k = 0; k < 4; k++) red[threadIdx.x >> 5][k] = v[k];
+    }
+    __syncthreads();
+    if (threadIdx.x < 4) {
+        double s = 0.0;
+        for (int w = 0; w < kThreads / 32; w++) s += red[w][threadIdx.x];
+        part[((size_t)b * gridDim.x + blockIdx.x) * 4 + threadIdx.x] = s;
+    }
+}
+
+// Potts, one thread per pixel over the label quads: the terms to the block sums or (BWD) grad_q = the local part
+// + g_2 (-w2 F_sp) + g_2 (-w2 F_sp^T) + g_3 (-w1 F_bi) + g_3 (-w1 F_bi^T), in k_crf_energy's order
+template <bool BWD>
+__global__ void __launch_bounds__(kThreads)
+k_wide_energy_potts(WideEnergyArgs a) {
+    const int b = blockIdx.y, i = blockIdx.x * kThreads + threadIdx.x;
+    float acc[4] = {0.0f, 0.0f, 0.0f, 0.0f};
+    if (i < a.N) {
+        const float w1 = a.potts ? __ldg(a.potts) : a.w1, w2 = a.potts ? __ldg(a.potts + 1) : a.w2;
+        float g0 = 0.0f, g1 = 0.0f, g2 = 0.0f, g3 = 0.0f;
+        if constexpr (BWD) {
+            g0 = __ldg(a.grad_terms + 4 * b);
+            g1 = __ldg(a.grad_terms + 4 * b + 1);
+            g2 = __ldg(a.grad_terms + 4 * b + 2);
+            g3 = __ldg(a.grad_terms + 4 * b + 3);
+        }
+        for (int c = 0; c < a.CH; c++) {
+            float q[4], g[4];
+#pragma unroll
+            for (int k = 0; k < 4; k++) {
+                const int l = 4 * c + k;
+                const size_t at = ((size_t)b * a.M + l) * a.N + i;
+                q[k] = l < a.M ? __ldg(a.q + at) : 0.0f;
+                g[k] = l < a.M ? wide_energy_local<BWD>(a, at, q[k], g0, g1, acc) : 0.0f;
+            }
+#pragma unroll
+            for (int kk = 0; kk < 2; kk++) {
+                const float w = kk == 0 ? w2 : w1, gk = kk == 0 ? g2 : g3;
+                float f[4] = {0.0f, 0.0f, 0.0f, 0.0f};
+                wide_slice_quad(kk == 0 ? a.sp : a.bi, kk == 0 ? a.a_sp : a.a_bi, b, i, c, a.N, a.CH, f);
+#pragma unroll
+                for (int k = 0; k < 4; k++) {
+                    const float m = -w * f[k];
+                    acc[2 + kk] = fmaf(q[k], m, acc[2 + kk]);
+                    if constexpr (BWD) g[k] = fmaf(gk, m, g[k]);
+                }
+                if constexpr (BWD) {
+                    float t[4] = {0.0f, 0.0f, 0.0f, 0.0f};
+                    wide_slice_quad(kk == 0 ? a.spt : a.bit, kk == 0 ? a.a_sp : a.a_bi, b, i, c, a.N, a.CH, t);
+#pragma unroll
+                    for (int k = 0; k < 4; k++) g[k] = fmaf(gk, -w * t[k], g[k]);
+                }
+            }
+            if constexpr (BWD) {
+#pragma unroll
+                for (int k = 0; k < 4; k++)
+                    if (4 * c + k < a.M) a.grad_q[((size_t)b * a.M + 4 * c + k) * a.N + i] = g[k];
+            }
+        }
+    }
+    if constexpr (!BWD) wide_energy_block_sum(acc, a.part, b);
+}
+
+// Matrices, the forward: one thread per pixel, terms 0 / 1 over the labels and e_k = sum_l q_l (mu_k F_k)_l with
+// (mu F)_l an fma chain over l' from zero, labels ascending.  mu's rows are staged kWideEnergyRows at a time, transposed
+// ([l'][row]), so a stage reads each F_k[l'] once for all of its rows; any label count fits.  F_sp, F_bi [B][M][N].
+constexpr int kWideEnergyRows = 16;
+__global__ void __launch_bounds__(kThreads)
+k_wide_energy_mat(WideEnergyArgs a, const float *compat, const float *F_sp, const float *F_bi) {
+    constexpr int R = kWideEnergyRows;
+    extern __shared__ float4 mus4[];   // [M][R / 4]
+    const int b = blockIdx.y, i = blockIdx.x * kThreads + threadIdx.x, M = a.M, N = a.N;
+    const bool in = i < N;
+    const size_t px = (size_t)b * M * N + i;
+    float acc[4] = {0.0f, 0.0f, 0.0f, 0.0f};
+    if (in)
+        for (int l = 0; l < M; l++) wide_energy_local<false>(a, px + (size_t)l * N, __ldg(a.q + px + (size_t)l * N), 0.0f, 0.0f, acc);
+#pragma unroll 1
+    for (int kk = 0; kk < 2; kk++) {
+        const float *mu = compat + (kk == 0 ? (size_t)M * M : 0);   // compat = {mu_bi, mu_sp}
+        const float *F = (kk == 0 ? F_sp : F_bi) + px;
+        float ek = 0.0f;
+        for (int l0 = 0; l0 < M; l0 += R) {
+            __syncthreads();
+            for (int e = threadIdx.x; e < R * M; e += kThreads) {
+                const int l2 = e / R, r = e % R;
+                reinterpret_cast<float *>(mus4)[e] = l0 + r < M ? __ldg(mu + (size_t)(l0 + r) * M + l2) : 0.0f;
+            }
+            __syncthreads();
+            if (!in) continue;
+            float m[R];
+#pragma unroll
+            for (int r = 0; r < R; r++) m[r] = 0.0f;
+            for (int l2 = 0; l2 < M; l2++) {
+                const float f = __ldg(F + (size_t)l2 * N);
+#pragma unroll
+                for (int r4 = 0; r4 < R / 4; r4++) {
+                    const float4 v = mus4[l2 * (R / 4) + r4];
+                    m[4 * r4] = fmaf(v.x, f, m[4 * r4]);
+                    m[4 * r4 + 1] = fmaf(v.y, f, m[4 * r4 + 1]);
+                    m[4 * r4 + 2] = fmaf(v.z, f, m[4 * r4 + 2]);
+                    m[4 * r4 + 3] = fmaf(v.w, f, m[4 * r4 + 3]);
+                }
+            }
+#pragma unroll
+            for (int r = 0; r < R; r++)
+                if (l0 + r < M) ek = fmaf(__ldg(a.q + px + (size_t)(l0 + r) * N), m[r], ek);
+        }
+        acc[2 + kk] = ek;
+    }
+    wide_energy_block_sum(acc, a.part, b);
+}
+
+// Matrices, the backward of one lattice (first: the spatial one, g_2, writing grad_q; else the bilateral one, g_3,
+// adding to it): grad_q_l += g_k (mu F)_l, then mu[l'][l] (g_k F^T_l') over l' ascending, k_crf_energy's order.  One
+// thread per (pixel, label quad); the quad's four rows and four columns of mu, 8 M floats in shared memory
+// ([2 = rows, columns][M][4]).  F, Ft [B][M][N].
+__global__ void __launch_bounds__(kThreads)
+k_wide_energy_mat_bwd(WideEnergyArgs a, const float *mu, const float *F, const float *Ft, int first) {
+    extern __shared__ float4 mq[];
+    const int b = blockIdx.z, c = blockIdx.y, M = a.M, N = a.N;
+    for (int e = threadIdx.x; e < 8 * M; e += blockDim.x) {
+        const int m = e / (4 * M), l2 = (e / 4) % M, k = e & 3, l = 4 * c + k;
+        reinterpret_cast<float *>(mq)[e] = l < M ? __ldg(m ? mu + (size_t)l2 * M + l : mu + (size_t)l * M + l2) : 0.0f;
+    }
+    __syncthreads();
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= N) return;
+    const float gk = __ldg(a.grad_terms + 4 * b + (first ? 2 : 3));
+    float g[4], m[4] = {0.0f, 0.0f, 0.0f, 0.0f}, unused[4] = {0.0f, 0.0f, 0.0f, 0.0f};
+#pragma unroll
+    for (int k = 0; k < 4; k++) {
+        const int l = 4 * c + k;
+        const size_t at = ((size_t)b * M + l) * N + i;
+        if (l >= M)
+            g[k] = 0.0f;
+        else if (first)
+            g[k] = wide_energy_local<true>(a, at, __ldg(a.q + at), __ldg(a.grad_terms + 4 * b),
+                                           __ldg(a.grad_terms + 4 * b + 1), unused);
+        else
+            g[k] = a.grad_q[at];
+    }
+    const float *fp = F + (size_t)b * M * N + i, *tp = Ft + (size_t)b * M * N + i;
+    for (int l2 = 0; l2 < M; l2++) {
+        const float f = __ldg(fp + (size_t)l2 * N);
+        const float4 r = mq[l2];
+        m[0] = fmaf(r.x, f, m[0]);
+        m[1] = fmaf(r.y, f, m[1]);
+        m[2] = fmaf(r.z, f, m[2]);
+        m[3] = fmaf(r.w, f, m[3]);
+    }
+#pragma unroll
+    for (int k = 0; k < 4; k++) g[k] = fmaf(gk, m[k], g[k]);
+    for (int l2 = 0; l2 < M; l2++) {
+        const float t = gk * __ldg(tp + (size_t)l2 * N);
+        const float4 r = mq[M + l2];
+        g[0] = fmaf(r.x, t, g[0]);
+        g[1] = fmaf(r.y, t, g[1]);
+        g[2] = fmaf(r.z, t, g[2]);
+        g[3] = fmaf(r.w, t, g[3]);
+    }
+#pragma unroll
+    for (int k = 0; k < 4; k++)
+        if (4 * c + k < M) a.grad_q[((size_t)b * M + 4 * c + k) * N + i] = g[k];
+}
+
+// copy the B images' rows of both lattices' splat targets (row counts device-resident, as k_wide_zero)
+__global__ void __launch_bounds__(kThreads)
+k_wide_energy_copy(const float4 *a, float4 *a2, const int32_t *rowbase_a, const float4 *c, float4 *c2,
+                   const int32_t *rowbase_c, int B, int CH) {
+    const long long na = (long long)rowbase_a[B] * CH, nc = (long long)rowbase_c[B] * CH;
+    for (long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x; t < na + nc; t += (long long)gridDim.x * blockDim.x) {
+        if (t < na) a2[t] = a[t]; else c2[t - na] = c[t - na];
+    }
+}
+
+int meanfield_energy_wide(Engine *e, int B, const float *q, const float *unary, const float *potts, const float *compat,
+                          const dsrg_crf_params &p, float *terms, const float *grad_terms, float *grad_q,
+                          float *grad_unary, cudaStream_t s) {
+    const int M = e->M, N = e->N, CH = e->MP / 4, nblk = cdiv(N, kThreads), grid = 8 * e->sm_count;
+    const bool bwd = grad_terms != nullptr;
+    const dim3 gp(nblk, B), gq(nblk, CH, B);
+    const float a_sp = wide_alpha(e->sp), a_bi = wide_alpha(e->bi);
+    const int tag = T_CRF_ENERGY;
+    // S(wn q) into A, and for the gradient a copy in C.  K S(wn q) from A with B as scratch; K^T S(wn q) from C with
+    // whichever of A / B the first result left free
+    DSRG_LAUNCH(e, tag, s, k_wide_zero<<<grid, kThreads, 0, s>>>((float4 *)e->spA, e->sp.rowbase, (float4 *)e->biA, e->bi.rowbase, B, CH));
+    DSRG_LAUNCH(e, tag, s, k_wide_splat<<<gq, kThreads, 0, s>>>(q, wide_lat(e->sp, e->spA), wide_lat(e->bi, e->biA), M, N, CH));
+    if (bwd)
+        DSRG_LAUNCH(e, tag, s,
+                    k_wide_energy_copy<<<grid, kThreads, 0, s>>>((const float4 *)e->spA, (float4 *)e->spC, e->sp.rowbase,
+                                                                 (const float4 *)e->biA, (float4 *)e->biC, e->bi.rowbase,
+                                                                 B, CH));
+    float *vf_sp = e->spA, *free_sp = e->spB, *vf_bi = e->biA, *free_bi = e->biB, *vt_sp = e->spC, *vt_bi = e->biC;
+    wide_blur_axes(e, e->sp, B, false, tag, s, &vf_sp, &free_sp);
+    wide_blur_axes(e, e->bi, B, false, tag, s, &vf_bi, &free_bi);
+    if (bwd) {
+        wide_blur_axes(e, e->sp, B, true, tag, s, &vt_sp, &free_sp);
+        wide_blur_axes(e, e->bi, B, true, tag, s, &vt_bi, &free_bi);
+    }
+    const WideEnergyArgs a{wide_lat(e->sp, vf_sp), wide_lat(e->bi, vf_bi), wide_lat(e->sp, vt_sp),
+                           wide_lat(e->bi, vt_bi), q, unary, potts, p.w1, p.w2, a_sp, a_bi, grad_terms, grad_q,
+                           grad_unary, e->en_part, M, N, CH};
+    if (!compat) {
+        if (bwd)
+            DSRG_LAUNCH(e, tag, s, k_wide_energy_potts<true><<<gp, kThreads, 0, s>>>(a));
+        else
+            DSRG_LAUNCH(e, tag, s, k_wide_energy_potts<false><<<gp, kThreads, 0, s>>>(a));
+    } else if (!bwd) {   // e->U, e->Q0: F_sp, F_bi
+        DSRG_LAUNCH(e, tag, s, k_wide_slice_planar<<<gq, kThreads, 0, s>>>(e->U, e->Q0, a.sp, a.bi, a_sp, a_bi, M, N, CH));
+        DSRG_LAUNCH(e, tag, s,
+                    k_wide_energy_mat<<<gp, kThreads, kWideEnergyRows * M * sizeof(float), s>>>(a, compat, e->U, e->Q0));
+    } else {             // per lattice, e->U, e->Q0: F_k, F_k^T
+        for (int kk = 0; kk < 2; kk++) {
+            const float al = kk == 0 ? a_sp : a_bi;
+            DSRG_LAUNCH(e, tag, s,
+                        k_wide_slice_planar<<<gq, kThreads, 0, s>>>(e->U, e->Q0, kk == 0 ? a.sp : a.bi,
+                                                                    kk == 0 ? a.spt : a.bit, al, al, M, N, CH));
+            DSRG_LAUNCH(e, tag, s,
+                        k_wide_energy_mat_bwd<<<gq, kThreads, 8 * M * sizeof(float), s>>>(
+                            a, compat + (kk == 0 ? (size_t)M * M : 0), e->U, e->Q0, kk == 0));
+        }
+    }
+    if (!bwd) DSRG_LAUNCH(e, tag, s, k_crf_energy_reduce<<<B, 32, 0, s>>>(e->en_part, nblk, terms));
     DSRG_CUDA_TRY(cudaGetLastError());
     return DSRG_OK;
 }

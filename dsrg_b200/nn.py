@@ -659,16 +659,17 @@ def dense_crf_inference(unary, image, scale_factor=1.0, color_factor=13, maxiter
 
 
 class _DenseCrfEnergy(torch.autograd.Function):
-    """dense_crf_energy's terms (N, 4) and their gradient to q and unary; the parameters carry none."""
+    """dense_crf_energy's terms (N, 4) and their gradient to q and unary; the parameters carry none.  wide: the
+    label-chunked entry points above 32 labels."""
 
     @staticmethod
     @_fwd
-    def forward(ctx, q, unary, image, features, compat, params):
+    def forward(ctx, q, unary, image, features, compat, params, wide):
         terms = torch.empty((q.shape[0], 4), dtype=torch.float32, device=q.device)
-        _engine_for(q).crf_energy_dev(q, unary, image, params, terms, features=features, compat=compat,
-                                      stream=_stream(q))
+        fwd = _engine_for(q).crf_energy_wide_dev if wide else _engine_for(q).crf_energy_dev
+        fwd(q, unary, image, params, terms, features=features, compat=compat, stream=_stream(q))
         ctx.save_for_backward(q, unary, image, features, compat)
-        ctx.params = params
+        ctx.params, ctx.wide = params, wide
         return terms
 
     @staticmethod
@@ -677,10 +678,41 @@ class _DenseCrfEnergy(torch.autograd.Function):
         q, unary, image, features, compat = ctx.saved_tensors
         grad_q = torch.empty_like(q)
         grad_u = torch.empty_like(q) if unary is not None and ctx.needs_input_grad[1] else None
-        _engine_for(q).crf_energy_backward_dev(q, unary, image, ctx.params, g.float().contiguous(), grad_q,
-                                               grad_unary=grad_u, features=features, compat=compat,
-                                               stream=_stream(q))
-        return grad_q if ctx.needs_input_grad[0] else None, grad_u, None, None, None, None
+        eng = _engine_for(q)
+        bwd = eng.crf_energy_backward_wide_dev if ctx.wide else eng.crf_energy_backward_dev
+        bwd(q, unary, image, ctx.params, g.float().contiguous(), grad_q, grad_unary=grad_u, features=features,
+            compat=compat, stream=_stream(q))
+        return grad_q if ctx.needs_input_grad[0] else None, grad_u, None, None, None, None, None
+
+
+def _energy_args(q, unary, image, scale_factor, color_factor, w1, w2, compat_bi, compat_sp, theta_bi, theta_sp,
+                 features_bi, wide):
+    """dense_crf_energy's and dense_crf_energy_wide's arguments, every check before the first launch -> the arguments
+    of _DenseCrfEnergy.  wide: dense_crf_energy_wide, which takes 1 to 255 labels and runs 32 or fewer as
+    dense_crf_energy does."""
+    if torch.is_autocast_enabled("cuda"):
+        q = q.float() if isinstance(q, torch.Tensor) and q.is_floating_point() else q
+        unary = unary.float() if isinstance(unary, torch.Tensor) and unary.is_floating_point() else unary
+        if isinstance(features_bi, torch.Tensor) and features_bi.is_floating_point():
+            features_bi = features_bi.float()
+    name_of = "dense_crf_energy_wide" if wide else "dense_crf_energy"
+    for name, t in (("w1", w1), ("w2", w2), ("compat_bi", compat_bi), ("compat_sp", compat_sp),
+                    ("theta_bi", theta_bi), ("theta_sp", theta_sp), ("features_bi", features_bi)):
+        if isinstance(t, torch.Tensor) and t.requires_grad:
+            raise ValueError("%s requires grad: %s differentiates q and unary only (detach it)" % (name, name_of))
+    qq = _maps(q, "q")
+    M = qq.shape[1]
+    if not wide and M > FUSED_LABELS:
+        raise ValueError("dense_crf_energy supports at most %d labels (got %d)" % (FUSED_LABELS, M))
+    u = None if unary is None else _like(unary, qq, "unary")
+    if features_bi is None:
+        image = _image(image, qq)
+    elif image is not None:
+        raise ValueError("image is not used when features_bi is given: pass None")
+    _cuda(qq, "q")
+    params = api.crf_params(float(scale_factor), float(color_factor), 0)
+    f, compat = _learned_crf(qq, *qq.shape, params, w1, w2, compat_bi, compat_sp, theta_bi, theta_sp, features_bi)
+    return qq, u, image, f, compat, params, M > FUSED_LABELS
 
 
 def dense_crf_energy(q, unary, image, scale_factor=1.0, color_factor=13, w1=None, w2=None, compat_bi=None,
@@ -698,29 +730,19 @@ def dense_crf_energy(q, unary, image, scale_factor=1.0, color_factor=13, w1=None
     exact for the function the device computes.  A term's pairwise energy alone (``terms[:, 2:].sum()``) is the
     dense-CRF regulariser of weakly-supervised segmentation.  The parameters get no gradient: a parameter tensor that
     requires grad is refused.  A features_bi image whose lattice keys leave the packed range gets NaN terms and
-    gradients."""
-    if torch.is_autocast_enabled("cuda"):
-        q = q.float() if isinstance(q, torch.Tensor) and q.is_floating_point() else q
-        unary = unary.float() if isinstance(unary, torch.Tensor) and unary.is_floating_point() else unary
-        if isinstance(features_bi, torch.Tensor) and features_bi.is_floating_point():
-            features_bi = features_bi.float()
-    for name, t in (("w1", w1), ("w2", w2), ("compat_bi", compat_bi), ("compat_sp", compat_sp),
-                    ("theta_bi", theta_bi), ("theta_sp", theta_sp), ("features_bi", features_bi)):
-        if isinstance(t, torch.Tensor) and t.requires_grad:
-            raise ValueError("%s requires grad: dense_crf_energy differentiates q and unary only (detach it)" % name)
-    qq = _maps(q, "q")
-    M = qq.shape[1]
-    if M > FUSED_LABELS:
-        raise ValueError("dense_crf_energy supports at most %d labels (got %d)" % (FUSED_LABELS, M))
-    u = None if unary is None else _like(unary, qq, "unary")
-    if features_bi is None:
-        image = _image(image, qq)
-    elif image is not None:
-        raise ValueError("image is not used when features_bi is given: pass None")
-    _cuda(qq, "q")
-    params = api.crf_params(float(scale_factor), float(color_factor), 0)
-    f, compat = _learned_crf(qq, *qq.shape, params, w1, w2, compat_bi, compat_sp, theta_bi, theta_sp, features_bi)
-    return _DenseCrfEnergy.apply(qq, u, image, f, compat, params)
+    gradients.  dense_crf_energy_wide takes up to 255 labels."""
+    return _DenseCrfEnergy.apply(*_energy_args(q, unary, image, scale_factor, color_factor, w1, w2, compat_bi,
+                                               compat_sp, theta_bi, theta_sp, features_bi, wide=False))
+
+
+def dense_crf_energy_wide(q, unary, image, scale_factor=1.0, color_factor=13, w1=None, w2=None, compat_bi=None,
+                          compat_sp=None, theta_bi=None, theta_sp=None, features_bi=None):
+    """dense_crf_energy for any label count from 1 to 255 (COCO's 81 classes): the same arguments, checks, terms and
+    gradients to q and unary.  At 32 labels or fewer it is dense_crf_energy itself; above that the energy and its
+    gradient run on the label-chunked kernels, with the same operation order per value and no device memory beyond
+    dense_crf_energy's per-block sums."""
+    return _DenseCrfEnergy.apply(*_energy_args(q, unary, image, scale_factor, color_factor, w1, w2, compat_bi,
+                                               compat_sp, theta_bi, theta_sp, features_bi, wide=True))
 
 
 def softmax(fc8):

@@ -259,6 +259,25 @@ int dsrg_crf_energy_backward_dev(dsrg_engine *e, const float *q_dev, int B, cons
                                  const float *potts_dev, const float *compat_dev, const float *grad_terms_dev,
                                  float *grad_q_dev, float *grad_unary_dev, void *stream);
 /*
+ * The energy and its gradient above DSRG_MAX_LABELS labels (DSRG_MAX_LABELS < M <= DSRG_MAX_LABELS_WIDE, e.g. COCO's
+ * 81): the label-chunked twins of dsrg_crf_energy_dev / dsrg_crf_energy_backward_dev, with the same arguments in the
+ * same order, the same terms, gradient, feature-range policy and graph capture, and the same operation order per value.
+ * An engine of 32 labels or fewer is refused with DSRG_E_INVALID before anything is allocated or queued: the fused pair
+ * serves it, so each label count has one path.  Neither call leaves marginals for the *_last_* entry points.  The
+ * first call of either allocates what the fused energy's does, the per-block sums: maxB * ceil(H*W/256) * 32 bytes,
+ * 4480 bytes for an engine of batch 20 @ 41x41 and 103168 bytes for one of batch 8 @ 321x321, both with 81 labels
+ * (dsrg_engine_device_bytes before and after; the backward adds nothing), and with features the feature passes'
+ * flags.  The blurred values use the mean field's value buffers, and the matrices' messages its marginal planes.
+ */
+int dsrg_crf_energy_wide_dev(dsrg_engine *e, const float *q_dev, int B, const float *unary_dev,
+                             const uint8_t *image_dev, const float *features_dev, const dsrg_crf_params *params,
+                             const float *potts_dev, const float *compat_dev, float *terms_dev, void *stream);
+int dsrg_crf_energy_backward_wide_dev(dsrg_engine *e, const float *q_dev, int B, const float *unary_dev,
+                                      const uint8_t *image_dev, const float *features_dev,
+                                      const dsrg_crf_params *params, const float *potts_dev, const float *compat_dev,
+                                      const float *grad_terms_dev, float *grad_q_dev, float *grad_unary_dev,
+                                      void *stream);
+/*
  * The training forward and its backward above DSRG_MAX_LABELS labels (DSRG_MAX_LABELS < M <= DSRG_MAX_LABELS_WIDE,
  * e.g. COCO's 81), on the label-chunked kernels of dsrg_crf_batch_dev at those counts.  The arguments mean what they
  * mean in dsrg_crf_forward_train_dev / dsrg_crf_backward_dev and their _compat twins: potts_dev ({w1, w2}) or
